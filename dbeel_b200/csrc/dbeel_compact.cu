@@ -24,6 +24,7 @@
 #include "merge_final.cuh"
 #include "gather_async.cuh"
 #include "gather_fb.cuh"
+#include "gather_h.cuh"
 #include "lookup.cuh"
 #include "route.cuh"
 #include "wal.cuh"
@@ -85,7 +86,7 @@ struct dbeel_engine {
     int sm_count = 0; // multiProcessorCount of the device, set at engine creation
     int merge_variant = 1;      // DBEEL_MERGE: 0 = one CTA per tile with plain loads, 1 = persistent TMA (default)
     int narrow_loads = 1;       // DBEEL_NARROW: .L2::64B loads for random accesses in extract / resolve (A/B switch)
-    int gather_variant = 10;    // DBEEL_GATHER: 10 = k_gather32 with the lean entry-boundary pass (default), 0 = 16 bytes per lane (k_gather),
+    int gather_variant = 11;    // DBEEL_GATHER: 11 = k_gather_h (default), 10 = k_gather32 with the lean entry-boundary pass, 0 = 16 bytes per lane (k_gather),
                                 //               1 = 32 bytes per lane + 32-byte block stores (k_gather32, the two-halves boundary pass),
                                 //               2 = 1 with the payload staged into shared memory by TMA bulk copies (k_gather_tma)
     int fused_emit = 0;         // DBEEL_FUSED_EMIT: 1 = resolve + offsets scan + .index writes in one kernel (single jobs), 0 = four kernels
@@ -607,7 +608,9 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
     // ---- K5: gather + bloom (fused epilogue)
     if (gather_tiles) {
         const bool al32 = ((uintptr_t)out->data & 31) == 0; // 32-byte block stores
-        if (e->gather_variant == 2 && al32) { // persistent, payload staged through shared memory by the bulk-copy engine
+        if (e->gather_variant == 11) { // the default: 16-byte vectors, the filter kept in L2 (gather_h.cuh)
+            launch_k(e, k_gather_h, (uint32_t)gather_tiles, kGhThreads, 0, s, p);
+        } else if (e->gather_variant == 2 && al32) { // persistent, payload staged through shared memory by the bulk-copy engine
             uint64_t grid = (uint64_t)e->sm_count * DBEEL_GT_CTAS;
             if (grid > gather_tiles) grid = gather_tiles;
             launch_k(e, k_gather_tma, (uint32_t)grid, kGtThreads, kGtSmem, s, p);
@@ -621,7 +624,7 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
             launch_k(e, k_gather_fb, (uint32_t)gather_tiles, kFbThreads, 0, s, p);
         } else if (e->gather_variant == 7 && al32) { // payload lands in shared memory (cp.async), boundary blocks + filter while it travels
             launch_k(e, k_gather_async, (uint32_t)gather_tiles, kGatherThreads, 0, s, p);
-        } else if (e->gather_variant >= 9 && al32) { // the default: k_gather32 with the lean entry-boundary pass (aligned 32-byte chunks, one store per block)
+        } else if (e->gather_variant >= 9 && al32) { // k_gather32 with the lean entry-boundary pass (aligned 32-byte chunks, one store per block)
             launch_k(e, k_gather32<false, false, false, true>, (uint32_t)gather_tiles, kGatherThreads, 0, s, p);
         } else if (e->gather_variant == 5 && al32) { // k_gather32, boundary blocks and filter on different warps (no gain)
             launch_k(e, k_gather32<false, true, false>, (uint32_t)gather_tiles, kGatherThreads, 0, s, p);

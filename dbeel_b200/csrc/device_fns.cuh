@@ -203,6 +203,23 @@ DB_HD void realign16(const uint32_t A[4], const uint32_t B[4], uint32_t sh, uint
     out[3] = funnel_r(w3, w4, bits);
 }
 
+// Which aligned 16-byte chunks of the window {A, B} that realign16(A, B, s0) reads hold output bytes [lo, hi)
+// (0 <= lo < hi <= 16): bit 0 = A (bytes [0, 16 - s0) of the output), bit 1 = B (the rest).  A chunk whose bit is
+// clear may hold anything.
+DB_HD uint32_t chunks16(uint32_t s0, uint32_t lo, uint32_t hi) {
+    return (lo < 16u - s0 ? 1u : 0u) | (hi > 16u - s0 ? 2u : 0u);
+}
+
+// out = bytes [0, t) of T followed by bytes [t, 16) of H, t in 0..16.
+DB_HD void blend16(const uint32_t T[4], const uint32_t H[4], uint32_t t, uint32_t out[4]) {
+    const uint32_t wfull = t >> 2, bits = (t & 3) * 8;
+    const uint32_t mmix = bits ? (0xFFFFFFFFu >> (32 - bits)) : 0u;
+    for (uint32_t q = 0; q < 4; q++) {
+        const uint32_t mk = q < wfull ? 0xFFFFFFFFu : (q == wfull ? mmix : 0u);
+        out[q] = (T[q] & mk) | (H[q] & ~mk);
+    }
+}
+
 // 32 output bytes starting `s0` (0..31) bytes into the 64-byte window w[0..16) (little-endian words, lower address first).
 // Words of the window that hold no wanted byte may contain anything.
 DB_HD void window32(const uint32_t w[16], uint32_t s0, uint32_t out[8]) {

@@ -185,6 +185,18 @@ __device__ __forceinline__ uint64_t ld_u64_unaligned(const uint8_t *p) {
     return (lo >> sh) | (hi << (64 - sh));
 }
 
+// Per-instruction L2 cache policy (it travels in the access's memory descriptor; no device-level carve-out).  The gather
+// streams ~4 GB of payload through the 50 MB L2 while the bloom filter (~10 MB at the benchmark shapes) takes scattered
+// REDs: marking the REDs evict_last keeps filter sectors resident between two touches.
+__device__ __forceinline__ uint64_t l2_evict_last() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ void red_or_keep(uint32_t *q, uint32_t v, uint64_t pol) {
+    asm volatile("red.global.or.L2::cache_hint.b32 [%0], %1, %2;" ::"l"(q), "r"(v), "l"(pol) : "memory");
+}
+
 __device__ __forceinline__ Rec ld_rec(const Rec *p) {
     uint4 v = *reinterpret_cast<const uint4 *>(p);
     Rec r;
