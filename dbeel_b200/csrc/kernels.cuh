@@ -774,7 +774,7 @@ __device__ __forceinline__ uint32_t find_pair(const uint32_t *tb, uint32_t pairs
 // one ballot), 5 rounds for a 4M-record diagonal instead of 22 dependent global-memory round trips.
 constexpr int kPartitionThreads = 256;
 
-__global__ void __launch_bounds__(kPartitionThreads) k_merge_partition(Params p, uint32_t level, const Rec *src) {
+__global__ void __launch_bounds__(kPartitionThreads) k_merge_partition(const __grid_constant__ Params p, uint32_t level, const Rec *src) {
     pdl_trigger();
     pdl_wait();
     const uint32_t pairs = p.nseg[level + 1];
@@ -967,7 +967,7 @@ __device__ __forceinline__ void tma_store_1d(void *gmem_dst, const void *smem_sr
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gmem_dst), "r"(smem_u32(smem_src)), "r"(bytes) : "memory");
 }
 
-__global__ void __launch_bounds__(kMergeThreads, kMergeCtasPerSM) k_merge_tma(Params p, uint32_t level, const Rec *src, Rec *dst) {
+__global__ void __launch_bounds__(kMergeThreads, kMergeCtasPerSM) k_merge_tma(const __grid_constant__ Params p, uint32_t level, const Rec *src, Rec *dst) {
     pdl_trigger();
     pdl_wait();
     extern __shared__ __align__(128) uint8_t s_raw[];

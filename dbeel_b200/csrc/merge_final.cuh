@@ -12,10 +12,10 @@
 //   resolve                         7 independent chains per thread: index record by gid (64-byte granule), timestamp only
 //                                   for members of a group; the head of a group picks max (timestamp, run position) over
 //                                   shared memory (lsm_tree.rs:1036-1066, mod.rs:75-81) and applies the tombstone rule
-//   scan                            (bytes, entries) of the tile's survivors; chained scan over the tiles with a 256-wide
-//                                   look-back (tiles are taken in order by co-resident persistent CTAs, so a predecessor is
-//                                   always running or done)
-//   emit                            output .index records, src_ptr, tile_first (entry_writer.rs:76-86) straight from registers
+//   scan                            (bytes, entries) of the tile's survivors; chained scan over the tiles, the aggregate
+//                                   published at once, the one-warp look-back deferred by one tile (see the tile loop)
+//   emit                            output .index records, src_ptr, tile_first (entry_writer.rs:76-86) from the survivors
+//                                   kept in shared memory, one tile later
 //
 // What no longer exists: the last level's 16 B/entry write, k_resolve's 16 B read + 16 B `res` write, k_emit's 16 B read,
 // three kernel boundaries and the two scan kernels.
@@ -35,6 +35,33 @@ constexpr int kFinMaxRunsSmem = 64;            // run tables (base / index / dat
 #endif
 constexpr uint32_t kFinSmem = 2u * kFinBufRecs * 16u + 2u * kFinTile * 8u + (uint32_t)kFinTile + 16u;
 
+// Measurement builds only (`python -m dbeel_b200._build --variant phases DBEEL_FIN_PHASES`): thread 0 of every CTA books the
+// clock64() time between consecutive marks -- most taken right after a CTA-wide wait, so such a phase is its slowest
+// thread's -- and the last CTA of a launch prints the sums over all CTAs, then clears them.  Outputs are those of the
+// normal build.
+#ifdef DBEEL_FIN_PHASES
+constexpr int kFinPhases = 8;
+__device__ unsigned long long g_fin_phase[kFinPhases];
+__device__ unsigned int g_fin_done;
+#define FIN_PH_DECL unsigned long long ph_acc[kFinPhases] = {}; long long ph_t = clock64();
+#define FIN_PH(k) do { if (tid == 0) { const long long ph_n = clock64(); ph_acc[k] += (unsigned long long)(ph_n - ph_t); ph_t = ph_n; } } while (0)
+__device__ __forceinline__ void fin_phase_flush(const unsigned long long *acc, uint32_t n_tiles) { // thread 0
+    for (int k = 0; k < kFinPhases; k++) atomicAdd(&g_fin_phase[k], acc[k]);
+    __threadfence();
+    if (atomicAdd(&g_fin_done, 1u) + 1 == (gridDim.x < n_tiles ? gridDim.x : n_tiles)) { // CTAs without a tile return early
+        __threadfence();
+        unsigned long long v[kFinPhases], tot = 0;
+        for (int k = 0; k < kFinPhases; k++) { v[k] = atomicExch(&g_fin_phase[k], 0ull); tot += v[k]; }
+        g_fin_done = 0;
+        printf("fin_phases ctas=%u cycles=%llu tma=%llu merge=%llu index_issue=%llu index_wait=%llu lookback=%llu emit=%llu "
+               "ts_wait=%llu heads_scan=%llu\n", gridDim.x, tot, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+    }
+}
+#else
+#define FIN_PH_DECL
+#define FIN_PH(k) do {} while (0)
+#endif
+
 struct FinDesc {
     uint32_t a_src, n_a, b_src, n_b; // record offsets into src, counts
     uint32_t a_end, b_end;           // one past the last record of segment A / B (absolute)
@@ -42,8 +69,59 @@ struct FinDesc {
     uint32_t nb;                     // bit 0: A[a0-1] exists, 1: A[a1] exists, 2: B[b0-1] exists, 3: B[b1] exists
 };
 
+// Decoupled look-back of tile t > 0 by one warp: lane l reads the state of predecessors t-1-4l ... t-4-4l (all four loads in
+// flight together), waits only for a predecessor that has published nothing yet, and the walk stops at the nearest one that
+// holds an inclusive prefix.  (eb, ec) = bytes and entries of every tile before t, in every lane.
+__device__ __forceinline__ void fin_lookback(const unsigned long long *scan_state, uint32_t t, uint32_t lane, unsigned long long &eb,
+                                             uint32_t &ec) {
+    constexpr int kPer = 4;
+    eb = 0;
+    ec = 0;
+    for (int base = (int)t - 1;; base -= 32 * kPer) {
+        unsigned long long vb[kPer], vc[kPer];
+#pragma unroll
+        for (int k = 0; k < kPer; k++) {
+            const int idx = base - (int)lane * kPer - k;
+            vb[k] = kScanPrefix << 62; // tiles before the first one: a prefix of nothing
+            vc[k] = kScanPrefix << 32;
+            if (idx >= 0) {
+                vc[k] = ld_volatile_u64(scan_state + 2ull * (uint32_t)idx + 1);
+                vb[k] = ld_volatile_u64(scan_state + 2ull * (uint32_t)idx);
+            }
+        }
+        bool found = false;
+        unsigned long long sb = 0;
+        uint32_t sc = 0;
+#pragma unroll
+        for (int k = 0; k < kPer; k++) {
+            const int idx = base - (int)lane * kPer - k;
+            // each word says what it holds: both at the same stage, or read the pair again
+            while ((vc[k] >> 32) == 0 || (vc[k] >> 32) != (vb[k] >> 62)) {
+                vc[k] = ld_volatile_u64(scan_state + 2ull * (uint32_t)idx + 1);
+                vb[k] = ld_volatile_u64(scan_state + 2ull * (uint32_t)idx);
+            }
+            if (!found) {
+                sb += vb[k] & ((1ull << 62) - 1);
+                sc += (uint32_t)vc[k];
+                found = (vc[k] >> 32) == kScanPrefix;
+            }
+        }
+        const uint32_t fm = __ballot_sync(0xFFFFFFFFu, found);
+        const uint32_t first = fm ? (uint32_t)__ffs((int)fm) - 1u : 32u; // the lane holding the nearest prefix
+        if (lane > first) { sb = 0; sc = 0; }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            sb += __shfl_xor_sync(0xFFFFFFFFu, sb, o);
+            sc += __shfl_xor_sync(0xFFFFFFFFu, sc, o);
+        }
+        eb += sb;
+        ec += sc;
+        if (fm) return;
+    }
+}
+
 template <bool kNarrow>
-__global__ void __launch_bounds__(kFinThreads, DBEEL_FIN_CTAS) k_merge_final(Params p, uint32_t level, const Rec *src) {
+__global__ void __launch_bounds__(kFinThreads, DBEEL_FIN_CTAS) k_merge_final(const __grid_constant__ Params p, uint32_t level, const Rec *src) {
     constexpr int NT = kFinThreads, VT = kFinVT;
     extern __shared__ __align__(128) uint8_t f_raw[];
     Rec *bufs[2] = {reinterpret_cast<Rec *>(f_raw), reinterpret_cast<Rec *>(f_raw) + kFinBufRecs};
@@ -54,9 +132,7 @@ __global__ void __launch_bounds__(kFinThreads, DBEEL_FIN_CTAS) k_merge_final(Par
     __shared__ Rec s_bnd[5]; // A[a0-1], A[a1], B[b0-1], B[b1], the tile's last record
     __shared__ unsigned long long s_wb[NT / 32];
     __shared__ uint32_t s_wc[NT / 32];
-    __shared__ unsigned long long s_pref_b;
-    __shared__ uint32_t s_pref_c;
-    __shared__ uint32_t s_first[NT / 32];
+    __shared__ unsigned long long s_pref[2];
     __shared__ uint32_t s_rbase[kFinMaxRunsSmem + 1];
     __shared__ uint8_t s_rlut[256]; // run that holds gid (b << lut_shift): a record's run is that one or a close successor
     __shared__ const uint4 *s_rindex[kFinMaxRunsSmem];
@@ -85,9 +161,11 @@ __global__ void __launch_bounds__(kFinThreads, DBEEL_FIN_CTAS) k_merge_final(Par
     if (tid == 0) {
         mbar_init(&s_bar[0], 1);
         mbar_init(&s_bar[1], 1);
+        s_pref[0] = s_pref[1] = ~0ull; // tag 0xFFFF: no tile's
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
+    FIN_PH_DECL
 
     // entry address / key_size / full_size of the entry behind a gid: its run's index record (64-byte granule)
     auto run_of = [&](uint32_t gid) -> uint32_t {
@@ -137,7 +215,71 @@ __global__ void __launch_bounds__(kFinThreads, DBEEL_FIN_CTAS) k_merge_final(Par
     if (tid == 0) issue(cur, bufs[0], &s_bar[0]);
     const int keep_tombstones = p.keep_tombstones;
 
-    for (uint32_t q = 0;; q++) {
+    // One-tile software pipeline: tile q publishes its aggregate as soon as it is resolved, and its look-back and emit run in
+    // the next iteration, after tile q+1 has been merged and its index loads are in flight (or after the loop, for the CTA's
+    // last tile).  By then the tiles before q have had one iteration to publish, so the look-back rarely waits.
+    // Why a tile never waits on a CTA that is waiting on it: the look-back of tile t waits only for tiles < t to publish their
+    // aggregates, and a CTA publishes the aggregate of its tile t after running only the look-backs of its own earlier tiles
+    // (all < t) and nothing that waits on a later tile.  By induction on t every aggregate gets published, given that every
+    // CTA holding a tile is resident -- the same co-residency as a non-pipelined chained scan, which the grid is sized for
+    // at engine creation.
+    // Tile q's survivors wait in s_tlo / s_thi (entry address / {key_size, full_size}), free between the last head of q and
+    // the timestamp stores of q+1.  A thread keeps its survivors in the very slots it later stores its own timestamps to
+    // (d + i, d = 7 * tid whenever it has records), so neither the emit nor those stores need a CTA barrier -- a barrier
+    // would wait for the timestamp loads in flight.  The look-back's result reaches the other warps the same way, through
+    // two shared words that each carry the tile's tag.
+    uint32_t prev_tile = 0, prev_d = 0, prev_act = 0, prev_pos = 0, prev_tc = 0;
+    unsigned long long prev_off = 0, prev_tb = 0;
+    volatile unsigned long long *vpref = s_pref; // {tag << 48 | bytes before the tile (< 2^48), tag << 32 | entries before it}
+    auto finish_prev = [&](uint32_t prev_q) {
+        const unsigned long long tag = prev_q & 0xFFFFu; // differs from the previous tile's (and from the initial 0xFFFF at q = 0)
+        if (warp == 0) { // the look-back is one warp's: 128 predecessors per step, stops at the nearest inclusive prefix
+            unsigned long long eb = 0;
+            uint32_t ec = 0;
+            if (prev_tile > 0) fin_lookback(p.scan_state, prev_tile, lane, eb, ec);
+            if (lane == 0) {
+                if (prev_tile > 0) {
+                    unsigned long long *mine = p.scan_state + 2ull * prev_tile;
+                    st_volatile_u64(mine, (kScanPrefix << 62) | (eb + prev_tb));
+                    st_volatile_u64(mine + 1, (kScanPrefix << 32) | (unsigned long long)(ec + prev_tc));
+                }
+                vpref[0] = (tag << 48) | eb;
+                vpref[1] = (tag << 32) | ec;
+                if (prev_tile + 1 == n_tiles) { // the last tile holds the totals
+                    Ctl *cw = p.ctl;
+                    cw->out_data_len = eb + prev_tb;
+                    cw->out_items = ec + prev_tc;
+                }
+            }
+        }
+        unsigned long long pb, pc;
+        do {
+            pb = vpref[0];
+            pc = vpref[1];
+        } while ((pb >> 48) != tag || (pc >> 32) != tag);
+        FIN_PH(4);
+        // ---- emit: .index records (entry_writer.rs:76-86), source addresses, gather-tile markers
+        unsigned long long off = (pb & ((1ull << 48) - 1)) + prev_off; // within this job's .data
+        uint32_t pos = (uint32_t)pc + prev_pos;
+        constexpr unsigned long long gt = kGatherTileBytes;
+#pragma unroll
+        for (int i = 0; i < VT; i++) {
+            if (!((prev_act >> i) & 1u)) continue;
+            const unsigned long long sz = s_thi[prev_d + i];
+            const uint32_t fs = (uint32_t)(sz >> 32);
+            if (!fs) continue;
+            const unsigned long long file_off = off + p.out_offset_base;
+            p.out_index[pos] = make_uint4((uint32_t)file_off, (uint32_t)(file_off >> 32), (uint32_t)sz, fs);
+            p.src_ptr[pos] = s_tlo[prev_d + i];
+            for (unsigned long long bq = (off + gt - 1) / gt; bq * gt < off + fs && bq < p.tile_first_n; bq++) p.tile_first[bq] = pos;
+            off += fs;
+            pos++;
+        }
+        FIN_PH(5);
+    };
+
+    uint32_t q = 0;
+    for (;; q++) {
         Rec *s = bufs[q & 1];
         uint4 *s4 = reinterpret_cast<uint4 *>(s);
         const bool has_next = tile + G < n_tiles;
@@ -145,6 +287,7 @@ __global__ void __launch_bounds__(kFinThreads, DBEEL_FIN_CTAS) k_merge_final(Par
         const FinDesc nn = mk_desc(bidx2);            // consumed one iteration from now
         const uint32_t bidx3 = ld_bidx(tile + 3 * G); // ... and two iterations from now
         while (!mbar_try_wait(&s_bar[q & 1], (q >> 1) & 1)) {}
+        FIN_PH(0);
 
         // ---- merge-path: thread t produces merged records [7t, 7t + 7) of the tile
         const uint32_t nA = cur.n_a, nB = cur.n_b, n = nA + nB;
@@ -183,6 +326,7 @@ __global__ void __launch_bounds__(kFinThreads, DBEEL_FIN_CTAS) k_merge_final(Par
                 if (d + i == n - 1) s_bnd[4] = me[i];
         }
         __syncthreads();
+        FIN_PH(1);
 
         // ---- resolve, part 1: group flags from the neighbours' keys, index record of every entry
         uint32_t m_act = 0, m_eqn = 0, m_eqp = 0;
@@ -224,43 +368,47 @@ __global__ void __launch_bounds__(kFinThreads, DBEEL_FIN_CTAS) k_merge_final(Par
             }
         }
         __syncthreads(); // every neighbour key has been read: the tile's slots may now hold {entry address, key_size, full_size}
-        uint4 we[VT]; // what is written for position d + i: {entry address, key_size, full_size or 0}; first the entry itself
+        FIN_PH(2);
         {
             const uint32_t m_grp = m_act & (m_eqn | m_eqp); // members of a group of two or more
             unsigned long long tlo[VT], thi[VT];
 #pragma unroll
             for (int i = 0; i < VT; i++) {
                 tlo[i] = thi[i] = 0;
-                we[i] = make_uint4(0, 0, 0, 0);
                 if (!(m_act & (1u << i))) continue;
                 const uint32_t r = run_of(gidv[i]);
                 const uint8_t *entry = data_ptr(r) + ((uint64_t)irec[i].x | ((uint64_t)irec[i].y << 32));
                 const unsigned long long ea = (unsigned long long)(uintptr_t)entry;
-                we[i] = make_uint4((uint32_t)ea, (uint32_t)(ea >> 32), irec[i].z, irec[i].w);
-                if ((m_grp >> i) & 1u) { // its timestamp decides (mod.rs:80); only group members go through shared memory
+                // {entry address, key_size, full_size} of position d + i; in shared memory, not registers, across the emit below
+                s4[d + i] = make_uint4((uint32_t)ea, (uint32_t)(ea >> 32), irec[i].z, irec[i].w);
+                if ((m_grp >> i) & 1u) { // its timestamp decides (mod.rs:80)
                     const uint8_t *t = entry + irec[i].w - 16;
                     if (kNarrow) { tlo[i] = ld_u64_unaligned_narrow(t); thi[i] = ld_u64_unaligned_narrow(t + 8); }
                     else { tlo[i] = ld_u64_unaligned(t); thi[i] = ld_u64_unaligned(t + 8); }
-                    s4[d + i] = we[i];
                     s_flag[d + i] = (uint8_t)((m_eqn >> i) & 1u);
                 }
             }
+            FIN_PH(3);
+            // the previous tile's look-back and emit while this tile's timestamps travel: no CTA barrier until they are stored
+            if (q > 0) finish_prev(q - 1);
 #pragma unroll
             for (int i = 0; i < VT; i++) {
                 if ((m_grp >> i) & 1u) { s_tlo[d + i] = tlo[i]; s_thi[d + i] = thi[i]; }
             }
         }
         __syncthreads();
+        FIN_PH(6);
 
         // ---- resolve, part 2: heads pick their group's winner; the tombstone rule (lsm_tree.rs:1045-1046)
         unsigned long long vb = 0;
         uint32_t vc = 0;
+        uint4 we[VT]; // what is written for position d + i: {entry address, key_size, full_size or 0}
 #pragma unroll
         for (int i = 0; i < VT; i++) {
-            uint4 info = we[i];
-            we[i].w = 0;
+            we[i] = make_uint4(0, 0, 0, 0);
             if (!((m_act >> i) & 1u) || ((m_eqp >> i) & 1u)) continue; // not a head
             const uint32_t k = d + i;
+            uint4 info = s4[k];
             if ((m_eqn >> i) & 1u) {
                 unsigned long long wlo = s_tlo[k], whi = s_thi[k];
                 uint32_t j = k;
@@ -312,7 +460,7 @@ __global__ void __launch_bounds__(kFinThreads, DBEEL_FIN_CTAS) k_merge_final(Par
             if (lane >= (uint32_t)o) { ib += xb; ic += xc; }
         }
         if (lane == 31) { s_wb[warp] = ib; s_wc[warp] = ic; }
-        __syncthreads();
+        __syncthreads(); // every head is done with s_tlo / s_thi / s4
         unsigned long long tb = 0, wbefore = 0;
         uint32_t tc = 0, wcbefore = 0;
 #pragma unroll
@@ -321,102 +469,44 @@ __global__ void __launch_bounds__(kFinThreads, DBEEL_FIN_CTAS) k_merge_final(Par
             tb += s_wb[w];
             tc += s_wc[w];
         }
-        unsigned long long *mine = p.scan_state + 2ull * tile;
-        if (tile == 0) {
-            if (tid == 0) {
-                st_volatile_u64(mine, (kScanPrefix << 62) | tb);
-                st_volatile_u64(mine + 1, (kScanPrefix << 32) | tc);
-                s_pref_b = 0;
-                s_pref_c = 0;
-            }
-            __syncthreads();
-        } else {
-            // Each word says what it holds (aggregate or inclusive prefix): a reader needs both words at the same stage and simply
-            // reads again when it caught the pair mid-update -- no fence on either side.
-            if (tid == 0) {
-                st_volatile_u64(mine, (kScanAgg << 62) | tb);
-                st_volatile_u64(mine + 1, (kScanAgg << 32) | tc);
-            }
-            unsigned long long eb = 0;
-            uint32_t ec = 0;
-            int base = (int)tile - 1;
-            while (true) { // 256 predecessors per step: thread t looks at tile base - t
-                const int idx = base - (int)tid;
-                unsigned long long vb2 = 0, vc2 = 0, stat = kScanPrefix; // tiles before the first one: a prefix of nothing
-                if (idx >= 0) {
-                    const unsigned long long *qs = p.scan_state + 2ull * (uint32_t)idx;
-                    while (true) {
-                        vc2 = ld_volatile_u64(qs + 1);
-                        vb2 = ld_volatile_u64(qs);
-                        if ((vc2 >> 32) != 0 && (vc2 >> 32) == (vb2 >> 62)) break;
-                    }
-                    stat = vc2 >> 32;
-                    vb2 &= (1ull << 62) - 1;
-                    vc2 &= 0xFFFFFFFFull;
-                }
-                // the nearest predecessor that already holds an inclusive prefix ends the walk
-                const uint32_t pm = __ballot_sync(0xFFFFFFFFu, stat == kScanPrefix);
-                __syncthreads(); // s_first / s_wb / s_wc of the previous step (or of the tile scan) have been read
-                if (lane == 0) s_first[warp] = pm ? (warp * 32u + (uint32_t)__ffs((int)pm) - 1u) : 0xFFFFFFFFu;
-                __syncthreads();
-                uint32_t first = 0xFFFFFFFFu;
-#pragma unroll
-                for (int w = 0; w < NT / 32; w++) first = s_first[w] < first ? s_first[w] : first;
-                unsigned long long cb = tid <= first ? vb2 : 0ull;
-                uint32_t cc = tid <= first ? (uint32_t)vc2 : 0u;
-#pragma unroll
-                for (int o = 16; o; o >>= 1) {
-                    cb += __shfl_xor_sync(0xFFFFFFFFu, cb, o);
-                    cc += __shfl_xor_sync(0xFFFFFFFFu, cc, o);
-                }
-                if (lane == 0) { s_wb[warp] = cb; s_wc[warp] = cc; }
-                __syncthreads();
-#pragma unroll
-                for (int w = 0; w < NT / 32; w++) { eb += s_wb[w]; ec += s_wc[w]; }
-                if (first != 0xFFFFFFFFu) break;
-                base -= NT;
-            }
-            if (tid == 0) {
-                st_volatile_u64(mine, (kScanPrefix << 62) | (eb + tb));
-                st_volatile_u64(mine + 1, (kScanPrefix << 32) | (unsigned long long)(ec + tc));
-                s_pref_b = eb;
-                s_pref_c = ec;
-            }
-            __syncthreads();
+        if (tid == 0) { // tile 0's aggregate is its inclusive prefix; no other tile waits for anything before publishing
+            // Each word says what it holds (aggregate or inclusive prefix): a reader needs both words at the same stage and
+            // simply reads again when it caught the pair mid-update -- no fence on either side.
+            const unsigned long long st = tile == 0 ? kScanPrefix : kScanAgg;
+            unsigned long long *mine = p.scan_state + 2ull * tile;
+            st_volatile_u64(mine, (st << 62) | tb);
+            st_volatile_u64(mine + 1, (st << 32) | tc);
         }
-        const unsigned long long pref_b = s_pref_b;
-        const uint32_t pref_c = s_pref_c;
-        if (tile + 1 == n_tiles && tid == 0) { // the last tile holds the totals
-            Ctl *cw = p.ctl;
-            cw->out_data_len = pref_b + tb;
-            cw->out_items = pref_c + tc;
-        }
-
-        // ---- emit: .index records (entry_writer.rs:76-86), source addresses, gather-tile markers
-        {
-            unsigned long long off = pref_b + wbefore + ib - vb; // within this job's .data
-            uint32_t pos = pref_c + wcbefore + ic - vc;
-            constexpr unsigned long long gt = kGatherTileBytes;
 #pragma unroll
-            for (int i = 0; i < VT; i++) {
-                const uint32_t fs = we[i].w;
-                if (!fs) continue;
-                const unsigned long long file_off = off + p.out_offset_base;
-                p.out_index[pos] = make_uint4((uint32_t)file_off, (uint32_t)(file_off >> 32), we[i].z, fs);
-                p.src_ptr[pos] = (unsigned long long)we[i].x | ((unsigned long long)we[i].y << 32);
-                for (unsigned long long bq = (off + gt - 1) / gt; bq * gt < off + fs && bq < p.tile_first_n; bq++) p.tile_first[bq] = pos;
-                off += fs;
-                pos++;
+        for (int i = 0; i < VT; i++) {
+            if ((m_act >> i) & 1u) {
+                s_tlo[d + i] = (unsigned long long)we[i].x | ((unsigned long long)we[i].y << 32);
+                s_thi[d + i] = (unsigned long long)we[i].z | ((unsigned long long)we[i].w << 32);
             }
         }
-        if (!has_next) break;
+        prev_tile = tile;
+        prev_d = d;
+        prev_act = m_act;
+        prev_off = wbefore + ib - vb;
+        prev_pos = wcbefore + ic - vc;
+        prev_tb = tb;
+        prev_tc = tc;
+        if (!has_next) {
+            FIN_PH(7);
+            break;
+        }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy accesses of this buffer before the next bulk copy into it
-        __syncthreads(); // s_pref / s_bnd / the tile buffer are free for the next tile
+        __syncthreads(); // s_bnd / the tile buffer are free for the next tile
+        FIN_PH(7);
         tile += G;
         cur = nxt;
         nxt = nn;
         bidx2 = bidx3;
     }
+    finish_prev(q);
+#ifdef DBEEL_FIN_PHASES
+    if (tid == 0) fin_phase_flush(ph_acc, n_tiles);
+#endif
 }
 
 } // namespace dbeel

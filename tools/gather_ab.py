@@ -145,10 +145,10 @@ def main():
     print("\nspec: median [min, max] over rounds, ms")
     for s in specs:
         summary[s or "default"] = row = {}
-        for k in ("ms_gather", "ms_total"):
+        for k in STAGES:
             v = [t[k] for t in times[s]]
             row[k] = {"median": round(statistics.median(v), 4), "min": round(min(v), 4), "max": round(max(v), 4)}
-        print(f"{s or 'default':50s} gather {row['ms_gather']}  total {row['ms_total']}")
+        print(f"{s or 'default':50s} " + "  ".join(f"{k[3:]} {row[k]}" for k in STAGES))
     out["ab"] = summary
     out["profile"] = {}
     for s in args.profile:
