@@ -22,6 +22,9 @@ DEFAULT_TREE_CAPACITY = 8192  # mod.rs:18
 LOOKUP_REFERENCE = 0  # the reference's binary_search loop, step for step (lsm_tree.rs:605-670)
 LOOKUP_EXACT = 1      # lower-bound search: every present key is found
 LOOKUP_CORRUPT = 0x80000000
+SCAN_HASH = 0  # ranges: (start, end) u32 pairs, murmur3_32(key) tested with migration.rs's between_cmp
+SCAN_KEY = 1   # ranges: (start, end) byte strings, start <= key < end
+SCAN_STOP_NONE, SCAN_STOP_ERR, SCAN_STOP_PANIC = 0, 1, 2
 ERR_UNSORTED_RUN = 8
 ERR_CAPACITY = 2
 ERR_INVALID_ARG = 1
@@ -39,7 +42,8 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_bloom_bitmap_bytes", "dbeel_bloom_k_num", "dbeel_bloom_file_size", "dbeel_host_alloc",
            "dbeel_host_free", "dbeel_last_stats", "dbeel_last_error", "dbeel_strerror",
            "dbeel_murmur3_32", "dbeel_ring_owner", "dbeel_shard_ring", "dbeel_route_device", "dbeel_flush_many_sparse_device",
-           "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream"]
+           "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream",
+           "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device"]
 
 
 class Run(C.Structure):
@@ -78,6 +82,29 @@ class JobResult(C.Structure):
 class Table(C.Structure):
     _fields_ = [("data", C.c_void_p), ("data_len", C.c_uint64), ("index", C.c_void_p), ("index_len", C.c_uint64),
                 ("bloom", C.c_void_p), ("bloom_len", C.c_uint64)]
+
+
+class KeyRanges(C.Structure):
+    _fields_ = [("keys", C.c_void_p), ("key_offsets", C.c_void_p)]
+
+
+class ScanStop(C.Structure):
+    _fields_ = [("table", C.c_int32), ("reason", C.c_uint32), ("record", C.c_uint64)]
+
+    def as_tuple(self):
+        """(table, reason, record); (-1, SCAN_STOP_NONE, 0) when every record was read."""
+        return int(self.table), int(self.reason), int(self.record)
+
+
+def pack_ranges(kind: int, ranges):
+    """The `ranges` argument of dbeel_scan: hash ranges as a u32 array, key ranges as a KeyRanges over a packed blob.
+    Returns (pointer-bearing object, things to keep alive)."""
+    if kind == SCAN_HASH:
+        arr = np.ascontiguousarray(np.array([[int(a), int(b)] for a, b in ranges], dtype=np.uint32).reshape(-1))
+        return arr.ctypes.data, (arr,)
+    blob, off = pack_keys([bytes(k) for pair in ranges for k in pair])
+    kr = KeyRanges(blob.ctypes.data if blob.size else None, off.ctypes.data)
+    return C.addressof(kr), (kr, blob, off)
 
 
 class LookupResult(C.Structure):
@@ -171,6 +198,13 @@ def lib():
             f.restype = C.c_int
             f.argtypes = [C.c_void_p, C.POINTER(Table), C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
                           C.c_void_p]
+        L.dbeel_scan_bound.restype = C.c_int
+        L.dbeel_scan_bound.argtypes = [C.POINTER(Table), C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+        for name in ("dbeel_scan", "dbeel_scan_device"):
+            f = getattr(L, name)
+            f.restype = C.c_int
+            f.argtypes = [C.c_void_p, C.POINTER(Table), C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(Out),
+                          C.POINTER(JobResult), C.POINTER(ScanStop)]
         L.dbeel_compact_many_bound.restype = C.c_int
         L.dbeel_compact_many_bound.argtypes = [C.POINTER(Job), C.c_uint32, C.c_uint64, C.c_double] + [C.POINTER(C.c_uint64)] * 3
         for name in ("dbeel_compact_many", "dbeel_compact_many_device"):
@@ -567,6 +601,45 @@ class Engine:
             arr[j] = Table(t[0], t[1], t[2], t[3], t[4] if t[5] else None, t[5])
         self._check(lib().dbeel_get_many_device(self._h, arr, len(tables), keys_ptr, offsets_ptr, n_keys, mode,
                                                 results_ptr), "dbeel_get_many_device")
+
+    # ---- N5: scans (LSMTree::iter_filter) ---------------------------------------------------
+    def scan(self, tables: Sequence[Tuple[object, ...]], ranges, kind: int = SCAN_HASH):
+        """dbeel_scan over host buffers.  tables: (data, index[, bloom]) oldest first; ranges: (start, end) u32 pairs
+        (SCAN_HASH) or byte strings (SCAN_KEY).  Returns ([(data, index)] per range, (table, reason, record) of the stop)."""
+        keep = [(_u8(t[0]), _u8(t[1])) for t in tables]
+        arr = (Table * max(1, len(keep)))()
+        for j, (d, i) in enumerate(keep):
+            arr[j] = Table(d.ctypes.data, d.size, i.ctypes.data, i.size, None, 0)
+        rptr, _rkeep = pack_ranges(kind, ranges)
+        # dbeel_scan_bound (the files' sizes), or more when index records share .data bytes: each record is delivered at most once
+        dc = sum(max(d.size, int(i[:i.size // 16 * 16].reshape(-1, 16)[:, 12:16].copy().view("<u4").astype(np.uint64).sum()))
+                 for d, i in keep)
+        ic = sum(i.size for _, i in keep)
+        od, oi = np.empty(max(1, dc), np.uint8), np.empty(max(16, ic), np.uint8)
+        out = Out(od.ctypes.data, dc, 0, oi.ctypes.data, ic, 0, None, 0, 0, 0)
+        n = len(ranges)
+        res = (JobResult * max(1, n))()
+        stop = ScanStop()
+        self._check(lib().dbeel_scan(self._h, arr, len(keep), kind, rptr, n, C.byref(out), res, C.byref(stop)), "dbeel_scan")
+        return ([(od[r.data_off:r.data_off + r.data_len], oi[r.index_off:r.index_off + r.index_len]) for r in res[:n]],
+                stop.as_tuple())
+
+    def scan_device(self, tables: Sequence[Tuple[int, int, int, int]], ranges, out_ptrs: Tuple[int, int, int, int],
+                    kind: int = SCAN_HASH):
+        """dbeel_scan_device: tables (data_ptr, data_len, index_ptr, index_len) and out_ptrs (data_ptr, data_cap, index_ptr,
+        index_cap) in device memory.  Returns (JobResult rows as dicts, (table, reason, record) of the stop)."""
+        arr = (Table * max(1, len(tables)))()
+        for j, t in enumerate(tables):
+            arr[j] = Table(t[0], t[1], t[2], t[3], None, 0)
+        rptr, _rkeep = pack_ranges(kind, ranges)
+        dp, dc, ip, ic = out_ptrs
+        out = Out(dp, dc, 0, ip, ic, 0, None, 0, 0, 0)
+        n = len(ranges)
+        res = (JobResult * max(1, n))()
+        stop = ScanStop()
+        self._check(lib().dbeel_scan_device(self._h, arr, len(tables), kind, rptr, n, C.byref(out), res, C.byref(stop)),
+                    "dbeel_scan_device")
+        return [{k: int(getattr(r, k)) for k, _ in JobResult._fields_} for r in res[:n]], stop.as_tuple()
 
     # ---- device buffers (raw pointers; torch tensors own the memory) -------------------
     def compact_device(self, runs: Sequence[Tuple[int, int, int, int]], out_ptrs: Tuple[int, int, int, int, int, int],

@@ -27,6 +27,7 @@
 #include "gather_h.cuh"
 #include "lookup.cuh"
 #include "route.cuh"
+#include "scan.cuh"
 #include "wal.cuh"
 #include "host/stream_pump.h"
 
@@ -1845,6 +1846,244 @@ int compact_many_entry(dbeel_engine *e, const dbeel_job *jobs, uint32_t n_jobs, 
     return DBEEL_OK;
 }
 
+// ------------------------------------------------------------------------------------ N5: scans (iter_filter)
+
+int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges, uint32_t n_ranges,
+               dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop, bool device) {
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (!out || !results || !stop || !ranges || (n_tables && !tables)) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    if (kind > DBEEL_SCAN_KEY) return fail(e, DBEEL_ERR_INVALID_ARG, "unknown scan kind");
+    if (n_ranges == 0 || n_ranges > DBEEL_MAX_SCAN_RANGES) return fail(e, DBEEL_ERR_INVALID_ARG, "1 to DBEEL_MAX_SCAN_RANGES ranges");
+    if (n_tables > DBEEL_MAX_RUNS) return fail(e, DBEEL_ERR_INVALID_ARG, "more than DBEEL_MAX_RUNS tables");
+    const dbeel_key_ranges *kr = static_cast<const dbeel_key_ranges *>(ranges);
+    uint64_t key_bytes = 0;
+    if (kind == DBEEL_SCAN_KEY) {
+        if (!kr->key_offsets) return fail(e, DBEEL_ERR_INVALID_ARG, "null key offsets");
+        for (uint32_t k = 0; k < 2 * n_ranges; k++)
+            if (kr->key_offsets[k + 1] < kr->key_offsets[k]) return fail(e, DBEEL_ERR_INVALID_ARG, "key offsets must ascend");
+        key_bytes = kr->key_offsets[2 * n_ranges] - kr->key_offsets[0];
+        if (key_bytes && !kr->keys) return fail(e, DBEEL_ERR_INVALID_ARG, "null range keys");
+    }
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    e->stats = dbeel_stats{};
+    out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
+    for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+    *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+    uint64_t n64 = 0, data_total = 0, index_total = 0;
+    unsigned long long stop0 = ~0ull; // an empty table: its first index read runs past EOF
+    for (uint32_t t = 0; t < n_tables; t++) {
+        const dbeel_table &tb = tables[t];
+        if ((tb.data_len && !tb.data) || (tb.index_len >= 16 && !tb.index)) return fail(e, DBEEL_ERR_INVALID_ARG, "null table buffer");
+        if (device && ((uintptr_t)tb.index & 15)) return fail(e, DBEEL_ERR_INVALID_ARG, "device .index buffers must be 16-byte aligned");
+        if (tb.index_len < 16 && stop0 == ~0ull) stop0 = (n64 << 12) | ((unsigned long long)t << 2) | kScanStopPanic;
+        n64 += tb.index_len / DBEEL_INDEX_ENTRY_SIZE;
+        data_total += tb.data_len;
+        index_total += tb.index_len;
+    }
+    if (n64 >= 0xFFFFFFF0ull) return fail(e, DBEEL_ERR_INVALID_ARG, "too many index records");
+    if (device && (((uintptr_t)out->data | (uintptr_t)out->index) & 15))
+        return fail(e, DBEEL_ERR_INVALID_ARG, "device output buffers must be 16-byte aligned");
+    e->stats.input_bytes = data_total + index_total;
+    e->stats.entries_in = n64;
+    const uint32_t n = (uint32_t)n64;
+    std::vector<uint32_t> base(n_tables + 1, 0);
+    for (uint32_t t = 0; t < n_tables; t++) base[t + 1] = base[t] + (uint32_t)(tables[t].index_len / DBEEL_INDEX_ENTRY_SIZE);
+    auto set_stop = [&](unsigned long long key) {
+        if (key == ~0ull) return;
+        const uint32_t t = (uint32_t)((key >> 2) & 1023);
+        *stop = dbeel_scan_stop{(int32_t)t, (uint32_t)(key & 3), (key >> 12) - base[t]};
+    };
+    if (n == 0) { set_stop(stop0); return DBEEL_OK; }
+    cudaError_t ce = cudaSetDevice(e->device);
+    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    cudaStream_t s = e->stream;
+
+    // host tables go down whole (16 bytes of slack behind every buffer: the 8-byte header loads may run past an entry)
+    std::vector<ScanTable> td(n_tables);
+    if (!device) {
+        uint64_t need = 0;
+        for (uint32_t t = 0; t < n_tables; t++) need += align_up(tables[t].data_len + 32, kAlign) + align_up(tables[t].index_len + 16, kAlign);
+        int rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, need);
+        if (rc) return rc;
+        uint64_t pos = 0;
+        for (uint32_t t = 0; t < n_tables; t++) {
+            const dbeel_table &tb = tables[t];
+            uint8_t *dd = e->stage_in + pos;
+            pos += align_up(tb.data_len + 32, kAlign);
+            uint8_t *di = e->stage_in + pos;
+            pos += align_up(tb.index_len + 16, kAlign);
+            if (tb.data_len) CU(cudaMemcpyAsync(dd, tb.data, tb.data_len, cudaMemcpyHostToDevice, s));
+            if (tb.index_len) CU(cudaMemcpyAsync(di, tb.index, tb.index_len, cudaMemcpyHostToDevice, s));
+            td[t] = ScanTable{dd, tb.data_len, reinterpret_cast<const uint4 *>(di), base[t + 1] - base[t], base[t]};
+        }
+    } else {
+        for (uint32_t t = 0; t < n_tables; t++)
+            td[t] = ScanTable{static_cast<const uint8_t *>(tables[t].data), tables[t].data_len, static_cast<const uint4 *>(tables[t].index),
+                              base[t + 1] - base[t], base[t]};
+    }
+
+    // ---- workspace (the engine's grow-only one: a compaction after a scan reuses it as it is)
+    const uint32_t nd = n_ranges;
+    const uint32_t n_blocks = (n + kRouteThreads - 1) / kRouteThreads;
+    const uint64_t res_tiles = (n + kResolveThreads - 1) / kResolveThreads, res_chunks = (res_tiles + 1023) / 1024;
+    uint64_t off = 0;
+    auto carve = [&](uint64_t b) { uint64_t o2 = off; off = align_up(off + b, kAlign); return o2; };
+    // header block, one copy through the mapped pinned block: tables | hash ranges or key offsets | range keys
+    const uint64_t o_tab = carve(sizeof(ScanTable) * n_tables);
+    const uint64_t o_rng = carve(kind == DBEEL_SCAN_KEY ? 8ull * (2 * nd + 1) : 8ull * nd);
+    const uint64_t o_keys = carve(key_bytes + 16);
+    const uint64_t header_bytes = off;
+    // second header, after the split is known: control block | per-destination (bytes, entries) before it
+    const uint64_t o_ctl = carve(sizeof(Ctl));
+    const uint64_t o_memtab = carve(16ull * (nd + 1));
+    const uint64_t header2_bytes = off - o_ctl;
+    const uint64_t o_tot = carve(8ull * (3 * nd + 1));
+    const uint64_t o_dest = carve(4ull * n), o_flat = carve(16ull * n), o_split = carve(16ull * n);
+    const uint64_t o_hist = carve(4ull * n_blocks * nd);
+    const uint64_t o_tbytes = carve(8 * res_tiles), o_tcount = carve(4 * res_tiles);
+    const uint64_t o_cbytes = carve(8 * res_chunks), o_ccount = carve(4 * res_chunks);
+    const uint64_t o_src = carve(8ull * n);
+    int rc = ensure_device(e, &e->ws, &e->ws_cap, off);
+    const uint64_t pin_tot = align_up(std::max(header_bytes, header2_bytes), 64);
+    if (!rc) rc = ensure_pinned(e, pin_tot + 8ull * (3 * nd + 1));
+    if (rc) return rc;
+    uint8_t *ws = e->ws, *h = e->pin;
+    memcpy(h + o_tab, td.data(), sizeof(ScanTable) * n_tables);
+    if (kind == DBEEL_SCAN_KEY) {
+        uint64_t *ko = reinterpret_cast<uint64_t *>(h + o_rng);
+        for (uint32_t k = 0; k <= 2 * nd; k++) ko[k] = kr->key_offsets[k] - kr->key_offsets[0];
+        if (key_bytes) memcpy(h + o_keys, static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0], key_bytes);
+    } else {
+        memcpy(h + o_rng, ranges, 8ull * nd);
+    }
+
+    ScanParams sp = {};
+    sp.tables = reinterpret_cast<const ScanTable *>(ws + o_tab);
+    sp.n_tables = n_tables;
+    sp.n = n;
+    sp.key_kind = kind == DBEEL_SCAN_KEY ? 1u : 0u;
+    sp.n_ranges = nd;
+    sp.hash_ranges = reinterpret_cast<const uint32_t *>(ws + o_rng);
+    sp.key_off = reinterpret_cast<const unsigned long long *>(ws + o_rng);
+    sp.keys = ws + o_keys;
+    sp.dest = reinterpret_cast<uint32_t *>(ws + o_dest);
+    sp.flat = reinterpret_cast<uint4 *>(ws + o_flat);
+    sp.stop = reinterpret_cast<unsigned long long *>(ws + o_tot) + 3ull * nd;
+    sp.stop0 = stop0;
+    RouteParams rp = {};
+    rp.index = sp.flat;
+    rp.n = n;
+    rp.n_shards = nd;
+    rp.n_blocks = n_blocks;
+    rp.shard_of = sp.dest;
+    rp.hist = reinterpret_cast<uint32_t *>(ws + o_hist);
+    rp.totals = reinterpret_cast<unsigned long long *>(ws + o_tot);
+    rp.out_index = reinterpret_cast<uint4 *>(ws + o_split);
+
+    // ---- phase 1: classify, split; the per-destination counts and bytes come back to size phase 2
+    uint32_t launches = 0;
+    CU(cudaEventRecord(e->ev[EV_START], s));
+    launch_k(e, k_copy_words, (uint32_t)((header_bytes / 4 + 255) / 256), 256, 0, s, reinterpret_cast<uint32_t *>(ws),
+             reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(header_bytes / 4));
+    CU(cudaMemsetAsync(rp.totals, 0, 8ull * 3 * nd, s));
+    CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
+    launch_k(e, k_scan_classify, (n + 255) / 256, 256, 0, s, sp);
+    launch_k(e, k_scan_hist, n_blocks, kRouteThreads, 0, s, sp, rp);
+    launch_k(e, k_route_scan, nd, 1024, 0, s, rp);
+    unsigned long long *host_tot = reinterpret_cast<unsigned long long *>(e->pin + pin_tot);
+    launch_k(e, k_route_starts, 1, 256, 0, s, rp, reinterpret_cast<unsigned long long *>(e->pin_dev + pin_tot));
+    launch_k(e, k_route_scatter, n_blocks, kRouteThreads, 0, s, rp);
+    launches += 6;
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(s));
+    const unsigned long long stop_key = std::min<unsigned long long>(host_tot[3 * nd], stop0);
+    set_stop(stop_key);
+    e->stats.entries_valid = stop_key == ~0ull ? n : (stop_key >> 12);
+    uint64_t items = 0, bytes = 0;
+    for (uint32_t d = 0; d < nd; d++) {
+        dbeel_job_result &r = results[d];
+        r.data_off = bytes;
+        r.data_len = host_tot[nd + d];
+        r.index_off = 16 * items;
+        r.items_written = host_tot[d];
+        r.index_len = 16 * host_tot[d];
+        items += host_tot[d];
+        bytes += host_tot[nd + d];
+    }
+    if (bytes > out->data_cap || 16 * items > out->index_cap) {
+        for (uint32_t d = 0; d < nd; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+        return fail(e, DBEEL_ERR_CAPACITY, "scan output larger than the buffers (index records that overlap in .data)");
+    }
+    if (device && ((bytes && !out->data) || (items && !out->index))) return fail(e, DBEEL_ERR_INVALID_ARG, "null output buffer");
+    // What depends on the output size is sized now that it is known -- records that share .data bytes can make the output
+    // larger than the inputs: the gather's tile_first (one entry per 8 KB output tile) and, for host callers, the staged
+    // outputs.  They live in stage_out, so the phase-1 workspace (the split records) stays where it is.
+    const uint64_t gather_tiles = (bytes + kGatherTileBytes - 1) / kGatherTileBytes;
+    const uint64_t tf_bytes = align_up(4ull * (gather_tiles + 2), kAlign);
+    rc = ensure_device(e, &e->stage_out, &e->stage_out_cap,
+                       tf_bytes + (device ? 0 : align_up(bytes + 16, kAlign) + align_up(16 * items + 16, kAlign)));
+    if (rc) return rc;
+    uint32_t *tile_first = reinterpret_cast<uint32_t *>(e->stage_out);
+    uint8_t *o_data = device ? static_cast<uint8_t *>(out->data) : e->stage_out + tf_bytes;
+    uint8_t *o_index = device ? static_cast<uint8_t *>(out->index) : e->stage_out + tf_bytes + align_up(bytes + 16, kAlign);
+
+    // ---- phase 2: .index (k_emit's offsets scan), payload gather, per-destination file offsets
+    if (items) {
+        Ctl *hc = reinterpret_cast<Ctl *>(h);
+        memset(hc, 0, sizeof(Ctl));
+        hc->span = (uint32_t)items;
+        hc->total = (uint32_t)items;
+        unsigned long long *hm = reinterpret_cast<unsigned long long *>(h + (o_memtab - o_ctl));
+        for (uint32_t d = 0; d <= nd; d++) {
+            hm[2 * d] = d < nd ? results[d].data_off : bytes;
+            hm[2 * d + 1] = d < nd ? results[d].index_off / 16 : items;
+        }
+        Params p;
+        memset(&p, 0, sizeof p);
+        p.ctl = reinterpret_cast<Ctl *>(ws + o_ctl);
+        p.tile_bytes = reinterpret_cast<unsigned long long *>(ws + o_tbytes);
+        p.tile_count = reinterpret_cast<uint32_t *>(ws + o_tcount);
+        p.chunk_bytes = reinterpret_cast<unsigned long long *>(ws + o_cbytes);
+        p.chunk_count = reinterpret_cast<uint32_t *>(ws + o_ccount);
+        p.src_ptr = reinterpret_cast<unsigned long long *>(ws + o_src);
+        p.tile_first = tile_first;
+        p.tile_first_n = (uint32_t)(gather_tiles + 2);
+        p.n_groups = nd;
+        p.mem_table = reinterpret_cast<unsigned long long *>(ws + o_memtab);
+        p.out_data = o_data;
+        p.out_index = reinterpret_cast<uint4 *>(o_index);
+        const uint4 *split = rp.out_index;
+        const uint32_t tiles = (uint32_t)((items + kResolveThreads - 1) / kResolveThreads);
+        launch_k(e, k_copy_words, (uint32_t)((header2_bytes / 4 + 255) / 256), 256, 0, s, reinterpret_cast<uint32_t *>(ws + o_ctl),
+                 reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(header2_bytes / 4));
+        launch_k(e, k_scan_tile_sums, tiles, kResolveThreads, 0, s, p, split, (uint32_t)items);
+        launch_k(e, k_scan_tiles, (tiles + 1023) / 1024, 1024, 0, s, p);
+        launch_k(e, k_scan_chunks, 1, 1024, 0, s, p);
+        launch_k(e, k_emit, tiles, kResolveThreads, 0, s, p, split);
+        launch_k(e, k_gather_h, (uint32_t)gather_tiles, kGhThreads, 0, s, p); // no filter: Params.bloom.words is null
+        launch_k(e, k_rebase_index, (uint32_t)((items + 255) / 256), 256, 0, s, p);
+        launches += 7;
+    }
+    CU(cudaEventRecord(e->ev[EV_GATHER], s));
+    CU(cudaGetLastError());
+    if (!device) {
+        if (bytes) CU(cudaMemcpyAsync(out->data, o_data, bytes, cudaMemcpyDeviceToHost, s));
+        if (items) CU(cudaMemcpyAsync(out->index, o_index, 16 * items, cudaMemcpyDeviceToHost, s));
+    }
+    CU(cudaStreamSynchronize(s));
+    cudaEventElapsedTime(&e->stats.ms_total, e->ev[EV_START], e->ev[EV_GATHER]);
+    e->stats.kernel_launches = launches;
+    e->stats.entries_out = items;
+    e->stats.output_bytes = bytes + 16 * items;
+    e->stats.gather_bytes = 2 * bytes + 16 * items + 8 * items;
+    out->data_len = bytes;
+    out->index_len = 16 * items;
+    out->items_written = items;
+    return DBEEL_OK;
+}
+
 } // namespace
 
 // ------------------------------------------------------------------------------------ C ABI
@@ -2153,6 +2392,27 @@ int dbeel_get_many_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n
                           const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_lookup_result *results) {
     REFUSE_WHILE_ASYNC(e);
     return lookup_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, results, true);
+}
+
+int dbeel_scan_bound(const dbeel_table *tables, uint32_t n_tables, uint64_t *data_cap, uint64_t *index_cap) {
+    if (n_tables && !tables) return DBEEL_ERR_INVALID_ARG;
+    uint64_t d = 0, i = 0;
+    for (uint32_t t = 0; t < n_tables; t++) { d += tables[t].data_len; i += tables[t].index_len; }
+    if (data_cap) *data_cap = d;
+    if (index_cap) *index_cap = i;
+    return DBEEL_OK;
+}
+
+int dbeel_scan(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges, uint32_t n_ranges,
+               dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop) {
+    REFUSE_WHILE_ASYNC(e);
+    return scan_entry(e, tables, n_tables, kind, ranges, n_ranges, out, results, stop, false);
+}
+
+int dbeel_scan_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
+                      uint32_t n_ranges, dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop) {
+    REFUSE_WHILE_ASYNC(e);
+    return scan_entry(e, tables, n_tables, kind, ranges, n_ranges, out, results, stop, true);
 }
 
 int dbeel_compact_many_bound(const dbeel_job *jobs, uint32_t n_jobs, uint64_t bloom_min_size, double bloom_fp, uint64_t *data_cap,

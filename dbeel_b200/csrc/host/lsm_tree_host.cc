@@ -631,6 +631,26 @@ int dbeel_tree_get_many(dbeel_tree *t, const void *keys, const uint64_t *key_off
     return rc;
 }
 
+int dbeel_tree_scan(dbeel_tree *t, uint32_t kind, const void *ranges, uint32_t n_ranges, dbeel_out *out, dbeel_job_result *results,
+                    dbeel_scan_stop *stop) {
+    if (!t) return DBEEL_ERR_INVALID_ARG;
+    t->err.clear();
+    // AsyncIter reads `self.sstables` (ascending index) oldest first (lsm_tree.rs:182-188, 214-246)
+    const size_t n = t->sstables.size();
+    std::vector<PinnedBuf> data(n), index(n);
+    std::vector<dbeel_table> tables(n);
+    for (size_t i = 0; i < n; i++) {
+        const uint64_t idx = t->sstables[i].index;
+        int rc = read_file(t, file_path(t->dir, idx, kData), &data[i]);
+        if (!rc) rc = read_file(t, file_path(t->dir, idx, kIndex), &index[i]);
+        if (rc) return rc;
+        tables[i] = dbeel_table{data[i].p, data[i].len, index[i].p, index[i].len, nullptr, 0};
+    }
+    int rc = dbeel_scan(t->engine, tables.data(), (uint32_t)n, kind, ranges, n_ranges, out, results, stop);
+    if (rc) t->err = dbeel_last_error(t->engine);
+    return rc;
+}
+
 int dbeel_tree_recover_wal(dbeel_tree *t, uint32_t tree_capacity, uint64_t *wal_file_index, uint64_t *items_written) {
     if (!t) return DBEEL_ERR_INVALID_ARG;
     t->err.clear();

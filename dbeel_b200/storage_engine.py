@@ -9,6 +9,7 @@ All the work happens in the C++/CUDA library; this file only marshals arguments.
 from __future__ import annotations
 
 import ctypes as C
+import os
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -48,6 +49,9 @@ def _lib():
                                               C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.c_char_p]
         L.dbeel_tree_get_many.restype = C.c_int
         L.dbeel_tree_get_many.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p]
+        L.dbeel_tree_scan.restype = C.c_int
+        L.dbeel_tree_scan.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(capi.Out),
+                                      C.POINTER(capi.JobResult), C.POINTER(capi.ScanStop)]
         L.dbeel_tree_recover_wal.restype = C.c_int
         L.dbeel_tree_recover_wal.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         L.dbeel_tree_last_error.restype = C.c_char_p
@@ -67,7 +71,7 @@ def _lib():
 
 
 TREE_EXPORTS = ["dbeel_tree_open", "dbeel_tree_close", "dbeel_tree_sstables", "dbeel_tree_write_sstable_index",
-                "dbeel_tree_compact", "dbeel_tree_compact_many", "dbeel_tree_flush", "dbeel_tree_recover_wal", "dbeel_tree_get_many", "dbeel_tree_last_error", "dbeel_memtable_cut",
+                "dbeel_tree_compact", "dbeel_tree_compact_many", "dbeel_tree_flush", "dbeel_tree_recover_wal", "dbeel_tree_get_many", "dbeel_tree_scan", "dbeel_tree_last_error", "dbeel_memtable_cut",
                 "dbeel_plan_compactions", "dbeel_out_pages", "dbeel_tree_set_page_sink"]
 
 
@@ -184,6 +188,26 @@ class LSMTree:
             o, ks, fs = int.from_bytes(rec[:8], "little"), int.from_bytes(rec[8:12], "little"), int.from_bytes(rec[12:], "little")
             out.append(bytes(d[o + ks + 8:o + fs - 16]))  # EntryValue.data (entry = key | dlen | data | ts)
         return out
+
+    def scan(self, ranges, kind: int = capi.SCAN_HASH):
+        """The SSTable part of iter_filter (lsm_tree.rs:133-282) over the tree's files, oldest table first: every entry
+        goes to the first of `ranges` that accepts it ((start, end) u32 hash ranges with between_cmp, or byte-string key
+        ranges).  Returns ([(data, index)] per range, (table, reason, record) of the first record the reference's iterator
+        fails on, table = position in sstable_indices_and_sizes() order).  The memtables are the caller's."""
+        from . import sstable
+        dc = ic = 0
+        for idx, _ in self.sstable_indices_and_sizes():
+            dc += os.path.getsize(os.path.join(self.dir, sstable.file_name(idx, sstable.DATA_FILE_EXT)))
+            ic += os.path.getsize(os.path.join(self.dir, sstable.file_name(idx, sstable.INDEX_FILE_EXT)))
+        od, oi = np.empty(max(1, dc), np.uint8), np.empty(max(16, ic), np.uint8)
+        out = capi.Out(od.ctypes.data, dc, 0, oi.ctypes.data, ic, 0, None, 0, 0, 0)
+        rptr, _keep = capi.pack_ranges(kind, ranges)
+        n = len(ranges)
+        res = (capi.JobResult * max(1, n))()
+        stop = capi.ScanStop()
+        self._check(_lib().dbeel_tree_scan(self._h, kind, rptr, n, C.byref(out), res, C.byref(stop)), "LSMTree.scan")
+        return ([(od[r.data_off:r.data_off + r.data_len].copy(), oi[r.index_off:r.index_off + r.index_len].copy())
+                 for r in res[:n]], stop.as_tuple())
 
     def recover_wal(self, tree_capacity: int = capi.DEFAULT_TREE_CAPACITY) -> Tuple[int, int]:
         """open_or_create_ex's WAL step (lsm_tree.rs:466-513): with two `.memtable` files the older one is replayed and

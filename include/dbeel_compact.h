@@ -27,6 +27,8 @@
  *                          (lsm_tree.rs:605-670, 686-719) for a batch of keys        ["next" row N2]
  *   dbeel_wal_flush*    <- read_memtable_from_wal_file + the recovery flush of open_or_create_ex
  *                          (lsm_tree.rs:552-574, 478-513)                            ["next" row N4]
+ *   dbeel_scan*         <- the SSTable part of LSMTree::iter_filter (lsm_tree.rs:133-282) with migrate_actions' hash-range
+ *                          filter (src/tasks/migration.rs:54-131) or a key range                ["next" row N5]
  *   dbeel_bloom_*       <- Bloom::new_for_fp_rate sizing (lsm_tree.rs:1028-1031)
  *   error codes         <- src/error.rs:8-74 (only the variants this path can raise)
  *
@@ -327,6 +329,57 @@ int dbeel_get_many(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables
                    const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_lookup_result *results);
 int dbeel_get_many_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys,
                           const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_lookup_result *results);
+
+/* ---- N5: scans -- LSMTree::iter_filter over a tree's SSTables ------------------------------------------------------
+ * Replaces the SSTable part of AsyncIter (src/storage_engine/lsm_tree.rs:133-282, iter_filter :1183-1189) with its filter
+ * for the two uses the reference has: migration (migrate_actions, src/tasks/migration.rs:62-131: murmur3_32 of the key in
+ * one of a list of hash ranges) and key-range reads ([start, end) in Vec<u8> order, lsm_tree.rs:1363-1397).
+ * tables[] is the tree's `sstables` vector, oldest first, read in that order; every table's floor(index_len / 16) records in
+ * order, each entry read at its EntryOffset's (offset, full_size) -- key_size is ignored, offsets need not be running.  No
+ * dedupe, no tombstone rule: duplicates across tables and tombstones come out as stored.  The memtable part of the
+ * iterator (emitted after the tables, :155-173) stays with the caller.
+ *
+ * Every accepted entry goes to the FIRST range that accepts it:
+ *   DBEEL_SCAN_HASH  ranges = uint32_t[2 * n_ranges] (start, end) pairs; range d accepts murmur3_32(key, 0) = h when
+ *                    between_cmp(h, start, end) (migration.rs:54-60, restated literally: for end < start every hash, for
+ *                    start == end none).
+ *   DBEEL_SCAN_KEY   ranges = a dbeel_key_ranges: range d accepts start_d <= key < end_d.
+ * Destination d's entries are written, in iteration order, as one SSTable pair: results[d] says where it lies in out->data /
+ * out->index (file-relative .index offsets, key_size = 8 + key length, bloom_len = 0).  Each pair is a valid arrival
+ * batch for dbeel_flush / dbeel_route_device.
+ *
+ * The reference decodes before it filters (lsm_tree.rs:273), so the first record that does not decode ends the scan even
+ * where no range would have taken it; what precedes it is delivered.  *stop reports it:
+ *   DBEEL_SCAN_STOP_ERR    next() returns Err: the entry is not exactly one bincode Entry of full_size bytes, or its
+ *                          timestamp is outside time's +-9999 years (utils/timestamp_nanos.rs:15-24).
+ *   DBEEL_SCAN_STOP_PANIC  the reference panics: full_size == 0 (cached_file_reader.rs:82), bytes past the end of .data
+ *                          (:68), or a table with no index record (its first index read runs past EOF).
+ * Limits: n_tables <= DBEEL_MAX_RUNS, 1 <= n_ranges <= DBEEL_MAX_SCAN_RANGES, fewer than 2^32 - 16 records in all; else
+ * DBEEL_ERR_INVALID_ARG.  Output caps: dbeel_scan_bound (entries whose index records overlap can exceed it:
+ * DBEEL_ERR_CAPACITY, nothing written).  The tables' bloom fields are ignored.
+ * dbeel_scan takes host memory and uploads the tables whole; dbeel_scan_device takes device pointers for tables / out
+ * (.index 16-byte aligned, outputs 16-byte aligned), ranges / results / stop stay in host memory in both. */
+#define DBEEL_SCAN_HASH 0u
+#define DBEEL_SCAN_KEY 1u
+#define DBEEL_MAX_SCAN_RANGES 256u
+#define DBEEL_SCAN_STOP_NONE 0u
+#define DBEEL_SCAN_STOP_ERR 1u
+#define DBEEL_SCAN_STOP_PANIC 2u
+typedef struct dbeel_key_ranges {
+    const void *keys;            /* start_d = keys[off[2d] .. off[2d+1]), end_d = keys[off[2d+1] .. off[2d+2]) */
+    const uint64_t *key_offsets; /* 2 * n_ranges + 1 byte offsets */
+} dbeel_key_ranges;
+typedef struct dbeel_scan_stop {
+    int32_t table;   /* position in tables[] of the first failing record, -1 = the scan read every record */
+    uint32_t reason; /* DBEEL_SCAN_STOP_* */
+    uint64_t record; /* its index record number in that table */
+} dbeel_scan_stop;
+/* data_cap = sum(data_len), index_cap = sum(index_len) (host arithmetic only) */
+int dbeel_scan_bound(const dbeel_table *tables, uint32_t n_tables, uint64_t *data_cap, uint64_t *index_cap);
+int dbeel_scan(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
+               uint32_t n_ranges, dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop);
+int dbeel_scan_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
+                      uint32_t n_ranges, dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop);
 
 /* ---- N4: write-ahead-log replay + flush ------------------------------------------------------------------------
  * Replaces LSMTree::read_memtable_from_wal_file (lsm_tree.rs:552-574) followed by flush_memtable_to_disk, i.e. the

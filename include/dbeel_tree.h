@@ -17,6 +17,7 @@
  *                             next even index through dbeel_flush(), no bloom
  *   dbeel_tree_sstables    <- LSMTree::sstable_indices_and_sizes (lsm_tree.rs:592-598)
  *   dbeel_tree_get_many    <- the SSTable loop of LSMTree::get_entry (lsm_tree.rs:686-719) through dbeel_get_many()
+ *   dbeel_tree_scan        <- the SSTable part of LSMTree::iter_filter (lsm_tree.rs:133-282, :1183-1189) through dbeel_scan()
  *   dbeel_memtable_cut     <- RedBlackTree::set + active_memtable_full (rbtree_arena lib.rs:497-534,
  *                             lsm_tree.rs:600-603,757-765): how many arrivals fill one memtable
  *   dbeel_plan_compactions <- compact_tree's size-tiered picker (src/tasks/compaction.rs:35-102),
@@ -75,6 +76,13 @@ int dbeel_tree_flush(dbeel_tree *t, const dbeel_run *batch, uint64_t *written_in
  * rows as in dbeel_get_many.  The memtable look-ups in front of it (:677-684) are the caller's. */
 int dbeel_tree_get_many(dbeel_tree *t, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
                         dbeel_lookup_result *results);
+
+/* The SSTable part of LSMTree::iter_filter over the tree's files: every table's .data / .index in dbeel_tree_sstables()
+ * order (oldest first, the iterator's order) through one dbeel_scan().  kind / ranges / results / stop as in dbeel_scan;
+ * out holds host buffers (caps: the sums of the tables' .data and .index file sizes).  stop->table is a position in
+ * dbeel_tree_sstables() order.  The memtables the iterator emits after the tables (:155-173) are the caller's. */
+int dbeel_tree_scan(dbeel_tree *t, uint32_t kind, const void *ranges, uint32_t n_ranges, dbeel_out *out,
+                    dbeel_job_result *results, dbeel_scan_stop *stop);
 
 /* WAL recovery step of open_or_create_ex.  0 logs: *wal_file_index = 0; 1 log: its index; 2 logs: the older one is
  * replayed (memtable of `tree_capacity` entries, DBEEL_ERR_TREE_FULL like the reference's ReachedCapacity), flushed
