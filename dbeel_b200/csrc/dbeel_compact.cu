@@ -420,6 +420,7 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
     p.src_ptr = reinterpret_cast<unsigned long long *>(ws + o_src);
     p.tile_first = reinterpret_cast<uint32_t *>(ws + o_tfirst);
     p.tile_first_n = (uint32_t)(gather_tiles + 2);
+    p.data_bound = sh.data_total;
     p.mem_table = reinterpret_cast<unsigned long long *>(ws + o_memtab);
     p.ref_reader = ref_reader ? 1 : 0;
     p.fix_index = reinterpret_cast<uint4 *>(ws + o_fix);
@@ -2050,6 +2051,7 @@ int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
         p.src_ptr = reinterpret_cast<unsigned long long *>(ws + o_src);
         p.tile_first = tile_first;
         p.tile_first_n = (uint32_t)(gather_tiles + 2);
+        p.data_bound = bytes;
         p.n_groups = nd;
         p.mem_table = reinterpret_cast<unsigned long long *>(ws + o_memtab);
         p.out_data = o_data;

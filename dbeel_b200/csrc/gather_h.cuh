@@ -50,11 +50,14 @@ __global__ void __launch_bounds__(kGhThreads, DBEEL_GATHER_H_MINB) k_gather_h(Pa
     __shared__ uint32_t s_ks[kGatherMaxEntries];
     const Ctl *c = p.ctl;
     const unsigned long long out_len = c->out_data_len;
+    // A caller's payload bound that turns out too low (sparse batches) is only reported after the job: the grid was sized
+    // from the bound, so the tiles stop writing there and entries keep their places in the true stream (out_len).
+    const unsigned long long out_end = out_len < p.data_bound ? out_len : p.data_bound;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t tile_id = blockIdx.x;
     const unsigned long long T0 = (unsigned long long)tile_id * kGatherTileBytes;
-    if (T0 >= out_len) return;
-    const uint32_t tile_len = out_len - T0 < kGatherTileBytes ? (uint32_t)(out_len - T0) : (uint32_t)kGatherTileBytes;
+    if (T0 >= out_end) return;
+    const uint32_t tile_len = out_end - T0 < kGatherTileBytes ? (uint32_t)(out_end - T0) : (uint32_t)kGatherTileBytes;
     const uint32_t e_lo = p.tile_first[tile_id];
     const uint32_t e_hi = T0 + kGatherTileBytes < out_len ? p.tile_first[tile_id + 1] : c->out_items - 1;
     const uint32_t ne = e_hi - e_lo + 1; // <= kGatherMaxEntries: every entry is >= 32 bytes

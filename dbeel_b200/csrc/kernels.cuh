@@ -128,6 +128,7 @@ struct Params {
     unsigned long long *src_ptr; // [n_total] device address of each surviving entry's bytes
     uint32_t *tile_first;        // [ceil(data bytes / 16 KB) + 2] entry holding each gather tile's first byte
     uint32_t tile_first_n;       // gather tiles the buffers were sized for (sparse batches: the caller's bound may be too low)
+    unsigned long long data_bound; // .data bytes the job checked against out->data_cap: k_gather_h writes nothing at or past it
     unsigned long long out_offset_base; // .data bytes written by earlier key-range partitions of the same output file
     BloomParams bloom;
     uint4 *hash_rec; // [n_total] {h0, h1} = both SipHash-1-3 values of every entry's key (k_extract), or null: the gather hashes
