@@ -43,7 +43,7 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_host_free", "dbeel_last_stats", "dbeel_last_error", "dbeel_strerror",
            "dbeel_murmur3_32", "dbeel_ring_owner", "dbeel_shard_ring", "dbeel_route_device", "dbeel_flush_many_sparse_device",
            "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream",
-           "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device"]
+           "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device", "dbeel_scan_stream"]
 
 
 class Run(C.Structure):
@@ -56,6 +56,13 @@ STREAM_WRITE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.c_uint64, C.c_v
 
 class StreamIO(C.Structure):
     _fields_ = [("read", STREAM_READ_FN), ("write", STREAM_WRITE_FN), ("ctx", C.c_void_p)]
+
+
+SCAN_WRITE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint64, C.c_void_p, C.c_uint64)
+
+
+class ScanIO(C.Structure):
+    _fields_ = [("read", STREAM_READ_FN), ("write", SCAN_WRITE_FN), ("ctx", C.c_void_p)]
 
 
 class Out(C.Structure):
@@ -205,6 +212,9 @@ def lib():
             f.restype = C.c_int
             f.argtypes = [C.c_void_p, C.POINTER(Table), C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(Out),
                           C.POINTER(JobResult), C.POINTER(ScanStop)]
+        L.dbeel_scan_stream.restype = C.c_int
+        L.dbeel_scan_stream.argtypes = [C.c_void_p, C.POINTER(Table), C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32,
+                                        C.POINTER(ScanIO), C.POINTER(JobResult), C.POINTER(ScanStop)]
         L.dbeel_compact_many_bound.restype = C.c_int
         L.dbeel_compact_many_bound.argtypes = [C.POINTER(Job), C.c_uint32, C.c_uint64, C.c_double] + [C.POINTER(C.c_uint64)] * 3
         for name in ("dbeel_compact_many", "dbeel_compact_many_device"):
@@ -623,6 +633,62 @@ class Engine:
         self._check(lib().dbeel_scan(self._h, arr, len(keep), kind, rptr, n, C.byref(out), res, C.byref(stop)), "dbeel_scan")
         return ([(od[r.data_off:r.data_off + r.data_len], oi[r.index_off:r.index_off + r.index_len]) for r in res[:n]],
                 stop.as_tuple())
+
+    def scan_stream(self, tables: Sequence[Tuple[object, ...]], ranges, kind: int = SCAN_HASH, fail_read_at: int = -1,
+                    fail_write_at: int = -1):
+        """dbeel_scan_stream with in-memory "files": the engine pulls the tables through a read callback and pushes every
+        destination's .data / .index through a write callback (both called from several engine threads).  Returns what
+        scan() returns; fail_*_at = n makes the n-th callback call return error code 4242 (tests), and
+        last_stream_calls holds the (read, write) callback calls of the call."""
+        keep = [(_u8(t[0]), _u8(t[1])) for t in tables]
+        arr = (Table * max(1, len(keep)))()
+        for j, (d, i) in enumerate(keep):
+            arr[j] = Table(None, d.size, None, i.size, None, 0)
+        rptr, _rkeep = pack_ranges(kind, ranges)
+        n = len(ranges)
+        outs = [{1: bytearray(), 2: bytearray()} for _ in range(n)]
+        calls = {"r": 0, "w": 0}
+        import threading
+        mu = threading.Lock()
+
+        def rd(_ctx, table, kind_, off, size, dst):
+            with mu:
+                k = calls["r"]
+                calls["r"] += 1
+            if k == fail_read_at:
+                return 4242
+            src = keep[table][0] if kind_ == 1 else keep[table][1]
+            if off + size > src.size:
+                return 4243
+            C.memmove(dst, src.ctypes.data + off, size)
+            return 0
+
+        def wr(_ctx, dest, kind_, off, src, size):
+            with mu:
+                k = calls["w"]
+                calls["w"] += 1
+                if k == fail_write_at:
+                    return 4242
+                if dest >= n or kind_ not in (1, 2):
+                    return 4244
+                f = outs[dest][kind_]
+                if len(f) < off + size:
+                    f.extend(bytes(off + size - len(f)))
+                f[off:off + size] = C.string_at(src, size)
+            return 0
+
+        io = ScanIO(STREAM_READ_FN(rd), SCAN_WRITE_FN(wr), None)
+        res = (JobResult * max(1, n))()
+        stop = ScanStop()
+        rc = lib().dbeel_scan_stream(self._h, arr, len(keep), kind, rptr, n, C.byref(io), res, C.byref(stop))
+        self.last_stream_calls = (calls["r"], calls["w"])
+        self._check(rc, "dbeel_scan_stream")
+        out = []
+        for d, (r, f) in enumerate(zip(res[:n], outs)):
+            if (r.data_off, r.index_off, r.bloom_len, len(f[1]), len(f[2])) != (0, 0, 0, r.data_len, r.index_len):
+                raise RuntimeError(f"dbeel_scan_stream: destination {d}'s files do not match its result row")
+            out.append((np.frombuffer(bytes(f[1]), np.uint8), np.frombuffer(bytes(f[2]), np.uint8)))
+        return out, stop.as_tuple()
 
     def scan_device(self, tables: Sequence[Tuple[int, int, int, int]], ranges, out_ptrs: Tuple[int, int, int, int],
                     kind: int = SCAN_HASH):

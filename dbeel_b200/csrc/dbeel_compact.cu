@@ -29,6 +29,7 @@
 #include "route.cuh"
 #include "scan.cuh"
 #include "wal.cuh"
+#include "host/scan_plan.h"
 #include "host/stream_pump.h"
 
 using namespace dbeel;
@@ -190,6 +191,19 @@ int parallel_pieces(size_t n, F fn) {
     work();
     for (auto &t : pool) t.join();
     return err.load();
+}
+
+// the copy streams and events of the pipelined host paths (created on first use)
+int ensure_copy_streams(dbeel_engine *e) {
+    if (e->s_h2d) return DBEEL_OK;
+    CU(cudaStreamCreateWithFlags(&e->s_h2d, cudaStreamNonBlocking));
+    CU(cudaStreamCreateWithFlags(&e->s_d2h, cudaStreamNonBlocking));
+    for (int i = 0; i < 2; i++) {
+        CU(cudaEventCreateWithFlags(&e->ev_h2d[i], cudaEventDisableTiming));
+        CU(cudaEventCreateWithFlags(&e->ev_comp[i], cudaEventDisableTiming));
+        CU(cudaEventCreateWithFlags(&e->ev_d2h[i], cudaEventDisableTiming));
+    }
+    return DBEEL_OK;
 }
 
 void default_opts(dbeel_compact_opts *o) {
@@ -920,16 +934,8 @@ int run_job_host_pipelined(dbeel_engine *e, const dbeel_run *runs, uint32_t n_ru
     if (!rc) rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, max_out);
     if (!rc) rc = ensure_device(e, &e->stage_out2, &e->stage_out2_cap, max_out);
     if (!rc && sh.bloom_file) rc = ensure_device(e, &e->bloom_dev, &e->bloom_dev_cap, sh.bloom_file + 16);
+    if (!rc) rc = ensure_copy_streams(e);
     if (rc) return rc;
-    if (!e->s_h2d) {
-        CU(cudaStreamCreateWithFlags(&e->s_h2d, cudaStreamNonBlocking));
-        CU(cudaStreamCreateWithFlags(&e->s_d2h, cudaStreamNonBlocking));
-        for (int i = 0; i < 2; i++) {
-            CU(cudaEventCreateWithFlags(&e->ev_h2d[i], cudaEventDisableTiming));
-            CU(cudaEventCreateWithFlags(&e->ev_comp[i], cudaEventDisableTiming));
-            CU(cudaEventCreateWithFlags(&e->ev_d2h[i], cudaEventDisableTiming));
-        }
-    }
     uint8_t *sin[2] = {e->stage_in, e->stage_in2}, *sout[2] = {e->stage_out, e->stage_out2};
     // streaming: R-slot pinned rings on both sides, one event per partition for the writer threads, the pump itself.
     // Declared in this order so that the pump's threads are joined before the events they wait on are destroyed.
@@ -1849,22 +1855,43 @@ int compact_many_entry(dbeel_engine *e, const dbeel_job *jobs, uint32_t n_jobs, 
 
 // ------------------------------------------------------------------------------------ N5: scans (iter_filter)
 
-int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges, uint32_t n_ranges,
-               dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop, bool device) {
-    if (!e) return DBEEL_ERR_INVALID_ARG;
-    if (!out || !results || !stop || !ranges || (n_tables && !tables)) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+// the argument checks both scan entry points share; *key_bytes = the key ranges' bytes (0 for hash ranges)
+int scan_args(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges, uint32_t n_ranges,
+              const dbeel_job_result *results, const dbeel_scan_stop *stop, uint64_t *key_bytes) {
+    if (!results || !stop || !ranges || (n_tables && !tables)) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     if (kind > DBEEL_SCAN_KEY) return fail(e, DBEEL_ERR_INVALID_ARG, "unknown scan kind");
     if (n_ranges == 0 || n_ranges > DBEEL_MAX_SCAN_RANGES) return fail(e, DBEEL_ERR_INVALID_ARG, "1 to DBEEL_MAX_SCAN_RANGES ranges");
     if (n_tables > DBEEL_MAX_RUNS) return fail(e, DBEEL_ERR_INVALID_ARG, "more than DBEEL_MAX_RUNS tables");
     const dbeel_key_ranges *kr = static_cast<const dbeel_key_ranges *>(ranges);
-    uint64_t key_bytes = 0;
+    *key_bytes = 0;
     if (kind == DBEEL_SCAN_KEY) {
         if (!kr->key_offsets) return fail(e, DBEEL_ERR_INVALID_ARG, "null key offsets");
         for (uint32_t k = 0; k < 2 * n_ranges; k++)
             if (kr->key_offsets[k + 1] < kr->key_offsets[k]) return fail(e, DBEEL_ERR_INVALID_ARG, "key offsets must ascend");
-        key_bytes = kr->key_offsets[2 * n_ranges] - kr->key_offsets[0];
-        if (key_bytes && !kr->keys) return fail(e, DBEEL_ERR_INVALID_ARG, "null range keys");
+        *key_bytes = kr->key_offsets[2 * n_ranges] - kr->key_offsets[0];
+        if (*key_bytes && !kr->keys) return fail(e, DBEEL_ERR_INVALID_ARG, "null range keys");
     }
+    return DBEEL_OK;
+}
+
+// The ranges as the kernels read them (ScanParams.hash_ranges / key_off / keys), written into the pinned header block.
+void scan_range_header(uint32_t kind, const void *ranges, uint32_t nd, uint64_t key_bytes, uint8_t *rng, uint8_t *keys) {
+    if (kind == DBEEL_SCAN_KEY) {
+        const dbeel_key_ranges *kr = static_cast<const dbeel_key_ranges *>(ranges);
+        uint64_t *ko = reinterpret_cast<uint64_t *>(rng);
+        for (uint32_t k = 0; k <= 2 * nd; k++) ko[k] = kr->key_offsets[k] - kr->key_offsets[0];
+        if (key_bytes) memcpy(keys, static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0], key_bytes);
+    } else {
+        memcpy(rng, ranges, 8ull * nd);
+    }
+}
+
+int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges, uint32_t n_ranges,
+               dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop, bool device) {
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (!out) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    uint64_t key_bytes = 0;
+    if (const int arc = scan_args(e, tables, n_tables, kind, ranges, n_ranges, results, stop, &key_bytes)) return arc;
     if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
     BusyGuard g(e);
     e->err.clear();
@@ -1952,13 +1979,7 @@ int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
     if (rc) return rc;
     uint8_t *ws = e->ws, *h = e->pin;
     memcpy(h + o_tab, td.data(), sizeof(ScanTable) * n_tables);
-    if (kind == DBEEL_SCAN_KEY) {
-        uint64_t *ko = reinterpret_cast<uint64_t *>(h + o_rng);
-        for (uint32_t k = 0; k <= 2 * nd; k++) ko[k] = kr->key_offsets[k] - kr->key_offsets[0];
-        if (key_bytes) memcpy(h + o_keys, static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0], key_bytes);
-    } else {
-        memcpy(h + o_rng, ranges, 8ull * nd);
-    }
+    scan_range_header(kind, ranges, nd, key_bytes, h + o_rng, h + o_keys);
 
     ScanParams sp = {};
     sp.tables = reinterpret_cast<const ScanTable *>(ws + o_tab);
@@ -2060,7 +2081,7 @@ int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
         const uint32_t tiles = (uint32_t)((items + kResolveThreads - 1) / kResolveThreads);
         launch_k(e, k_copy_words, (uint32_t)((header2_bytes / 4 + 255) / 256), 256, 0, s, reinterpret_cast<uint32_t *>(ws + o_ctl),
                  reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(header2_bytes / 4));
-        launch_k(e, k_scan_tile_sums, tiles, kResolveThreads, 0, s, p, split, (uint32_t)items);
+        launch_k(e, k_scan_tile_sums, tiles, kResolveThreads, 0, s, p, split);
         launch_k(e, k_scan_tiles, (tiles + 1023) / 1024, 1024, 0, s, p);
         launch_k(e, k_scan_chunks, 1, 1024, 0, s, p);
         launch_k(e, k_emit, tiles, kResolveThreads, 0, s, p, split);
@@ -2083,6 +2104,299 @@ int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
     out->data_len = bytes;
     out->index_len = 16 * items;
     out->items_written = items;
+    return DBEEL_OK;
+}
+
+
+// ------------------------------------------------------------------------------------ N5 streamed: dbeel_scan_stream
+// The plan (host/scan_plan.h) cuts the record sequence into partitions; each goes file -> pinned ring slot -> device slot
+// c & 1 in ONE H2D copy of its slot image (table headers | per table: index slice, .data window), runs the scan chain with
+// phase 2 sized from the plan's bound, and comes back with an exact D2H of what it selected.  H2D of c + 1, the kernels of c
+// and the D2H of c - 1 overlap; the engine thread enqueues partition c + 1's kernels before it waits for c's published sizes.
+int scan_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
+                      uint32_t n_ranges, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop) {
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (!io || !io->read || !io->write) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    uint64_t key_bytes = 0;
+    if (const int arc = scan_args(e, tables, n_tables, kind, ranges, n_ranges, results, stop, &key_bytes)) return arc;
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    e->stats = dbeel_stats{};
+    for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+    *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+
+    // ---- 1. the plan, from the .index files read in pieces
+    std::vector<uint64_t> dlen(n_tables), ilen(n_tables);
+    for (uint32_t t = 0; t < n_tables; t++) {
+        dlen[t] = tables[t].data_len;
+        ilen[t] = tables[t].index_len;
+        e->stats.entries_in += ilen[t] / DBEEL_INDEX_ENTRY_SIZE;
+    }
+    ScanPlan plan;
+    int rc = plan_scan(dlen.data(), ilen.data(), n_tables, e->partition_bytes,
+                       [io](uint32_t t, uint64_t off, uint64_t len, void *dst) { return io->read(io->ctx, t, DBEEL_STREAM_INDEX, off, len, dst); },
+                       &plan);
+    if (rc) return fail(e, rc, "stream read callback failed (.index, planning)");
+    const uint32_t np = (uint32_t)plan.parts.size();
+    e->stats.partitions = np;
+    auto host_stop = [&]() {
+        if (plan.panic_table >= 0) *stop = dbeel_scan_stop{plan.panic_table, DBEEL_SCAN_STOP_PANIC, plan.panic_record};
+    };
+    if (np == 0) { host_stop(); return DBEEL_OK; }
+    cudaError_t ce = cudaSetDevice(e->device);
+    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    cudaStream_t s = e->stream;
+
+    // ---- 2. slot layouts: [ScanTable per slice | per slice: index slice (+16), .data window (+32)], 256-byte aligned pieces
+    auto slot_layout = [&](uint32_t c, auto &&fn) { // fn(slice, index position, window position); returns the slot's bytes
+        const ScanPart &pt = plan.parts[c];
+        uint64_t pos = align_up(sizeof(ScanTable) * pt.n_slices, kAlign);
+        for (uint32_t k = 0; k < pt.n_slices; k++) {
+            const ScanSlice &sl = plan.slices[pt.first_slice + k];
+            const uint64_t ip = pos;
+            pos += align_up(16 * (sl.rec_hi - sl.rec_lo) + 16, kAlign);
+            fn(k, sl, ip, pos);
+            pos += align_up(sl.win_hi - sl.win_lo + 32, kAlign);
+        }
+        return pos;
+    };
+    const uint32_t nd = n_ranges;
+    uint64_t max_in = 0, max_rec = 0, max_bound = 0, h2d_bytes = 0;
+    for (uint32_t c = 0; c < np; c++) {
+        const uint64_t in = slot_layout(c, [](uint32_t, const ScanSlice &, uint64_t, uint64_t) {});
+        max_in = std::max(max_in, in);
+        max_rec = std::max(max_rec, plan.parts[c].n_rec);
+        max_bound = std::max(max_bound, plan.parts[c].data_bound);
+        h2d_bytes += in;
+    }
+    const uint64_t out_index_at = align_up(max_bound + 16, kAlign), max_out = out_index_at + align_up(16 * max_rec + 16, kAlign);
+    const uint32_t n_max = (uint32_t)max_rec;
+    const uint32_t n_blocks = (n_max + kRouteThreads - 1) / kRouteThreads;
+    const uint64_t res_tiles = (max_rec + kResolveThreads - 1) / kResolveThreads, res_chunks = (res_tiles + 1023) / 1024;
+    const uint64_t gather_tiles_max = (max_bound + kGatherTileBytes - 1) / kGatherTileBytes;
+    uint64_t off = 0;
+    auto carve = [&](uint64_t b) { uint64_t o2 = off; off = align_up(off + b, kAlign); return o2; };
+    const uint64_t o_rng = carve(kind == DBEEL_SCAN_KEY ? 8ull * (2 * nd + 1) : 8ull * nd);
+    const uint64_t o_keys = carve(key_bytes + 16);
+    const uint64_t header_bytes = off;
+    const uint64_t o_ctl = carve(sizeof(Ctl)), o_memtab = carve(16ull * (nd + 1));
+    const uint64_t o_tot = carve(8ull * (3 * nd + 1)), o_carry = carve(8ull * (2 * nd + 1));
+    const uint64_t o_dest = carve(4ull * n_max), o_flat = carve(16ull * n_max), o_split = carve(16ull * n_max);
+    const uint64_t o_hist = carve(4ull * n_blocks * nd);
+    const uint64_t o_tbytes = carve(8 * res_tiles), o_tcount = carve(4 * res_tiles);
+    const uint64_t o_cbytes = carve(8 * res_chunks), o_ccount = carve(4 * res_chunks);
+    const uint64_t o_src = carve(8ull * n_max), o_tf = carve(4ull * (gather_tiles_max + 2));
+    const uint64_t pub_words = 5ull * nd + 2, pub_stride = align_up(8 * pub_words, 64), pin_pub = align_up(header_bytes, 64);
+    const uint32_t R = (uint32_t)std::max(2, e->stream_ring);
+    rc = ensure_device(e, &e->ws, &e->ws_cap, off);
+    if (!rc) rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, max_in);
+    if (!rc) rc = ensure_device(e, &e->stage_in2, &e->stage_in2_cap, max_in);
+    if (!rc) rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, max_out);
+    if (!rc) rc = ensure_device(e, &e->stage_out2, &e->stage_out2_cap, max_out);
+    if (!rc) rc = ensure_pinned(e, pin_pub + 2 * pub_stride);
+    if (!rc) rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, (uint64_t)R * max_in);
+    if (!rc) rc = ensure_host(e, &e->ring_out, &e->ring_out_cap, (uint64_t)R * max_out);
+    if (!rc) rc = ensure_copy_streams(e);
+    if (rc) return rc;
+    uint8_t *ws = e->ws;
+    uint8_t *sin[2] = {e->stage_in, e->stage_in2}, *sout[2] = {e->stage_out, e->stage_out2};
+
+    // ---- 3. the pump: every partition's index slices and windows into its ring slot, the outputs to the write callback
+    struct EventList {
+        std::vector<cudaEvent_t> ev;
+        ~EventList() { for (auto &x : ev) if (x) cudaEventDestroy(x); }
+    } ev_out;
+    ev_out.ev.assign(np, nullptr);
+    for (uint32_t c = 0; c < np; c++) CU(cudaEventCreateWithFlags(&ev_out.ev[c], cudaEventDisableTiming | cudaEventBlockingSync));
+    const int dev = e->device;
+    EventList *evl = &ev_out;
+    StreamPump pump(io, np, R, stream_threads(), [evl](uint32_t c) { cudaEventSynchronize(evl->ev[c]); }, [dev]() { cudaSetDevice(dev); });
+    for (uint32_t c = 0; c < np; c++) {
+        uint8_t *slot = e->ring_in + (uint64_t)(c % R) * max_in;
+        slot_layout(c, [&](uint32_t, const ScanSlice &sl, uint64_t ip, uint64_t wp) {
+            pump.add_read(c, sl.table, DBEEL_STREAM_INDEX, 16 * sl.rec_lo, 16 * (sl.rec_hi - sl.rec_lo), slot + ip);
+            pump.add_read(c, sl.table, DBEEL_STREAM_DATA, sl.win_lo, sl.win_hi - sl.win_lo, slot + wp);
+        });
+    }
+    pump.start();
+
+    // ---- 4. per-scan state on the device: ranges (once), carry, stop word
+    scan_range_header(kind, ranges, nd, key_bytes, e->pin + o_rng, e->pin + o_keys);
+    ScanParams sp = {};
+    sp.n_ranges = nd;
+    sp.key_kind = kind == DBEEL_SCAN_KEY ? 1u : 0u;
+    sp.hash_ranges = reinterpret_cast<const uint32_t *>(ws + o_rng);
+    sp.key_off = reinterpret_cast<const unsigned long long *>(ws + o_rng);
+    sp.keys = ws + o_keys;
+    sp.dest = reinterpret_cast<uint32_t *>(ws + o_dest);
+    sp.flat = reinterpret_cast<uint4 *>(ws + o_flat);
+    sp.stop = reinterpret_cast<unsigned long long *>(ws + o_tot) + 3ull * nd;
+    sp.stop0 = ~0ull; // the plan ends before every stop the index shows (empty tables included)
+    RouteParams rp = {};
+    rp.index = sp.flat;
+    rp.n_shards = nd;
+    rp.shard_of = sp.dest;
+    rp.hist = reinterpret_cast<uint32_t *>(ws + o_hist);
+    rp.totals = reinterpret_cast<unsigned long long *>(ws + o_tot);
+    rp.out_index = reinterpret_cast<uint4 *>(ws + o_split);
+    Params p;
+    memset(&p, 0, sizeof p);
+    p.ctl = reinterpret_cast<Ctl *>(ws + o_ctl);
+    p.tile_bytes = reinterpret_cast<unsigned long long *>(ws + o_tbytes);
+    p.tile_count = reinterpret_cast<uint32_t *>(ws + o_tcount);
+    p.chunk_bytes = reinterpret_cast<unsigned long long *>(ws + o_cbytes);
+    p.chunk_count = reinterpret_cast<uint32_t *>(ws + o_ccount);
+    p.src_ptr = reinterpret_cast<unsigned long long *>(ws + o_src);
+    p.tile_first = reinterpret_cast<uint32_t *>(ws + o_tf);
+    p.n_groups = nd;
+    p.mem_table = reinterpret_cast<unsigned long long *>(ws + o_memtab);
+    unsigned long long *carry = reinterpret_cast<unsigned long long *>(ws + o_carry);
+    CU(cudaEventRecord(e->ev[EV_START], s));
+    launch_k(e, k_copy_words, (uint32_t)((header_bytes / 4 + 255) / 256), 256, 0, s, reinterpret_cast<uint32_t *>(ws),
+             reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(header_bytes / 4));
+    CU(cudaMemsetAsync(carry, 0, 8ull * (2 * nd + 1), s));
+    CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
+
+    // ---- 5. the pipeline
+    auto enqueue_h2d = [&](uint32_t c) -> int {
+        const int prc = pump.wait_reads(c);
+        if (prc) return fail(e, prc, "stream read callback failed");
+        uint8_t *slot = e->ring_in + (uint64_t)(c % R) * max_in, *base = sin[c & 1];
+        ScanTable *td = reinterpret_cast<ScanTable *>(slot);
+        uint32_t local = 0;
+        const uint64_t bytes = slot_layout(c, [&](uint32_t k, const ScanSlice &sl, uint64_t ip, uint64_t wp) {
+            const uint32_t nr = (uint32_t)(sl.rec_hi - sl.rec_lo);
+            // biased: .data offset `off` of the table lives at data + off, inside the window
+            td[k] = ScanTable{reinterpret_cast<const uint8_t *>(reinterpret_cast<uintptr_t>(base + wp) - sl.win_lo), tables[sl.table].data_len,
+                              reinterpret_cast<const uint4 *>(base + ip), nr, local};
+            local += nr;
+        });
+        CU(cudaMemcpyAsync(base, slot, bytes, cudaMemcpyHostToDevice, e->s_h2d));
+        CU(cudaEventRecord(e->ev_h2d[c & 1], e->s_h2d));
+        return DBEEL_OK;
+    };
+    uint32_t launches = 0;
+    auto enqueue_kernels = [&](uint32_t c) -> int {
+        const ScanPart &pt = plan.parts[c];
+        const uint32_t n = (uint32_t)pt.n_rec, nb = (n + kRouteThreads - 1) / kRouteThreads;
+        const uint32_t tiles = (n + kResolveThreads - 1) / kResolveThreads;
+        const uint64_t gtiles = (pt.data_bound + kGatherTileBytes - 1) / kGatherTileBytes;
+        CU(cudaStreamWaitEvent(s, e->ev_h2d[c & 1], 0));
+        if (c >= 2) CU(cudaStreamWaitEvent(s, e->ev_d2h[c & 1], 0)); // output slot c & 1 has gone back to the host
+        ScanParams spc = sp;
+        spc.tables = reinterpret_cast<const ScanTable *>(sin[c & 1]);
+        spc.n_tables = pt.n_slices;
+        spc.n = n;
+        RouteParams rpc = rp;
+        rpc.n = n;
+        rpc.n_blocks = nb;
+        Params pc = p;
+        pc.tile_first_n = (uint32_t)(gtiles + 2);
+        pc.data_bound = pt.data_bound;
+        pc.out_data = sout[c & 1];
+        pc.out_index = reinterpret_cast<uint4 *>(sout[c & 1] + out_index_at);
+        unsigned long long *pub = reinterpret_cast<unsigned long long *>(e->pin_dev + pin_pub + (c & 1) * pub_stride);
+        CU(cudaMemsetAsync(rp.totals, 0, 8ull * 3 * nd, s));
+        launch_k(e, k_scan_classify, (n + 255) / 256, 256, 0, s, spc);
+        launch_k(e, k_scan_hist, nb, kRouteThreads, 0, s, spc, rpc);
+        launch_k(e, k_route_scan, nd, 1024, 0, s, rpc);
+        launch_k(e, k_route_starts, 1, 256, 0, s, rpc, pub);
+        launch_k(e, k_route_scatter, nb, kRouteThreads, 0, s, rpc);
+        launch_k(e, k_scan_stream_carry, 1, 32, 0, s, rpc, pc, carry, pub);
+        const uint4 *split = rpc.out_index;
+        launch_k(e, k_scan_tile_sums, tiles, kResolveThreads, 0, s, pc, split);
+        launch_k(e, k_scan_tiles, (tiles + 1023) / 1024, 1024, 0, s, pc);
+        launch_k(e, k_scan_chunks, 1, 1024, 0, s, pc);
+        launch_k(e, k_emit, tiles, kResolveThreads, 0, s, pc, split);
+        launch_k(e, k_gather_h, (uint32_t)gtiles, kGhThreads, 0, s, pc); // tiles past Ctl.out_data_len return at once
+        launch_k(e, k_rebase_index, (n + 255) / 256, 256, 0, s, pc);
+        launches += 12;
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(e->ev_comp[c & 1], s));
+        return DBEEL_OK;
+    };
+    uint64_t out_bytes = 0;
+    std::vector<unsigned long long> hdr(pub_words);
+    bool stopped = false;
+    rc = enqueue_h2d(0);
+    if (!rc && np > 1) rc = enqueue_h2d(1);
+    if (!rc) rc = enqueue_kernels(0);
+    for (uint32_t c = 0; c < np && !rc; c++) {
+        if (c + 1 < np) {
+            rc = enqueue_kernels(c + 1);
+            if (rc) break;
+        }
+        ce = cudaEventSynchronize(e->ev_comp[c & 1]);
+        if (ce != cudaSuccess) { rc = fail(e, DBEEL_ERR_CUDA, "scan kernels", ce); break; }
+        pump.release_input(c); // H2D c (out of ring slot c mod R) has completed
+        memcpy(hdr.data(), e->pin + pin_pub + (c & 1) * pub_stride, 8 * pub_words);
+        // counts | bytes | starts | stop | carry bytes | carry entries | halted before this partition
+        const ScanPart &pt = plan.parts[c];
+        if (!hdr[5 * nd + 1] && hdr[3 * nd] != ~0ull && !stopped) {
+            const unsigned long long key = hdr[3 * nd];
+            const uint32_t lt = (uint32_t)((key >> 2) & 1023);
+            uint64_t local = 0;
+            for (uint32_t k = 0; k < lt; k++) local += plan.slices[pt.first_slice + k].rec_hi - plan.slices[pt.first_slice + k].rec_lo;
+            const ScanSlice &sl = plan.slices[pt.first_slice + lt];
+            *stop = dbeel_scan_stop{(int32_t)sl.table, (uint32_t)(key & 3), sl.rec_lo + ((key >> 12) - local)};
+            stopped = true;
+        }
+        uint64_t bytes = 0, items = 0;
+        for (uint32_t d = 0; d < nd; d++) { bytes += hdr[nd + d]; items += hdr[d]; }
+        rc = pump.wait_out_slot(c);
+        if (rc) { fail(e, rc, "stream write callback failed"); break; }
+        uint8_t *oslot = e->ring_out + (uint64_t)(c % R) * max_out;
+        CU(cudaStreamWaitEvent(e->s_d2h, e->ev_comp[c & 1], 0));
+        if (bytes) CU(cudaMemcpyAsync(oslot, sout[c & 1], bytes, cudaMemcpyDeviceToHost, e->s_d2h));
+        if (items) CU(cudaMemcpyAsync(oslot + out_index_at, sout[c & 1] + out_index_at, 16 * items, cudaMemcpyDeviceToHost, e->s_d2h));
+        CU(cudaEventRecord(ev_out.ev[c], e->s_d2h));
+        CU(cudaEventRecord(e->ev_d2h[c & 1], e->s_d2h));
+        std::vector<StreamPump::OutPiece> pieces;
+        uint64_t before = 0; // destination d's bytes start here in the partition's output (its entries at starts[d])
+        for (uint32_t d = 0; d < nd; d++) {
+            const uint64_t db = hdr[nd + d], di = hdr[d];
+            if (di) {
+                pieces.push_back({d, DBEEL_STREAM_DATA, hdr[3 * nd + 1 + d], oslot + before, db});
+                pieces.push_back({d, DBEEL_STREAM_INDEX, 16 * hdr[4 * nd + 1 + d], oslot + out_index_at + 16 * hdr[2 * nd + d], 16 * di});
+            }
+            before += db;
+            results[d].data_len += db;
+            results[d].items_written += di;
+        }
+        out_bytes += bytes + 16 * items;
+        pump.publish_pieces(c, std::move(pieces));
+        if (c + 2 < np) rc = enqueue_h2d(c + 2);
+    }
+    if (rc) { // drain: nothing of this scan may touch the engine's buffers after it returns
+        cudaStreamSynchronize(e->s_h2d);
+        cudaStreamSynchronize(s);
+        cudaStreamSynchronize(e->s_d2h);
+        pump.abort(rc);
+        for (uint32_t d = 0; d < nd; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+        *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+        return rc;
+    }
+    CU(cudaEventRecord(e->ev[EV_GATHER], s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaStreamSynchronize(e->s_d2h));
+    const int frc = pump.finish(); // every destination's bytes have gone through the write callback
+    if (frc) {
+        for (uint32_t d = 0; d < nd; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+        *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+        return fail(e, frc, "stream write callback failed");
+    }
+    if (!stopped) host_stop();
+    uint64_t items = 0;
+    for (uint32_t d = 0; d < nd; d++) {
+        results[d].index_len = 16 * results[d].items_written;
+        items += results[d].items_written;
+    }
+    cudaEventElapsedTime(&e->stats.ms_total, e->ev[EV_START], e->ev[EV_GATHER]);
+    e->stats.kernel_launches = launches + 1;
+    e->stats.input_bytes = h2d_bytes;
+    e->stats.output_bytes = out_bytes;
+    e->stats.entries_out = items;
     return DBEEL_OK;
 }
 
@@ -2415,6 +2729,11 @@ int dbeel_scan_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tab
                       uint32_t n_ranges, dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop) {
     REFUSE_WHILE_ASYNC(e);
     return scan_entry(e, tables, n_tables, kind, ranges, n_ranges, out, results, stop, true);
+}
+
+int dbeel_scan_stream(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
+                      uint32_t n_ranges, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop) {
+    return scan_stream_entry(e, tables, n_tables, kind, ranges, n_ranges, io, results, stop);
 }
 
 int dbeel_compact_many_bound(const dbeel_job *jobs, uint32_t n_jobs, uint64_t bloom_min_size, double bloom_fp, uint64_t *data_cap,

@@ -651,6 +651,50 @@ int dbeel_tree_scan(dbeel_tree *t, uint32_t kind, const void *ranges, uint32_t n
     return rc;
 }
 
+namespace {
+struct ScanStreamFiles { // the tables' descriptors (read side of StreamFiles) and the caller's write callback
+    StreamFiles in;
+    int (*write)(void *, uint32_t, uint32_t, uint64_t, const void *, uint64_t);
+    void *ctx;
+};
+int scan_stream_read(void *ctx, uint32_t table, uint32_t kind, uint64_t off, uint64_t len, void *dst) {
+    return stream_read(&static_cast<ScanStreamFiles *>(ctx)->in, table, kind, off, len, dst);
+}
+int scan_stream_write(void *ctx, uint32_t dest, uint32_t kind, uint64_t off, const void *src, uint64_t len) {
+    auto *f = static_cast<ScanStreamFiles *>(ctx);
+    return f->write(f->ctx, dest, kind, off, src, len);
+}
+} // namespace
+
+int dbeel_tree_scan_stream(dbeel_tree *t, uint32_t kind, const void *ranges, uint32_t n_ranges,
+                           int (*write)(void *ctx, uint32_t dest, uint32_t kind, uint64_t offset, const void *src, uint64_t len),
+                           void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop) {
+    if (!t || !write) return DBEEL_ERR_INVALID_ARG;
+    t->err.clear();
+    // AsyncIter reads `self.sstables` (ascending index) oldest first (lsm_tree.rs:182-188, 214-246)
+    const size_t n = t->sstables.size();
+    ScanStreamFiles f;
+    f.write = write;
+    f.ctx = ctx;
+    f.in.data_fd.assign(n, -1);
+    f.in.index_fd.assign(n, -1);
+    std::vector<dbeel_table> tables(n);
+    for (size_t i = 0; i < n; i++) {
+        const std::string dp = file_path(t->dir, t->sstables[i].index, kData), ip = file_path(t->dir, t->sstables[i].index, kIndex);
+        f.in.data_fd[i] = open(dp.c_str(), O_RDONLY);
+        f.in.index_fd[i] = open(ip.c_str(), O_RDONLY);
+        struct stat sd, si;
+        if (f.in.data_fd[i] < 0 || f.in.index_fd[i] < 0 || fstat(f.in.data_fd[i], &sd) != 0 || fstat(f.in.index_fd[i], &si) != 0)
+            return io_fail(t, "open " + dp);
+        tables[i] = dbeel_table{nullptr, (uint64_t)sd.st_size, nullptr, (uint64_t)si.st_size, nullptr, 0};
+    }
+    const dbeel_scan_io io{scan_stream_read, scan_stream_write, &f};
+    const int rc = dbeel_scan_stream(t->engine, tables.data(), (uint32_t)n, kind, ranges, n_ranges, &io, results, stop);
+    if (rc == DBEEL_ERR_IO && f.in.saved_errno.load()) { errno = f.in.saved_errno.load(); io_fail(t, "streamed scan"); }
+    else if (rc) t->err = dbeel_last_error(t->engine);
+    return rc;
+}
+
 int dbeel_tree_recover_wal(dbeel_tree *t, uint32_t tree_capacity, uint64_t *wal_file_index, uint64_t *items_written) {
     if (!t) return DBEEL_ERR_INVALID_ARG;
     t->err.clear();

@@ -14,6 +14,9 @@
 //
 // so file reads, both PCIe directions and file writes all overlap, and the pinned memory is R slots however large the
 // SSTables are.  Any callback error aborts the pump; the first error code is what every wait returns from then on.
+//
+// A partition's output is a list of pieces {destination, kind, file offset, bytes}: the compaction publishes two (its .data
+// and .index), the streamed scan (dbeel_scan_stream) two per destination that received something.
 #pragma once
 #include <stdint.h>
 
@@ -42,17 +45,23 @@ class StreamPump {
         const uint8_t *index = nullptr;
         uint64_t index_len = 0, index_off = 0;
     };
+    struct OutPiece { // len bytes at src go to offset `off` of destination `dest`'s file of kind `kind` (DBEEL_STREAM_*)
+        uint32_t dest, kind;
+        uint64_t off;
+        const uint8_t *src;
+        uint64_t len;
+    };
     static constexpr uint64_t kPiece = 8ull << 20; // bytes per callback call
 
     // wait_out(c): blocks until partition c's output has arrived in host memory (the engine: cudaEventSynchronize).
     // thread_init(): run once on every pump thread (the engine: cudaSetDevice).
     StreamPump(const dbeel_stream_io *io, uint32_t n_parts, uint32_t ring, int n_threads, std::function<void(uint32_t)> wait_out,
                std::function<void()> thread_init = nullptr)
-        : io_(io), np_(n_parts), ring_(ring ? ring : 1), nt_(n_threads > 0 ? n_threads : 1), wait_out_(std::move(wait_out)),
-          thread_init_(std::move(thread_init)), r_left_(n_parts, 0), w_left_(n_parts, 0), w_next_(new std::atomic<uint64_t>[n_parts ? n_parts : 1]),
-          outs_(n_parts) {
-        for (uint32_t c = 0; c < n_parts; c++) w_next_[c].store(0);
-    }
+        : StreamPump(io->read, io->write, nullptr, io->ctx, n_parts, ring, n_threads, std::move(wait_out), std::move(thread_init)) {}
+    // The scan's callbacks: the same read, a write that names the destination.
+    StreamPump(const dbeel_scan_io *io, uint32_t n_parts, uint32_t ring, int n_threads, std::function<void(uint32_t)> wait_out,
+               std::function<void()> thread_init = nullptr)
+        : StreamPump(io->read, nullptr, io->write, io->ctx, n_parts, ring, n_threads, std::move(wait_out), std::move(thread_init)) {}
     StreamPump(const StreamPump &) = delete;
     StreamPump &operator=(const StreamPump &) = delete;
     ~StreamPump() {
@@ -97,9 +106,18 @@ class StreamPump {
     }
 
     void publish_out(uint32_t part, const OutPart &o) {
+        publish_pieces(part, {OutPiece{0, DBEEL_STREAM_DATA, o.data_off, o.data, o.data_len},
+                              OutPiece{0, DBEEL_STREAM_INDEX, o.index_off, o.index, o.index_len}});
+    }
+
+    // In partition order.  Pieces longer than kPiece go out in several callback calls.
+    void publish_pieces(uint32_t part, std::vector<OutPiece> ps) {
+        uint64_t calls = 0;
+        for (const OutPiece &q : ps) calls += pieces(q.len);
         std::lock_guard<std::mutex> lk(mu_);
-        outs_[part] = o;
-        w_left_[part] = pieces(o.data_len) + pieces(o.index_len);
+        outs_[part] = std::move(ps);
+        w_total_[part] = calls;
+        w_left_[part] = calls;
         published_ = part + 1;
         cv_.notify_all();
     }
@@ -132,6 +150,18 @@ class StreamPump {
     }
 
   private:
+    using ReadFn = int (*)(void *, uint32_t, uint32_t, uint64_t, uint64_t, void *);
+    using WriteFn = int (*)(void *, uint32_t, uint64_t, const void *, uint64_t);
+    using WriteDestFn = int (*)(void *, uint32_t, uint32_t, uint64_t, const void *, uint64_t);
+
+    StreamPump(ReadFn read, WriteFn write, WriteDestFn write_dest, void *ctx, uint32_t n_parts, uint32_t ring, int n_threads,
+               std::function<void(uint32_t)> wait_out, std::function<void()> thread_init)
+        : read_(read), write_(write), write_dest_(write_dest), ctx_(ctx), np_(n_parts), ring_(ring ? ring : 1), nt_(n_threads > 0 ? n_threads : 1),
+          wait_out_(std::move(wait_out)), thread_init_(std::move(thread_init)), r_left_(n_parts, 0), w_total_(n_parts, 0), w_left_(n_parts, 0),
+          w_next_(new std::atomic<uint64_t>[n_parts ? n_parts : 1]), outs_(n_parts) {
+        for (uint32_t c = 0; c < n_parts; c++) w_next_[c].store(0);
+    }
+
     static uint64_t pieces(uint64_t len) { return (len + kPiece - 1) / kPiece; }
 
     void join() {
@@ -158,7 +188,7 @@ class StreamPump {
                 cv_.wait(lk, [&] { return failed_ || t.part < consumed_ + ring_; });
                 if (failed_) return;
             }
-            const int rc = io_->read(io_->ctx, t.run, t.kind, t.off, t.len, t.dst);
+            const int rc = read_(ctx_, t.run, t.kind, t.off, t.len, t.dst);
             std::lock_guard<std::mutex> lk(mu_);
             if (rc) fail_locked(rc);
             r_left_[t.part]--;
@@ -170,24 +200,27 @@ class StreamPump {
     void writer() {
         if (thread_init_) thread_init_();
         for (uint32_t c = 0; c < np_; c++) {
-            OutPart o;
+            const std::vector<OutPiece> *ps;
+            uint64_t total;
             {
                 std::unique_lock<std::mutex> lk(mu_);
                 cv_.wait(lk, [&] { return failed_ || published_ > c; });
                 if (failed_) return;
-                o = outs_[c];
+                ps = &outs_[c]; // neither changes once published
+                total = w_total_[c];
             }
-            const uint64_t nd = pieces(o.data_len), total = nd + pieces(o.index_len);
             if (total == 0) continue;
             if (wait_out_) wait_out_(c);
+            size_t p = 0;      // the piece that holds call k (k only grows on this thread)
+            uint64_t p0 = 0;   // calls of the pieces before it
             while (true) {
                 const uint64_t k = w_next_[c].fetch_add(1);
                 if (k >= total) break;
-                const bool is_data = k < nd;
-                const uint64_t q = is_data ? k : k - nd, len_all = is_data ? o.data_len : o.index_len;
-                const uint64_t off = q * kPiece, n = len_all - off < kPiece ? len_all - off : kPiece;
-                const int rc = io_->write(io_->ctx, is_data ? DBEEL_STREAM_DATA : DBEEL_STREAM_INDEX, (is_data ? o.data_off : o.index_off) + off,
-                                          (is_data ? o.data : o.index) + off, n);
+                while (k >= p0 + pieces((*ps)[p].len)) p0 += pieces((*ps)[p++].len);
+                const OutPiece &o = (*ps)[p];
+                const uint64_t off = (k - p0) * kPiece, n = o.len - off < kPiece ? o.len - off : kPiece;
+                const int rc = write_dest_ ? write_dest_(ctx_, o.dest, o.kind, o.off + off, o.src + off, n)
+                                           : write_(ctx_, o.kind, o.off + off, o.src + off, n);
                 std::lock_guard<std::mutex> lk(mu_);
                 if (rc) fail_locked(rc);
                 w_left_[c]--;
@@ -197,7 +230,10 @@ class StreamPump {
         }
     }
 
-    const dbeel_stream_io *io_;
+    const ReadFn read_;
+    const WriteFn write_;
+    const WriteDestFn write_dest_;
+    void *const ctx_;
     const uint32_t np_, ring_;
     const int nt_;
     std::function<void(uint32_t)> wait_out_;
@@ -208,9 +244,9 @@ class StreamPump {
     std::condition_variable cv_;
     // all below under mu_
     std::vector<uint32_t> r_left_;
-    std::vector<uint64_t> w_left_;
+    std::vector<uint64_t> w_total_, w_left_; // callback calls of each partition's output: all / not yet done
     std::unique_ptr<std::atomic<uint64_t>[]> w_next_;
-    std::vector<OutPart> outs_;
+    std::vector<std::vector<OutPiece>> outs_;
     uint32_t consumed_ = 0;  // partitions [0, consumed_) have released their input slot
     uint32_t published_ = 0; // partitions [0, published_) have their output described
     bool failed_ = false, done_ = false, started_ = false;

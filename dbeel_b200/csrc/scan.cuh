@@ -11,6 +11,10 @@
 //
 // The records the split moves are 16 bytes {source address, 8 + key length, full_size}: the layout k_emit reads, so the
 // payload is read once (k_gather_h) and nothing else touches it.
+//
+// Streamed (dbeel_scan_stream): one partition of the record sequence per chain, the tables' .data windows passed as biased
+// pointers (ScanTable.data + offset = the entry inside the window), so k_scan_classify runs unchanged on partition-local
+// positions.  k_scan_stream_carry sits between the split and phase 2 and replaces dbeel_scan's host round trip there.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -170,11 +174,14 @@ __global__ void __launch_bounds__(kRouteThreads) k_scan_hist(ScanParams sp, Rout
     }
 }
 
-// Per resolve tile (kResolveThreads split records): bytes and entries, the aggregates k_scan_tiles scans.
-__global__ void __launch_bounds__(kResolveThreads) k_scan_tile_sums(Params p, const uint4 *split, uint32_t span) {
+// Per resolve tile (kResolveThreads split records): bytes and entries, the aggregates k_scan_tiles scans.  The split's
+// length is Ctl.span, so the grid may be sized from a bound (streamed partitions).
+__global__ void __launch_bounds__(kResolveThreads) k_scan_tile_sums(Params p, const uint4 *split) {
     pdl_trigger();
     pdl_wait();
     __shared__ unsigned long long s_b[kResolveThreads / 32];
+    const uint32_t span = p.ctl->span;
+    if (blockIdx.x * (uint32_t)kResolveThreads >= span) return;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t i = blockIdx.x * (uint32_t)kResolveThreads + tid;
     unsigned long long b = i < span ? (unsigned long long)split[i].w : 0ull;
@@ -189,6 +196,50 @@ __global__ void __launch_bounds__(kResolveThreads) k_scan_tile_sums(Params p, co
         p.tile_bytes[blockIdx.x] = tb;
         p.tile_count[blockIdx.x] = span - i0 < (uint32_t)kResolveThreads ? span - i0 : (uint32_t)kResolveThreads;
     }
+}
+
+// Streamed scans: one thread, after k_route_starts of a partition (totals = counts | bytes | starts | stop, nd each + 1).
+// carry[2 nd + 1] (device, zeroed before the first partition) = .data bytes | entries every destination received from the
+// partitions before, | halted (an earlier partition found the stop).  Partitions run in order on one stream, so this is
+// exact with no host in the loop.  The thread
+//   * publishes the carry before this partition behind k_route_starts's totals in the mapped pinned header (pub[3 nd + 1 ..
+//     5 nd + 1] and the halted word at pub[5 nd + 1]): the host learns the exact D2H sizes and the file offsets from it;
+//   * makes k_rebase_index write destination-file offsets across partitions: mem_table[2d] = (bytes before d in this
+//     partition) - carry bytes of d, so off - mem_table[2d] = offset inside d's part here + what d had before (mod 2^64);
+//   * sets Ctl.span / total for phase 2, whose grids come from the host's bound;
+//   * adds the partition to the carry, and arms the next partition's stop word: 0 once halted (k_scan_hist then drops every
+//     record: nothing is delivered after the reference's iteration ended), else none.
+__global__ void k_scan_stream_carry(RouteParams rp, Params p, unsigned long long *carry, unsigned long long *pub) {
+    pdl_trigger();
+    pdl_wait();
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    const uint32_t nd = rp.n_shards;
+    unsigned long long *tot = rp.totals;
+    const unsigned long long halted = carry[2 * nd];
+    unsigned long long before = 0, items = 0;
+    for (uint32_t d = 0; d < nd; d++) {
+        const unsigned long long cb = carry[d], ci = carry[nd + d], b = tot[nd + d], n = tot[d];
+        pub[3 * nd + 1 + d] = cb;
+        pub[4 * nd + 1 + d] = ci;
+        p.mem_table[2 * d] = before - cb;
+        p.mem_table[2 * d + 1] = tot[2 * nd + d];
+        carry[d] = cb + b;
+        carry[nd + d] = ci + n;
+        before += b;
+        items += n;
+    }
+    p.mem_table[2 * nd] = before;
+    p.mem_table[2 * nd + 1] = items;
+    pub[5 * nd + 1] = halted;
+    Ctl *c = p.ctl;
+    c->flags = 0;
+    c->span = c->total = (uint32_t)items;
+    c->out_data_len = 0;
+    c->out_items = 0;
+    const bool halts = halted || tot[3 * nd] != ~0ull;
+    carry[2 * nd] = halts ? 1ull : 0ull;
+    tot[3 * nd] = halts ? 0ull : ~0ull;
+    __threadfence_system();
 }
 
 } // namespace dbeel

@@ -52,6 +52,9 @@ def _lib():
         L.dbeel_tree_scan.restype = C.c_int
         L.dbeel_tree_scan.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(capi.Out),
                                       C.POINTER(capi.JobResult), C.POINTER(capi.ScanStop)]
+        L.dbeel_tree_scan_stream.restype = C.c_int
+        L.dbeel_tree_scan_stream.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, capi.SCAN_WRITE_FN, C.c_void_p,
+                                             C.POINTER(capi.JobResult), C.POINTER(capi.ScanStop)]
         L.dbeel_tree_recover_wal.restype = C.c_int
         L.dbeel_tree_recover_wal.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         L.dbeel_tree_last_error.restype = C.c_char_p
@@ -71,7 +74,7 @@ def _lib():
 
 
 TREE_EXPORTS = ["dbeel_tree_open", "dbeel_tree_close", "dbeel_tree_sstables", "dbeel_tree_write_sstable_index",
-                "dbeel_tree_compact", "dbeel_tree_compact_many", "dbeel_tree_flush", "dbeel_tree_recover_wal", "dbeel_tree_get_many", "dbeel_tree_scan", "dbeel_tree_last_error", "dbeel_memtable_cut",
+                "dbeel_tree_compact", "dbeel_tree_compact_many", "dbeel_tree_flush", "dbeel_tree_recover_wal", "dbeel_tree_get_many", "dbeel_tree_scan", "dbeel_tree_scan_stream", "dbeel_tree_last_error", "dbeel_memtable_cut",
                 "dbeel_plan_compactions", "dbeel_out_pages", "dbeel_tree_set_page_sink"]
 
 
@@ -208,6 +211,35 @@ class LSMTree:
         self._check(_lib().dbeel_tree_scan(self._h, kind, rptr, n, C.byref(out), res, C.byref(stop)), "LSMTree.scan")
         return ([(od[r.data_off:r.data_off + r.data_len].copy(), oi[r.index_off:r.index_off + r.index_len].copy())
                  for r in res[:n]], stop.as_tuple())
+
+    def scan_stream(self, ranges, kind: int = capi.SCAN_HASH, write=None):
+        """scan() with the files streamed through the engine (dbeel_tree_scan_stream): nothing is read whole, so trees
+        larger than memory scan too.  write(dest, kind, offset, src_address, length) -> 0 or an error code receives every
+        piece of every destination's .data (kind 1) / .index (kind 2), from several threads (src_address: host memory
+        valid during the call); without one the pieces are collected in memory.  Returns ([(data_len, index_len, items)]
+        per range when `write` is given, else [(data, index)] per range like scan(), and the stop as scan() does."""
+        import threading
+        n = len(ranges)
+        files = [{1: bytearray(), 2: bytearray()} for _ in range(n)]
+        mu = threading.Lock()
+
+        def collect(dest, kind_, off, src, size):
+            with mu:
+                f = files[dest][kind_]
+                if len(f) < off + size:
+                    f.extend(bytes(off + size - len(f)))
+                f[off:off + size] = C.string_at(src, size)
+            return 0
+
+        cb = capi.SCAN_WRITE_FN(lambda _ctx, dest, kind_, off, src, size: (write or collect)(dest, kind_, off, src, size))
+        rptr, _keep = capi.pack_ranges(kind, ranges)
+        res = (capi.JobResult * max(1, n))()
+        stop = capi.ScanStop()
+        self._check(_lib().dbeel_tree_scan_stream(self._h, kind, rptr, n, cb, None, res, C.byref(stop)), "LSMTree.scan_stream")
+        if write is not None:
+            return [(int(r.data_len), int(r.index_len), int(r.items_written)) for r in res[:n]], stop.as_tuple()
+        return ([(np.frombuffer(bytes(f[1]), np.uint8).copy(), np.frombuffer(bytes(f[2]), np.uint8).copy()) for f in files],
+                stop.as_tuple())
 
     def recover_wal(self, tree_capacity: int = capi.DEFAULT_TREE_CAPACITY) -> Tuple[int, int]:
         """open_or_create_ex's WAL step (lsm_tree.rs:466-513): with two `.memtable` files the older one is replayed and

@@ -381,6 +381,33 @@ int dbeel_scan(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
 int dbeel_scan_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
                       uint32_t n_ranges, dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop);
 
+/* The same scan fed from files, for trees of any size (LSMTree::iter_filter's SSTable part, lsm_tree.rs:210-281): migration
+ * reads a shard's whole tree, which is the tree that grows until the node is rebalanced.  The engine moves the bytes
+ *     file -> read() -> pinned ring -> H2D -> kernels -> D2H -> pinned ring -> write() -> file
+ * one partition at a time: a partition is a contiguous run of records in iteration order (it may span tables) with, per
+ * table, its index slice and the .data window that holds them.  Device and page-locked memory are bounded by the partition
+ * budget (DBEEL_PARTITION_MB / DBEEL_PARTITION_KB) and the ring depth (DBEEL_STREAM_RING), not by the tree; the planner reads
+ * the .index files in pieces and keeps one row per partition.  tables[i].data / .index are ignored (lengths only).
+ *   read : as dbeel_stream_io.read: [offset, offset + len) of table `table`'s .data (DBEEL_STREAM_DATA) or .index
+ *          (DBEEL_STREAM_INDEX).  The .index files are read twice: once to plan, once into the ring.
+ *   write: len bytes at `offset` of destination `dest`'s .data (DBEEL_STREAM_DATA) or .index (DBEEL_STREAM_INDEX) file.
+ *          Every destination's two files start at offset 0 (.index offsets are relative to its own .data file); pieces
+ *          arrive in any order, from several threads, at their final offsets.
+ * Both return 0 or an error code of the caller's, which dbeel_scan_stream returns unchanged; the engine stays usable.
+ * results[d]: data_len / index_len / items_written of destination d's files, *_off = 0, bloom_len = 0.  The files and
+ * *stop are byte-identical to what dbeel_scan returns for the same tables (stop in (table, record) of tables[]).  Only the
+ * selected bytes cross PCIe back; dbeel_last_stats reports input_bytes = bytes copied to the device (windows, index slices,
+ * table headers), output_bytes = the selected output, partitions = partitions run.
+ * Limits and argument checks as dbeel_scan, except that the record limit (fewer than 2^32 - 16) applies per partition, not
+ * to the tree. */
+typedef struct dbeel_scan_io {
+    int (*read)(void *ctx, uint32_t table, uint32_t kind, uint64_t offset, uint64_t len, void *dst);
+    int (*write)(void *ctx, uint32_t dest, uint32_t kind, uint64_t offset, const void *src, uint64_t len);
+    void *ctx;
+} dbeel_scan_io;
+int dbeel_scan_stream(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
+                      uint32_t n_ranges, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop);
+
 /* ---- N4: write-ahead-log replay + flush ------------------------------------------------------------------------
  * Replaces LSMTree::read_memtable_from_wal_file (lsm_tree.rs:552-574) followed by flush_memtable_to_disk, i.e. the
  * recovery of an unflushed memtable in open_or_create_ex (:478-513).  `wal` is the whole `.memtable` file: bincode

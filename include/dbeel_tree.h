@@ -18,6 +18,7 @@
  *   dbeel_tree_sstables    <- LSMTree::sstable_indices_and_sizes (lsm_tree.rs:592-598)
  *   dbeel_tree_get_many    <- the SSTable loop of LSMTree::get_entry (lsm_tree.rs:686-719) through dbeel_get_many()
  *   dbeel_tree_scan        <- the SSTable part of LSMTree::iter_filter (lsm_tree.rs:133-282, :1183-1189) through dbeel_scan()
+ *   dbeel_tree_scan_stream <- the same through dbeel_scan_stream(): the files are streamed, trees of any size
  *   dbeel_memtable_cut     <- RedBlackTree::set + active_memtable_full (rbtree_arena lib.rs:497-534,
  *                             lsm_tree.rs:600-603,757-765): how many arrivals fill one memtable
  *   dbeel_plan_compactions <- compact_tree's size-tiered picker (src/tasks/compaction.rs:35-102),
@@ -83,6 +84,14 @@ int dbeel_tree_get_many(dbeel_tree *t, const void *keys, const uint64_t *key_off
  * dbeel_tree_sstables() order.  The memtables the iterator emits after the tables (:155-173) are the caller's. */
 int dbeel_tree_scan(dbeel_tree *t, uint32_t kind, const void *ranges, uint32_t n_ranges, dbeel_out *out,
                     dbeel_job_result *results, dbeel_scan_stop *stop);
+
+/* The same scan with the files streamed through the engine (dbeel_scan_stream): the tables are pread in pieces, nothing is
+ * held whole in memory, so a tree larger than device or host memory scans too (migration of a shard's whole tree).  Every
+ * destination's output goes to `write` (dbeel_scan_io.write: destination d's .data / .index from offset 0, pieces in any
+ * order, from several threads); its error code comes back unchanged.  results / stop as dbeel_scan_stream. */
+int dbeel_tree_scan_stream(dbeel_tree *t, uint32_t kind, const void *ranges, uint32_t n_ranges,
+                           int (*write)(void *ctx, uint32_t dest, uint32_t kind, uint64_t offset, const void *src, uint64_t len),
+                           void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop);
 
 /* WAL recovery step of open_or_create_ex.  0 logs: *wal_file_index = 0; 1 log: its index; 2 logs: the older one is
  * replayed (memtable of `tree_capacity` entries, DBEEL_ERR_TREE_FULL like the reference's ReachedCapacity), flushed
