@@ -3,6 +3,7 @@
 //   pump              StreamPump with per-destination output pieces (the scan's writer side): every byte of every
 //                     destination's two files arrives exactly once at its offset, pieces longer than kPiece included;
 //                     an error from either callback stops the pump and the first code wins.
+//   pump-far          the same writer loop with file offsets past 2^32, for the scan's pieces and the compaction's OutPart.
 //   plan B1 B2 ...    reads a tree from stdin ("n_tables", then per table "data_len index_path"), plans it with
 //                     dbeel_b200/csrc/host/scan_plan.h at every budget and prints the plan (tests/test_scan_stream_host.py
 //                     checks it against the records and the scan oracle).
@@ -12,6 +13,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+#include <array>
 #include <chrono>
 #include <random>
 #include <string>
@@ -147,6 +150,140 @@ int run_pump() {
     return bad ? 1 : 0;
 }
 
+// Output pieces at file offsets past 2^32 (a destination file larger than 4 GiB): destination d's files start a little
+// over one kPiece below (d + 1) << 32, so pieces, and the kPiece-sized calls a long piece is split into, cross 2^32 and
+// 2^33.  No file is kept: the write callback checks every byte against a pattern of its absolute 64-bit offset (a write
+// at an offset truncated to 32 bits fails it) and records the range it covered.
+uint8_t far_byte(uint32_t d, uint32_t k, uint64_t off) {
+    return (uint8_t)((off >> 32) * 37 + off * 13 + (off >> 11) + d * 31 + k * 7);
+}
+
+struct FarFiles {
+    std::mutex mu;
+    std::vector<std::array<uint64_t, 4>> calls; // dest, kind, offset, len
+    int bad = 0;
+};
+
+int far_check(FarFiles *f, uint32_t dest, uint32_t kind, uint64_t off, const void *src, uint64_t len) {
+    const uint8_t *p = static_cast<const uint8_t *>(src);
+    for (uint64_t i = 0; i < len; i++)
+        if (p[i] != far_byte(dest, kind, off + i)) return 91;
+    std::lock_guard<std::mutex> lk(f->mu);
+    f->calls.push_back({dest, kind, off, len});
+    return 0;
+}
+
+int wr_far(void *ctx, uint32_t dest, uint32_t kind, uint64_t off, const void *src, uint64_t len) {
+    return far_check(static_cast<FarFiles *>(ctx), dest, kind, off, src, len);
+}
+
+int wr_far_compact(void *ctx, uint32_t kind, uint64_t off, const void *src, uint64_t len) {
+    return far_check(static_cast<FarFiles *>(ctx), 0, kind, off, src, len);
+}
+
+int rd_none(void *, uint32_t, uint32_t, uint64_t, uint64_t, void *) { return 0; }
+
+// The calls of every (dest, kind) tile [start, start + total) exactly once; returns the number of calls crossing a
+// multiple of 2^32, or -1.
+long far_coverage(FarFiles &f, uint32_t nd, const std::vector<std::array<uint64_t, 3>> &start,
+                  const std::vector<std::array<uint64_t, 3>> &total) {
+    long crossing = 0;
+    for (uint32_t d = 0; d < nd; d++)
+        for (uint32_t k = 1; k <= 2; k++) {
+            std::vector<std::pair<uint64_t, uint64_t>> r;
+            for (const auto &c : f.calls)
+                if (c[0] == d && c[1] == k) r.push_back({c[2], c[3]});
+            std::sort(r.begin(), r.end());
+            uint64_t at = start[d][k];
+            for (const auto &x : r) {
+                if (x.first != at) {
+                    fprintf(stderr, "dest %u kind %u: call at %llu, expected %llu\n", d, k, (unsigned long long)x.first,
+                            (unsigned long long)at);
+                    return -1;
+                }
+                if (x.first >> 32 != (x.first + x.second - 1) >> 32) crossing++;
+                at += x.second;
+            }
+            if (at != start[d][k] + total[d][k]) {
+                fprintf(stderr, "dest %u kind %u: ends at %llu, expected %llu\n", d, k, (unsigned long long)at,
+                        (unsigned long long)(start[d][k] + total[d][k]));
+                return -1;
+            }
+        }
+    return crossing;
+}
+
+int pump_far_scenario(uint32_t np, uint32_t nd, uint32_t ring, int threads, unsigned seed, bool compact) {
+    std::mt19937_64 rng(seed);
+    FarFiles f;
+    const uint64_t P = StreamPump::kPiece;
+    std::vector<std::array<uint64_t, 3>> start(nd), total(nd, {0, 0, 0}), at(nd);
+    for (uint32_t d = 0; d < nd; d++)
+        for (uint32_t k = 1; k <= 2; k++) start[d][k] = at[d][k] = ((uint64_t)(d + 1) << 32) - P - P / 2 - 5 - 11 * k;
+    std::vector<std::vector<uint8_t>> bufs(np);
+    dbeel_scan_io sio{rd_none, wr_far, &f};
+    dbeel_stream_io cio{rd_none, wr_far_compact, &f};
+    std::unique_ptr<StreamPump> pump(compact ? new StreamPump(&cio, np, ring, threads, [](uint32_t) {})
+                                             : new StreamPump(&sio, np, ring, threads, [](uint32_t) {}));
+    pump->start();
+    for (uint32_t c = 0; c < np; c++) {
+        if (pump->wait_out_slot(c)) return -3;
+        uint64_t len[64][3] = {};
+        uint64_t sz = 0;
+        for (uint32_t d = 0; d < nd; d++)
+            for (uint32_t k = 1; k <= 2; k++) {
+                // partition 0's piece alone runs past (d + 1) << 32; later ones: empty, short or longer than kPiece
+                len[d][k] = c == 0 ? P + P / 2 + 5 + 11 * k + 1 + rng() % P
+                                   : rng() % 5 == 0 ? 0 : (rng() % 3 == 0 ? P + rng() % (P + P / 2) : 1 + rng() % (P / 3));
+                sz += len[d][k];
+            }
+        bufs[c].resize(sz);
+        std::vector<StreamPump::OutPiece> ps;
+        uint64_t pos = 0;
+        for (uint32_t d = 0; d < nd; d++)
+            for (uint32_t k = 1; k <= 2; k++) {
+                for (uint64_t i = 0; i < len[d][k]; i++) bufs[c][pos + i] = far_byte(d, k, at[d][k] + i);
+                ps.push_back({d, k, at[d][k], bufs[c].data() + pos, len[d][k]});
+                at[d][k] += len[d][k];
+                total[d][k] += len[d][k];
+                pos += len[d][k];
+            }
+        if (compact) {
+            StreamPump::OutPart o;
+            o.data = ps[0].src, o.data_len = ps[0].len, o.data_off = ps[0].off;
+            o.index = ps[1].src, o.index_len = ps[1].len, o.index_off = ps[1].off;
+            pump->publish_out(c, o);
+        } else {
+            pump->publish_pieces(c, std::move(ps));
+        }
+    }
+    const int rc = pump->finish();
+    if (rc) return rc;
+    const long crossing = far_coverage(f, nd, start, total);
+    if (crossing < 0) return -2;
+    for (uint32_t d = 0; d < nd; d++)
+        for (uint32_t k = 1; k <= 2; k++)
+            if (start[d][k] + total[d][k] <= ((uint64_t)(d + 1) << 32)) {
+                fprintf(stderr, "dest %u kind %u never reaches %u << 32\n", d, k, d + 1);
+                return -4;
+            }
+    return crossing > 0 ? 0 : -5;
+}
+
+int run_pump_far() {
+    int bad = 0;
+    unsigned seed = 40;
+    for (bool compact : {false, true})
+        for (uint32_t ring : {2u, 3u})
+            for (int threads : {1, 4}) {
+                const uint32_t nd = compact ? 1 : 3;
+                const int rc = pump_far_scenario(5, nd, ring, threads, seed++, compact);
+                if (rc) { fprintf(stderr, "%s ring=%u threads=%d -> %d\n", compact ? "OutPart" : "pieces", ring, threads, rc); bad++; }
+            }
+    printf(bad ? "FAILED %d\n" : "ok\n", bad);
+    return bad ? 1 : 0;
+}
+
 int run_plan(int argc, char **argv) {
     uint32_t n = 0;
     if (scanf("%u", &n) != 1) return 2;
@@ -196,7 +333,8 @@ int run_plan(int argc, char **argv) {
 
 int main(int argc, char **argv) {
     if (argc >= 2 && !strcmp(argv[1], "pump")) return run_pump();
+    if (argc >= 2 && !strcmp(argv[1], "pump-far")) return run_pump_far();
     if (argc >= 3 && !strcmp(argv[1], "plan")) return run_plan(argc, argv);
-    fprintf(stderr, "usage: %s pump | plan BUDGET... < tree\n", argv[0]);
+    fprintf(stderr, "usage: %s pump | pump-far | plan BUDGET... < tree\n", argv[0]);
     return 2;
 }

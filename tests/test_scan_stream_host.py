@@ -149,3 +149,94 @@ def test_plan_ends_at_the_first_panic(exe, tmp_path, kind):
         for plan in _plan(exe, tmp_path, bad, [1, 300, 4096, 1 << 30]):
             _check_plan(bad, plan)
             _check_against_oracle(bad, plan)
+
+
+def test_pump_writes_at_offsets_past_4gib(exe):
+    """Destination files larger than 4 GiB: pieces and their kPiece-sized calls cross 2^32 and 2^33, for the scan's
+    per-destination pieces and the compaction's OutPart, and every byte lands at its full 64-bit offset once."""
+    out = subprocess.run([exe, "pump-far"], capture_output=True, text=True, timeout=300)
+    assert out.returncode == 0, out.stdout + out.stderr
+    assert out.stdout.strip().endswith("ok")
+
+
+class _Virtual:
+    """A .data file that only has a length: the planner never reads .data."""
+
+    def __init__(self, size: int):
+        self.size = size
+
+
+def _virtual_table(rng, panic=None):
+    """About 6 GiB of .data as index records only: small records with every ~800th one a ~270 MiB record, running offsets.
+    panic = (record, kind) damages one record past 2^32: "past_end" points it past the end of .data with a nonzero high
+    word (truncated to 32 bits it would point inside the file), "zero" gives it full_size 0."""
+    n = 20_000
+    fs = rng.integers(40, 300, n).astype(np.int64)
+    fs[400::800] = (270 << 20) + rng.integers(1, 4096, fs[400::800].size)
+    off = np.zeros(n, np.int64)
+    np.cumsum(fs[:-1], out=off[1:])
+    data_len = int(off[-1] + fs[-1]) + 123
+    assert data_len > 6 << 30
+    if panic is not None:
+        r, kind = panic
+        assert off[r] > 1 << 32
+        if kind == "past_end":
+            off[r] = (2 << 32) | (int(off[r]) & 0xFFFFFFFF)
+            assert off[r] > data_len and off[r] & 0xFFFFFFFF < data_len
+        else:
+            fs[r] = 0
+    idx = np.zeros((n, 4), "<u4")
+    idx[:, 0:2] = off.astype("<u8").view("<u4").reshape(n, 2)
+    idx[:, 2] = 20
+    idx[:, 3] = fs
+    return data_len, off, fs, idx.view(np.uint8).reshape(-1)
+
+
+def _plan_model(data_len, off, fs, budget):
+    """plan_scan restated for one table: cut before the record that would take the window or the output bound
+    (sum of full_size + 16) past the budget; end before the first record the reference would panic on."""
+    parts, cur = [], None
+
+    def close():
+        if cur is not None:
+            parts.append({"n_rec": cur[1] - cur[0], "data_bound": cur[4], "slices": [(0, cur[0], cur[1], cur[2], cur[3])]})
+
+    for r in range(off.size):
+        o, f = int(off[r]), int(fs[r])
+        if f == 0 or o > data_len or f > data_len - o:
+            close()
+            return parts, (0, r)
+        if cur is not None and (max(o + f, cur[3]) - min(o, cur[2]) > budget or cur[5] + f + 16 > budget):
+            close()
+            cur = None
+        if cur is None:
+            cur = [r, r, o, o + f, 0, 0]   # rec_lo, rec_hi, win_lo, win_hi, data_bound, out_bound
+        cur[1], cur[2], cur[3] = r + 1, min(cur[2], o), max(cur[3], o + f)
+        cur[4] += f
+        cur[5] += f + 16
+    close()
+    return parts, (-1, 0)
+
+
+@pytest.mark.parametrize("panic", [None, "past_end", "zero"])
+def test_plan_of_a_virtual_6gib_table(exe, tmp_path, panic):
+    """plan_scan over a 6 GiB table that exists only as index records: partition windows, index slices and the PANIC cut
+    past 2^32 equal the Python restatement, at budgets below, at and above one large record and above 4 GiB."""
+    rng = np.random.default_rng(61)
+    data_len, off, fs, idx = _virtual_table(rng)
+    if panic:
+        r = int(np.searchsorted(off, (1 << 32) + (700 << 20)))
+        data_len, off, fs, idx = _virtual_table(np.random.default_rng(61), (r, panic))
+    budgets = [64 << 20, 256 << 20, 1 << 30, 5 << 30, 8 << 30]
+    plans = _plan(exe, tmp_path, [(_Virtual(data_len), idx)], budgets)
+    for plan in plans:
+        parts, stop = _plan_model(data_len, off, fs, plan["budget"])
+        assert plan["panic"] == stop
+        assert plan["parts"] == parts, f"budget {plan['budget']}"
+        if panic:
+            assert stop[1] == r
+        wins = [s[3:] for p in plan["parts"] for s in p["slices"]]
+        assert any(hi > 1 << 32 for _, hi in wins), "no window reaches past 2^32"
+        if plan["budget"] <= 256 << 20:
+            assert any(lo > 1 << 32 for lo, _ in wins), "no window starts past 2^32"
+    assert len(plans[-1]["parts"]) <= 2 and max(p["data_bound"] for p in plans[-1]["parts"]) > 4 << 30
