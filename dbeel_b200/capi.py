@@ -22,6 +22,7 @@ DEFAULT_TREE_CAPACITY = 8192  # mod.rs:18
 LOOKUP_REFERENCE = 0  # the reference's binary_search loop, step for step (lsm_tree.rs:605-670)
 LOOKUP_EXACT = 1      # lower-bound search: every present key is found
 LOOKUP_CORRUPT = 0x80000000
+LOOKUP_BAD_ENTRY = 0x40000000  # get_values: the hit's entry does not decode (the reference's get returns Err)
 SCAN_HASH = 0  # ranges: (start, end) u32 pairs, murmur3_32(key) tested with migration.rs's between_cmp
 SCAN_KEY = 1   # ranges: (start, end) byte strings, start <= key < end
 SCAN_STOP_NONE, SCAN_STOP_ERR, SCAN_STOP_PANIC = 0, 1, 2
@@ -43,7 +44,8 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_host_free", "dbeel_last_stats", "dbeel_last_error", "dbeel_strerror",
            "dbeel_murmur3_32", "dbeel_ring_owner", "dbeel_shard_ring", "dbeel_route_device", "dbeel_flush_many_sparse_device",
            "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream",
-           "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device", "dbeel_scan_stream"]
+           "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device", "dbeel_scan_stream", "dbeel_get_values",
+           "dbeel_get_values_device"]
 
 
 class Run(C.Structure):
@@ -151,6 +153,7 @@ class DbeelError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"dbeel error {code} ({ERR_NAMES.get(code, '?')}): {msg}")
         self.code = code
+        self.needed = None  # get_values*: (data_len, index_len) the output needs, on ERR_CAPACITY
 
 
 _lib = None
@@ -205,6 +208,11 @@ def lib():
             f.restype = C.c_int
             f.argtypes = [C.c_void_p, C.POINTER(Table), C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
                           C.c_void_p]
+        for name in ("dbeel_get_values", "dbeel_get_values_device"):
+            f = getattr(L, name)
+            f.restype = C.c_int
+            f.argtypes = [C.c_void_p, C.POINTER(Table), C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
+                          C.POINTER(Out), C.c_void_p]
         L.dbeel_scan_bound.restype = C.c_int
         L.dbeel_scan_bound.argtypes = [C.POINTER(Table), C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         for name in ("dbeel_scan", "dbeel_scan_device"):
@@ -611,6 +619,56 @@ class Engine:
             arr[j] = Table(t[0], t[1], t[2], t[3], t[4] if t[5] else None, t[5])
         self._check(lib().dbeel_get_many_device(self._h, arr, len(tables), keys_ptr, offsets_ptr, n_keys, mode,
                                                 results_ptr), "dbeel_get_many_device")
+
+    def _get_values_call(self, fn, name: str, arr, n_tables: int, keys_ptr, offsets_ptr, n_keys: int, mode: int, out: Out,
+                         results_ptr):
+        rc = fn(self._h, arr, n_tables, keys_ptr, offsets_ptr, n_keys, mode, C.byref(out), results_ptr)
+        if rc:
+            err = DbeelError(rc, f"{name}: {lib().dbeel_last_error(self._h).decode()}")
+            if rc == ERR_CAPACITY:
+                err.needed = (int(out.data_len), int(out.index_len))
+            raise err
+
+    def get_values(self, tables: Sequence[Tuple[object, object, object]], keys: Sequence[bytes], mode: int = LOOKUP_REFERENCE,
+                   caps: Optional[Tuple[int, int]] = None):
+        """dbeel_get_values over host buffers: get_many's rows plus the entry of every answered row (table >= 0, no
+        LOOKUP_BAD_ENTRY), in query order, as an arrival batch.  Returns (rows, data, index); row i's entry is entry number
+        (answered rows before i).  caps = (data_cap, index_cap); by default the tables' .data sizes and 16 bytes per key,
+        and one more call with the sizes the engine reports when duplicate or overlapping hits need more."""
+        keep = [(_u8(d), _u8(i), _u8(b) if b is not None and len(b) else None) for d, i, b in tables]
+        arr = (Table * max(1, len(keep)))()
+        for j, (d, i, b) in enumerate(keep):
+            arr[j] = Table(d.ctypes.data, d.size, i.ctypes.data, i.size, b.ctypes.data if b is not None else None,
+                           b.size if b is not None else 0)
+        blob, off = pack_keys(keys)
+        res = np.zeros(len(keys), dtype=LOOKUP_DTYPE)
+        dc, ic = caps if caps is not None else (sum(d.size for d, _, _ in keep), 16 * len(keys))
+        for attempt in range(2):
+            od, oi = np.empty(max(1, dc), np.uint8), np.empty(max(1, ic), np.uint8)
+            out = Out(od.ctypes.data, dc, 0, oi.ctypes.data, ic, 0, None, 0, 0, 0)
+            try:
+                self._get_values_call(lib().dbeel_get_values, "dbeel_get_values", arr, len(keep),
+                                      blob.ctypes.data if blob.size else None, off.ctypes.data, len(keys), mode, out, res.ctypes.data)
+                return res, od[:out.data_len], oi[:out.index_len]
+            except DbeelError as ex:
+                if caps is not None or attempt or ex.code != ERR_CAPACITY:
+                    raise
+                dc, ic = ex.needed
+
+    def get_values_device(self, tables: Sequence[Tuple[int, int, int, int, int, int]], keys_ptr: int, offsets_ptr: int,
+                          n_keys: int, results_ptr: int, out_ptrs: Tuple[int, int, int, int],
+                          mode: int = LOOKUP_REFERENCE) -> Tuple[int, int, int]:
+        """dbeel_get_values_device: every pointer is a device pointer; tables as in get_many_device, out_ptrs = (data_ptr,
+        data_cap, index_ptr, index_cap), 16-byte aligned.  Returns (data_len, index_len, items); on ERR_CAPACITY the
+        DbeelError carries .needed = (data_len, index_len)."""
+        arr = (Table * max(1, len(tables)))()
+        for j, t in enumerate(tables):
+            arr[j] = Table(t[0], t[1], t[2], t[3], t[4] if t[5] else None, t[5])
+        dp, dc, ip, ic = out_ptrs
+        out = Out(dp, dc, 0, ip, ic, 0, None, 0, 0, 0)
+        self._get_values_call(lib().dbeel_get_values_device, "dbeel_get_values_device", arr, len(tables), keys_ptr, offsets_ptr,
+                              n_keys, mode, out, results_ptr)
+        return int(out.data_len), int(out.index_len), int(out.items_written)
 
     # ---- N5: scans (LSMTree::iter_filter) ---------------------------------------------------
     def scan(self, tables: Sequence[Tuple[object, ...]], ranges, kind: int = SCAN_HASH):

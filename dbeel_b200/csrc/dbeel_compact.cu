@@ -1350,20 +1350,20 @@ int parse_bloom(dbeel_engine *e, const uint8_t *head, const uint8_t *tail, uint6
     return DBEEL_OK;
 }
 
-int lookup_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys, const uint64_t *key_off,
-                 uint64_t n_keys, uint32_t mode, dbeel_lookup_result *results, bool device) {
-    static_assert(sizeof(dbeel_lookup_result) == 16, "result rows are written as uint4");
-    if (!e) return DBEEL_ERR_INVALID_ARG;
+// The argument checks of both batched reads (dbeel_get_many*, dbeel_get_values*), before the engine is taken.
+int lookup_args(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const uint64_t *key_off, uint64_t n_keys,
+                uint32_t mode, const dbeel_lookup_result *results) {
     if ((n_tables && !tables) || (n_keys && (!key_off || !results))) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     if (mode > DBEEL_LOOKUP_EXACT) return fail(e, DBEEL_ERR_INVALID_ARG, "unknown lookup mode");
     if (n_tables > 65536) return fail(e, DBEEL_ERR_TOO_MANY_RUNS, "more than 65536 tables");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
-    if (n_keys == 0) return DBEEL_OK;
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    return DBEEL_OK;
+}
+
+// The tables as k_lookup reads them, shared by both batched reads: table checks, the bloom trailers parsed on the host and,
+// for host callers, the tables, keys and offsets staged into stage_in (the device path reads only each trailer back).  The
+// TableDesc array goes down from the pinned block into `d_desc`; the pinned block is at least `pin_min` bytes.
+int stage_lookup(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys, const uint64_t *key_off,
+                 uint64_t n_keys, bool device, uint64_t pin_min, TableDesc *d_desc, const uint8_t **d_keys, const uint64_t **d_off) {
     cudaStream_t s = e->stream;
     for (uint32_t i = 0; i < n_tables; i++) {
         const dbeel_table &t = tables[i];
@@ -1374,10 +1374,9 @@ int lookup_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, 
         if (device && (((uintptr_t)t.index & 15) || ((uintptr_t)t.bloom & 3))) return fail(e, DBEEL_ERR_INVALID_ARG, "misaligned device buffer");
     }
     std::vector<TableDesc> td(n_tables);
-    const uint8_t *d_keys = static_cast<const uint8_t *>(keys);
-    const uint64_t *d_off = key_off;
-    uint4 *d_res = reinterpret_cast<uint4 *>(results);
-    int rc = ensure_pinned(e, std::max<uint64_t>(4096, (uint64_t)n_tables * (8 + kBloomTrailer) + n_tables * sizeof(TableDesc)));
+    *d_keys = static_cast<const uint8_t *>(keys);
+    *d_off = key_off;
+    int rc = ensure_pinned(e, std::max<uint64_t>({4096, pin_min, (uint64_t)n_tables * (8 + kBloomTrailer) + n_tables * sizeof(TableDesc)}));
     if (rc) return rc;
     uint8_t *pin_desc = e->pin + (uint64_t)n_tables * (8 + kBloomTrailer);
     if (device) {
@@ -1398,14 +1397,13 @@ int lookup_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, 
                 const uint8_t *hp = e->pin + (uint64_t)i * (8 + kBloomTrailer);
                 if ((rc = parse_bloom(e, hp, hp + 8, tables[i].bloom_len, &td[i]))) return rc;
             }
-    } else { // host buffers: the tables, the keys and the offsets go down, the result rows come back
+    } else { // host buffers: the tables, the keys and the offsets go down
         if (!keys && key_off[n_keys]) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
         const uint64_t key_bytes = key_off[n_keys];
         uint64_t need = align_up(key_bytes + 16, kAlign) + align_up((n_keys + 1) * 8, kAlign);
         for (uint32_t i = 0; i < n_tables; i++)
             need += align_up(tables[i].data_len + 16, kAlign) + align_up(tables[i].index_len + 16, kAlign) + align_up(tables[i].bloom_len + 16, kAlign);
         rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, need);
-        if (!rc) rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, n_keys * 16);
         if (rc) return rc;
         uint64_t pos = 0;
         auto put = [&](const void *src, uint64_t len, uint64_t slack) -> const uint8_t * {
@@ -1414,9 +1412,9 @@ int lookup_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, 
             if (len && cudaMemcpyAsync(dst, src, len, cudaMemcpyHostToDevice, s) != cudaSuccess) return nullptr;
             return dst;
         };
-        d_keys = put(keys, key_bytes, 16);
-        d_off = reinterpret_cast<const uint64_t *>(put(key_off, (n_keys + 1) * 8, 0));
-        if (!d_keys || !d_off) return fail(e, DBEEL_ERR_CUDA, "cudaMemcpyAsync(keys)", cudaGetLastError());
+        *d_keys = put(keys, key_bytes, 16);
+        *d_off = reinterpret_cast<const uint64_t *>(put(key_off, (n_keys + 1) * 8, 0));
+        if (!*d_keys || !*d_off) return fail(e, DBEEL_ERR_CUDA, "cudaMemcpyAsync(keys)", cudaGetLastError());
         for (uint32_t i = 0; i < n_tables; i++) {
             const dbeel_table &t = tables[i];
             const uint8_t *dd = put(t.data, t.data_len, 16), *di = put(t.index, t.index_len, 16), *db = put(t.bloom, t.bloom_len, 16);
@@ -1427,14 +1425,35 @@ int lookup_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, 
             if ((rc = parse_bloom(e, b, b + t.bloom_len - kBloomTrailer, t.bloom_len, &td[i]))) return rc;
             td[i].words = reinterpret_cast<const uint32_t *>(db + 8);
         }
-        d_res = reinterpret_cast<uint4 *>(e->stage_out);
     }
-    rc = ensure_device(e, &e->ws, &e->ws_cap, std::max<uint64_t>(4096, n_tables * sizeof(TableDesc)));
-    if (rc) return rc;
     if (n_tables) {
         memcpy(pin_desc, td.data(), n_tables * sizeof(TableDesc));
-        CU(cudaMemcpyAsync(e->ws, pin_desc, n_tables * sizeof(TableDesc), cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(d_desc, pin_desc, n_tables * sizeof(TableDesc), cudaMemcpyHostToDevice, s));
     }
+    return DBEEL_OK;
+}
+
+int lookup_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys, const uint64_t *key_off,
+                 uint64_t n_keys, uint32_t mode, dbeel_lookup_result *results, bool device) {
+    static_assert(sizeof(dbeel_lookup_result) == 16, "result rows are written as uint4");
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (const int arc = lookup_args(e, tables, n_tables, key_off, n_keys, mode, results)) return arc;
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    e->stats = dbeel_stats{};
+    if (n_keys == 0) return DBEEL_OK;
+    cudaError_t ce = cudaSetDevice(e->device);
+    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    cudaStream_t s = e->stream;
+    int rc = ensure_device(e, &e->ws, &e->ws_cap, std::max<uint64_t>(4096, n_tables * sizeof(TableDesc)));
+    if (!rc && !device) rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, n_keys * 16);
+    if (rc) return rc;
+    const uint8_t *d_keys;
+    const uint64_t *d_off;
+    if ((rc = stage_lookup(e, tables, n_tables, keys, key_off, n_keys, device, 0, reinterpret_cast<TableDesc *>(e->ws), &d_keys, &d_off)))
+        return rc;
+    uint4 *d_res = device ? reinterpret_cast<uint4 *>(results) : reinterpret_cast<uint4 *>(e->stage_out);
     LookupParams lp{reinterpret_cast<const TableDesc *>(e->ws), n_tables, mode, d_keys, d_off, n_keys, d_res};
     CU(cudaEventRecord(e->ev[EV_START], s));
     k_lookup<<<(uint32_t)((n_keys + 255) / 256), 256, 0, s>>>(lp);
@@ -1886,6 +1905,161 @@ void scan_range_header(uint32_t kind, const void *ranges, uint32_t nd, uint64_t 
     }
 }
 
+// ---- the split and phase 2 of a scan, shared with dbeel_get_values*
+// Input: n 16-byte records {source address, 8 + klen, full_size} (ScanParams.flat) and a destination per record
+// (ScanParams.dest, kScanNone = not delivered).  Output: the nd streams back to back in out->data / out->index, in record
+// order inside each stream, every stream's .index offsets relative to its own first byte -- nd arrival batches.  The
+// output can be larger than the inputs (records may share .data bytes), so it is sized from a read-back.
+struct SplitLayout {
+    uint64_t o_ctl, o_memtab, header2_bytes; // second header, after the split is known: control block | (bytes, entries) before each stream
+    uint64_t o_tot, o_dest, o_flat, o_split, o_hist, o_tbytes, o_tcount, o_cbytes, o_ccount, o_src;
+    uint32_t n, nd, n_blocks;
+};
+
+uint64_t carve_ws(uint64_t *off, uint64_t b) {
+    const uint64_t o = *off;
+    *off = align_up(*off + b, kAlign);
+    return o;
+}
+
+SplitLayout carve_split(uint64_t *off, uint32_t n, uint32_t nd) {
+    SplitLayout w;
+    w.n = n;
+    w.nd = nd;
+    w.n_blocks = (n + kRouteThreads - 1) / kRouteThreads;
+    const uint64_t res_tiles = (n + kResolveThreads - 1) / kResolveThreads, res_chunks = (res_tiles + 1023) / 1024;
+    w.o_ctl = carve_ws(off, sizeof(Ctl));
+    w.o_memtab = carve_ws(off, 16ull * (nd + 1));
+    w.header2_bytes = *off - w.o_ctl;
+    w.o_tot = carve_ws(off, 8ull * (3 * nd + 1));
+    w.o_dest = carve_ws(off, 4ull * n);
+    w.o_flat = carve_ws(off, 16ull * n);
+    w.o_split = carve_ws(off, 16ull * n);
+    w.o_hist = carve_ws(off, 4ull * w.n_blocks * nd);
+    w.o_tbytes = carve_ws(off, 8 * res_tiles);
+    w.o_tcount = carve_ws(off, 4 * res_tiles);
+    w.o_cbytes = carve_ws(off, 8 * res_chunks);
+    w.o_ccount = carve_ws(off, 4 * res_chunks);
+    w.o_src = carve_ws(off, 8ull * n);
+    return w;
+}
+
+// ScanParams fields the split reads: records, destinations, the stop word (totals[3 nd], stop0 = none)
+void split_params(const SplitLayout &w, uint8_t *ws, ScanParams *sp) {
+    sp->dest = reinterpret_cast<uint32_t *>(ws + w.o_dest);
+    sp->flat = reinterpret_cast<uint4 *>(ws + w.o_flat);
+    sp->stop = reinterpret_cast<unsigned long long *>(ws + w.o_tot) + 3ull * w.nd;
+    sp->stop0 = ~0ull;
+}
+
+// Enqueued behind the kernels that wrote sp.flat / sp.dest (totals zeroed, the stop word set).  k_scan_hist drops what lies
+// at or past the stop, k_route_scan / k_route_starts / k_route_scatter split the records stably, and k_route_starts publishes
+// the totals (counts | bytes | starts | stop, nd each + 1) to the mapped pinned block at pin_tot.  `sized(totals)` runs on
+// them before the caps are checked: DBEEL_ERR_CAPACITY (nothing written, *items / *bytes = the required sizes) is the
+// caller's to report.  Then k_scan_tile_sums .. k_rebase_index write the output; ms_total runs from EV_START.
+template <class F>
+int split_emit(dbeel_engine *e, const SplitLayout &w, const ScanParams &sp, uint64_t pin_tot, bool device, dbeel_out *out,
+               uint32_t *launches, uint64_t *items_out, uint64_t *bytes_out, F &&sized) {
+    cudaStream_t s = e->stream;
+    uint8_t *ws = e->ws, *h = e->pin;
+    const uint32_t n = w.n, nd = w.nd;
+    RouteParams rp = {};
+    rp.index = sp.flat;
+    rp.n = n;
+    rp.n_shards = nd;
+    rp.n_blocks = w.n_blocks;
+    rp.shard_of = sp.dest;
+    rp.hist = reinterpret_cast<uint32_t *>(ws + w.o_hist);
+    rp.totals = reinterpret_cast<unsigned long long *>(ws + w.o_tot);
+    rp.out_index = reinterpret_cast<uint4 *>(ws + w.o_split);
+    launch_k(e, k_scan_hist, w.n_blocks, kRouteThreads, 0, s, sp, rp);
+    launch_k(e, k_route_scan, nd, 1024, 0, s, rp);
+    unsigned long long *host_tot = reinterpret_cast<unsigned long long *>(e->pin + pin_tot);
+    launch_k(e, k_route_starts, 1, 256, 0, s, rp, reinterpret_cast<unsigned long long *>(e->pin_dev + pin_tot));
+    launch_k(e, k_route_scatter, w.n_blocks, kRouteThreads, 0, s, rp);
+    *launches += 4;
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(s));
+    sized(static_cast<const unsigned long long *>(host_tot));
+    uint64_t items = 0, bytes = 0;
+    for (uint32_t d = 0; d < nd; d++) {
+        items += host_tot[d];
+        bytes += host_tot[nd + d];
+    }
+    *items_out = items;
+    *bytes_out = bytes;
+    if (bytes > out->data_cap || 16 * items > out->index_cap) return DBEEL_ERR_CAPACITY;
+    if (device && ((bytes && !out->data) || (items && !out->index))) return fail(e, DBEEL_ERR_INVALID_ARG, "null output buffer");
+    // What depends on the output size is sized now that it is known -- records that share .data bytes can make the output
+    // larger than the inputs: the gather's tile_first (one entry per 8 KB output tile) and, for host callers, the staged
+    // outputs.  They live in stage_out, so the phase-1 workspace (the split records) stays where it is.
+    const uint64_t gather_tiles = (bytes + kGatherTileBytes - 1) / kGatherTileBytes;
+    const uint64_t tf_bytes = align_up(4ull * (gather_tiles + 2), kAlign);
+    int rc = ensure_device(e, &e->stage_out, &e->stage_out_cap,
+                           tf_bytes + (device ? 0 : align_up(bytes + 16, kAlign) + align_up(16 * items + 16, kAlign)));
+    if (rc) return rc;
+    uint32_t *tile_first = reinterpret_cast<uint32_t *>(e->stage_out);
+    uint8_t *o_data = device ? static_cast<uint8_t *>(out->data) : e->stage_out + tf_bytes;
+    uint8_t *o_index = device ? static_cast<uint8_t *>(out->index) : e->stage_out + tf_bytes + align_up(bytes + 16, kAlign);
+
+    // ---- phase 2: .index (k_emit's offsets scan), payload gather, per-destination file offsets
+    if (items) {
+        Ctl *hc = reinterpret_cast<Ctl *>(h);
+        memset(hc, 0, sizeof(Ctl));
+        hc->span = (uint32_t)items;
+        hc->total = (uint32_t)items;
+        unsigned long long *hm = reinterpret_cast<unsigned long long *>(h + (w.o_memtab - w.o_ctl));
+        unsigned long long before_b = 0, before_i = 0;
+        for (uint32_t d = 0; d <= nd; d++) {
+            hm[2 * d] = before_b;
+            hm[2 * d + 1] = before_i;
+            if (d < nd) { before_b += host_tot[nd + d]; before_i += host_tot[d]; }
+        }
+        Params p;
+        memset(&p, 0, sizeof p);
+        p.ctl = reinterpret_cast<Ctl *>(ws + w.o_ctl);
+        p.tile_bytes = reinterpret_cast<unsigned long long *>(ws + w.o_tbytes);
+        p.tile_count = reinterpret_cast<uint32_t *>(ws + w.o_tcount);
+        p.chunk_bytes = reinterpret_cast<unsigned long long *>(ws + w.o_cbytes);
+        p.chunk_count = reinterpret_cast<uint32_t *>(ws + w.o_ccount);
+        p.src_ptr = reinterpret_cast<unsigned long long *>(ws + w.o_src);
+        p.tile_first = tile_first;
+        p.tile_first_n = (uint32_t)(gather_tiles + 2);
+        p.data_bound = bytes;
+        p.n_groups = nd;
+        p.mem_table = reinterpret_cast<unsigned long long *>(ws + w.o_memtab);
+        p.out_data = o_data;
+        p.out_index = reinterpret_cast<uint4 *>(o_index);
+        const uint4 *split = rp.out_index;
+        const uint32_t tiles = (uint32_t)((items + kResolveThreads - 1) / kResolveThreads);
+        launch_k(e, k_copy_words, (uint32_t)((w.header2_bytes / 4 + 255) / 256), 256, 0, s, reinterpret_cast<uint32_t *>(ws + w.o_ctl),
+                 reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(w.header2_bytes / 4));
+        launch_k(e, k_scan_tile_sums, tiles, kResolveThreads, 0, s, p, split);
+        launch_k(e, k_scan_tiles, (tiles + 1023) / 1024, 1024, 0, s, p);
+        launch_k(e, k_scan_chunks, 1, 1024, 0, s, p);
+        launch_k(e, k_emit, tiles, kResolveThreads, 0, s, p, split);
+        launch_k(e, k_gather_h, (uint32_t)gather_tiles, kGhThreads, 0, s, p); // no filter: Params.bloom.words is null
+        launch_k(e, k_rebase_index, (uint32_t)((items + 255) / 256), 256, 0, s, p);
+        *launches += 7;
+    }
+    CU(cudaEventRecord(e->ev[EV_GATHER], s));
+    CU(cudaGetLastError());
+    if (!device) {
+        if (bytes) CU(cudaMemcpyAsync(out->data, o_data, bytes, cudaMemcpyDeviceToHost, s));
+        if (items) CU(cudaMemcpyAsync(out->index, o_index, 16 * items, cudaMemcpyDeviceToHost, s));
+    }
+    CU(cudaStreamSynchronize(s));
+    cudaEventElapsedTime(&e->stats.ms_total, e->ev[EV_START], e->ev[EV_GATHER]);
+    e->stats.kernel_launches = *launches;
+    e->stats.entries_out = items;
+    e->stats.output_bytes = bytes + 16 * items;
+    e->stats.gather_bytes = 2 * bytes + 16 * items + 8 * items;
+    out->data_len = bytes;
+    out->index_len = 16 * items;
+    out->items_written = items;
+    return DBEEL_OK;
+}
+
 int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges, uint32_t n_ranges,
                dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop, bool device) {
     if (!e) return DBEEL_ERR_INVALID_ARG;
@@ -1954,27 +2128,15 @@ int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
 
     // ---- workspace (the engine's grow-only one: a compaction after a scan reuses it as it is)
     const uint32_t nd = n_ranges;
-    const uint32_t n_blocks = (n + kRouteThreads - 1) / kRouteThreads;
-    const uint64_t res_tiles = (n + kResolveThreads - 1) / kResolveThreads, res_chunks = (res_tiles + 1023) / 1024;
     uint64_t off = 0;
-    auto carve = [&](uint64_t b) { uint64_t o2 = off; off = align_up(off + b, kAlign); return o2; };
     // header block, one copy through the mapped pinned block: tables | hash ranges or key offsets | range keys
-    const uint64_t o_tab = carve(sizeof(ScanTable) * n_tables);
-    const uint64_t o_rng = carve(kind == DBEEL_SCAN_KEY ? 8ull * (2 * nd + 1) : 8ull * nd);
-    const uint64_t o_keys = carve(key_bytes + 16);
+    const uint64_t o_tab = carve_ws(&off, sizeof(ScanTable) * n_tables);
+    const uint64_t o_rng = carve_ws(&off, kind == DBEEL_SCAN_KEY ? 8ull * (2 * nd + 1) : 8ull * nd);
+    const uint64_t o_keys = carve_ws(&off, key_bytes + 16);
     const uint64_t header_bytes = off;
-    // second header, after the split is known: control block | per-destination (bytes, entries) before it
-    const uint64_t o_ctl = carve(sizeof(Ctl));
-    const uint64_t o_memtab = carve(16ull * (nd + 1));
-    const uint64_t header2_bytes = off - o_ctl;
-    const uint64_t o_tot = carve(8ull * (3 * nd + 1));
-    const uint64_t o_dest = carve(4ull * n), o_flat = carve(16ull * n), o_split = carve(16ull * n);
-    const uint64_t o_hist = carve(4ull * n_blocks * nd);
-    const uint64_t o_tbytes = carve(8 * res_tiles), o_tcount = carve(4 * res_tiles);
-    const uint64_t o_cbytes = carve(8 * res_chunks), o_ccount = carve(4 * res_chunks);
-    const uint64_t o_src = carve(8ull * n);
+    const SplitLayout w = carve_split(&off, n, nd);
     int rc = ensure_device(e, &e->ws, &e->ws_cap, off);
-    const uint64_t pin_tot = align_up(std::max(header_bytes, header2_bytes), 64);
+    const uint64_t pin_tot = align_up(std::max(header_bytes, w.header2_bytes), 64);
     if (!rc) rc = ensure_pinned(e, pin_tot + 8ull * (3 * nd + 1));
     if (rc) return rc;
     uint8_t *ws = e->ws, *h = e->pin;
@@ -1990,121 +2152,96 @@ int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
     sp.hash_ranges = reinterpret_cast<const uint32_t *>(ws + o_rng);
     sp.key_off = reinterpret_cast<const unsigned long long *>(ws + o_rng);
     sp.keys = ws + o_keys;
-    sp.dest = reinterpret_cast<uint32_t *>(ws + o_dest);
-    sp.flat = reinterpret_cast<uint4 *>(ws + o_flat);
-    sp.stop = reinterpret_cast<unsigned long long *>(ws + o_tot) + 3ull * nd;
+    split_params(w, ws, &sp);
     sp.stop0 = stop0;
-    RouteParams rp = {};
-    rp.index = sp.flat;
-    rp.n = n;
-    rp.n_shards = nd;
-    rp.n_blocks = n_blocks;
-    rp.shard_of = sp.dest;
-    rp.hist = reinterpret_cast<uint32_t *>(ws + o_hist);
-    rp.totals = reinterpret_cast<unsigned long long *>(ws + o_tot);
-    rp.out_index = reinterpret_cast<uint4 *>(ws + o_split);
 
-    // ---- phase 1: classify, split; the per-destination counts and bytes come back to size phase 2
+    // ---- phase 1: classify; the split and phase 2 (split_emit) size the output from what it selected
     uint32_t launches = 0;
     CU(cudaEventRecord(e->ev[EV_START], s));
     launch_k(e, k_copy_words, (uint32_t)((header_bytes / 4 + 255) / 256), 256, 0, s, reinterpret_cast<uint32_t *>(ws),
              reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(header_bytes / 4));
-    CU(cudaMemsetAsync(rp.totals, 0, 8ull * 3 * nd, s));
+    CU(cudaMemsetAsync(ws + w.o_tot, 0, 8ull * 3 * nd, s));
     CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
     launch_k(e, k_scan_classify, (n + 255) / 256, 256, 0, s, sp);
-    launch_k(e, k_scan_hist, n_blocks, kRouteThreads, 0, s, sp, rp);
-    launch_k(e, k_route_scan, nd, 1024, 0, s, rp);
-    unsigned long long *host_tot = reinterpret_cast<unsigned long long *>(e->pin + pin_tot);
-    launch_k(e, k_route_starts, 1, 256, 0, s, rp, reinterpret_cast<unsigned long long *>(e->pin_dev + pin_tot));
-    launch_k(e, k_route_scatter, n_blocks, kRouteThreads, 0, s, rp);
-    launches += 6;
-    CU(cudaGetLastError());
-    CU(cudaStreamSynchronize(s));
-    const unsigned long long stop_key = std::min<unsigned long long>(host_tot[3 * nd], stop0);
-    set_stop(stop_key);
-    e->stats.entries_valid = stop_key == ~0ull ? n : (stop_key >> 12);
+    launches += 2;
     uint64_t items = 0, bytes = 0;
-    for (uint32_t d = 0; d < nd; d++) {
-        dbeel_job_result &r = results[d];
-        r.data_off = bytes;
-        r.data_len = host_tot[nd + d];
-        r.index_off = 16 * items;
-        r.items_written = host_tot[d];
-        r.index_len = 16 * host_tot[d];
-        items += host_tot[d];
-        bytes += host_tot[nd + d];
-    }
-    if (bytes > out->data_cap || 16 * items > out->index_cap) {
+    rc = split_emit(e, w, sp, pin_tot, device, out, &launches, &items, &bytes, [&](const unsigned long long *host_tot) {
+        const unsigned long long stop_key = std::min<unsigned long long>(host_tot[3 * nd], stop0);
+        set_stop(stop_key);
+        e->stats.entries_valid = stop_key == ~0ull ? n : (stop_key >> 12);
+        uint64_t it = 0, by = 0;
+        for (uint32_t d = 0; d < nd; d++) {
+            dbeel_job_result &r = results[d];
+            r.data_off = by;
+            r.data_len = host_tot[nd + d];
+            r.index_off = 16 * it;
+            r.items_written = host_tot[d];
+            r.index_len = 16 * host_tot[d];
+            it += host_tot[d];
+            by += host_tot[nd + d];
+        }
+    });
+    if (rc == DBEEL_ERR_CAPACITY) {
         for (uint32_t d = 0; d < nd; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
         return fail(e, DBEEL_ERR_CAPACITY, "scan output larger than the buffers (index records that overlap in .data)");
     }
-    if (device && ((bytes && !out->data) || (items && !out->index))) return fail(e, DBEEL_ERR_INVALID_ARG, "null output buffer");
-    // What depends on the output size is sized now that it is known -- records that share .data bytes can make the output
-    // larger than the inputs: the gather's tile_first (one entry per 8 KB output tile) and, for host callers, the staged
-    // outputs.  They live in stage_out, so the phase-1 workspace (the split records) stays where it is.
-    const uint64_t gather_tiles = (bytes + kGatherTileBytes - 1) / kGatherTileBytes;
-    const uint64_t tf_bytes = align_up(4ull * (gather_tiles + 2), kAlign);
-    rc = ensure_device(e, &e->stage_out, &e->stage_out_cap,
-                       tf_bytes + (device ? 0 : align_up(bytes + 16, kAlign) + align_up(16 * items + 16, kAlign)));
-    if (rc) return rc;
-    uint32_t *tile_first = reinterpret_cast<uint32_t *>(e->stage_out);
-    uint8_t *o_data = device ? static_cast<uint8_t *>(out->data) : e->stage_out + tf_bytes;
-    uint8_t *o_index = device ? static_cast<uint8_t *>(out->index) : e->stage_out + tf_bytes + align_up(bytes + 16, kAlign);
+    return rc;
+}
 
-    // ---- phase 2: .index (k_emit's offsets scan), payload gather, per-destination file offsets
-    if (items) {
-        Ctl *hc = reinterpret_cast<Ctl *>(h);
-        memset(hc, 0, sizeof(Ctl));
-        hc->span = (uint32_t)items;
-        hc->total = (uint32_t)items;
-        unsigned long long *hm = reinterpret_cast<unsigned long long *>(h + (o_memtab - o_ctl));
-        for (uint32_t d = 0; d <= nd; d++) {
-            hm[2 * d] = d < nd ? results[d].data_off : bytes;
-            hm[2 * d + 1] = d < nd ? results[d].index_off / 16 : items;
-        }
-        Params p;
-        memset(&p, 0, sizeof p);
-        p.ctl = reinterpret_cast<Ctl *>(ws + o_ctl);
-        p.tile_bytes = reinterpret_cast<unsigned long long *>(ws + o_tbytes);
-        p.tile_count = reinterpret_cast<uint32_t *>(ws + o_tcount);
-        p.chunk_bytes = reinterpret_cast<unsigned long long *>(ws + o_cbytes);
-        p.chunk_count = reinterpret_cast<uint32_t *>(ws + o_ccount);
-        p.src_ptr = reinterpret_cast<unsigned long long *>(ws + o_src);
-        p.tile_first = tile_first;
-        p.tile_first_n = (uint32_t)(gather_tiles + 2);
-        p.data_bound = bytes;
-        p.n_groups = nd;
-        p.mem_table = reinterpret_cast<unsigned long long *>(ws + o_memtab);
-        p.out_data = o_data;
-        p.out_index = reinterpret_cast<uint4 *>(o_index);
-        const uint4 *split = rp.out_index;
-        const uint32_t tiles = (uint32_t)((items + kResolveThreads - 1) / kResolveThreads);
-        launch_k(e, k_copy_words, (uint32_t)((header2_bytes / 4 + 255) / 256), 256, 0, s, reinterpret_cast<uint32_t *>(ws + o_ctl),
-                 reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(header2_bytes / 4));
-        launch_k(e, k_scan_tile_sums, tiles, kResolveThreads, 0, s, p, split);
-        launch_k(e, k_scan_tiles, (tiles + 1023) / 1024, 1024, 0, s, p);
-        launch_k(e, k_scan_chunks, 1, 1024, 0, s, p);
-        launch_k(e, k_emit, tiles, kResolveThreads, 0, s, p, split);
-        launch_k(e, k_gather_h, (uint32_t)gather_tiles, kGhThreads, 0, s, p); // no filter: Params.bloom.words is null
-        launch_k(e, k_rebase_index, (uint32_t)((items + 255) / 256), 256, 0, s, p);
-        launches += 7;
+
+// ------------------------------------------------------------------------------------ N2 with values: dbeel_get_values*
+// k_lookup_emit writes the rows and, per query, its hit's entry as a split record for destination 0 (or kScanNone: no
+// entry); split_emit turns those into one arrival batch in query order.  Only the rows and the selected bytes come back.
+int get_values_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys, const uint64_t *key_off,
+                     uint64_t n_keys, uint32_t mode, dbeel_out *out, dbeel_lookup_result *results, bool device) {
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (!out) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    if (const int arc = lookup_args(e, tables, n_tables, key_off, n_keys, mode, results)) return arc;
+    if (n_keys >= 0xFFFFFFF0ull) return fail(e, DBEEL_ERR_INVALID_ARG, "2^32 - 16 keys or more");
+    if (device && (((uintptr_t)out->data | (uintptr_t)out->index) & 15))
+        return fail(e, DBEEL_ERR_INVALID_ARG, "device output buffers must be 16-byte aligned");
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    e->stats = dbeel_stats{};
+    out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
+    if (n_keys == 0) return DBEEL_OK;
+    cudaError_t ce = cudaSetDevice(e->device);
+    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    cudaStream_t s = e->stream;
+    const uint32_t n = (uint32_t)n_keys;
+    uint64_t off = 0;
+    const uint64_t o_desc = carve_ws(&off, sizeof(TableDesc) * n_tables);
+    const uint64_t o_rows = carve_ws(&off, device ? 0 : 16ull * n); // host callers: the rows before their D2H
+    const SplitLayout w = carve_split(&off, n, 1);
+    int rc = ensure_device(e, &e->ws, &e->ws_cap, off);
+    if (rc) return rc;
+    const uint64_t pin_tot = align_up(w.header2_bytes, 64);
+    const uint8_t *d_keys;
+    const uint64_t *d_off;
+    rc = stage_lookup(e, tables, n_tables, keys, key_off, n_keys, device, pin_tot + 8ull * 4, reinterpret_cast<TableDesc *>(e->ws + o_desc),
+                      &d_keys, &d_off);
+    if (rc) return rc;
+    uint8_t *ws = e->ws;
+    ScanParams sp = {};
+    split_params(w, ws, &sp);
+    uint4 *d_res = device ? reinterpret_cast<uint4 *>(results) : reinterpret_cast<uint4 *>(ws + o_rows);
+    LookupParams lp{reinterpret_cast<const TableDesc *>(ws + o_desc), n_tables, mode, d_keys, d_off, n_keys, d_res};
+    e->stats.entries_in = n_keys;
+    uint32_t launches = 1;
+    CU(cudaEventRecord(e->ev[EV_START], s));
+    CU(cudaMemsetAsync(ws + w.o_tot, 0, 8ull * 3, s));
+    CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
+    launch_k(e, k_lookup_emit, (n + 255) / 256, 256, 0, s, lp, LookupEmit{sp.dest, sp.flat});
+    if (!device) CU(cudaMemcpyAsync(results, d_res, 16ull * n, cudaMemcpyDeviceToHost, s)); // back with the sizes: filled on ERR_CAPACITY too
+    uint64_t items = 0, bytes = 0;
+    rc = split_emit(e, w, sp, pin_tot, device, out, &launches, &items, &bytes, [](const unsigned long long *) {});
+    if (rc == DBEEL_ERR_CAPACITY) {
+        out->data_len = bytes;
+        out->index_len = 16 * items;
+        return fail(e, DBEEL_ERR_CAPACITY, "the entries found are larger than the output buffers (data_len / index_len: the sizes needed)");
     }
-    CU(cudaEventRecord(e->ev[EV_GATHER], s));
-    CU(cudaGetLastError());
-    if (!device) {
-        if (bytes) CU(cudaMemcpyAsync(out->data, o_data, bytes, cudaMemcpyDeviceToHost, s));
-        if (items) CU(cudaMemcpyAsync(out->index, o_index, 16 * items, cudaMemcpyDeviceToHost, s));
-    }
-    CU(cudaStreamSynchronize(s));
-    cudaEventElapsedTime(&e->stats.ms_total, e->ev[EV_START], e->ev[EV_GATHER]);
-    e->stats.kernel_launches = launches;
-    e->stats.entries_out = items;
-    e->stats.output_bytes = bytes + 16 * items;
-    e->stats.gather_bytes = 2 * bytes + 16 * items + 8 * items;
-    out->data_len = bytes;
-    out->index_len = 16 * items;
-    out->items_written = items;
-    return DBEEL_OK;
+    return rc;
 }
 
 
@@ -2708,6 +2845,18 @@ int dbeel_get_many_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n
                           const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_lookup_result *results) {
     REFUSE_WHILE_ASYNC(e);
     return lookup_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, results, true);
+}
+
+int dbeel_get_values(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys, const uint64_t *key_offsets,
+                     uint64_t n_keys, uint32_t mode, dbeel_out *out, dbeel_lookup_result *results) {
+    REFUSE_WHILE_ASYNC(e);
+    return get_values_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, out, results, false);
+}
+
+int dbeel_get_values_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys,
+                            const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_out *out, dbeel_lookup_result *results) {
+    REFUSE_WHILE_ASYNC(e);
+    return get_values_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, out, results, true);
 }
 
 int dbeel_scan_bound(const dbeel_table *tables, uint32_t n_tables, uint64_t *data_cap, uint64_t *index_cap) {

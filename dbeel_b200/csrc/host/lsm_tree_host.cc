@@ -608,12 +608,10 @@ int dbeel_tree_flush(dbeel_tree *t, const dbeel_run *batch, uint64_t *written_in
     return DBEEL_OK;
 }
 
-int dbeel_tree_get_many(dbeel_tree *t, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
-                        dbeel_lookup_result *results) {
-    if (!t || (n_keys && (!key_offsets || !results))) return DBEEL_ERR_INVALID_ARG;
-    t->err.clear();
-    // get_entry walks `self.sstables` (ascending index) newest first (lsm_tree.rs:686-688); every table brings its
-    // .bloom if one exists on disk (SSTable::new_with_bloom_read, :94-101)
+// get_entry walks `self.sstables` (ascending index) newest first (lsm_tree.rs:686-688); every table brings its .bloom if one
+// exists on disk (SSTable::new_with_bloom_read, :94-101).  `read(tables)` runs on the tree's files read whole.
+extern "C++" template <class F>
+int with_lookup_tables(dbeel_tree *t, F &&read) {
     const size_t n = t->sstables.size();
     std::vector<PinnedBuf> data(n), index(n), bloom(n);
     std::vector<dbeel_table> tables(n);
@@ -626,9 +624,27 @@ int dbeel_tree_get_many(dbeel_tree *t, const void *keys, const uint64_t *key_off
         if (rc) return rc;
         tables[i] = dbeel_table{data[i].p, data[i].len, index[i].p, index[i].len, bloom[i].len ? bloom[i].p : nullptr, bloom[i].len};
     }
-    int rc = dbeel_get_many(t->engine, tables.data(), (uint32_t)n, keys, key_offsets, n_keys, mode, results);
+    int rc = read(tables.data(), (uint32_t)n);
     if (rc) t->err = dbeel_last_error(t->engine);
     return rc;
+}
+
+int dbeel_tree_get_many(dbeel_tree *t, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
+                        dbeel_lookup_result *results) {
+    if (!t || (n_keys && (!key_offsets || !results))) return DBEEL_ERR_INVALID_ARG;
+    t->err.clear();
+    return with_lookup_tables(t, [&](const dbeel_table *tables, uint32_t n) {
+        return dbeel_get_many(t->engine, tables, n, keys, key_offsets, n_keys, mode, results);
+    });
+}
+
+int dbeel_tree_get_values(dbeel_tree *t, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
+                          dbeel_out *out, dbeel_lookup_result *results) {
+    if (!t || !out || (n_keys && (!key_offsets || !results))) return DBEEL_ERR_INVALID_ARG;
+    t->err.clear();
+    return with_lookup_tables(t, [&](const dbeel_table *tables, uint32_t n) {
+        return dbeel_get_values(t->engine, tables, n, keys, key_offsets, n_keys, mode, out, results);
+    });
 }
 
 int dbeel_tree_scan(dbeel_tree *t, uint32_t kind, const void *ranges, uint32_t n_ranges, dbeel_out *out, dbeel_job_result *results,

@@ -11,9 +11,13 @@
 //                           are reported absent, exactly as the reference reports them
 //                           (oracle: orc_sstable_lookup; tests/test_oracle_goldens.py);
 //   DBEEL_LOOKUP_EXACT      a plain lower-bound search that finds every key that is present.
+//
+// k_lookup writes the rows (dbeel_get_many*); k_lookup_emit runs the same search and also hands each query's entry to the
+// scan's split and phase 2 (dbeel_get_values*: the entries come back as one arrival batch in query order).
 #pragma once
 
 #include "kernels.cuh"
+#include "scan.cuh"
 
 namespace dbeel {
 
@@ -71,11 +75,14 @@ __device__ __forceinline__ int cmp_key_bytes(const uint8_t *a, uint64_t alen, co
     return alen < blen ? -1 : (alen > blen ? 1 : 0);
 }
 
-constexpr uint32_t kLookupCorrupt = 0x80000000u; // an index record pointed outside its .data file
+constexpr uint32_t kLookupCorrupt = 0x80000000u;  // an index record pointed outside its .data file
+constexpr uint32_t kLookupBadEntry = 0x40000000u; // k_lookup_emit: the hit's entry does not decode (get_entry returns Err)
 
-// compare the key of entry `rec` of table t with the query: sets *bad when the record cannot be decoded
-__device__ __forceinline__ int probe(const TableDesc &t, uint64_t rec, const uint8_t *key, uint64_t klen, bool *bad) {
+// compare the key of entry `rec` of table t with the query: sets *bad when the record cannot be decoded; *ix_out = the index
+// record (the emitting form decodes a hit's entry from it without loading it again)
+__device__ __forceinline__ int probe(const TableDesc &t, uint64_t rec, const uint8_t *key, uint64_t klen, bool *bad, uint4 *ix_out) {
     const uint4 ix = ldg128_narrow(&t.index[rec]);
+    *ix_out = ix;
     const uint64_t off = (uint64_t)ix.x | ((uint64_t)ix.y << 32);
     if (off > t.data_len || t.data_len - off < 8) { *bad = true; return 0; }
     const uint64_t cur_klen = ld_bytes_le<true>(t.data + off, 8); // bincode Vec<u8>: u64 length, then the bytes
@@ -86,9 +93,21 @@ __device__ __forceinline__ int probe(const TableDesc &t, uint64_t rec, const uin
 #ifndef DBEEL_LOOKUP_MINB
 #define DBEEL_LOOKUP_MINB 4 // 4 CTAs of 256 threads per SM = a 64-register cap
 #endif
-__global__ void __launch_bounds__(256, DBEEL_LOOKUP_MINB) k_lookup(LookupParams p) {
-    pdl_trigger();
-    pdl_wait();
+// dbeel_get_values*: per query the destination of its entry (0 = answered, kScanNone = no entry) and the 16-byte record
+// {source address, 8 + klen, full_size} the scan's phase 2 splits and gathers (scan.cuh)
+struct LookupEmit {
+    uint32_t *dest;
+    uint4 *flat;
+};
+
+// The search of one query key, shared by k_lookup (rows only) and k_lookup_emit (rows + the hit's entry as a split record).
+// kEmit decodes the hit the way binary_search does after the key compared equal (lsm_tree.rs:628-651): the key frame
+// read_at(offset, key_size) must be exactly the key (bincode reject_trailing_bytes: key_size == 8 + klen), and
+// read_at(offset + key_size, full_size - key_size) exactly one EntryValue (u64 dlen | data | i128 ts inside `time`'s
+// range) inside .data.  A hit that does not decode gets kLookupBadEntry and no entry: the reference's `?` returns Err
+// there, so no older table is tried either.
+template <bool kEmit>
+__device__ __forceinline__ void lookup_query(const LookupParams &p, const LookupEmit &em) {
     const uint64_t q = (uint64_t)blockIdx.x * 256u + threadIdx.x;
     if (q >= p.n_keys) return;
     const uint64_t k0 = p.key_off[q];
@@ -97,6 +116,7 @@ __global__ void __launch_bounds__(256, DBEEL_LOOKUP_MINB) k_lookup(LookupParams 
     int32_t found_table = -1;
     uint32_t rejects = 0;
     uint64_t record = 0;
+    uint4 hit_ix = make_uint4(0, 0, 0, 0);
     for (uint32_t ti = p.n_tables; ti-- > 0 && found_table < 0;) { // sstables.iter().rev(): newest first (:688)
         const TableDesc &t = p.tables[ti];
         if (t.words != nullptr) { // :691-696
@@ -121,9 +141,10 @@ __global__ void __launch_bounds__(256, DBEEL_LOOKUP_MINB) k_lookup(LookupParams 
             uint64_t half = n / 2, high = n - 1, low = 0;
             bool done = false;
             while (!done) {
-                const int c = probe(t, half, key, klen, &bad);
+                uint4 ix;
+                const int c = probe(t, half, key, klen, &bad, &ix);
                 const bool hit = c == 0 && !bad;
-                if (hit) { found_table = (int32_t)ti; record = half; }
+                if (hit) { found_table = (int32_t)ti; record = half; hit_ix = ix; }
                 low = c < 0 ? half + 1 : low;                              // Ordering::Less
                 high = c > 0 ? (half > 1 ? half : 1) - 1 : high;           // Ordering::Greater: max(half, 1) - 1
                 done = hit || bad || half == 0 || half == n;               // `if half == 0 || half == length { break }`
@@ -134,14 +155,51 @@ __global__ void __launch_bounds__(256, DBEEL_LOOKUP_MINB) k_lookup(LookupParams 
             uint64_t lo = 0, hi = n;
             while (lo < hi && !bad) {
                 const uint64_t mid = lo + (hi - lo) / 2;
-                const int c = probe(t, mid, key, klen, &bad);
-                if (c == 0 && !bad) { found_table = (int32_t)ti; record = mid; break; }
+                uint4 ix;
+                const int c = probe(t, mid, key, klen, &bad, &ix);
+                if (c == 0 && !bad) { found_table = (int32_t)ti; record = mid; hit_ix = ix; break; }
                 if (c < 0) lo = mid + 1; else hi = mid;
             }
         }
         if (bad) { rejects |= kLookupCorrupt; break; } // the reference's read_at would fail here: the whole get errors out
     }
+    if constexpr (kEmit) {
+        uint32_t d = kScanNone;
+        uint4 rec = make_uint4(0, 0, 0, 0);
+        if (found_table >= 0) {
+            const TableDesc &t = p.tables[found_table];
+            const uint64_t off = (uint64_t)hit_ix.x | ((uint64_t)hit_ix.y << 32); // off + 8 + klen <= data_len: probe checked it
+            const uint64_t ks = hit_ix.z, fs = hit_ix.w;
+            bool ok = ks == 8 + klen && fs >= ks + 24 && fs <= t.data_len - off;
+            if (ok) {
+                const uint8_t *e = t.data + off;
+                ok = ld_bytes_le<true>(e + ks, 8) == fs - ks - 24 &&
+                     ts_decodes(ld_bytes_le<true>(e + fs - 16, 8), ld_bytes_le<true>(e + fs - 8, 8));
+            }
+            if (ok) {
+                d = 0;
+                const unsigned long long src = reinterpret_cast<unsigned long long>(t.data + off);
+                rec = make_uint4((uint32_t)src, (uint32_t)(src >> 32), (uint32_t)ks, (uint32_t)fs);
+            } else {
+                rejects |= kLookupBadEntry;
+            }
+        }
+        em.dest[q] = d;
+        em.flat[q] = rec;
+    }
     p.out[q] = make_uint4((uint32_t)found_table, rejects, (uint32_t)record, (uint32_t)(record >> 32));
+}
+
+__global__ void __launch_bounds__(256, DBEEL_LOOKUP_MINB) k_lookup(LookupParams p) {
+    pdl_trigger();
+    pdl_wait();
+    lookup_query<false>(p, LookupEmit{nullptr, nullptr});
+}
+
+__global__ void __launch_bounds__(256, DBEEL_LOOKUP_MINB) k_lookup_emit(LookupParams p, LookupEmit em) {
+    pdl_trigger();
+    pdl_wait();
+    lookup_query<true>(p, em);
 }
 
 } // namespace dbeel

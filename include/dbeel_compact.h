@@ -25,6 +25,7 @@
  *                          read / write callbacks feeding a pinned ring                 ["next" row N3]
  *   dbeel_get_many*     <- the SSTable loop of LSMTree::get_entry: Bloom::check + binary_search
  *                          (lsm_tree.rs:605-670, 686-719) for a batch of keys        ["next" row N2]
+ *   dbeel_get_values*   <- the same, returning the entries binary_search decodes (:628-651)
  *   dbeel_wal_flush*    <- read_memtable_from_wal_file + the recovery flush of open_or_create_ex
  *                          (lsm_tree.rs:552-574, 478-513)                            ["next" row N4]
  *   dbeel_scan*         <- the SSTable part of LSMTree::iter_filter (lsm_tree.rs:133-282) with migrate_actions' hash-range
@@ -329,6 +330,28 @@ int dbeel_get_many(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables
                    const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_lookup_result *results);
 int dbeel_get_many_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys,
                           const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_lookup_result *results);
+
+/* Batched reads that return the entries: the rows of dbeel_get_many for the same arguments, plus the entry every
+ * answered row names (what get_entry returns, :674-723), so nothing is read a second time.
+ * A row answers when table >= 0 and its hit decodes the way binary_search decodes one (:628-651): read_at(offset,
+ * key_size) is exactly the key (key_size == 8 + klen), and read_at(offset + key_size, full_size - key_size) exactly one
+ * EntryValue (u64 dlen | data | i128 timestamp, 8 + dlen + 16 == full_size - key_size) inside .data, with the timestamp
+ * inside `time`'s +-9999 years.  A hit that does not decode gets DBEEL_LOOKUP_BAD_ENTRY and no entry, and no older table
+ * is tried (the reference's get returns Err).  The search itself is dbeel_get_many's (key_size is not read while probing).
+ * out->data / out->index receive one entry per answered row, in query order, bytes as stored (a tombstone comes back with
+ * dlen == 0 and its timestamp; a key asked twice comes back twice): an arrival batch whose .index offsets start at 0, like
+ * a scan destination.  out->items_written = entries; row i's entry is entry number (answered rows before i).
+ * Caps: the sum of full_size over the hits is enough.  When out->data_cap or out->index_cap is smaller than needed:
+ * DBEEL_ERR_CAPACITY, out->data_len / index_len = the sizes needed, the rows filled, nothing written to out.
+ * Limits: n_keys < 2^32 - 16 (DBEEL_ERR_INVALID_ARG).  out->bloom is not used.  dbeel_get_values takes host memory (tables uploaded whole, only the rows and the selected bytes come
+ * back); dbeel_get_values_device takes device memory for tables, keys, offsets, results and out (out 16-byte aligned). */
+#define DBEEL_LOOKUP_BAD_ENTRY 0x40000000u /* in bloom_rejects: the hit's entry does not decode (get_entry returns Err) */
+int dbeel_get_values(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys,
+                     const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_out *out,
+                     dbeel_lookup_result *results);
+int dbeel_get_values_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys,
+                            const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_out *out,
+                            dbeel_lookup_result *results);
 
 /* ---- N5: scans -- LSMTree::iter_filter over a tree's SSTables ------------------------------------------------------
  * Replaces the SSTable part of AsyncIter (src/storage_engine/lsm_tree.rs:133-282, iter_filter :1183-1189) with its filter

@@ -17,6 +17,7 @@
  *                             next even index through dbeel_flush(), no bloom
  *   dbeel_tree_sstables    <- LSMTree::sstable_indices_and_sizes (lsm_tree.rs:592-598)
  *   dbeel_tree_get_many    <- the SSTable loop of LSMTree::get_entry (lsm_tree.rs:686-719) through dbeel_get_many()
+ *   dbeel_tree_get_values  <- the same with the entries (:674-723) through dbeel_get_values()
  *   dbeel_tree_scan        <- the SSTable part of LSMTree::iter_filter (lsm_tree.rs:133-282, :1183-1189) through dbeel_scan()
  *   dbeel_tree_scan_stream <- the same through dbeel_scan_stream(): the files are streamed, trees of any size
  *   dbeel_memtable_cut     <- RedBlackTree::set + active_memtable_full (rbtree_arena lib.rs:497-534,
@@ -77,6 +78,11 @@ int dbeel_tree_flush(dbeel_tree *t, const dbeel_run *batch, uint64_t *written_in
  * rows as in dbeel_get_many.  The memtable look-ups in front of it (:677-684) are the caller's. */
 int dbeel_tree_get_many(dbeel_tree *t, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
                         dbeel_lookup_result *results);
+
+/* dbeel_tree_get_many with the entries: the tree's files read whole as there, then dbeel_get_values() (rows, output,
+ * caps and DBEEL_ERR_CAPACITY as described there).  out is host memory. */
+int dbeel_tree_get_values(dbeel_tree *t, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
+                          dbeel_out *out, dbeel_lookup_result *results);
 
 /* The SSTable part of LSMTree::iter_filter over the tree's files: every table's .data / .index in dbeel_tree_sstables()
  * order (oldest first, the iterator's order) through one dbeel_scan().  kind / ranges / results / stop as in dbeel_scan;
