@@ -45,7 +45,7 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_murmur3_32", "dbeel_ring_owner", "dbeel_shard_ring", "dbeel_route_device", "dbeel_flush_many_sparse_device",
            "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream",
            "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device", "dbeel_scan_stream", "dbeel_get_values",
-           "dbeel_get_values_device"]
+           "dbeel_get_values_device", "dbeel_get_values_stream"]
 
 
 class Run(C.Structure):
@@ -213,6 +213,9 @@ def lib():
             f.restype = C.c_int
             f.argtypes = [C.c_void_p, C.POINTER(Table), C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
                           C.POINTER(Out), C.c_void_p]
+        L.dbeel_get_values_stream.restype = C.c_int
+        L.dbeel_get_values_stream.argtypes = [C.c_void_p, C.POINTER(Table), C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64,
+                                              C.c_uint32, C.POINTER(ScanIO), C.POINTER(Out), C.c_void_p]
         L.dbeel_scan_bound.restype = C.c_int
         L.dbeel_scan_bound.argtypes = [C.POINTER(Table), C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         for name in ("dbeel_scan", "dbeel_scan_device"):
@@ -654,6 +657,68 @@ class Engine:
                 if caps is not None or attempt or ex.code != ERR_CAPACITY:
                     raise
                 dc, ic = ex.needed
+
+    def get_values_stream(self, tables: Sequence[Tuple[object, object, object]], keys: Sequence[bytes],
+                          mode: int = LOOKUP_REFERENCE, read=None, fail_read_at: int = -1,
+                          caps: Optional[Tuple[int, int]] = None):
+        """dbeel_get_values_stream: get_values' result for tables the engine reads through a callback, only where the
+        searches reach.  tables: (data, index, bloom | None) oldest first.  Without `read` the callback serves data / index
+        from memory; with it, data / index may be sizes, and read(table, kind, offset, size) returns the bytes (kind 1 =
+        .data, 2 = .index; called from several engine threads) or a nonzero int error code.  fail_read_at = n makes the n-th
+        read return 4242 (tests).  last_stream_reads lists every (table, kind, offset, size) read.  Returns (rows, data,
+        index); caps as in get_values (by default at most 64 MiB of .data, retried once with the sizes needed)."""
+        def size_of(x):
+            return int(x) if isinstance(x, (int, np.integer)) else _u8(x).size
+        keep = [(None if read else _u8(d), None if read else _u8(i), _u8(b) if b is not None and len(b) else None)
+                for d, i, b in tables]
+        sizes = [(size_of(d), size_of(i)) for d, i, _ in tables]
+        arr = (Table * max(1, len(keep)))()
+        for j, ((_, _, b), (ds, isz)) in enumerate(zip(keep, sizes)):
+            arr[j] = Table(None, ds, None, isz, b.ctypes.data if b is not None else None, b.size if b is not None else 0)
+        blob, off = pack_keys(keys)
+        res = np.zeros(len(keys), dtype=LOOKUP_DTYPE)
+        import threading
+        mu = threading.Lock()
+        log = []
+
+        def rd(_ctx, table, kind_, offset, size, dst):
+            with mu:
+                k = len(log)
+                log.append((int(table), int(kind_), int(offset), int(size)))
+            if k == fail_read_at:
+                return 4242
+            if read is None:
+                src = keep[table][0] if kind_ == 1 else keep[table][1]
+                if offset + size > src.size:
+                    return 4243
+                C.memmove(dst, src.ctypes.data + offset, size)
+                return 0
+            got = read(int(table), int(kind_), int(offset), int(size))
+            if isinstance(got, (int, np.integer)):
+                return int(got)
+            b = np.ascontiguousarray(np.frombuffer(got, np.uint8) if isinstance(got, (bytes, bytearray)) else _u8(got))
+            if b.size != size:
+                return 4243
+            C.memmove(dst, b.ctypes.data, size)
+            return 0
+
+        io = ScanIO(STREAM_READ_FN(rd), C.cast(None, SCAN_WRITE_FN), None)
+        dc, ic = caps if caps is not None else (min(sum(d for d, _ in sizes), 64 << 20), 16 * len(keys))
+        for attempt in range(2):
+            od, oi = np.empty(max(1, dc), np.uint8), np.empty(max(1, ic), np.uint8)
+            out = Out(od.ctypes.data, dc, 0, oi.ctypes.data, ic, 0, None, 0, 0, 0)
+            log.clear()
+            rc = lib().dbeel_get_values_stream(self._h, arr, len(keep), blob.ctypes.data if blob.size else None, off.ctypes.data,
+                                               len(keys), mode, C.byref(io), C.byref(out), res.ctypes.data)
+            self.last_stream_reads = list(log)
+            if rc == 0:
+                return res, od[:out.data_len], oi[:out.index_len]
+            err = DbeelError(rc, f"dbeel_get_values_stream: {lib().dbeel_last_error(self._h).decode()}")
+            if rc == ERR_CAPACITY:
+                err.needed = (int(out.data_len), int(out.index_len))
+            if caps is not None or attempt or rc != ERR_CAPACITY:
+                raise err
+            dc, ic = err.needed
 
     def get_values_device(self, tables: Sequence[Tuple[int, int, int, int, int, int]], keys_ptr: int, offsets_ptr: int,
                           n_keys: int, results_ptr: int, out_ptrs: Tuple[int, int, int, int],

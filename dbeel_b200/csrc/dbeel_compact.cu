@@ -26,6 +26,7 @@
 #include "gather_fb.cuh"
 #include "gather_h.cuh"
 #include "lookup.cuh"
+#include "lookup_stream.cuh"
 #include "route.cuh"
 #include "scan.cuh"
 #include "wal.cuh"
@@ -2245,6 +2246,338 @@ int get_values_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tabl
 }
 
 
+// ------------------------------------------------------------------------------------ N2 streamed: dbeel_get_values_stream
+// Ranges of one file laid out in a staging buffer: run k (merged ranges) at pos[k], congruent to its file offset modulo 16
+// with 16 bytes of slack on both sides, so the kernels' aligned 8-byte loads stay inside the buffer.
+struct GvsStaged {
+    std::vector<ByteRange> runs;
+    std::vector<uint64_t> pos;
+    uint64_t end = 0;
+    uint64_t at(uint64_t off) const { // staging position of file offset `off` (inside some run)
+        const size_t k = std::upper_bound(runs.begin(), runs.end(), off, [](uint64_t o, const ByteRange &r) { return o < r.lo; }) - runs.begin() - 1;
+        return pos[k] + (off - runs[k].lo);
+    }
+};
+
+GvsStaged gvs_stage(std::vector<ByteRange> r, uint64_t gap, uint64_t base) {
+    GvsStaged s;
+    s.runs = merge_ranges(std::move(r), gap);
+    uint64_t p = base;
+    for (const ByteRange &x : s.runs) {
+        const uint64_t at = align_up(p + 16, 16) + (x.lo & 15);
+        s.pos.push_back(at);
+        p = at + (x.hi - x.lo) + 16;
+    }
+    s.end = align_up(p, kAlign);
+    return s;
+}
+
+// Every run of `s` of table t's file `kind` into dst + pos, through the read callback from a few threads, in pieces of at
+// most StreamPump::kPiece bytes; the callback's code comes back unchanged.  A batch of many small reads (fences, scattered
+// hits) is dominated by the per-call cost, so this takes parallel_pieces' lock-free loop rather than the pump's
+// partition-ordered one.
+int gvs_read(dbeel_engine *e, const dbeel_scan_io *io, uint32_t t, uint32_t kind, const GvsStaged &s, uint8_t *dst) {
+    struct Piece { uint64_t off, len; uint8_t *dst; };
+    std::vector<Piece> ps;
+    for (size_t k = 0; k < s.runs.size(); k++) {
+        const uint64_t len = s.runs[k].hi - s.runs[k].lo;
+        for (uint64_t done = 0; done < len; done += StreamPump::kPiece)
+            ps.push_back({s.runs[k].lo + done, std::min(len - done, StreamPump::kPiece), dst + s.pos[k] + done});
+        e->stats.input_bytes += len;
+    }
+    return parallel_pieces(ps.size(), [&](size_t k) { return io->read(io->ctx, t, kind, ps[k].off, ps[k].len, ps[k].dst); });
+}
+
+// Per table, newest first: k_gvs_filter -> fences read, k_lookup_fence -> touched leaves read in groups under the partition
+// budget, k_lookup_leaf per group and k_gvs_copy for the group's hits (their entries leave the window for the hit heap).
+// Then the entries of hits at fences are read into the heap, k_gvs_hit decodes every hit and split_emit writes `out` in
+// query order, as dbeel_get_values does.  Every phase ends in a stream synchronise before its pinned
+// buffers are refilled.
+int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys, const uint64_t *key_off,
+                            uint64_t n_keys, uint32_t mode, const dbeel_scan_io *io, dbeel_out *out, dbeel_lookup_result *results) {
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (!out || !io || !io->read) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    if (const int arc = lookup_args(e, tables, n_tables, key_off, n_keys, mode, results)) return arc;
+    if (n_keys >= 0xFFFFFFF0ull) return fail(e, DBEEL_ERR_INVALID_ARG, "2^32 - 16 keys or more");
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    e->stats = dbeel_stats{};
+    out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
+    if (n_keys == 0) return DBEEL_OK;
+    for (uint32_t i = 0; i < n_tables; i++) { // as stage_lookup; .data and .index come through the callback
+        const dbeel_table &t = tables[i];
+        if (t.index_len % DBEEL_INDEX_ENTRY_SIZE) return fail(e, DBEEL_ERR_INVALID_ARG, "index length is not a multiple of 16");
+        if (t.bloom_len && !t.bloom) return fail(e, DBEEL_ERR_INVALID_ARG, "null table buffer");
+        if (t.bloom_len && (t.bloom_len < 8 + kBloomTrailer || (t.bloom_len - 8 - kBloomTrailer) % 4))
+            return fail(e, DBEEL_ERR_BAD_BLOOM, "bloom file length is not 8 + 4 * words + 164");
+    }
+    const uint64_t key_bytes = key_off[n_keys];
+    if (!keys && key_bytes) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    cudaError_t ce = cudaSetDevice(e->device);
+    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    cudaStream_t s = e->stream;
+    const uint32_t n = (uint32_t)n_keys;
+    uint64_t max_klen = 0;
+    for (uint64_t q = 0; q < n_keys; q++) max_klen = std::max(max_klen, key_off[q + 1] - key_off[q]);
+
+    // ---- per-query state and the split's workspace
+    uint64_t off = 0;
+    const uint64_t o_keys = carve_ws(&off, key_bytes + 16), o_off = carve_ws(&off, 8ull * (n + 1));
+    const uint64_t o_rows = carve_ws(&off, 16ull * n), o_hix = carve_ws(&off, 16ull * n), o_state = carve_ws(&off, sizeof(SearchState) * n);
+    const uint64_t o_node = carve_ws(&off, 4ull * n), o_src = carve_ws(&off, 8ull * n), o_hoff = carve_ws(&off, 8ull * n);
+    const uint64_t o_touched = carve_ws(&off, 1ull << kLookupMaxDepth), o_cnt = carve_ws(&off, 8), o_need = carve_ws(&off, 8);
+    const uint64_t o_cursor = carve_ws(&off, 8);
+    const SplitLayout w = carve_split(&off, n, 1);
+    int rc = ensure_device(e, &e->ws, &e->ws_cap, off);
+    const uint64_t pin_tot = align_up(w.header2_bytes, 64);
+    if (!rc) rc = ensure_pinned(e, std::max<uint64_t>(pin_tot + 8ull * 4, (1ull << kLookupMaxDepth) + 64));
+    if (rc) return rc;
+    uint64_t bloom_bytes = 0;
+    for (uint32_t i = 0; i < n_tables; i++) bloom_bytes += align_up(tables[i].bloom_len + 16, kAlign);
+    if ((rc = ensure_device(e, &e->bloom_dev, &e->bloom_dev_cap, std::max<uint64_t>(bloom_bytes, 256)))) return rc;
+    uint8_t *ws = e->ws;
+    std::vector<TableDesc> td(n_tables);
+    uint64_t bpos = 0;
+    for (uint32_t i = 0; i < n_tables; i++) {
+        const dbeel_table &t = tables[i];
+        td[i] = TableDesc{nullptr, t.data_len, nullptr, t.index_len / DBEEL_INDEX_ENTRY_SIZE, nullptr, 0, 0, 0, 0, {0, 0, 0, 0}};
+        if (!t.bloom_len) continue;
+        const uint8_t *b = static_cast<const uint8_t *>(t.bloom);
+        if ((rc = parse_bloom(e, b, b + t.bloom_len - kBloomTrailer, t.bloom_len, &td[i]))) return rc;
+        CU(cudaMemcpyAsync(e->bloom_dev + bpos, b, t.bloom_len, cudaMemcpyHostToDevice, s));
+        td[i].words = reinterpret_cast<const uint32_t *>(e->bloom_dev + bpos + 8);
+        bpos += align_up(t.bloom_len + 16, kAlign);
+    }
+    CU(cudaEventRecord(e->ev[EV_START], s));
+    for (uint64_t q = 0; q < n_keys; q++) results[q] = dbeel_lookup_result{-1, 0, 0};
+    static_assert(sizeof(dbeel_lookup_result) == 16, "result rows are written as uint4");
+    if (key_bytes) CU(cudaMemcpyAsync(ws + o_keys, keys, key_bytes, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_off, key_off, 8ull * (n + 1), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_rows, results, 16ull * n, cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(ws + o_src, 0, 8ull * n, s));
+    CU(cudaMemsetAsync(ws + o_hoff, 0xFF, 8ull * n, s)); // kGvsNoEntry
+    CU(cudaMemsetAsync(ws + o_cursor, 0, 8, s));
+    GvsQueries gq{ws + o_keys, reinterpret_cast<const uint64_t *>(ws + o_off), n_keys, reinterpret_cast<uint4 *>(ws + o_rows),
+                  reinterpret_cast<uint4 *>(ws + o_hix), reinterpret_cast<SearchState *>(ws + o_state), reinterpret_cast<uint32_t *>(ws + o_node),
+                  reinterpret_cast<unsigned long long *>(ws + o_src), reinterpret_cast<unsigned long long *>(ws + o_hoff), mode};
+    unsigned long long *d_need = reinterpret_cast<unsigned long long *>(ws + o_need), *d_cursor = reinterpret_cast<unsigned long long *>(ws + o_cursor);
+    // The hit heap (stage_out2) holds every answered entry until split_emit gathers them; it grows keeping what it holds.
+    uint64_t heap_bound = 0;
+    auto heap_reserve = [&](uint64_t need) -> int {
+        if (need <= e->stage_out2_cap) return DBEEL_OK;
+        uint8_t *old = e->stage_out2;
+        const uint64_t old_cap = e->stage_out2_cap;
+        e->stage_out2 = nullptr;
+        e->stage_out2_cap = 0;
+        int rc2 = ensure_device(e, &e->stage_out2, &e->stage_out2_cap, need);
+        if (!rc2 && old && heap_bound) CU(cudaMemcpyAsync(e->stage_out2, old, std::min(old_cap, heap_bound), cudaMemcpyDeviceToDevice, s));
+        CU(cudaStreamSynchronize(s));
+        if (old) cudaFree(old);
+        return rc2;
+    };
+    unsigned long long *d_cnt = reinterpret_cast<unsigned long long *>(ws + o_cnt);
+    uint8_t *d_touched = ws + o_touched;
+    const uint32_t grid = (n + 255) / 256;
+    uint32_t launches = 0, groups = 0;
+    const uint64_t budget = e->partition_bytes;
+    std::vector<uint8_t> touched;
+
+    for (uint32_t ti = n_tables; ti-- > 0;) { // sstables.iter().rev(): newest first
+        const TableDesc &t = td[ti];
+        const uint64_t data_len = t.data_len, nrec = t.n;
+        CU(cudaMemsetAsync(d_cnt, 0, 8, s));
+        launch_k(e, k_gvs_filter, grid, 256, 0, s, gq, t, d_cnt);
+        CU(cudaMemcpyAsync(e->pin, d_cnt, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        launches++;
+        const uint64_t m = rd64(e->pin);
+        if (m == 0) continue; // no query reaches the table: nothing of it is read
+        const uint32_t depth = lookup_depth(m, nrec, data_len, 8 + max_klen, budget);
+        ProbeTree pt;
+        plan_probe_tree(mode, nrec, depth, &pt);
+        const uint64_t leaf0 = 1ull << depth;
+        CU(cudaMemsetAsync(d_touched, 0, leaf0, s));
+
+        // ---- fences: the index records of the open internal nodes, then their key frames
+        if (depth > 0) {
+            std::vector<ByteRange> ir;
+            for (uint64_t k = 1; k < leaf0; k++)
+                if (pt.open[k]) { const uint64_t p = search_pos(mode, pt.state[k]); ir.push_back({16 * p, 16 * p + 16}); }
+            const GvsStaged si = gvs_stage(ir, kLookupMergeGap, 0);
+            if ((rc = ensure_host(e, &e->ring_out, &e->ring_out_cap, si.end))) return rc;
+            if ((rc = gvs_read(e, io, ti, DBEEL_STREAM_INDEX, si, e->ring_out))) return fail(e, rc, "stream read callback failed (.index, fences)");
+            std::vector<uint4> fix(leaf0, make_uint4(0, 0, 0, 0));
+            std::vector<ByteRange> fr;
+            std::vector<uint8_t> has(leaf0, 0);
+            std::vector<ByteRange> frame(leaf0);
+            for (uint64_t k = 1; k < leaf0; k++) {
+                if (!pt.open[k]) continue;
+                memcpy(&fix[k], e->ring_out + si.at(16 * search_pos(mode, pt.state[k])), 16);
+                if (probe_frame(reinterpret_cast<const uint8_t *>(&fix[k]), data_len, max_klen, &frame[k])) { has[k] = 1; fr.push_back(frame[k]); }
+            }
+            const uint64_t o_fix = 0, o_ffr = align_up(16 * leaf0, kAlign);
+            const GvsStaged sf = gvs_stage(fr, 0, align_up(o_ffr + 8 * leaf0, kAlign));
+            if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, sf.end))) return rc;
+            if ((rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, sf.end))) return rc;
+            if ((rc = gvs_read(e, io, ti, DBEEL_STREAM_DATA, sf, e->ring_in))) return fail(e, rc, "stream read callback failed (.data, fences)");
+            uint8_t *img = e->ring_in;
+            memcpy(img + o_fix, fix.data(), 16 * leaf0);
+            unsigned long long *ffr = reinterpret_cast<unsigned long long *>(img + o_ffr);
+            for (uint64_t k = 0; k < leaf0; k++) {
+                ffr[k] = 0;
+                if (!has[k]) continue;
+                const uint64_t p = sf.at(frame[k].lo), cur_klen = rd64(img + p);
+                if (cur_klen <= data_len - frame[k].lo - 8) ffr[k] = reinterpret_cast<unsigned long long>(e->stage_in + p); // else as probe(): corrupt
+            }
+            CU(cudaMemcpyAsync(e->stage_in, img, sf.end, cudaMemcpyHostToDevice, s));
+            GvsFences gf{reinterpret_cast<const uint4 *>(e->stage_in + o_fix), reinterpret_cast<const unsigned long long *>(e->stage_in + o_ffr),
+                         depth, ti, nrec, d_touched};
+            launch_k(e, k_lookup_fence, grid, 256, 0, s, gq, gf);
+            launches++;
+        } else {
+            CU(cudaMemsetAsync(d_touched, 1, 1, s));
+        }
+        CU(cudaMemcpyAsync(e->pin, d_touched, leaf0, cudaMemcpyDeviceToHost, s));
+        CU(cudaGetLastError());
+        CU(cudaStreamSynchronize(s));
+        touched.assign(e->pin, e->pin + leaf0);
+
+        // ---- leaves, in groups of about `budget` bytes: index slices, then the windows their records point at
+        const uint64_t per_rec = 16 + (nrec ? (data_len + nrec - 1) / nrec : 0);
+        std::vector<uint32_t> group;
+        auto run_group = [&]() -> int {
+            const uint32_t nl = (uint32_t)group.size();
+            std::vector<ByteRange> sr(nl);
+            for (uint32_t k = 0; k < nl; k++) {
+                uint64_t a, b;
+                search_interval(mode, pt.state[leaf0 + group[k]], &a, &b);
+                sr[k] = {16 * a, 16 * b};
+            }
+            const uint64_t o_hdr = 0;
+            const GvsStaged ss = gvs_stage(sr, kLookupMergeGap, align_up(sizeof(GvsLeaf) * nl, kAlign));
+            int rc2 = ensure_host(e, &e->ring_in, &e->ring_in_cap, ss.end);
+            if (!rc2) rc2 = ensure_device(e, &e->stage_in, &e->stage_in_cap, ss.end);
+            if (rc2) return rc2;
+            if ((rc2 = gvs_read(e, io, ti, DBEEL_STREAM_INDEX, ss, e->ring_in))) return fail(e, rc2, "stream read callback failed (.index, leaves)");
+            std::vector<ByteRange> win(nl);
+            std::vector<uint8_t> has(nl, 0);
+            std::vector<ByteRange> wr;
+            for (uint32_t k = 0; k < nl; k++)
+                if (leaf_window(e->ring_in + ss.at(sr[k].lo), (sr[k].hi - sr[k].lo) / 16, data_len, max_klen, &win[k])) { has[k] = 1; wr.push_back(win[k]); }
+            const GvsStaged sw = gvs_stage(wr, 0, 0);
+            rc2 = ensure_host(e, &e->ring_out, &e->ring_out_cap, sw.end);
+            if (!rc2) rc2 = ensure_device(e, &e->stage_in2, &e->stage_in2_cap, sw.end);
+            if (rc2) return rc2;
+            if ((rc2 = gvs_read(e, io, ti, DBEEL_STREAM_DATA, sw, e->ring_out))) return fail(e, rc2, "stream read callback failed (.data, leaves)");
+            GvsLeaf *hl = reinterpret_cast<GvsLeaf *>(e->ring_in + o_hdr);
+            for (uint32_t k = 0; k < nl; k++) {
+                // biased: record r of the table at index + r, file offset o at data + o (a leaf whose records all point past
+                // the file never dereferences data: probe() reports them corrupt first)
+                const uintptr_t ib = reinterpret_cast<uintptr_t>(e->stage_in + ss.at(sr[k].lo)) - sr[k].lo;
+                const uintptr_t db = has[k] ? reinterpret_cast<uintptr_t>(e->stage_in2 + sw.at(win[k].lo)) - win[k].lo
+                                            : reinterpret_cast<uintptr_t>(e->stage_in2);
+                hl[k] = GvsLeaf{reinterpret_cast<const uint8_t *>(db), reinterpret_cast<const uint4 *>(ib), group[k], 0, 0};
+            }
+            CU(cudaMemcpyAsync(e->stage_in, e->ring_in, ss.end, cudaMemcpyHostToDevice, s));
+            if (sw.end) CU(cudaMemcpyAsync(e->stage_in2, e->ring_out, sw.end, cudaMemcpyHostToDevice, s));
+            CU(cudaMemsetAsync(d_need, 0, 8, s));
+            launch_k(e, k_lookup_leaf, grid, 256, 0, s, gq, t, reinterpret_cast<const GvsLeaf *>(e->stage_in + o_hdr), nl, depth, ti, d_need);
+            CU(cudaMemcpyAsync(e->pin, d_need, 8, cudaMemcpyDeviceToHost, s));
+            CU(cudaGetLastError());
+            CU(cudaStreamSynchronize(s));
+            launches++;
+            if (const uint64_t need = rd64(e->pin)) { // the group's hits leave the window for the heap before it is reused
+                if ((rc2 = heap_reserve(heap_bound + need))) return rc2;
+                heap_bound += need;
+                launch_k(e, k_gvs_copy, (uint32_t)((32 * n_keys + 255) / 256), 256, 0, s, gq, e->stage_out2, d_cursor);
+                CU(cudaGetLastError());
+                CU(cudaStreamSynchronize(s));
+                launches++;
+            }
+            groups++;
+            group.clear();
+            return DBEEL_OK;
+        };
+        uint64_t est = 0;
+        for (uint64_t L = 0; L < leaf0; L++) {
+            if (!touched[L]) continue;
+            uint64_t a, b;
+            search_interval(mode, pt.state[leaf0 + L], &a, &b);
+            const uint64_t bytes = (b - a) * per_rec + 8 + max_klen;
+            if (!group.empty() && est + bytes > budget) {
+                if ((rc = run_group())) return rc;
+                est = 0;
+            }
+            group.push_back((uint32_t)L);
+            est += bytes;
+        }
+        if (!group.empty() && (rc = run_group())) return rc;
+    }
+
+    // ---- hits at fences: their entries, one record each (runs that touch as one read), into the heap behind the copies
+    std::vector<uint4> hix(n);
+    std::vector<unsigned long long> hoff(n);
+    CU(cudaMemcpyAsync(results, ws + o_rows, 16ull * n, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(hix.data(), ws + o_hix, 16ull * n, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(hoff.data(), ws + o_hoff, 8ull * n, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    std::vector<std::vector<ByteRange>> er(n_tables);
+    auto fence_entry = [&](uint64_t q, ByteRange *r) { // a fence hit whose entry k_gvs_hit can decode
+        if (hoff[q] != kGvsFenceHit) return false;
+        const uint4 ix = hix[q];
+        const uint64_t o = (uint64_t)ix.x | ((uint64_t)ix.y << 32), dl = tables[results[q].table].data_len;
+        if (!gvs_entry_fits(o, ix.z, ix.w, key_off[q + 1] - key_off[q], dl)) return false;
+        *r = ByteRange{o, o + ix.w};
+        return true;
+    };
+    bool any_fence_hit = false;
+    for (uint64_t q = 0; q < n_keys; q++) {
+        ByteRange r;
+        if (fence_entry(q, &r)) er[results[q].table].push_back(r);
+        any_fence_hit = any_fence_hit || hoff[q] == kGvsFenceHit;
+    }
+    if (any_fence_hit) {
+        const uint64_t base = align_up(heap_bound, kAlign);
+        std::vector<GvsStaged> sh(n_tables);
+        uint64_t staged = 0;
+        for (uint32_t i = 0; i < n_tables; i++) {
+            sh[i] = gvs_stage(std::move(er[i]), 0, staged);
+            staged = sh[i].end;
+        }
+        if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, std::max<uint64_t>(staged, 256)))) return rc;
+        if ((rc = heap_reserve(base + staged + 256))) return rc;
+        for (uint32_t i = 0; i < n_tables; i++)
+            if ((rc = gvs_read(e, io, i, DBEEL_STREAM_DATA, sh[i], e->ring_in))) return fail(e, rc, "stream read callback failed (.data, entries)");
+        if (staged) CU(cudaMemcpyAsync(e->stage_out2 + base, e->ring_in, staged, cudaMemcpyHostToDevice, s));
+        for (uint64_t q = 0; q < n_keys; q++) {
+            ByteRange r;
+            if (hoff[q] != kGvsFenceHit) continue;
+            hoff[q] = fence_entry(q, &r) ? base + sh[results[q].table].at(r.lo) : kGvsNoEntry;
+        }
+        CU(cudaMemcpyAsync(ws + o_hoff, hoff.data(), 8ull * n, cudaMemcpyHostToDevice, s));
+        CU(cudaStreamSynchronize(s));
+    }
+    ScanParams sp = {};
+    split_params(w, ws, &sp);
+    CU(cudaMemsetAsync(ws + w.o_tot, 0, 8ull * 3, s));
+    CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
+    launch_k(e, k_gvs_hit, grid, 256, 0, s, gq, static_cast<const uint8_t *>(e->stage_out2), LookupEmit{sp.dest, sp.flat});
+    launches++;
+    CU(cudaMemcpyAsync(results, ws + o_rows, 16ull * n, cudaMemcpyDeviceToHost, s)); // back with the sizes: filled on ERR_CAPACITY too
+    e->stats.entries_in = n_keys;
+    e->stats.partitions = groups;
+    uint64_t items = 0, bytes = 0;
+    rc = split_emit(e, w, sp, pin_tot, false, out, &launches, &items, &bytes, [](const unsigned long long *) {});
+    if (rc == DBEEL_ERR_CAPACITY) {
+        out->data_len = bytes;
+        out->index_len = 16 * items;
+        return fail(e, DBEEL_ERR_CAPACITY, "the entries found are larger than the output buffers (data_len / index_len: the sizes needed)");
+    }
+    return rc;
+}
+
+
 // ------------------------------------------------------------------------------------ N5 streamed: dbeel_scan_stream
 // The plan (host/scan_plan.h) cuts the record sequence into partitions; each goes file -> pinned ring slot -> device slot
 // c & 1 in ONE H2D copy of its slot image (table headers | per table: index slice, .data window), runs the scan chain with
@@ -2857,6 +3190,13 @@ int dbeel_get_values_device(dbeel_engine *e, const dbeel_table *tables, uint32_t
                             const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_out *out, dbeel_lookup_result *results) {
     REFUSE_WHILE_ASYNC(e);
     return get_values_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, out, results, true);
+}
+
+int dbeel_get_values_stream(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys,
+                            const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, const dbeel_scan_io *io,
+                            dbeel_out *out, dbeel_lookup_result *results) {
+    REFUSE_WHILE_ASYNC(e);
+    return get_values_stream_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, io, out, results);
 }
 
 int dbeel_scan_bound(const dbeel_table *tables, uint32_t n_tables, uint64_t *data_cap, uint64_t *index_cap) {

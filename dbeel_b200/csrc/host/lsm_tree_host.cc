@@ -711,6 +711,36 @@ int dbeel_tree_scan_stream(dbeel_tree *t, uint32_t kind, const void *ranges, uin
     return rc;
 }
 
+int dbeel_tree_get_values_stream(dbeel_tree *t, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
+                                 dbeel_out *out, dbeel_lookup_result *results) {
+    if (!t || !out || (n_keys && (!key_offsets || !results))) return DBEEL_ERR_INVALID_ARG;
+    t->err.clear();
+    const size_t n = t->sstables.size();
+    StreamFiles f;
+    f.data_fd.assign(n, -1);
+    f.index_fd.assign(n, -1);
+    std::vector<PinnedBuf> bloom(n);
+    std::vector<dbeel_table> tables(n);
+    for (size_t i = 0; i < n; i++) {
+        const uint64_t idx = t->sstables[i].index;
+        const std::string dp = file_path(t->dir, idx, kData), ip = file_path(t->dir, idx, kIndex), bp = file_path(t->dir, idx, kBloom);
+        f.data_fd[i] = open(dp.c_str(), O_RDONLY);
+        f.index_fd[i] = open(ip.c_str(), O_RDONLY);
+        struct stat sd, si;
+        if (f.data_fd[i] < 0 || f.index_fd[i] < 0 || fstat(f.data_fd[i], &sd) != 0 || fstat(f.index_fd[i], &si) != 0)
+            return io_fail(t, "open " + dp);
+        if (exists(bp)) { // the filter is read whole, as SSTable::new_with_bloom_read does (lsm_tree.rs:94-101)
+            if (const int rc = read_file(t, bp, &bloom[i])) return rc;
+        }
+        tables[i] = dbeel_table{nullptr, (uint64_t)sd.st_size, nullptr, (uint64_t)si.st_size, bloom[i].len ? bloom[i].p : nullptr, bloom[i].len};
+    }
+    const dbeel_scan_io io{stream_read, nullptr, &f};
+    const int rc = dbeel_get_values_stream(t->engine, tables.data(), (uint32_t)n, keys, key_offsets, n_keys, mode, &io, out, results);
+    if (rc == DBEEL_ERR_IO && f.saved_errno.load()) { errno = f.saved_errno.load(); io_fail(t, "streamed read"); }
+    else if (rc) t->err = dbeel_last_error(t->engine);
+    return rc;
+}
+
 int dbeel_tree_recover_wal(dbeel_tree *t, uint32_t tree_capacity, uint64_t *wal_file_index, uint64_t *items_written) {
     if (!t) return DBEEL_ERR_INVALID_ARG;
     t->err.clear();

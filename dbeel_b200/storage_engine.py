@@ -52,6 +52,9 @@ def _lib():
         L.dbeel_tree_get_values.restype = C.c_int
         L.dbeel_tree_get_values.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.POINTER(capi.Out),
                                             C.c_void_p]
+        L.dbeel_tree_get_values_stream.restype = C.c_int
+        L.dbeel_tree_get_values_stream.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
+                                                   C.POINTER(capi.Out), C.c_void_p]
         L.dbeel_tree_scan.restype = C.c_int
         L.dbeel_tree_scan.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(capi.Out),
                                       C.POINTER(capi.JobResult), C.POINTER(capi.ScanStop)]
@@ -77,7 +80,7 @@ def _lib():
 
 
 TREE_EXPORTS = ["dbeel_tree_open", "dbeel_tree_close", "dbeel_tree_sstables", "dbeel_tree_write_sstable_index",
-                "dbeel_tree_compact", "dbeel_tree_compact_many", "dbeel_tree_flush", "dbeel_tree_recover_wal", "dbeel_tree_get_many", "dbeel_tree_get_values", "dbeel_tree_scan", "dbeel_tree_scan_stream", "dbeel_tree_last_error", "dbeel_memtable_cut",
+                "dbeel_tree_compact", "dbeel_tree_compact_many", "dbeel_tree_flush", "dbeel_tree_recover_wal", "dbeel_tree_get_many", "dbeel_tree_get_values", "dbeel_tree_get_values_stream", "dbeel_tree_scan", "dbeel_tree_scan_stream", "dbeel_tree_last_error", "dbeel_memtable_cut",
                 "dbeel_plan_compactions", "dbeel_out_pages", "dbeel_tree_set_page_sink"]
 
 
@@ -215,6 +218,26 @@ class LSMTree:
                 dc, ic = int(out.data_len), int(out.index_len)
                 continue
             self._check(rc, "LSMTree.get_values")
+            return res, od[:out.data_len], oi[:out.index_len]
+
+    def get_values_stream(self, keys: Sequence[bytes], mode: int = capi.LOOKUP_REFERENCE):
+        """dbeel_tree_get_values_stream: what get_values returns, with .data and .index read from the files only where the
+        searches reach (each .bloom is read whole), so trees larger than device or host memory answer too."""
+        from . import sstable
+        blob, off = capi.pack_keys(keys)
+        res = np.zeros(len(keys), dtype=capi.LOOKUP_DTYPE)
+        dc = min(64 << 20, sum(os.path.getsize(os.path.join(self.dir, sstable.file_name(idx, sstable.DATA_FILE_EXT)))
+                               for idx, _ in self.sstable_indices_and_sizes()))
+        ic = 16 * len(keys)
+        for attempt in range(2):  # one more call with the reported sizes when the first caps are short
+            od, oi = np.empty(max(1, dc), np.uint8), np.empty(max(1, ic), np.uint8)
+            out = capi.Out(od.ctypes.data, dc, 0, oi.ctypes.data, ic, 0, None, 0, 0, 0)
+            rc = _lib().dbeel_tree_get_values_stream(self._h, blob.ctypes.data if blob.size else None, off.ctypes.data,
+                                                     len(keys), mode, C.byref(out), res.ctypes.data)
+            if rc == capi.ERR_CAPACITY and not attempt:
+                dc, ic = int(out.data_len), int(out.index_len)
+                continue
+            self._check(rc, "LSMTree.get_values_stream")
             return res, od[:out.data_len], oi[:out.index_len]
 
     def scan(self, ranges, kind: int = capi.SCAN_HASH):

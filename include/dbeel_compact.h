@@ -431,6 +431,28 @@ typedef struct dbeel_scan_io {
 int dbeel_scan_stream(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
                       uint32_t n_ranges, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop);
 
+/* dbeel_get_values on tables that stay in files: the same rows (DBEEL_LOOKUP_CORRUPT and DBEEL_LOOKUP_BAD_ENTRY included),
+ * the same out->data / out->index / items_written, the same DBEEL_ERR_CAPACITY behaviour, argument checks and limits, in
+ * both modes and on damaged tables -- but only the parts of .data and .index the batch's searches reach are read, which is
+ * what the reference reads per get: about log2(n) index records and key frames per table its filter lets through, plus
+ * the entry that answers (binary_search, lsm_tree.rs:605-670).
+ * tables[i].data_len / index_len give the file sizes (.data / .index pointers are ignored); tables[i].bloom is the .bloom
+ * file in host memory or NULL, as the reference keeps it in memory.  .data and .index are read only through io->read
+ * (io->write is not used and may be NULL), from the engine's reader threads; a nonzero return comes back unchanged and the
+ * engine stays usable.  Per table, newest first: the filter runs on the device, a table no open query passes is not read at
+ * all; the index records and key frames of the top levels of the search's probe tree are read (ranges that lie close
+ * together as one read), the searches descend on them on the device, and the index slices and .data windows of the leaves
+ * they end in are read in groups of about the partition budget (DBEEL_PARTITION_MB / _KB).  A hit's entry is copied out of
+ * its leaf's window on the device; a hit at a fence gets a one-record read after the last table.  Device and page-locked
+ * memory: a group, the fences, O(n_keys) and the answered entries -- not the tables.  A group holds at least one leaf, so
+ * one leaf's window can exceed the budget: about data_len / 2^16 bytes on very large tables, or more when a leaf holds
+ * multi-megabyte entries.
+ * dbeel_last_stats: input_bytes = bytes read through the callback, output_bytes / entries_out as dbeel_get_values,
+ * entries_in = n_keys, partitions = leaf groups run.  keys / key_offsets / results / out in host memory. */
+int dbeel_get_values_stream(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys,
+                            const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, const dbeel_scan_io *io,
+                            dbeel_out *out, dbeel_lookup_result *results);
+
 /* ---- N4: write-ahead-log replay + flush ------------------------------------------------------------------------
  * Replaces LSMTree::read_memtable_from_wal_file (lsm_tree.rs:552-574) followed by flush_memtable_to_disk, i.e. the
  * recovery of an unflushed memtable in open_or_create_ex (:478-513).  `wal` is the whole `.memtable` file: bincode

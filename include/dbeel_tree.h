@@ -84,6 +84,12 @@ int dbeel_tree_get_many(dbeel_tree *t, const void *keys, const uint64_t *key_off
 int dbeel_tree_get_values(dbeel_tree *t, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
                           dbeel_out *out, dbeel_lookup_result *results);
 
+/* dbeel_tree_get_values with the files left on disk (dbeel_get_values_stream): each .bloom is read whole, as the reference
+ * does when it opens a table; .data and .index are pread only where the batch's searches reach, so a tree larger than device
+ * or host memory answers too.  Rows, output, caps and DBEEL_ERR_CAPACITY equal dbeel_tree_get_values'.  out is host memory. */
+int dbeel_tree_get_values_stream(dbeel_tree *t, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
+                                 dbeel_out *out, dbeel_lookup_result *results);
+
 /* The SSTable part of LSMTree::iter_filter over the tree's files: every table's .data / .index in dbeel_tree_sstables()
  * order (oldest first, the iterator's order) through one dbeel_scan().  kind / ranges / results / stop as in dbeel_scan;
  * out holds host buffers (caps: the sums of the tables' .data and .index file sizes).  stop->table is a position in
