@@ -65,7 +65,7 @@ def build_variant(name: str, defines: list[str]) -> str:
 
 
 if __name__ == "__main__":
-    if "--variant" in sys.argv:  # python -m dbeel_b200._build --variant tpc2 DBEEL_GATHER_TPC=2
+    if "--variant" in sys.argv:  # python -m dbeel_b200._build --variant vpt2 DBEEL_GATHER_H_VPT=2
         k = sys.argv.index("--variant")
         print(build_variant(sys.argv[k + 1], sys.argv[k + 2:]))
     else:

@@ -22,8 +22,6 @@
 #include "../../include/dbeel_compact.h"
 #include "kernels.cuh"
 #include "merge_final.cuh"
-#include "gather_async.cuh"
-#include "gather_fb.cuh"
 #include "gather_h.cuh"
 #include "lookup.cuh"
 #include "lookup_stream.cuh"
@@ -87,16 +85,7 @@ struct dbeel_engine {
     dbeel_compact_opts async_opts = {};
     uint8_t async_seed[32] = {};
     int sm_count = 0; // multiProcessorCount of the device, set at engine creation
-    int merge_variant = 1;      // DBEEL_MERGE: 0 = one CTA per tile with plain loads, 1 = persistent TMA (default)
     int narrow_loads = 1;       // DBEEL_NARROW: .L2::64B loads for random accesses in extract / resolve (A/B switch)
-    int gather_variant = 11;    // DBEEL_GATHER: 11 = k_gather_h (default), 10 = k_gather32 with the lean entry-boundary pass, 0 = 16 bytes per lane (k_gather),
-                                //               1 = 32 bytes per lane + 32-byte block stores (k_gather32, the two-halves boundary pass),
-                                //               2 = 1 with the payload staged into shared memory by TMA bulk copies (k_gather_tma)
-    int fused_emit = 0;         // DBEEL_FUSED_EMIT: 1 = resolve + offsets scan + .index writes in one kernel (single jobs), 0 = four kernels
-    int bloom_side = 0;         // DBEEL_BLOOM_SIDE: 1 = k_bloom_res on a second stream (kernels of two streams do not co-run when each fills
-                                // the GPU, so the filter pass just moves in front of k_emit); 0 = the gather's fused epilogue
-    cudaStream_t s_side = nullptr;
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     int fused_final = 1;        // DBEEL_FUSED_FINAL: 1 = last merge level + resolve + offsets scan + .index writes in one persistent kernel
                                 // (k_merge_final, single compactions; the default: on an H100 it takes a cfg2 job from 5.91 ms with the five
                                 // kernels to 3.96 ms, DESIGN.md section 7), 0 = the five kernels
@@ -105,7 +94,6 @@ struct dbeel_engine {
     int stage_events = 1;       // DBEEL_STAGE_EVENTS: 0 = no per-stage event records inside a job (stage_ms read 0)
     int extract_persist = 6;    // DBEEL_EXTRACT_PERSIST: > 0 = k_extract runs as that many CTAs per SM, each thread fetching the next step's index
                                 // records while the current step's entry headers travel
-    int bloom_in_extract = 0;   // DBEEL_BLOOM_EXTRACT: 1 = k_extract hashes, k_resolve sets the bits; 0 = the gather's fused epilogue
 };
 
 namespace {
@@ -398,17 +386,11 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
     const uint64_t o_tfirst = carve(4ull * (gather_tiles + 2));
     const bool ref_reader = !flush && !jobs && (o->flags & DBEEL_FLAG_REFERENCE_READER);
     const uint64_t o_fix = carve(ref_reader ? 16ull * N : 0);
-    // single job with a filter: k_extract leaves both SipHash values of every key here and k_resolve sets the survivors' bits
-    const bool hash_early = e->bloom_in_extract && !flush && !jobs && (sh.bloom_file || (extra && extra->external_bloom && extra->bloom.words));
-    const uint64_t o_hash = carve(hash_early ? 16ull * N : 0);
-    // single compaction: resolve, the offsets scan and the .index writes in one kernel (chained scan over the tiles)
-    const bool fused_emit = e->fused_emit && !flush && !jobs && !many && !hash_early && !(e->bloom_side && sh.bloom_file);
     // single compaction: the last merge level, resolve, the offsets scan and the .index writes in one persistent kernel
-    const bool fused_final = e->fused_final && e->fin_ctas_per_sm > 0 && !flush && !jobs && !many && !hash_early && !fused_emit && levels >= 1 &&
-                             !(e->bloom_side && sh.bloom_file);
+    const bool fused_final = e->fused_final && e->fin_ctas_per_sm > 0 && !flush && !jobs && !many && levels >= 1;
     const uint64_t fin_tiles_ub = (uint64_t)(N + kFinNominal - 1) / kFinNominal + 1;
     p.fin_tile = fused_final ? (uint32_t)kFinNominal : 0u;
-    const uint64_t scan_bytes = fused_emit ? 16ull * res_tiles + 64 : (fused_final ? 16ull * fin_tiles_ub + 64 : 0);
+    const uint64_t scan_bytes = fused_final ? 16ull * fin_tiles_ub + 64 : 0;
     const uint64_t o_scan = carve(scan_bytes);
     int rc = ensure_device(e, &e->ws, &e->ws_cap, off);
     if (rc) return rc;
@@ -439,9 +421,7 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
     p.mem_table = reinterpret_cast<unsigned long long *>(ws + o_memtab);
     p.ref_reader = ref_reader ? 1 : 0;
     p.fix_index = reinterpret_cast<uint4 *>(ws + o_fix);
-    p.hash_rec = hash_early ? reinterpret_cast<uint4 *>(ws + o_hash) : nullptr;
     p.scan_state = reinterpret_cast<unsigned long long *>(ws + o_scan);
-    p.scan_ticket = reinterpret_cast<uint32_t *>(ws + o_scan + 16ull * res_tiles);
     p.out_data = static_cast<uint8_t *>(out->data);
     p.out_index = static_cast<uint4 *>(out->index);
 
@@ -517,13 +497,11 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
     const uint32_t g256 = (N + 255) / 256;
     const uint32_t gext = (N + 256 * kExtractEPT - 1) / (256 * kExtractEPT);
     auto launch_extract = [&](uint32_t grid, int mode) {
-        if (ref_reader && hash_early) launch_k(e, k_extract<true, true, true>, grid, 256, 0, s, p, mode);
-        else if (ref_reader) launch_k(e, k_extract<true, true, false>, grid, 256, 0, s, p, mode);
-        else if (hash_early) launch_k(e, k_extract<true, false, true>, grid, 256, 0, s, p, mode);
+        if (ref_reader) launch_k(e, k_extract<true, true>, grid, 256, 0, s, p, mode);
         else if (e->narrow_loads && e->extract_persist > 0 && mode == 0) // one resident wave, index records fetched a step ahead
-            launch_k(e, k_extract<true, false, false, true>, std::min<uint32_t>(grid, (uint32_t)(e->sm_count * e->extract_persist)), 256, 0, s, p, mode);
-        else if (e->narrow_loads) launch_k(e, k_extract<true, false, false>, grid, 256, 0, s, p, mode);
-        else launch_k(e, k_extract<false, false, false>, grid, 256, 0, s, p, mode);
+            launch_k(e, k_extract<true, false, true>, std::min<uint32_t>(grid, (uint32_t)(e->sm_count * e->extract_persist)), 256, 0, s, p, mode);
+        else if (e->narrow_loads) launch_k(e, k_extract<true, false>, grid, 256, 0, s, p, mode);
+        else launch_k(e, k_extract<false, false>, grid, 256, 0, s, p, mode);
     };
     if (flush) {
         launch_k(e, k_flush_prefix_init, 1, 1, 0, s, p);
@@ -573,8 +551,6 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
             if (grid > t_ub) grid = t_ub;
             if (e->narrow_loads) launch_k(e, k_merge_final<true>, (uint32_t)grid, kFinThreads, kFinSmem, s, p, l, src);
             else launch_k(e, k_merge_final<false>, (uint32_t)grid, kFinThreads, kFinSmem, s, p, l, src);
-        } else if (e->merge_variant == 0) { // one CTA per tile, plain loads (kept as the A/B baseline of the TMA kernel)
-            launch_k(e, k_merge, (uint32_t)t_ub, kMergeThreads, 0, s, p, l, src, dst);
         } else { // persistent, TMA bulk loads / stores + mbarrier
             uint64_t grid = (uint64_t)e->sm_count * kMergeCtasPerSM;
             if (grid > t_ub) grid = t_ub;
@@ -594,27 +570,13 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
         launches++;
     }
     uint4 *res = reinterpret_cast<uint4 *>(dst); // the ping-pong buffer that does not hold the merged order
-    const bool side_bloom = e->bloom_side && !flush && !jobs && !hash_early && p.bloom.words != nullptr;
-    p.bloom_elsewhere = side_bloom ? 1 : 0;
     if (!fused_final) {
-        if (hash_early) launch_k(e, k_resolve<true, false, true>, (uint32_t)res_tiles, kResolveThreads, 0, s, p, src, res);
-        else if (fused_emit) launch_k(e, k_resolve<true, true, false>, (uint32_t)res_tiles, kResolveThreads, 0, s, p, src, res);
-        else if (e->narrow_loads) launch_k(e, k_resolve<true, false, false>, (uint32_t)res_tiles, kResolveThreads, 0, s, p, src, res);
-        else launch_k(e, k_resolve<false, false, false>, (uint32_t)res_tiles, kResolveThreads, 0, s, p, src, res);
-        launches += 1;
-    }
-    if (side_bloom) { // fork: the filter is filled on the second stream while this one scans, emits and copies the payload
-        CU(cudaEventRecord(e->ev_fork, s));
-        CU(cudaStreamWaitEvent(e->s_side, e->ev_fork, 0));
-        k_bloom_res<<<g256, 256, 0, e->s_side>>>(p, res);
-        CU(cudaEventRecord(e->ev_join, e->s_side));
-        launches++;
-    }
-    if (!fused_emit && !fused_final) {
+        if (e->narrow_loads) launch_k(e, k_resolve<true>, (uint32_t)res_tiles, kResolveThreads, 0, s, p, src, res);
+        else launch_k(e, k_resolve<false>, (uint32_t)res_tiles, kResolveThreads, 0, s, p, src, res);
         launch_k(e, k_scan_tiles, (uint32_t)res_chunks, 1024, 0, s, p);
         launch_k(e, k_scan_chunks, 1, 1024, 0, s, p);
         launch_k(e, k_emit, (uint32_t)res_tiles, kResolveThreads, 0, s, p, res);
-        launches += 3;
+        launches += 4;
     }
     if (n_groups) {
         launch_k(e, k_flush_table, (uint32_t)((n_groups + 1 + 127) / 128), 128, 0, s, p, res);
@@ -623,39 +585,7 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
     if (stage_ev) CU(cudaEventRecord(e->ev[EV_RESOLVE], s));
 
     // ---- K5: gather + bloom (fused epilogue)
-    if (gather_tiles) {
-        const bool al32 = ((uintptr_t)out->data & 31) == 0; // 32-byte block stores
-        if (e->gather_variant == 11) { // the default: 16-byte vectors, the filter kept in L2 (gather_h.cuh)
-            launch_k(e, k_gather_h, (uint32_t)gather_tiles, kGhThreads, 0, s, p);
-        } else if (e->gather_variant == 2 && al32) { // persistent, payload staged through shared memory by the bulk-copy engine
-            uint64_t grid = (uint64_t)e->sm_count * DBEEL_GT_CTAS;
-            if (grid > gather_tiles) grid = gather_tiles;
-            launch_k(e, k_gather_tma, (uint32_t)grid, kGtThreads, kGtSmem, s, p);
-        } else if (e->gather_variant == 3 && al32) { // persistent, next tile's metadata prefetched with cp.async
-            uint64_t grid = (uint64_t)e->sm_count * DBEEL_GP_CTAS;
-            if (grid > gather_tiles) grid = gather_tiles;
-            launch_k(e, k_gather_p, (uint32_t)grid, kGatherThreads, 0, s, p);
-        } else if (e->gather_variant == 4 && al32) { // k_gather32 + a fifth warp per CTA that only fills the filter
-            launch_k(e, k_gather32<true, false, false>, (uint32_t)gather_tiles, kGatherThreads + 32, 0, s, p);
-        } else if (e->gather_variant == 8 && al32) { // entry-boundary blocks built by the lane that owns them in the copy loop
-            launch_k(e, k_gather_fb, (uint32_t)gather_tiles, kFbThreads, 0, s, p);
-        } else if (e->gather_variant == 7 && al32) { // payload lands in shared memory (cp.async), boundary blocks + filter while it travels
-            launch_k(e, k_gather_async, (uint32_t)gather_tiles, kGatherThreads, 0, s, p);
-        } else if (e->gather_variant >= 9 && al32) { // k_gather32 with the lean entry-boundary pass (aligned 32-byte chunks, one store per block)
-            launch_k(e, k_gather32<false, false, false, true>, (uint32_t)gather_tiles, kGatherThreads, 0, s, p);
-        } else if (e->gather_variant == 5 && al32) { // k_gather32, boundary blocks and filter on different warps (no gain)
-            launch_k(e, k_gather32<false, true, false>, (uint32_t)gather_tiles, kGatherThreads, 0, s, p);
-        } else if (e->gather_variant == 6 && al32 && p.bloom.words != nullptr && p.hash_rec == nullptr && !p.bloom_elsewhere &&
-                   gather_tiles + (N + kGatherThreads - 1) / kGatherThreads < 0x7FFFFFFFull) {
-            // k_gather32 with the filter on CTAs of their own, interleaved with the copy CTAs of the same grid
-            p.bloom_ctas = (uint32_t)((N + kGatherThreads - 1) / kGatherThreads); // one key per thread; N bounds the output entries
-            launch_k(e, k_gather32<false, false, true>, (uint32_t)(gather_tiles + p.bloom_ctas), kGatherThreads, 0, s, p);
-        } else if (e->gather_variant >= 1 && al32) { // k_gather32, filter as the copy CTA's epilogue
-            launch_k(e, k_gather32<false, false, false>, (uint32_t)gather_tiles, kGatherThreads, 0, s, p);
-        } else {
-            launch_k(e, k_gather, (uint32_t)gather_tiles, kGatherThreads, 0, s, p);
-        }
-    }
+    if (gather_tiles) launch_k(e, k_gather_h, (uint32_t)gather_tiles, kGhThreads, 0, s, p);
     launches++;
     if (jobs) { // per-job filters: their own pass over the output entries
         launch_k(e, k_bloom_many, g256, 256, 0, s, p);
@@ -665,7 +595,6 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
         launch_k(e, k_rebase_index, g256, 256, 0, s, p);
         launches++;
     }
-    if (side_bloom) CU(cudaStreamWaitEvent(s, e->ev_join, 0)); // join: the job ends when both streams are done
     CU(cudaEventRecord(e->ev[EV_GATHER], s));
     CU(cudaGetLastError());
 
@@ -2894,23 +2823,17 @@ int dbeel_engine_create(int device, dbeel_engine **out) {
     if (!e) return DBEEL_ERR_NOMEM;
     e->device = device;
     e->sm_count = prop.multiProcessorCount;
-    if (const char *v = getenv("DBEEL_MERGE")) e->merge_variant = atoi(v);
     if (const char *v = getenv("DBEEL_PIPELINE")) e->pipeline = atoi(v);
     if (const char *v = getenv("DBEEL_PIPELINE_MIN_KB")) e->pipeline_min_bytes = (uint64_t)(atoi(v) > 0 ? atoi(v) : 1) << 10;
     if (const char *v = getenv("DBEEL_PARTITION_KB")) e->partition_bytes = (uint64_t)(atoi(v) > 0 ? atoi(v) : 1) << 10;
     if (const char *v = getenv("DBEEL_PARTITION_TAPER")) e->partition_taper = atoi(v) != 0;
     if (const char *v = getenv("DBEEL_STREAM_RING")) e->stream_ring = std::max(2, atoi(v));
     if (const char *v = getenv("DBEEL_PARTITION_MB")) e->partition_bytes = (uint64_t)(atoi(v) > 0 ? atoi(v) : 128) << 20;
-    if (cudaFuncSetAttribute(k_merge_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * kMergeBufRecs * sizeof(Rec))) != cudaSuccess ||
-        cudaFuncSetAttribute(k_gather_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGtSmem) != cudaSuccess) {
+    if (cudaFuncSetAttribute(k_merge_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * kMergeBufRecs * sizeof(Rec))) != cudaSuccess) {
         dbeel_engine_destroy(e);
         return DBEEL_ERR_CUDA;
     }
     if (const char *v = getenv("DBEEL_NARROW")) e->narrow_loads = atoi(v);
-    if (const char *v = getenv("DBEEL_GATHER")) e->gather_variant = atoi(v);
-    if (const char *v = getenv("DBEEL_BLOOM_EXTRACT")) e->bloom_in_extract = atoi(v);
-    if (const char *v = getenv("DBEEL_BLOOM_SIDE")) e->bloom_side = atoi(v);
-    if (const char *v = getenv("DBEEL_FUSED_EMIT")) e->fused_emit = atoi(v);
     if (const char *v = getenv("DBEEL_FUSED_FINAL")) e->fused_final = atoi(v);
     if (const char *v = getenv("DBEEL_EXTRACT_PERSIST")) e->extract_persist = atoi(v);
     if (const char *v = getenv("DBEEL_PDL")) e->pdl = atoi(v);
@@ -2927,12 +2850,6 @@ int dbeel_engine_create(int device, dbeel_engine **out) {
             e->fin_ctas_per_sm = 0; // the five-kernel path
         }
         if (const char *v = getenv("DBEEL_FIN_CTAS_RT")) e->fin_ctas_per_sm = std::min(e->fin_ctas_per_sm, std::max(1, atoi(v)));
-    }
-    if (cudaStreamCreateWithFlags(&e->s_side, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming) != cudaSuccess) {
-        dbeel_engine_destroy(e);
-        return DBEEL_ERR_CUDA;
     }
     if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) { delete e; return DBEEL_ERR_CUDA; }
     for (int i = 0; i < EV_COUNT; i++)
@@ -2963,9 +2880,6 @@ void dbeel_engine_destroy(dbeel_engine *e) {
         if (e->ev_comp[i]) cudaEventDestroy(e->ev_comp[i]);
         if (e->ev_d2h[i]) cudaEventDestroy(e->ev_d2h[i]);
     }
-    if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-    if (e->ev_join) cudaEventDestroy(e->ev_join);
-    if (e->s_side) cudaStreamDestroy(e->s_side);
     if (e->s_h2d) cudaStreamDestroy(e->s_h2d);
     if (e->s_d2h) cudaStreamDestroy(e->s_d2h);
     if (e->pin) cudaFreeHost(e->pin);

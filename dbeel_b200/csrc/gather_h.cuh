@@ -1,26 +1,29 @@
-// gather_h.cuh -- K5 at Hopper's access width (k_gather_h, DBEEL_GATHER=11, the default).
+// gather_h.cuh -- K5: gather + bloom (k_gather_h), the roofline kernel.  Every surviving entry's bytes are read once from
+// its input run and written once at its output offset.
 //
-// k_gather32 was built around single 256-bit global accesses, which sm_90 does not have: there every 32-byte lane
-// granule is two 128-bit accesses 32 bytes apart, so one warp instruction spans 1 KB in 16-byte pieces.  This kernel
-// keeps k_gather32's skeleton -- short-lived CTAs, one 8 KB output tile each, one barrier after the metadata staging,
-// the payload held in registers, the OR-reduce + popcount vector -> entry map, a dense one-lane-per-entry boundary
-// pass, the filter as the epilogue -- and changes what the H100 does differently:
-//   * 16-byte output vectors, lane-contiguous (k_gather's mapping): a warp store covers 512 contiguous bytes, a warp
-//     load at most 528 contiguous source bytes of one entry.  The second aligned source vector is loaded only when the
-//     source shift is nonzero.
-//   * The boundary vector (the one holding entry j's last byte) gets its tail and its head from only the aligned 16-byte
-//     chunks that hold wanted bytes (chunks16), blended in registers (blend16), one 16-byte store.
-//   * The filter's REDs carry an L2 evict_last policy (kernels.cuh), so the ~4 GB payload stream does not push filter
-//     sectors out of the 50 MB L2 between two touches.  Marking the payload evict_first as well did not pay (DESIGN.md §7).
-// Same Params contract as k_gather32 (hash_rec, bloom_elsewhere, out_offset_base, multi-megabyte entries, no filter);
-// output buffers 16-byte aligned, which every entry point checks.
+// The output .data stream is cut into kGatherTileBytes (8 KB) tiles, one short-lived CTA each.  One pass stages the tile's
+// entries (source address, tile-relative start and end, key size) in shared memory, then ONE barrier.
+//   * Copy: 16-byte output vectors, lane-contiguous: a warp store covers 512 contiguous bytes, a warp load at most 528
+//     contiguous source bytes of one entry.  A vector inside one entry = one aligned 16-byte source load, a second only when
+//     the source shift is nonzero, and a byte funnel shift (realign16_sel); the payload is held in registers.  The entry under
+//     each lane's vector comes from one OR-reduction + popcount per 512-byte chunk over the sorted entry ends.
+//   * The vector that holds the last byte of entry j (at most one per entry: entries are >= 32 bytes) is left to a dense
+//     pass, one thread per entry: its tail and the head of entry j + 1 from only the aligned 16-byte chunks that hold wanted
+//     bytes (chunks16), blended in registers (blend16), one 16-byte store.
+//   No byte stores (bar the last < 16 bytes of the stream), no overlap between CTAs: every output vector has one writer.
+//   * Bloom (fused epilogue, when the job has a filter): the CTA hashes the key of every entry whose first byte lies in its
+//     tile (2 x SipHash-1-3 in one walk, one thread per entry) from lines the copy has just touched, and sets k bits with REDs
+//     that carry an L2 evict_last policy (kernels.cuh), so the ~4 GB payload stream does not push filter sectors out of the
+//     50 MB L2 between two touches.  Marking the payload evict_first as well did not pay (DESIGN.md §7).
+// Handles out_offset_base (key-range partitions of one output file) and multi-megabyte entries; output buffers are 16-byte
+// aligned, which every entry point checks.
 #pragma once
 #include "kernels.cuh"
 
 namespace dbeel {
 
 #ifndef DBEEL_GATHER_H_VPT
-#define DBEEL_GATHER_H_VPT 4 // 16-byte output vectors per thread: 64 bytes of payload in flight, as k_gather32
+#define DBEEL_GATHER_H_VPT 4 // 16-byte output vectors per thread: 64 bytes of payload in flight
 #endif
 constexpr int kGhVpt = DBEEL_GATHER_H_VPT;
 constexpr int kGhThreads = (int)(kGatherTileBytes / (16ull * 32 * kGhVpt)) * 32; // one 8 KB tile per CTA
@@ -28,6 +31,17 @@ static_assert(kGatherTileBytes == 16ull * kGhThreads * kGhVpt, "gather tile = 16
 #ifndef DBEEL_GATHER_H_MINB
 #define DBEEL_GATHER_H_MINB (1024 / kGhThreads) // 8 CTAs of 128 threads: 64 registers, no spills
 #endif
+
+__device__ __forceinline__ uint4 realign16_sel(uint4 A, uint4 B, uint32_t sh) {
+    // branch-free version of realign16 for a per-lane shift
+    const uint32_t bits = (sh & 3) * 8;
+    const bool s2 = sh & 8, s1 = sh & 4;
+    uint32_t c0 = s2 ? A.z : A.x, c1 = s2 ? A.w : A.y, c2 = s2 ? B.x : A.z;
+    uint32_t c3 = s2 ? B.y : A.w, c4 = s2 ? B.z : B.x, c5 = s2 ? B.w : B.y;
+    uint32_t d0 = s1 ? c1 : c0, d1 = s1 ? c2 : c1, d2 = s1 ? c3 : c2, d3 = s1 ? c4 : c3, d4 = s1 ? c5 : c4;
+    return make_uint4(__funnelshift_r(d0, d1, bits), __funnelshift_r(d1, d2, bits), __funnelshift_r(d2, d3, bits),
+                      __funnelshift_r(d3, d4, bits));
+}
 
 // 16 bytes at an arbitrary address of which bytes [lo, hi) are wanted: only the aligned chunks that hold them are loaded
 __device__ __forceinline__ uint4 ld16_lean(uintptr_t a, uint32_t lo, uint32_t hi) {
@@ -61,7 +75,8 @@ __global__ void __launch_bounds__(kGhThreads, DBEEL_GATHER_H_MINB) k_gather_h(Pa
     const uint32_t e_lo = p.tile_first[tile_id];
     const uint32_t e_hi = T0 + kGatherTileBytes < out_len ? p.tile_first[tile_id + 1] : c->out_items - 1;
     const uint32_t ne = e_hi - e_lo + 1; // <= kGatherMaxEntries: every entry is >= 32 bytes
-    const bool hash_here = p.bloom.words != nullptr && p.hash_rec == nullptr && !p.bloom_elsewhere;
+    const bool hash_here = p.bloom.words != nullptr;
+#pragma unroll 1 // one entry per thread is the common case; unrolled, this loop is two 4x copies of itself (+240 instructions)
     for (uint32_t j = tid; j < ne; j += NT) {
         const uint4 rec = p.out_index[e_lo + j];
         const unsigned long long d0 = ((unsigned long long)rec.x | ((unsigned long long)rec.y << 32)) - p.out_offset_base;
@@ -139,7 +154,7 @@ __global__ void __launch_bounds__(kGhThreads, DBEEL_GATHER_H_MINB) k_gather_h(Pa
         }
     }
 
-    // ---- bloom (fused epilogue), only when k_extract did not hash: entries whose first byte lies in this tile
+    // ---- bloom (fused epilogue): entries whose first byte lies in this tile
     if (hash_here) {
         const uint64_t keep = l2_evict_last();
         for (uint32_t j = tid; j < ne; j += NT) {

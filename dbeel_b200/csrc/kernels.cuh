@@ -68,7 +68,7 @@ constexpr int kResolveThreads = DBEEL_RESOLVE_THREADS;
 constexpr int kGatherThreads = DBEEL_GATHER_THREADS; // 128 threads = 8 KB tiles at 12 CTAs/SM
 constexpr int kGatherVecsPerThread = 4;
 
-constexpr unsigned long long kGatherTileBytes = 16ull * kGatherThreads * kGatherVecsPerThread; // 16 KB of output per CTA
+constexpr unsigned long long kGatherTileBytes = 16ull * kGatherThreads * kGatherVecsPerThread; // 8 KB of output per CTA
 constexpr int kGatherMaxEntries = (int)(kGatherTileBytes / 32) + 2; // entries are >= 32 bytes
 constexpr int kMaxLevels = 16;      // >= ceil(log2(DBEEL_MAX_RUNS)); flush: 2^16 sort tiles of kMergeTile (1792) arrivals
 
@@ -126,19 +126,15 @@ struct Params {
     uint8_t *out_data;
     uint4 *out_index;
     unsigned long long *src_ptr; // [n_total] device address of each surviving entry's bytes
-    uint32_t *tile_first;        // [ceil(data bytes / 16 KB) + 2] entry holding each gather tile's first byte
+    uint32_t *tile_first;        // [ceil(data bytes / kGatherTileBytes) + 2] entry holding each gather tile's first byte
     uint32_t tile_first_n;       // gather tiles the buffers were sized for (sparse batches: the caller's bound may be too low)
     unsigned long long data_bound; // .data bytes the job checked against out->data_cap: k_gather_h writes nothing at or past it
     unsigned long long out_offset_base; // .data bytes written by earlier key-range partitions of the same output file
     BloomParams bloom;
-    uint4 *hash_rec; // [n_total] {h0, h1} = both SipHash-1-3 values of every entry's key (k_extract), or null: the gather hashes
-    uint32_t bloom_ctas;      // k_gather32<.., kSplit>: filter blocks interleaved with the copy blocks of the grid
-    uint32_t bloom_elsewhere; // 1: k_bloom_res fills the filter on a second stream, next to the gather (which then skips it)
-    // fused resolve + emit (single jobs): chained scan of the tiles' (bytes, entries), decoupled look-back
+    // fused last merge level + resolve + emit (k_merge_final, single jobs): chained scan of the tiles' (bytes, entries), decoupled look-back
     uint32_t fin_tile;   // k_merge_final: nominal records per tile of the LAST level (< kMergeTile: room for the extensions), 0 = off
     uint32_t *part_ext;  // [boundaries of the last level] records with the boundary's key that follow it in A (bits 0-7) and B (8-15)
-    unsigned long long *scan_state; // [resolve tiles][2]: {status << 62 | bytes, status << 32 | entries}, zeroed per job
-    uint32_t *scan_ticket;          // tiles are numbered in the order their CTAs start
+    unsigned long long *scan_state; // [k_merge_final tiles][2]: {status << 62 | bytes, status << 32 | entries}, zeroed per job
 };
 
 // ------------------------------------------------------------------------------------
@@ -393,7 +389,7 @@ constexpr int kExtractEPT = DBEEL_EXTRACT_EPT; // entries per thread = independe
 #ifndef DBEEL_EXTRACT_PERSIST_MINB
 #define DBEEL_EXTRACT_PERSIST_MINB 3
 #endif
-template <bool kNarrow, bool kRef, bool kHash, bool kPersist = false>
+template <bool kNarrow, bool kRef, bool kPersist = false>
 __global__ void __launch_bounds__(256, kRef ? 3 : (kPersist ? DBEEL_EXTRACT_PERSIST_MINB : DBEEL_EXTRACT_MINB)) k_extract(Params p, int mode) {
     pdl_trigger();
     pdl_wait();
@@ -524,18 +520,6 @@ __global__ void __launch_bounds__(256, kRef ? 3 : (kPersist ? DBEEL_EXTRACT_PERS
                 else atomicMin(&p.first_mismatch[r[u]], i[u]);
             }
             st_rec(&p.rec_a[g[u]], out);
-        }
-        // ---- bloom hashes, here rather than in the gather: this kernel waits on memory with its issue slots idle, the key
-        // bytes are in L1, and the gather is the kernel that has no instruction to spare (DESIGN.md section 5, K1 / K5)
-        if (kHash && !redo && p.hash_rec != nullptr) {
-#pragma unroll
-            for (int u = 0; u < kExtractEPT; u++) {
-                if (!act[u] || !ok[u]) continue;
-                const uint8_t *key = data[u] + off[u] + 8;
-                uint64_t h0, h1;
-                sip13_pair_vec_u8(p.bloom.sip, (uint64_t)(ks[u] - 8), [key](uint64_t q) { return ld_u64_unaligned(key + 8 * q); }, &h0, &h1);
-                p.hash_rec[g[u]] = make_uint4((uint32_t)h0, (uint32_t)(h0 >> 32), (uint32_t)h1, (uint32_t)(h1 >> 32));
-            }
         }
     }
 }
@@ -850,61 +834,6 @@ __global__ void __launch_bounds__(kPartitionThreads) k_merge_partition(const __g
     }
 }
 
-__global__ void __launch_bounds__(kMergeThreads, 4) k_merge(Params p, uint32_t level, const Rec *src, Rec *dst) {
-    pdl_trigger();
-    pdl_wait();
-    __shared__ Rec s[kMergeTile + kMergeVT + 1];
-    const uint32_t pairs = p.nseg[level + 1];
-    const uint32_t *tb = p.tile_base[level];
-    const uint32_t tile = blockIdx.x;
-    if (tile >= tb[pairs]) return;
-    const uint32_t tid = threadIdx.x;
-    const uint32_t skip = p.ctl->prefix_len + kWindowBytes;
-    uint32_t j = find_pair(tb, pairs, tile, 0);
-    uint32_t t = tile - tb[j];
-    Seg a = p.seg[level][2 * j];
-    Seg b;
-    b.start = 0; b.len = 0;
-    if (2 * j + 1 < p.nseg[level]) b = p.seg[level][2 * j + 1];
-    const uint32_t pidx = tb[j] + j + t;
-    const uint32_t a0 = p.part[pidx], a1 = p.part[pidx + 1];
-    const uint32_t total = a.len + b.len;
-    const uint32_t diag0 = t * kMergeTile;
-    const uint32_t diag1 = diag0 + kMergeTile < total ? diag0 + kMergeTile : total;
-    const uint32_t b0 = diag0 - a0, b1 = diag1 - a1;
-    const uint32_t nA = a1 - a0, nB = b1 - b0, n = nA + nB;
-
-    for (uint32_t i = tid; i < nA; i += kMergeThreads) s[i] = ld_rec(&src[a.start + a0 + i]);
-    for (uint32_t i = tid; i < nB; i += kMergeThreads) s[nA + i] = ld_rec(&src[b.start + b0 + i]);
-    __syncthreads();
-
-    uint32_t d = tid * kMergeVT;
-    if (d > n) d = n;
-    uint32_t lo = d > nB ? d - nB : 0;
-    uint32_t hi = d < nA ? d : nA;
-    while (lo < hi) {
-        uint32_t mid = (lo + hi) >> 1;
-        if (!key_less_smem(p, skip, &s[nA + d - 1 - mid], &s[mid])) lo = mid + 1; else hi = mid;
-    }
-    uint32_t ai = lo, bi = d - lo;
-    Rec ak = s[ai], bk = s[nA + bi]; // may read one slot past a range: slack + guarded below
-    Rec out[kMergeVT];
-#pragma unroll
-    for (int i = 0; i < kMergeVT; i++) {
-        bool has_a = ai < nA, has_b = bi < nB;
-        bool take_b = has_b && (!has_a || key_less(p, skip, bk, ak));
-        out[i] = take_b ? bk : ak;
-        if (take_b) { bi++; bk = s[nA + bi]; } else { ai++; ak = s[ai]; }
-    }
-    Rec *o = dst + a.start + diag0;
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < kMergeVT; i++)
-        if (d + i < n) s[d + i] = out[i];
-    __syncthreads();
-    for (uint32_t i = tid; i < n; i += kMergeThreads) st_rec(&o[i], s[i]);
-}
-
 // ------------------------------------------------------------------------------------
 // Tile descriptors for the persistent merge kernel: which records of src a tile consumes and where
 // its merged output goes.  Looked up two tiles ahead so the lookups never sit on the critical path.
@@ -1092,15 +1021,8 @@ __device__ __forceinline__ void st_volatile_u64(unsigned long long *q, unsigned 
     asm volatile("st.volatile.global.u64 [%0], %1;" ::"l"(q), "l"(v) : "memory");
 }
 
-// kFused: the offsets scan and k_emit's writes happen here too -- every tile publishes its (bytes, entries) aggregate, looks
-// back over its predecessors' aggregates / inclusive prefixes (one warp, 32 predecessors per step) and writes its survivors'
-// .index records, source addresses and gather-tile markers directly.  Saves the res[] round trip (2 x 16 B per merged
-// record), two scan kernels and k_emit's launch.  Single jobs only: the grouped paths cut the stream by res[] afterwards.
-#ifndef DBEEL_RESOLVE_FUSED_MINB
-#define DBEEL_RESOLVE_FUSED_MINB 12
-#endif
-template <bool kNarrow, bool kFused, bool kHashRec>
-__global__ void __launch_bounds__(kResolveThreads, kFused ? DBEEL_RESOLVE_FUSED_MINB : DBEEL_RESOLVE_MINB) k_resolve(Params p, const Rec *m, uint4 *res) {
+template <bool kNarrow>
+__global__ void __launch_bounds__(kResolveThreads, DBEEL_RESOLVE_MINB) k_resolve(Params p, const Rec *m, uint4 *res) {
     pdl_trigger();
     pdl_wait();
     constexpr int NT = kResolveThreads;
@@ -1112,13 +1034,7 @@ __global__ void __launch_bounds__(kResolveThreads, kFused ? DBEEL_RESOLVE_FUSED_
     const Ctl *c = p.ctl;
     const uint32_t tid = threadIdx.x;
     const uint32_t span = c->span;
-    __shared__ uint32_t s_tile;
-    if (kFused) { // tiles numbered by starting order: a tile only ever waits for tiles that are already running
-        if (tid == 0) s_tile = atomicAdd(p.scan_ticket, 1u);
-        __syncthreads();
-    }
-    const uint32_t tile_id = kFused ? s_tile : blockIdx.x;
-    const uint32_t i0 = tile_id * NT;
+    const uint32_t i0 = blockIdx.x * NT;
     if (i0 >= span) return;
     const uint32_t skip = c->prefix_len + kWindowBytes;
     const uint32_t i = i0 + tid;
@@ -1180,7 +1096,7 @@ __global__ void __launch_bounds__(kResolveThreads, kFused ? DBEEL_RESOLVE_FUSED_
     s_eqn[tid] = eq_next ? 1 : 0;
     __syncthreads();
 
-    uint32_t keep = 0, ks = 0, fs = 0, wgid = 0;
+    uint32_t keep = 0, ks = 0, fs = 0;
     unsigned long long src = 0;
     if (p.mode_flush) {
         // Arrival batches: the winner of a group of equal keys is simply its LAST member (RedBlackTree::set replaces in place,
@@ -1190,12 +1106,10 @@ __global__ void __launch_bounds__(kResolveThreads, kFused ? DBEEL_RESOLVE_FUSED_
         if (active && !eq_next) {
             keep = 1; // tombstones are ordinary entries of a flush (lsm_tree.rs:790-795)
             ks = s_ks[tid]; fs = s_fs[tid]; src = s_entry[tid];
-            wgid = cur.w;
         }
     } else if (active && !eq_prev) { // head of its group
         uint32_t w = tid; // winner so far, as an index into this tile's shared arrays
         ks = s_ks[tid]; fs = s_fs[tid]; src = s_entry[tid];
-        wgid = cur.w;
         if (eq_next) {
             uint64_t wlo = s_tlo[tid], whi = s_thi[tid];
             uint32_t j = tid;
@@ -1209,7 +1123,6 @@ __global__ void __launch_bounds__(kResolveThreads, kFused ? DBEEL_RESOLVE_FUSED_
                 more = s_eqn[j] != 0;
             }
             ks = s_ks[w]; fs = s_fs[w]; src = s_entry[w];
-            wgid = s_rec[w + 1].w;
             if (more) { // the group runs past the tile: finish it from global memory
                 uint32_t gj = i0 + NT; // first record of the next tile (known equal: s_eqn[NT-1])
                 while (true) {
@@ -1222,7 +1135,7 @@ __global__ void __launch_bounds__(kResolveThreads, kFused ? DBEEL_RESOLVE_FUSED_
                         better = !ts_greater(wlo, whi, clo, chi);
                         if (better) { wlo = clo; whi = chi; }
                     }
-                    if (better) { ks = ck.klen + 8; fs = ck.full_size; src = (unsigned long long)(uintptr_t)ck.entry; wgid = nx.w; }
+                    if (better) { ks = ck.klen + 8; fs = ck.full_size; src = (unsigned long long)(uintptr_t)ck.entry; }
                     gj++;
                     if (gj >= lim_hi) break;
                     if (!key_equal(p, skip, nx, ld_rec(&m[gj]))) break;
@@ -1231,135 +1144,35 @@ __global__ void __launch_bounds__(kResolveThreads, kFused ? DBEEL_RESOLVE_FUSED_
         }
         bool tomb = fs == ks + 24;
         keep = (keep_tombstones || p.mode_flush || !tomb) ? 1u : 0u;
-        // Bloom::set for every entry that is written (lsm_tree.rs:1049-1051), from the hashes k_extract left behind
-        if (kHashRec && keep && p.hash_rec != nullptr && p.bloom.words != nullptr) {
-            const uint4 hv = __ldg(&p.hash_rec[wgid]);
-            uint32_t *words = p.bloom.words;
-            bloom_probe_all((uint64_t)hv.x | ((uint64_t)hv.y << 32), (uint64_t)hv.z | ((uint64_t)hv.w << 32), p.bloom.k_num, p.bloom.bits,
-                            p.bloom.bits_magic, [words](uint64_t bit) { atomicOr(&words[bit >> 5], 1u << (bit & 31)); });
-        }
     }
-    if (!kFused) {
-        if (i < span) res[i] = make_uint4((uint32_t)src, (uint32_t)(src >> 32), ks, keep ? fs : 0u); // holes: nothing emitted
+    if (i < span) res[i] = make_uint4((uint32_t)src, (uint32_t)(src >> 32), ks, keep ? fs : 0u); // holes: nothing emitted
 
-        // tile aggregate (bytes, entries) for the offsets scan: three warp reductions (REDUX) -- the byte count in two 16-bit
-        // halves, so that 32 entries of up to 4 GB each cannot overflow a 32-bit partial sum
-        const uint32_t fk = keep ? fs : 0u;
-        const uint32_t s_lo = __reduce_add_sync(0xFFFFFFFFu, fk & 0xFFFFu), s_hi = __reduce_add_sync(0xFFFFFFFFu, fk >> 16);
-        unsigned long long vb = (unsigned long long)s_lo + ((unsigned long long)s_hi << 16);
-        uint32_t vc = __reduce_add_sync(0xFFFFFFFFu, keep);
-        __syncthreads(); // s_tlo / s_ks are dead: reuse them as the cross-warp scratch
-        if ((tid & 31) == 0) { s_tlo[tid >> 5] = vb; s_ks[tid >> 5] = vc; }
-        __syncthreads();
-        if (tid == 0) {
-            unsigned long long tb = 0;
-            uint32_t tc = 0;
-            for (int w = 0; w < NT / 32; w++) { tb += s_tlo[w]; tc += s_ks[w]; }
-            p.tile_bytes[blockIdx.x] = tb;
-            p.tile_count[blockIdx.x] = tc;
-        }
-        return;
-    }
-
-    // ---- fused: in-tile inclusive scan, chained scan over the tiles, then the writes k_emit would do
-    const uint32_t lane = tid & 31, warp = tid >> 5;
-    unsigned long long ib = keep ? fs : 0ull;
-    uint32_t ic = keep;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long xb = __shfl_up_sync(0xFFFFFFFFu, ib, o);
-        const uint32_t xc = __shfl_up_sync(0xFFFFFFFFu, ic, o);
-        if (lane >= (uint32_t)o) { ib += xb; ic += xc; }
-    }
-    __syncthreads(); // s_tlo / s_ks / s_thi are dead: cross-warp scratch
-    if (lane == 31) { s_tlo[warp] = ib; s_ks[warp] = ic; }
+    // tile aggregate (bytes, entries) for the offsets scan: three warp reductions (REDUX) -- the byte count in two 16-bit
+    // halves, so that 32 entries of up to 4 GB each cannot overflow a 32-bit partial sum
+    const uint32_t fk = keep ? fs : 0u;
+    const uint32_t s_lo = __reduce_add_sync(0xFFFFFFFFu, fk & 0xFFFFu), s_hi = __reduce_add_sync(0xFFFFFFFFu, fk >> 16);
+    unsigned long long vb = (unsigned long long)s_lo + ((unsigned long long)s_hi << 16);
+    uint32_t vc = __reduce_add_sync(0xFFFFFFFFu, keep);
+    __syncthreads(); // s_tlo / s_ks are dead: reuse them as the cross-warp scratch
+    if ((tid & 31) == 0) { s_tlo[tid >> 5] = vb; s_ks[tid >> 5] = vc; }
     __syncthreads();
-    unsigned long long tb = 0, wb = 0;
-    uint32_t tc = 0, wc = 0;
-    for (int w = 0; w < NT / 32; w++) {
-        if ((uint32_t)w < warp) { wb += s_tlo[w]; wc += s_ks[w]; }
-        tb += s_tlo[w];
-        tc += s_ks[w];
+    if (tid == 0) {
+        unsigned long long tb = 0;
+        uint32_t tc = 0;
+        for (int w = 0; w < NT / 32; w++) { tb += s_tlo[w]; tc += s_ks[w]; }
+        p.tile_bytes[blockIdx.x] = tb;
+        p.tile_count[blockIdx.x] = tc;
     }
-    if (warp == 0) {
-        unsigned long long *mine = p.scan_state + 2ull * tile_id;
-        unsigned long long eb = 0;
-        uint32_t ec = 0;
-        if (tile_id == 0) {
-            if (lane == 0) {
-                st_volatile_u64(mine, (kScanPrefix << 62) | tb);
-                __threadfence();
-                st_volatile_u64(mine + 1, (kScanPrefix << 32) | tc);
-            }
-        } else {
-            if (lane == 0) { // bytes word first, entries word second: a reader that sees the second sees the first
-                st_volatile_u64(mine, (kScanAgg << 62) | tb);
-                __threadfence();
-                st_volatile_u64(mine + 1, (kScanAgg << 32) | tc);
-            }
-            int t = (int)tile_id - 1;
-            while (true) {
-                const int idx = t - (int)lane;
-                unsigned long long vb2 = 0, vc2 = 0, stat = kScanPrefix;
-                if (idx >= 0) {
-                    const unsigned long long *q = p.scan_state + 2ull * (uint32_t)idx;
-                    while (true) { // entries word, then bytes word; both must be at the same stage
-                        vc2 = ld_volatile_u64(q + 1);
-                        __threadfence();
-                        vb2 = ld_volatile_u64(q);
-                        if ((vc2 >> 32) != 0 && (vc2 >> 32) == (vb2 >> 62)) break;
-                    }
-                    stat = vc2 >> 32;
-                }
-                // lanes below the nearest tile that already holds an inclusive prefix add their aggregates, that tile its prefix
-                const uint32_t pm = __ballot_sync(0xFFFFFFFFu, stat == kScanPrefix);
-                const uint32_t first = (uint32_t)__ffs((int)pm) - 1; // pm != 0: lanes with idx < 0 report "prefix" (of nothing)
-                unsigned long long cb = (lane <= first && idx >= 0) ? (vb2 & ((1ull << 62) - 1)) : 0ull;
-                uint32_t cc = (lane <= first && idx >= 0) ? (uint32_t)vc2 : 0u;
-#pragma unroll
-                for (int o = 16; o; o >>= 1) {
-                    cb += __shfl_xor_sync(0xFFFFFFFFu, cb, o);
-                    cc += __shfl_xor_sync(0xFFFFFFFFu, cc, o);
-                }
-                eb += cb;
-                ec += cc;
-                if (pm) break;
-                t -= 32;
-            }
-            if (lane == 0) {
-                st_volatile_u64(mine, (kScanPrefix << 62) | (eb + tb));
-                __threadfence();
-                st_volatile_u64(mine + 1, (kScanPrefix << 32) | (unsigned long long)(ec + tc));
-            }
-        }
-        if (lane == 0) {
-            s_thi[0] = eb;
-            s_fs[0] = ec;
-            if ((unsigned long long)(tile_id + 1) * NT >= span) { // the last tile holds the totals
-                Ctl *cw = p.ctl;
-                cw->out_data_len = eb + tb;
-                cw->out_items = ec + tc;
-            }
-        }
-    }
-    __syncthreads();
-    if (!keep) return;
-    const unsigned long long off = s_thi[0] + wb + ib - fs; // within this job's .data
-    const uint32_t pos = s_fs[0] + wc + ic - 1;
-    const unsigned long long file_off = off + p.out_offset_base;
-    p.out_index[pos] = make_uint4((uint32_t)file_off, (uint32_t)(file_off >> 32), ks, fs);
-    p.src_ptr[pos] = src;
-    constexpr unsigned long long gt = kGatherTileBytes;
-    for (unsigned long long bq = (off + gt - 1) / gt; bq * gt < off + fs && bq < p.tile_first_n; bq++) p.tile_first[bq] = pos;
 }
+
 
 // ------------------------------------------------------------------------------------
 // K4b: offsets.  The survivor at merged position i becomes output entry `count before i`, at
 // .data offset `bytes before i` (entry_writer.rs:81-86: offset = running sum of full_size).
 // No inter-CTA waiting: (1) the per-tile aggregates are scanned in chunks of 1024 tiles, (2) one
 // CTA scans the chunk totals, (3) every tile rescans its 256 records locally and emits
-// out_index (the output .index file itself), src_ptr, and -- for every 16 KB tile of the
-// output .data stream -- the entry that holds the tile's first byte (tile_first).
+// out_index (the output .index file itself), src_ptr, and -- for every gather tile (kGatherTileBytes)
+// of the output .data stream -- the entry that holds the tile's first byte (tile_first).
 
 // block-wide exclusive scan of (bytes, count) over 1024 threads; returns the block totals
 __device__ __forceinline__ void block_excl_scan_1024(unsigned long long &vb, uint32_t &vc, unsigned long long *s_b,
@@ -1532,928 +1345,6 @@ __global__ void __launch_bounds__(256) k_rebase_index(Params p) {
     p.out_index[e] = rec;
 }
 
-// ------------------------------------------------------------------------------------
-// K5: gather + bloom -- the roofline kernel.  Every surviving entry's bytes are read once
-// from its input run and written once at its output offset.
-//
-// The output .data stream is cut into 16 KB tiles (1024 aligned 16-byte vectors), one CTA each.
-//   * a vector that lies inside one entry = two aligned 16-byte source loads + a byte funnel
-//     shift (source and destination are misaligned by an arbitrary byte count);
-//   * a vector that straddles an entry boundary (one per entry) is built by a second, dense
-//     pass: tail of entry j blended with the shifted head of entry j+1.
-// No byte stores (bar the last <16 bytes of the stream), no overlap between CTAs: every output
-// vector has exactly one writer.
-// Bloom (fused epilogue): after its stores are issued the CTA hashes the key of every entry
-// whose first byte lies in its tile (2 x SipHash-1-3 in one walk, one thread per entry) and
-// sets k bits with atomicOr -- the filter (<= ~10 MB at the benchmark shapes) stays
-// L2-resident and the key bytes are lines the copy has just touched.
-
-__device__ __forceinline__ uint4 realign16_sel(uint4 A, uint4 B, uint32_t sh) {
-    // branch-free version of realign16 for a per-lane shift
-    const uint32_t bits = (sh & 3) * 8;
-    const bool s2 = sh & 8, s1 = sh & 4;
-    uint32_t c0 = s2 ? A.z : A.x, c1 = s2 ? A.w : A.y, c2 = s2 ? B.x : A.z;
-    uint32_t c3 = s2 ? B.y : A.w, c4 = s2 ? B.z : B.x, c5 = s2 ? B.w : B.y;
-    uint32_t d0 = s1 ? c1 : c0, d1 = s1 ? c2 : c1, d2 = s1 ? c3 : c2, d3 = s1 ? c4 : c3, d4 = s1 ? c5 : c4;
-    return make_uint4(__funnelshift_r(d0, d1, bits), __funnelshift_r(d1, d2, bits), __funnelshift_r(d2, d3, bits),
-                      __funnelshift_r(d3, d4, bits));
-}
-
-// ------------------------------------------------------------------------------------
-// One staging pass, ONE block barrier, dense (thread-per-entry) straddle and bloom passes; the copy
-// itself is done warp by warp on 2 KB sub-tiles: a warp finds the entry under its first byte once
-// and then walks the (sorted) entry ends 512 bytes at a time, each lane counting how many entries
-// end at or before its own vector (one OR-reduction + popcount per chunk).
-
-#ifndef DBEEL_GATHER_MINB
-#define DBEEL_GATHER_MINB (1536 / DBEEL_GATHER_THREADS) // 12 CTAs of 128 threads: 40 registers
-#endif
-__global__ void __launch_bounds__(kGatherThreads, DBEEL_GATHER_MINB) k_gather(Params p) {
-    pdl_trigger();
-    pdl_wait();
-    constexpr int NT = kGatherThreads;
-    constexpr int VPT = kGatherVecsPerThread;
-    __shared__ unsigned long long s_adj[kGatherMaxEntries]; // entry address minus its tile-relative start
-    __shared__ int s_r0[kGatherMaxEntries], s_r1[kGatherMaxEntries];
-    __shared__ uint32_t s_ks[kGatherMaxEntries];
-    const Ctl *c = p.ctl;
-    const unsigned long long out_len = c->out_data_len;
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t tile_id = blockIdx.x;
-    const unsigned long long T0 = (unsigned long long)tile_id * kGatherTileBytes;
-    if (T0 >= out_len) return;
-    const uint32_t tile_len = out_len - T0 < kGatherTileBytes ? (uint32_t)(out_len - T0) : (uint32_t)kGatherTileBytes;
-    const uint32_t e_lo = p.tile_first[tile_id];
-    const uint32_t e_hi = T0 + kGatherTileBytes < out_len ? p.tile_first[tile_id + 1] : c->out_items - 1;
-    const uint32_t ne = e_hi - e_lo + 1; // <= kGatherMaxEntries: every entry is >= 32 bytes
-    for (uint32_t j = tid; j < ne; j += NT) {
-        const uint4 rec = p.out_index[e_lo + j];
-        const unsigned long long d0 = ((unsigned long long)rec.x | ((unsigned long long)rec.y << 32)) - p.out_offset_base;
-        const long long r0 = (long long)d0 - (long long)T0; // < 0 only for the tile's first entry
-        const long long r1 = r0 + (long long)rec.w;
-        s_adj[j] = p.src_ptr[e_lo + j] - (unsigned long long)r0;
-        s_r0[j] = r0 < -0x7FFFFFFFll ? -0x7FFFFFFF : (int)r0;
-        s_r1[j] = r1 > 0x7FFFFFFFll ? 0x7FFFFFFF : (int)r1;
-        s_ks[j] = rec.z;
-    }
-    __syncthreads();
-
-    // ---- copy: warp w owns bytes [w * 2 KB, (w + 1) * 2 KB) of the tile
-    uint8_t *dst_tile = p.out_data + T0;
-    const int sub0 = (int)(warp * (uint32_t)(32 * VPT * 16));
-    if ((uint32_t)sub0 < tile_len) {
-        // j = the entry that holds byte sub0 = number of entries ending at or before it (ends ascend).
-        uint32_t j = 0;
-        for (uint32_t base = 0; base + 1 < ne; base += 32) { // ballot-count 32 entries at a time; the last entry never counts
-            const uint32_t i = base + lane;
-            j += __popc(__ballot_sync(0xFFFFFFFFu, i + 1 < ne && s_r1[i] <= sub0));
-        }
-        uint4 A[VPT], B[VPT];
-        uint32_t sh[VPT];
-        bool pure[VPT];
-        const uint32_t lanes_le = 0xFFFFFFFFu >> (31 - lane); // bits 0..lane
-#pragma unroll
-        for (int k = 0; k < VPT; k++) {
-            const int cb = sub0 + k * 512; // this 512-byte chunk: one vector per lane
-            const int b0 = cb + (int)lane * 16;
-            // Entries that end inside the chunk, i.e. in (cb, cb + 512]: at most 17 (entries are >= 32 bytes),
-            // lane l looks at entry j + l.  An end at r1 precedes the vectors t = ceil((r1 - cb) / 16) .. 31,
-            // and distinct entries have distinct t, so one OR-reduction builds the whole chunk's map.
-            const uint32_t i = j + lane;
-            const int r1 = i + 1 < ne ? s_r1[i] : 0x7FFFFFFF;
-            const bool ends_here = r1 <= cb + 512;
-            const uint32_t t = (uint32_t)((ends_here ? r1 : cb + 16) - cb + 15) >> 4; // 1..32 when ends_here
-            const uint32_t ends = __reduce_or_sync(0xFFFFFFFFu, (ends_here && t < 32) ? (1u << t) : 0u);
-            const uint32_t cnt = __popc(ends & lanes_le); // entries ending at or before my vector's first byte
-            const uint32_t adv = __popc(__ballot_sync(0xFFFFFFFFu, ends_here));
-            const uint32_t e = j + cnt; // entry that holds byte b0
-            j += adv;                   // entry that holds the next chunk's first byte
-            // Loads are unconditional (no divergent branch around them): a vector that is not wholly inside
-            // entry e -- it straddles e's end, or lies past the end of the stream -- reads the last full vector
-            // of e instead (always valid memory: entries are >= 32 bytes) and simply is not stored.
-            const int r1e = s_r1[e];
-            pure[k] = (uint32_t)b0 + 16 <= tile_len && b0 + 16 <= r1e;
-            const int bl = b0 + 16 <= r1e ? b0 : r1e - 16;
-            const uintptr_t sa = (uintptr_t)(s_adj[e] + (unsigned long long)(long long)bl);
-            sh[k] = (uint32_t)(sa & 15);
-            const uint4 *sv = reinterpret_cast<const uint4 *>(sa - sh[k]);
-            A[k] = __ldg(sv);
-            B[k] = __ldg(sh[k] ? sv + 1 : sv);
-        }
-#pragma unroll
-        for (int k = 0; k < VPT; k++) {
-            const uint32_t v = (uint32_t)(sub0 >> 4) + (uint32_t)k * 32 + lane;
-            if (pure[k]) reinterpret_cast<uint4 *>(dst_tile)[v] = realign16_sel(A[k], B[k], sh[k]);
-        }
-    }
-
-    // ---- the vector that holds the last byte of entry j: tail of j blended with the head of j+1
-    for (uint32_t j = tid; j < ne; j += NT) {
-        const int r1 = s_r1[j];
-        if (r1 <= 0 || (r1 & 15) == 0 || r1 > (int)tile_len) continue;
-        const uint32_t v = (uint32_t)r1 >> 4;
-        const uint32_t b0 = v * 16;
-        const uint32_t t = (uint32_t)r1 - b0; // tail bytes of entry j in this vector: 1..15
-        const uintptr_t sa = (uintptr_t)(s_adj[j] + b0);
-        const uint32_t s0 = (uint32_t)(sa & 15);
-        const uint4 *sv = reinterpret_cast<const uint4 *>(sa - s0);
-        const uint4 TA = __ldg(sv);
-        const uint4 TB = __ldg(s0 + t > 16 ? sv + 1 : sv);
-        uint4 o = realign16_sel(TA, TB, s0);
-        if (b0 + 16 <= tile_len) {
-            const uintptr_t ha = (uintptr_t)(s_adj[j + 1] + (unsigned long long)(long long)s_r0[j + 1]); // first byte of entry j+1
-            const uint32_t hs = (uint32_t)(ha & 15);
-            const uint4 *hv = reinterpret_cast<const uint4 *>(ha - hs);
-            const uint4 HA = __ldg(hv);
-            const uint4 HB = __ldg(hs ? hv + 1 : hv);
-            const uint4 H = realign16_sel(HA, HB, hs);
-            const uint4 HU = realign16_sel(make_uint4(0, 0, 0, 0), H, 16 - t);
-            const uint32_t wfull = t >> 2, bits = (t & 3) * 8;
-            const uint32_t mmix = bits ? (0xFFFFFFFFu >> (32 - bits)) : 0u;
-            uint32_t ow[4] = {o.x, o.y, o.z, o.w}, hw[4] = {HU.x, HU.y, HU.z, HU.w};
-#pragma unroll
-            for (uint32_t q = 0; q < 4; q++) {
-                const uint32_t mk = q < wfull ? 0xFFFFFFFFu : (q == wfull ? mmix : 0u);
-                ow[q] = (ow[q] & mk) | (hw[q] & ~mk);
-            }
-            reinterpret_cast<uint4 *>(dst_tile)[v] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-        } else { // ragged end of the whole stream: never write past out_data_len
-            const uint32_t ow[4] = {o.x, o.y, o.z, o.w};
-            for (uint32_t b = 0; b < t; b++) dst_tile[b0 + b] = (uint8_t)(ow[b >> 2] >> ((b & 3) * 8));
-        }
-    }
-
-    // ---- bloom (fused epilogue): entries whose first byte lies in this tile
-    if (p.bloom.words != nullptr && p.hash_rec == nullptr && !p.bloom_elsewhere) {
-        for (uint32_t j = tid; j < ne; j += NT) {
-            const int r0 = s_r0[j];
-            if (r0 < 0 || r0 >= (int)kGatherTileBytes) continue;
-            const uint8_t *key = reinterpret_cast<const uint8_t *>((uintptr_t)(s_adj[j] + (unsigned long long)r0)) + 8;
-            const uint64_t klen = s_ks[j] - 8;
-            uint64_t h0, h1;
-            sip13_pair_vec_u8(p.bloom.sip, klen, [key](uint64_t q) { return ld_u64_unaligned(key + 8 * q); }, &h0, &h1);
-            uint32_t *words = p.bloom.words;
-            bloom_probe_all(h0, h1, p.bloom.k_num, p.bloom.bits, p.bloom.bits_magic,
-                            [words](uint64_t bit) { atomicOr(&words[bit >> 5], 1u << (bit & 31)); });
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------
-// K5, 32 bytes per lane (the default).  Same tiles, same staging, same one barrier as k_gather; what changes is the
-// granule every lane moves: a 32-byte block = three aligned 16-byte loads + one 32-byte store (stg256) instead of
-// 2 x (two loads + one 128-bit store).  Per output byte that halves the vector -> entry mapping (one OR-reduction +
-// popcount now covers 1 KB) and the address arithmetic, and takes the load over-fetch from 2x to 1.5x.  A block that holds an entry boundary (one per entry at most: entries are >= 32 bytes) is
-// left to a second, dense pass that writes its two 16-byte halves: tail of entry j, head of entry j + 1, or a blend.
-// The bloom epilogue only runs when k_extract did not hash (p.hash_rec == null).
-
-__device__ __forceinline__ void realign32(const uint4 A, const uint4 B, const uint4 C, uint32_t sh, uint32_t out[8]) {
-    // 32 output bytes starting `sh` (0..15) bytes into the 48-byte window {A, B, C}; C is not read when sh == 0
-    const uint32_t bits = (sh & 3) * 8;
-    const bool s2 = sh & 8, s1 = sh & 4;
-    const uint32_t w[12] = {A.x, A.y, A.z, A.w, B.x, B.y, B.z, B.w, C.x, C.y, C.z, C.w};
-    uint32_t c[10], d[9];
-#pragma unroll
-    for (int i = 0; i < 10; i++) c[i] = s2 ? w[i + 2] : w[i];
-#pragma unroll
-    for (int i = 0; i < 9; i++) d[i] = s1 ? c[i + 1] : c[i];
-#pragma unroll
-    for (int i = 0; i < 8; i++) out[i] = __funnelshift_r(d[i], d[i + 1], bits);
-}
-
-// one 32-byte aligned block: sm_90 has no 256-bit global access, so it leaves as two 128-bit stores (STG.E.128)
-__device__ __forceinline__ void stg256(void *dst, const uint32_t v[8]) {
-    asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]) : "memory");
-    asm volatile("st.global.v4.b32 [%0+16], {%1, %2, %3, %4};" ::"l"(dst), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]) : "memory");
-}
-
-// 16 bytes at an arbitrary address, `need` of them wanted: the second aligned load is skipped when the first one holds them all
-__device__ __forceinline__ uint4 ld16_any(uintptr_t sa, uint32_t need) {
-    const uint32_t s0 = (uint32_t)(sa & 15);
-    const uint4 *sv = reinterpret_cast<const uint4 *>(sa - s0);
-    const uint4 TA = __ldg(sv);
-    const uint4 TB = __ldg(s0 + need > 16 ? sv + 1 : sv);
-    return realign16_sel(TA, TB, s0);
-}
-
-__device__ __forceinline__ void ldg256_nc(const void *p, uint32_t v[8]) { // one 32-byte aligned chunk as two LDG.E.128
-    asm volatile("ld.global.nc.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "l"(p));
-    asm volatile("ld.global.nc.v4.b32 {%0, %1, %2, %3}, [%4+16];" : "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]) : "l"(p));
-}
-
-// 32 bytes at an arbitrary address of which bytes [lo, hi) are wanted (0 <= lo < hi <= 32): only the aligned 32-byte chunks
-// that hold wanted bytes are loaded (a lane that needs one chunk costs the L1 data pipe one wavefront, not two)
-__device__ __forceinline__ void ld32_any(uintptr_t a, uint32_t lo, uint32_t hi, uint32_t out[8]) {
-    const uint32_t s0 = (uint32_t)(a & 31);
-    const uintptr_t base = a - s0;
-    uint32_t w[16];
-#pragma unroll
-    for (int i = 0; i < 16; i++) w[i] = 0u;
-    if (lo < 32u - s0) ldg256_nc(reinterpret_cast<const void *>(base), w);          // chunk 0 = bytes [0, 32 - s0) of the block
-    if (hi > 32u - s0) ldg256_nc(reinterpret_cast<const void *>(base + 32), w + 8); // chunk 1 = bytes [32 - s0, 32)
-    window32(w, s0, out);
-}
-
-constexpr int kG32Vpt = (int)(kGatherTileBytes / (32ull * kGatherThreads)); // 1 KB chunks per warp
-static_assert(kGatherTileBytes == 32ull * kGatherThreads * kG32Vpt, "gather tile = 32 bytes x lanes x chunks");
-
-#ifndef DBEEL_GATHER32_MINB
-#define DBEEL_GATHER32_MINB (1536 / DBEEL_GATHER_THREADS)
-#endif
-#ifndef DBEEL_GATHER32W_MINB
-#define DBEEL_GATHER32W_MINB 9
-#endif
-// kBloomWarp: a fifth warp does nothing but the filter -- the tile's keys are hashed WHILE the four copy warps wait for their
-// payload loads, instead of after their stores by the same threads (the fused epilogue is a ~600-instruction dependent chain
-// per entry on 27 of 128 lanes: it lengthens every CTA's life by about a fifth).
-// kRot: the two dense per-entry passes run on DIFFERENT warps -- entry j's boundary block is written by thread (j + 96) mod 128
-// (warp 3 first), its key is hashed by thread (j + 32) mod 128 (warp 1 first).  A tile holds ~27 entries of 305 bytes, so with
-// the plain j = tid mapping warp 0 alone walks copy -> boundary loads -> key loads -> 600 dependent hash instructions while
-// warps 1-3 have exited but still hold their slots: the CTA lives as long as its slowest warp.
-// kSplit: the filter is filled by CTAs OF THEIR OWN, interleaved with the copy CTAs in the same grid (every ~5th block): a
-// filter CTA takes 128 consecutive output entries, one key per thread, all lanes busy, and runs on an SM next to copy CTAs
-// that are waiting for their payload -- its ~600 dependent hash instructions per key fill issue slots the copy leaves idle
-// instead of lengthening every copy CTA's life.  (Two kernels on two streams do not co-run when each fills the GPU; blocks
-// of one grid do.)  The key bytes are the first granule of an entry the copy CTA of the same region touches within a few
-// microseconds either way: an L2 hit for whichever comes second.  Block b is a filter block iff floor((b+1) nb / G) >
-// floor(b nb / G) (nb filter blocks spread evenly over the G blocks of the grid); it is filter block floor(b nb / G), and
-// a copy block is tile b - floor(b nb / G).
-// kLean (the default since round 2, DBEEL_GATHER=10; 1 = the two-halves pass below): the entry-boundary blocks with fewer trips
-// through the L1 data pipe, where every lane's access is a wavefront of its own (the one-lane-per-entry passes -- boundary
-// blocks, key loads, the filter's REDs -- issue most of the kernel's wavefronts; the copy proper a minority).  The
-// tail of entry j and the head of entry j + 1 each come from the aligned 32-byte chunks that hold wanted bytes (ldg256_nc,
-// one or two per side), are blended in registers and leave in one 32-byte store instead of 6 loads + 2 stores.  The same idea
-// applied to the key loads (two aligned 16-byte chunks per key, or two lanes per key with one SipHash each) was slower.
-template <bool kBloomWarp, bool kRot, bool kSplit, bool kLean = false>
-__global__ void __launch_bounds__(kGatherThreads + (kBloomWarp ? 32 : 0), kBloomWarp ? DBEEL_GATHER32W_MINB : DBEEL_GATHER32_MINB)
-k_gather32(Params p) {
-    pdl_trigger();
-    pdl_wait();
-    constexpr int NT = kGatherThreads;            // copy threads
-    constexpr int NTA = NT + (kBloomWarp ? 32 : 0); // all threads
-    uint32_t tile_of_block = blockIdx.x;
-    if (kSplit) {
-        const uint64_t nb = p.bloom_ctas, G = gridDim.x;
-        const uint32_t q0 = (uint32_t)((uint64_t)blockIdx.x * nb / G), q1 = (uint32_t)(((uint64_t)blockIdx.x + 1) * nb / G);
-        if (q1 != q0) { // filter block q0: output entries [128 q0, 128 q0 + 128)
-            const uint32_t e = q0 * (uint32_t)NT + threadIdx.x;
-            if (p.bloom.words == nullptr || e >= p.ctl->out_items) return;
-            const uint8_t *key = reinterpret_cast<const uint8_t *>((uintptr_t)__ldg(&p.src_ptr[e])) + 8;
-            const uint64_t klen = __ldg(&p.out_index[e]).z - 8;
-            uint64_t h0, h1;
-            sip13_pair_vec_u8(p.bloom.sip, klen, [key](uint64_t q) { return ld_u64_unaligned(key + 8 * q); }, &h0, &h1);
-            uint32_t *words = p.bloom.words;
-            bloom_probe_all(h0, h1, p.bloom.k_num, p.bloom.bits, p.bloom.bits_magic,
-                            [words](uint64_t bit) { atomicOr(&words[bit >> 5], 1u << (bit & 31)); });
-            return;
-        }
-        tile_of_block = blockIdx.x - q0;
-    }
-    __shared__ unsigned long long s_adj[kGatherMaxEntries]; // entry address minus its tile-relative start
-    __shared__ int s_r0[kGatherMaxEntries], s_r1[kGatherMaxEntries];
-    __shared__ uint32_t s_ks[kGatherMaxEntries];
-    const Ctl *c = p.ctl;
-    const unsigned long long out_len = c->out_data_len;
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t tile_id = tile_of_block;
-    const unsigned long long T0 = (unsigned long long)tile_id * kGatherTileBytes;
-    if (T0 >= out_len) return;
-    const uint32_t tile_len = out_len - T0 < kGatherTileBytes ? (uint32_t)(out_len - T0) : (uint32_t)kGatherTileBytes;
-    const uint32_t e_lo = p.tile_first[tile_id];
-    const uint32_t e_hi = T0 + kGatherTileBytes < out_len ? p.tile_first[tile_id + 1] : c->out_items - 1;
-    const uint32_t ne = e_hi - e_lo + 1; // <= kGatherMaxEntries: every entry is >= 32 bytes
-    const bool hash_here = !kSplit && p.bloom.words != nullptr && p.hash_rec == nullptr && !p.bloom_elsewhere;
-    for (uint32_t j = tid; j < ne; j += NTA) {
-        const uint4 rec = p.out_index[e_lo + j];
-        const unsigned long long d0 = ((unsigned long long)rec.x | ((unsigned long long)rec.y << 32)) - p.out_offset_base;
-        const long long r0 = (long long)d0 - (long long)T0; // < 0 only for the tile's first entry
-        const long long r1 = r0 + (long long)rec.w;
-        s_adj[j] = p.src_ptr[e_lo + j] - (unsigned long long)r0;
-        s_r0[j] = r0 < -0x7FFFFFFFll ? -0x7FFFFFFF : (int)r0;
-        s_r1[j] = r1 > 0x7FFFFFFFll ? 0x7FFFFFFF : (int)r1;
-        if (hash_here) s_ks[j] = rec.z;
-    }
-    __syncthreads();
-
-    if (kBloomWarp && warp == NT / 32) { // the filter warp: entries whose first byte lies in this tile
-        if (hash_here) {
-            for (uint32_t j = lane; j < ne; j += 32) {
-                const int r0 = s_r0[j];
-                if (r0 < 0 || r0 >= (int)kGatherTileBytes) continue;
-                const uint8_t *key = reinterpret_cast<const uint8_t *>((uintptr_t)(s_adj[j] + (unsigned long long)r0)) + 8;
-                const uint64_t klen = s_ks[j] - 8;
-                uint64_t h0, h1;
-                sip13_pair_vec_u8(p.bloom.sip, klen, [key](uint64_t q) { return ld_u64_unaligned(key + 8 * q); }, &h0, &h1);
-                uint32_t *words = p.bloom.words;
-                bloom_probe_all(h0, h1, p.bloom.k_num, p.bloom.bits, p.bloom.bits_magic,
-                                [words](uint64_t bit) { atomicOr(&words[bit >> 5], 1u << (bit & 31)); });
-            }
-        }
-        return;
-    }
-
-    // ---- copy: warp w owns bytes [w * 2 KB, (w + 1) * 2 KB) of the tile, 1 KB (32 lanes x 32 bytes) at a time
-    uint8_t *dst_tile = p.out_data + T0;
-    const int sub0 = (int)(warp * (uint32_t)(kG32Vpt * 1024));
-    if ((uint32_t)sub0 < tile_len) {
-        uint32_t j = 0; // the entry that holds byte sub0 = number of entries ending at or before it (ends ascend)
-        for (uint32_t base = 0; base + 1 < ne; base += 32) {
-            const uint32_t i = base + lane;
-            j += __popc(__ballot_sync(0xFFFFFFFFu, i + 1 < ne && s_r1[i] <= sub0));
-        }
-        uint4 A[kG32Vpt], B[kG32Vpt], C[kG32Vpt];
-        uint32_t sh[kG32Vpt];
-        bool pure[kG32Vpt];
-        const uint32_t lanes_le = 0xFFFFFFFFu >> (31 - lane); // bits 0..lane
-#pragma unroll
-        for (int k = 0; k < kG32Vpt; k++) {
-            const int cb = sub0 + k * 1024;
-            const int b0 = cb + (int)lane * 32;
-            // Entries that end inside the chunk, i.e. in (cb, cb + 1024]: at most 32, lane l looks at entry j + l.  An end at
-            // r1 precedes the blocks t = ceil((r1 - cb) / 32) .. 31; distinct entries have distinct t.
-            const uint32_t i = j + lane;
-            const int r1 = i + 1 < ne ? s_r1[i] : 0x7FFFFFFF;
-            const bool ends_here = r1 <= cb + 1024;
-            const uint32_t t = (uint32_t)((ends_here ? r1 : cb + 32) - cb + 31) >> 5; // 1..32 when ends_here
-            const uint32_t ends = __reduce_or_sync(0xFFFFFFFFu, (ends_here && t < 32) ? (1u << t) : 0u);
-            const uint32_t cnt = __popc(ends & lanes_le); // entries ending at or before my block's first byte
-            const uint32_t adv = __popc(__ballot_sync(0xFFFFFFFFu, ends_here));
-            const uint32_t e = j + cnt; // entry that holds byte b0
-            j += adv;                   // entry that holds the next chunk's first byte
-            // Unconditional loads: a block that is not wholly inside entry e (it holds e's end, or lies past the end of the
-            // stream) reads the last 32 bytes of e instead (always valid: entries are >= 32 bytes) and is not stored here.
-            const int r1e = s_r1[e];
-            pure[k] = (uint32_t)b0 + 32 <= tile_len && b0 + 32 <= r1e;
-            const int bl = b0 + 32 <= r1e ? b0 : r1e - 32;
-            const uintptr_t sa = (uintptr_t)(s_adj[e] + (unsigned long long)(long long)bl);
-            sh[k] = (uint32_t)(sa & 15);
-            const uint4 *sv = reinterpret_cast<const uint4 *>(sa - sh[k]);
-            A[k] = __ldg(sv); // (skipping these loads for the ~27 blocks per tile that are not stored here was slower)
-            B[k] = __ldg(sv + 1);
-            C[k] = __ldg(sh[k] ? sv + 2 : sv + 1);
-        }
-#pragma unroll
-        for (int k = 0; k < kG32Vpt; k++) {
-            if (pure[k]) {
-                uint32_t o[8];
-                realign32(A[k], B[k], C[k], sh[k], o);
-                stg256(dst_tile + sub0 + k * 1024 + (int)lane * 32, o);
-            }
-        }
-    }
-
-    // ---- the 32-byte block that holds the last byte of entry j (unless j ends on a block boundary)
-    if (kLean) {
-        for (uint32_t j = tid; j < ne; j += NT) {
-            const int r1 = s_r1[j];
-            if (r1 <= 0 || (r1 & 31) == 0 || r1 > (int)tile_len) continue;
-            const uint32_t b0 = (uint32_t)r1 & ~31u, t = (uint32_t)r1 - b0; // t = 1..31 bytes of entry j in this block
-            uint32_t T[8];
-            ld32_any((uintptr_t)(s_adj[j] + b0), 0u, t, T);
-            if (b0 + 32u <= tile_len) { // the rest of the block is the head of entry j + 1 (entries are >= 32 bytes)
-                uint32_t H[8], O[8];
-                ld32_any((uintptr_t)(s_adj[j + 1] + b0), t, 32u, H);
-                blend32(T, H, t, O);
-                stg256(dst_tile + b0, O);
-            } else { // ragged end of the whole stream: never write past out_data_len
-                uint32_t tw[8];
-#pragma unroll
-                for (int q = 0; q < 8; q++) tw[q] = T[q];
-                for (uint32_t b = 0; b < t; b++) dst_tile[b0 + b] = (uint8_t)(tw[b >> 2] >> ((b & 3) * 8));
-            }
-        }
-    }
-    for (uint32_t j = kLean ? ne : (kRot ? (tid + NT - 96u) % NT : tid); j < ne; j += NT) {
-        const int r1 = s_r1[j];
-        if (r1 <= 0 || (r1 & 31) == 0 || r1 > (int)tile_len) continue;
-        const bool has_next = j + 1 < ne;
-#pragma unroll
-        for (int half = 0; half < 2; half++) {
-            const uint32_t b0 = ((uint32_t)r1 & ~31u) + 16u * half;
-            if (b0 >= tile_len) continue;     // past the end of the stream
-            const int t = r1 - (int)b0;       // bytes of entry j in this vector: <= 0 none, >= 16 all
-            uint4 o;
-            if (t >= 16) {
-                o = ld16_any((uintptr_t)(s_adj[j] + b0), 16);
-            } else if (t <= 0) {
-                if (!has_next) continue;
-                o = ld16_any((uintptr_t)(s_adj[j + 1] + b0), 16);
-            } else {
-                o = ld16_any((uintptr_t)(s_adj[j] + b0), (uint32_t)t);
-                if (b0 + 16 <= tile_len) { // blend with the head of entry j + 1
-                    const uint4 H = ld16_any((uintptr_t)(s_adj[j + 1] + (unsigned long long)(long long)r1), 16);
-                    const uint4 HU = realign16_sel(make_uint4(0, 0, 0, 0), H, 16 - (uint32_t)t);
-                    const uint32_t wfull = (uint32_t)t >> 2, bits = ((uint32_t)t & 3) * 8;
-                    const uint32_t mmix = bits ? (0xFFFFFFFFu >> (32 - bits)) : 0u;
-                    uint32_t ow[4] = {o.x, o.y, o.z, o.w}, hw[4] = {HU.x, HU.y, HU.z, HU.w};
-#pragma unroll
-                    for (uint32_t q = 0; q < 4; q++) {
-                        const uint32_t mk = q < wfull ? 0xFFFFFFFFu : (q == wfull ? mmix : 0u);
-                        ow[q] = (ow[q] & mk) | (hw[q] & ~mk);
-                    }
-                    o = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-                } else { // ragged end of the whole stream: never write past out_data_len
-                    const uint32_t ow[4] = {o.x, o.y, o.z, o.w};
-                    for (int b = 0; b < t; b++) dst_tile[b0 + b] = (uint8_t)(ow[b >> 2] >> ((b & 3) * 8));
-                    continue;
-                }
-            }
-            reinterpret_cast<uint4 *>(dst_tile)[b0 >> 4] = o;
-        }
-    }
-
-    // ---- bloom (fused epilogue), only when k_extract did not hash: entries whose first byte lies in this tile
-    if (!kBloomWarp && hash_here) {
-        for (uint32_t j = kRot ? (tid + NT - 32u) % NT : tid; j < ne; j += NT) {
-            const int r0 = s_r0[j];
-            if (r0 < 0 || r0 >= (int)kGatherTileBytes) continue;
-            const uint8_t *key = reinterpret_cast<const uint8_t *>((uintptr_t)(s_adj[j] + (unsigned long long)r0)) + 8;
-            const uint64_t klen = s_ks[j] - 8;
-            uint64_t h0, h1;
-            sip13_pair_vec_u8(p.bloom.sip, klen, [key](uint64_t q) { return ld_u64_unaligned(key + 8 * q); }, &h0, &h1);
-            uint32_t *words = p.bloom.words;
-            bloom_probe_all(h0, h1, p.bloom.k_num, p.bloom.bits, p.bloom.bits_magic,
-                            [words](uint64_t bit) { atomicOr(&words[bit >> 5], 1u << (bit & 31)); });
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------
-// K5, TMA-staged (the default): "SSTable data blocks staged from HBM into shared memory via TMA".
-//
-// Why: k_gather / k_gather32 are neither DRAM- nor issue-bound.  A CTA walks its phases one
-// after the other -- tile_first -> out_index / src_ptr -> payload loads -> stores -> boundary loads -> key loads -- and
-// every arrow is a memory round trip that only the OTHER resident CTAs can cover.  Here the payload of a tile comes in
-// through the bulk-copy engine instead: one cp.async.bulk per entry (its 16-byte-aligned superset, <= tile bytes + 30),
-// all completing on one mbarrier, issued a whole tile AHEAD (two shared-memory stages), with the metadata of the tile
-// after that already travelling in registers.  By the time a tile is processed its bytes are in shared memory; the byte
-// realignment (the bulk engine preserves address mod 16, source and destination offsets differ by an arbitrary byte
-// count) runs from shared memory with LDS.128 + funnel shifts, the output leaves in 32-byte blocks (stg256), and the bloom hashes
-// read their keys from shared memory too.  Persistent CTAs, one tile per iteration.
-//
-//   iteration q:   metadata of tile q+1 (registers) -> shared memory, prefix sum of the staged lengths, bulk copies issued
-//                  global loads for the metadata of tile q+2 and the tile_first pair of tile q+3 (consumed next iteration)
-//                  wait for tile q's mbarrier -> copy / boundary blocks / bloom from stage q & 1
-//
-// Staging layout of a tile: entry j's in-tile part [r0c, r1c) is copied from src_lo = src & ~15 as len = ceil16(sh + n) bytes
-// to stage offset base_j = sum of the earlier lengths, so its byte at tile position b lives at sadj_j + b with
-// sadj_j = base_j + sh - r0c.
-
-constexpr int kGtThreads = kGatherThreads;
-constexpr int kGtPer = (kGatherMaxEntries + kGtThreads - 1) / kGtThreads;          // entries a thread may have to stage
-constexpr uint32_t kGtStageBytes = (uint32_t)kGatherTileBytes + 32u * kGatherMaxEntries + 128u; // payload + per-entry slack
-#ifndef DBEEL_GT_CTAS
-#define DBEEL_GT_CTAS 4
-#endif
-
-struct GtMeta {
-    unsigned long long adj[kGatherMaxEntries]; // global address of the entry minus its tile-relative start
-    uint32_t sadj[kGatherMaxEntries];          // stage offset of the entry's byte at tile position 0
-    int r0[kGatherMaxEntries], r1[kGatherMaxEntries];
-    uint32_t ks[kGatherMaxEntries];
-    uint32_t ne, tile_len;
-    unsigned long long T0;
-};
-constexpr uint32_t kGtSmem = 2u * kGtStageBytes + 2u * (uint32_t)sizeof(GtMeta) + 64u;
-
-__device__ __forceinline__ uint4 lds16_any(const uint8_t *stage, uint32_t off, uint32_t need) {
-    const uint32_t s0 = off & 15u;
-    const uint4 *sv = reinterpret_cast<const uint4 *>(stage + (off - s0));
-    const uint4 TA = *sv;
-    const uint4 TB = *(s0 + need > 16 ? sv + 1 : sv);
-    return realign16_sel(TA, TB, s0);
-}
-
-__global__ void __launch_bounds__(kGtThreads, DBEEL_GT_CTAS) k_gather_tma(Params p) {
-    pdl_trigger();
-    pdl_wait();
-    constexpr int NT = kGtThreads;
-    extern __shared__ __align__(128) uint8_t gt_raw[];
-    auto stage_ptr = [&](uint32_t st) -> uint8_t * { return gt_raw + st * kGtStageBytes; };
-    auto meta_ptr = [&](uint32_t st) -> GtMeta * { return reinterpret_cast<GtMeta *>(gt_raw + 2 * kGtStageBytes) + st; };
-    __shared__ __align__(8) uint64_t s_bar[2];
-    __shared__ uint32_t s_scan[NT / 32];
-    const Ctl *c = p.ctl;
-    const unsigned long long out_len = c->out_data_len;
-    const uint32_t out_items = c->out_items;
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t n_tiles = (uint32_t)((out_len + kGatherTileBytes - 1) / kGatherTileBytes);
-    const uint32_t G = gridDim.x;
-    if (blockIdx.x >= n_tiles) return;
-    if (tid == 0) {
-        mbar_init(&s_bar[0], 1);
-        mbar_init(&s_bar[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-
-    // ---- the three pipeline steps that run ahead of the tile being copied
-    struct TF { uint32_t e_lo, ne; };
-    auto load_tf = [&](uint32_t t) -> TF { // which entries overlap tile t
-        TF r;
-        r.e_lo = 0; r.ne = 0;
-        if (t < n_tiles) {
-            r.e_lo = __ldg(&p.tile_first[t]);
-            const uint32_t e_hi = t + 1 < n_tiles ? __ldg(&p.tile_first[t + 1]) : out_items - 1;
-            r.ne = e_hi - r.e_lo + 1;
-        }
-        return r;
-    };
-    auto load_recs = [&](const TF &tf, uint4 rec[kGtPer], unsigned long long src[kGtPer]) { // their index records / addresses
-#pragma unroll
-        for (int k = 0; k < kGtPer; k++) {
-            const uint32_t j = tid + (uint32_t)k * NT;
-            rec[k] = make_uint4(0, 0, 0, 0);
-            src[k] = 0;
-            if (j < tf.ne) {
-                rec[k] = __ldg(&p.out_index[tf.e_lo + j]);
-                src[k] = __ldg(&p.src_ptr[tf.e_lo + j]);
-            }
-        }
-    };
-    auto publish = [&](uint32_t st, uint32_t t, const TF &tf, const uint4 rec[kGtPer], const unsigned long long src[kGtPer]) {
-        GtMeta &m = *meta_ptr(st);
-        const unsigned long long T0 = (unsigned long long)t * kGatherTileBytes;
-        const uint32_t tile_len = out_len - T0 < kGatherTileBytes ? (uint32_t)(out_len - T0) : (uint32_t)kGatherTileBytes;
-        uint32_t carry = 0;
-#pragma unroll
-        for (int k = 0; k < kGtPer; k++) {
-            if ((uint32_t)k * NT >= tf.ne) break; // uniform
-            const uint32_t j = tid + (uint32_t)k * NT;
-            uint32_t len = 0, sh = 0;
-            int r0c = 0;
-            unsigned long long src_lo = 0;
-            if (j < tf.ne) {
-                const unsigned long long d0 = ((unsigned long long)rec[k].x | ((unsigned long long)rec[k].y << 32)) - p.out_offset_base;
-                const long long r0 = (long long)d0 - (long long)T0; // < 0 only for the tile's first entry
-                const long long r1 = r0 + (long long)rec[k].w;
-                const unsigned long long adj = src[k] - (unsigned long long)r0;
-                m.adj[j] = adj;
-                m.r0[j] = r0 < -0x7FFFFFFFll ? -0x7FFFFFFF : (int)r0;
-                m.r1[j] = r1 > 0x7FFFFFFFll ? 0x7FFFFFFF : (int)r1;
-                m.ks[j] = rec[k].z;
-                r0c = r0 < 0 ? 0 : (int)r0;
-                const int r1c = r1 > (long long)tile_len ? (int)tile_len : (int)r1;
-                const unsigned long long src_c = adj + (unsigned long long)r0c;
-                sh = (uint32_t)(src_c & 15);
-                src_lo = src_c - sh;
-                len = (sh + (uint32_t)(r1c - r0c) + 15u) & ~15u;
-            }
-            // exclusive prefix of len over the 128 entries of this round, in entry order
-            uint32_t inc = len;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t x = __shfl_up_sync(0xFFFFFFFFu, inc, o);
-                if (lane >= (uint32_t)o) inc += x;
-            }
-            __syncthreads(); // s_scan of the previous round / call has been read
-            if (lane == 31) s_scan[warp] = inc;
-            __syncthreads();
-            uint32_t before = carry, total = 0;
-#pragma unroll
-            for (int w = 0; w < NT / 32; w++) {
-                if ((uint32_t)w < warp) before += s_scan[w];
-                total += s_scan[w];
-            }
-            const uint32_t base = before + inc - len;
-            carry += total;
-            if (j < tf.ne) {
-                m.sadj[j] = base + sh - (uint32_t)r0c;
-                tma_load_1d(stage_ptr(st) + base, reinterpret_cast<const void *>(src_lo), len, &s_bar[st]);
-            }
-        }
-        if (tid == 0) {
-            m.ne = tf.ne;
-            m.tile_len = tile_len;
-            m.T0 = T0;
-            mbar_expect_tx(&s_bar[st], carry); // one arrival: the phase completes when all `carry` bytes have landed
-        }
-    };
-
-    uint4 recA[kGtPer], recB[kGtPer];
-    unsigned long long srcA[kGtPer], srcB[kGtPer];
-    uint32_t tile = blockIdx.x;
-    TF tf_cur = load_tf(tile), tf_nxt = load_tf(tile + G);
-    load_recs(tf_cur, recA, srcA);
-    publish(0, tile, tf_cur, recA, srcA);
-    load_recs(tf_nxt, recA, srcA);        // metadata of the NEXT tile rides in registers
-    TF tf_nn = load_tf(tile + 2 * G);
-
-    for (uint32_t q = 0;; q++) {
-        const uint32_t st = q & 1;
-        const bool has_next = tile + G < n_tiles;
-        if (has_next) publish(st ^ 1, tile + G, tf_nxt, recA, srcA);
-        load_recs(tf_nn, recB, srcB);                 // tile q + 2
-        const TF tf_n3 = load_tf(tile + 3 * G);       // tile q + 3
-        __syncthreads();                              // meta[st] was written one iteration ago by other threads
-        while (!mbar_try_wait(&s_bar[st], (q >> 1) & 1)) {}
-
-        const GtMeta &m = *meta_ptr(st);
-        const uint8_t *sd = stage_ptr(st);
-        const uint32_t ne = m.ne, tile_len = m.tile_len;
-        uint8_t *dst_tile = p.out_data + m.T0;
-
-        // ---- copy: warp w owns bytes [w * 2 KB, (w + 1) * 2 KB) of the tile, 1 KB (32 lanes x 32 bytes) at a time
-        const int sub0 = (int)(warp * (uint32_t)(kG32Vpt * 1024));
-        if ((uint32_t)sub0 < tile_len) {
-            uint32_t j = 0;
-            for (uint32_t base = 0; base + 1 < ne; base += 32) {
-                const uint32_t i = base + lane;
-                j += __popc(__ballot_sync(0xFFFFFFFFu, i + 1 < ne && m.r1[i] <= sub0));
-            }
-            const uint32_t lanes_le = 0xFFFFFFFFu >> (31 - lane);
-#pragma unroll
-            for (int k = 0; k < kG32Vpt; k++) {
-                const int cb = sub0 + k * 1024;
-                const int b0 = cb + (int)lane * 32;
-                const uint32_t i = j + lane;
-                const int r1 = i + 1 < ne ? m.r1[i] : 0x7FFFFFFF;
-                const bool ends_here = r1 <= cb + 1024;
-                const uint32_t t = (uint32_t)((ends_here ? r1 : cb + 32) - cb + 31) >> 5;
-                const uint32_t ends = __reduce_or_sync(0xFFFFFFFFu, (ends_here && t < 32) ? (1u << t) : 0u);
-                const uint32_t cnt = __popc(ends & lanes_le);
-                const uint32_t adv = __popc(__ballot_sync(0xFFFFFFFFu, ends_here));
-                const uint32_t e = j + cnt;
-                j += adv;
-                const int r1e = m.r1[e];
-                const bool pure = (uint32_t)b0 + 32 <= tile_len && b0 + 32 <= r1e;
-                if (pure) { // divergence is cheap here: nothing is in flight, the operands are in shared memory
-                    const uint32_t sa = m.sadj[e] + (uint32_t)b0;
-                    const uint32_t sh = sa & 15u;
-                    const uint4 *sv = reinterpret_cast<const uint4 *>(sd + (sa - sh));
-                    const uint4 A = sv[0], B = sv[1], C = sv[sh ? 2 : 1];
-                    uint32_t o[8];
-                    realign32(A, B, C, sh, o);
-                    stg256(dst_tile + b0, o);
-                }
-            }
-        }
-
-        // ---- the 32-byte block that holds the last byte of entry j (unless j ends on a block boundary): its two halves
-        for (uint32_t j = tid; j < ne; j += NT) {
-            const int r1 = m.r1[j];
-            if (r1 <= 0 || (r1 & 31) == 0 || r1 > (int)tile_len) continue;
-            const bool has_nx = j + 1 < ne;
-#pragma unroll
-            for (int half = 0; half < 2; half++) {
-                const uint32_t b0 = ((uint32_t)r1 & ~31u) + 16u * half;
-                if (b0 >= tile_len) continue;
-                const int t = r1 - (int)b0;
-                uint4 o;
-                if (t >= 16) {
-                    o = lds16_any(sd, m.sadj[j] + b0, 16);
-                } else if (t <= 0) {
-                    if (!has_nx) continue;
-                    o = lds16_any(sd, m.sadj[j + 1] + b0, 16);
-                } else {
-                    o = lds16_any(sd, m.sadj[j] + b0, (uint32_t)t);
-                    if (b0 + 16 <= tile_len) {
-                        const uint4 H = lds16_any(sd, m.sadj[j + 1] + (uint32_t)r1, 16);
-                        const uint4 HU = realign16_sel(make_uint4(0, 0, 0, 0), H, 16 - (uint32_t)t);
-                        const uint32_t wfull = (uint32_t)t >> 2, bits = ((uint32_t)t & 3) * 8;
-                        const uint32_t mmix = bits ? (0xFFFFFFFFu >> (32 - bits)) : 0u;
-                        uint32_t ow[4] = {o.x, o.y, o.z, o.w}, hw[4] = {HU.x, HU.y, HU.z, HU.w};
-#pragma unroll
-                        for (uint32_t qq = 0; qq < 4; qq++) {
-                            const uint32_t mk = qq < wfull ? 0xFFFFFFFFu : (qq == wfull ? mmix : 0u);
-                            ow[qq] = (ow[qq] & mk) | (hw[qq] & ~mk);
-                        }
-                        o = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-                    } else { // ragged end of the whole stream
-                        const uint32_t ow[4] = {o.x, o.y, o.z, o.w};
-                        for (int b = 0; b < t; b++) dst_tile[b0 + b] = (uint8_t)(ow[b >> 2] >> ((b & 3) * 8));
-                        continue;
-                    }
-                }
-                reinterpret_cast<uint4 *>(dst_tile)[b0 >> 4] = o;
-            }
-        }
-
-        // ---- bloom (fused epilogue): entries whose first byte lies in this tile; keys from shared memory when they are
-        // wholly staged (an entry that runs into the next tile may have its key cut off: global loads then)
-        if (p.bloom.words != nullptr && p.hash_rec == nullptr && !p.bloom_elsewhere) {
-            for (uint32_t j = tid; j < ne; j += NT) {
-                const int r0 = m.r0[j];
-                if (r0 < 0 || r0 >= (int)kGatherTileBytes) continue;
-                const uint64_t klen = m.ks[j] - 8;
-                uint64_t h0, h1;
-                if ((uint64_t)r0 + 16 + klen <= (uint64_t)tile_len) {
-                    const uint8_t *key = sd + (m.sadj[j] + (uint32_t)r0 + 8u);
-                    sip13_pair_vec_u8(p.bloom.sip, klen, [key](uint64_t qq) {
-                        const uintptr_t a = reinterpret_cast<uintptr_t>(key + 8 * qq);
-                        const uint64_t *w = reinterpret_cast<const uint64_t *>(a & ~uintptr_t(7));
-                        const uint32_t shb = (uint32_t)(a & 7) * 8;
-                        const uint64_t lo = w[0];
-                        return shb ? (lo >> shb) | (w[1] << (64 - shb)) : lo;
-                    }, &h0, &h1);
-                } else {
-                    const uint8_t *key = reinterpret_cast<const uint8_t *>((uintptr_t)(m.adj[j] + (unsigned long long)r0)) + 8;
-                    sip13_pair_vec_u8(p.bloom.sip, klen, [key](uint64_t qq) { return ld_u64_unaligned(key + 8 * qq); }, &h0, &h1);
-                }
-                uint32_t *words = p.bloom.words;
-                bloom_probe_all(h0, h1, p.bloom.k_num, p.bloom.bits, p.bloom.bits_magic,
-                                [words](uint64_t bit) { atomicOr(&words[bit >> 5], 1u << (bit & 31)); });
-            }
-        }
-
-        if (!has_next) break;
-        __syncthreads(); // everyone is done with stage st and meta[st]: the next iteration's publish overwrites st ^ 1's peer
-        tile += G;
-        tf_nxt = tf_nn;
-        tf_nn = tf_n3;
-#pragma unroll
-        for (int k = 0; k < kGtPer; k++) { recA[k] = recB[k]; srcA[k] = srcB[k]; }
-    }
-}
-
-// ------------------------------------------------------------------------------------
-// K5, persistent with prefetched metadata (k_gather32's copy, different skeleton).  In k_gather32 a CTA's life is a chain
-// of memory round trips -- tile_first -> out_index / src_ptr -> payload -> boundary / key bytes -- and only the other
-// resident CTAs cover them.  Here a CTA keeps going tile after tile, and the first two links of the NEXT tile's chain run
-// while the current tile is copied: the tile_first pair two tiles ahead travels in registers, the out_index / src_ptr
-// records of the next tile arrive in shared memory through cp.async (LDGSTS: no registers held).  What is left on a
-// tile's critical path is one payload round trip.
-
-__device__ __forceinline__ void cp_async16(void *smem_dst, const void *gmem_src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
-}
-__device__ __forceinline__ void cp_async8(void *smem_dst, const void *gmem_src) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
-}
-
-#ifndef DBEEL_GP_CTAS
-#define DBEEL_GP_CTAS 10
-#endif
-__global__ void __launch_bounds__(kGatherThreads, DBEEL_GP_CTAS) k_gather_p(Params p) {
-    pdl_trigger();
-    pdl_wait();
-    constexpr int NT = kGatherThreads;
-    __shared__ __align__(16) uint4 s_rawi[2][kGatherMaxEntries];
-    __shared__ __align__(8) unsigned long long s_raws[2][kGatherMaxEntries];
-    __shared__ unsigned long long s_adj[kGatherMaxEntries];
-    __shared__ int s_r0[kGatherMaxEntries], s_r1[kGatherMaxEntries];
-    __shared__ uint32_t s_ks[kGatherMaxEntries];
-    const Ctl *c = p.ctl;
-    const unsigned long long out_len = c->out_data_len;
-    const uint32_t out_items = c->out_items;
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t n_tiles = (uint32_t)((out_len + kGatherTileBytes - 1) / kGatherTileBytes);
-    const uint32_t G = gridDim.x;
-    uint32_t tile = blockIdx.x;
-    if (tile >= n_tiles) return;
-    const bool hash_here = p.bloom.words != nullptr && p.hash_rec == nullptr && !p.bloom_elsewhere;
-
-    auto tf_lo = [&](uint32_t t) -> uint32_t { return t < n_tiles ? __ldg(&p.tile_first[t]) : 0u; };
-    auto tf_ne = [&](uint32_t t, uint32_t lo) -> uint32_t {
-        if (t >= n_tiles) return 0u;
-        const uint32_t hi = t + 1 < n_tiles ? __ldg(&p.tile_first[t + 1]) : out_items - 1;
-        return hi - lo + 1;
-    };
-    auto prefetch = [&](uint32_t buf, uint32_t lo, uint32_t ne) {
-        for (uint32_t j = tid; j < ne; j += NT) {
-            cp_async16(&s_rawi[buf][j], &p.out_index[lo + j]);
-            cp_async8(&s_raws[buf][j], &p.src_ptr[lo + j]);
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-
-    uint32_t lo0 = tf_lo(tile), ne0 = tf_ne(tile, lo0);
-    prefetch(0, lo0, ne0);
-    uint32_t lo1 = tf_lo(tile + G), ne1 = tf_ne(tile + G, lo1);
-
-    for (uint32_t q = 0;; q++) {
-        const uint32_t buf = q & 1;
-        const bool has_next = tile + G < n_tiles;
-        prefetch(buf ^ 1, lo1, ne1); // an empty group when there is no next tile
-        const uint32_t lo2 = tf_lo(tile + 2 * G), ne2 = tf_ne(tile + 2 * G, lo2); // consumed one iteration from now
-        asm volatile("cp.async.wait_group 1;" ::: "memory"); // everything but the group just committed has landed
-        __syncthreads();
-
-        const unsigned long long T0 = (unsigned long long)tile * kGatherTileBytes;
-        const uint32_t tile_len = out_len - T0 < kGatherTileBytes ? (uint32_t)(out_len - T0) : (uint32_t)kGatherTileBytes;
-        const uint32_t ne = ne0;
-        for (uint32_t j = tid; j < ne; j += NT) {
-            const uint4 rec = s_rawi[buf][j];
-            const unsigned long long d0 = ((unsigned long long)rec.x | ((unsigned long long)rec.y << 32)) - p.out_offset_base;
-            const long long r0 = (long long)d0 - (long long)T0;
-            const long long r1 = r0 + (long long)rec.w;
-            s_adj[j] = s_raws[buf][j] - (unsigned long long)r0;
-            s_r0[j] = r0 < -0x7FFFFFFFll ? -0x7FFFFFFF : (int)r0;
-            s_r1[j] = r1 > 0x7FFFFFFFll ? 0x7FFFFFFF : (int)r1;
-            if (hash_here) s_ks[j] = rec.z;
-        }
-        __syncthreads();
-
-        // ---- copy (k_gather32's): warp w owns bytes [w * 2 KB, (w + 1) * 2 KB) of the tile, 1 KB at a time
-        uint8_t *dst_tile = p.out_data + T0;
-        const int sub0 = (int)(warp * (uint32_t)(kG32Vpt * 1024));
-        if ((uint32_t)sub0 < tile_len) {
-            uint32_t j = 0;
-            for (uint32_t base = 0; base + 1 < ne; base += 32) {
-                const uint32_t i = base + lane;
-                j += __popc(__ballot_sync(0xFFFFFFFFu, i + 1 < ne && s_r1[i] <= sub0));
-            }
-            uint4 A[kG32Vpt], B[kG32Vpt], C[kG32Vpt];
-            uint32_t sh[kG32Vpt];
-            bool pure[kG32Vpt];
-            const uint32_t lanes_le = 0xFFFFFFFFu >> (31 - lane);
-#pragma unroll
-            for (int k = 0; k < kG32Vpt; k++) {
-                const int cb = sub0 + k * 1024;
-                const int b0 = cb + (int)lane * 32;
-                const uint32_t i = j + lane;
-                const int r1 = i + 1 < ne ? s_r1[i] : 0x7FFFFFFF;
-                const bool ends_here = r1 <= cb + 1024;
-                const uint32_t t = (uint32_t)((ends_here ? r1 : cb + 32) - cb + 31) >> 5;
-                const uint32_t ends = __reduce_or_sync(0xFFFFFFFFu, (ends_here && t < 32) ? (1u << t) : 0u);
-                const uint32_t cnt = __popc(ends & lanes_le);
-                const uint32_t adv = __popc(__ballot_sync(0xFFFFFFFFu, ends_here));
-                const uint32_t e = j + cnt;
-                j += adv;
-                const int r1e = s_r1[e];
-                pure[k] = (uint32_t)b0 + 32 <= tile_len && b0 + 32 <= r1e;
-                const int bl = b0 + 32 <= r1e ? b0 : r1e - 32;
-                const uintptr_t sa = (uintptr_t)(s_adj[e] + (unsigned long long)(long long)bl);
-                sh[k] = (uint32_t)(sa & 15);
-                const uint4 *sv = reinterpret_cast<const uint4 *>(sa - sh[k]);
-                A[k] = __ldg(sv);
-                B[k] = __ldg(sv + 1);
-                C[k] = __ldg(sh[k] ? sv + 2 : sv + 1);
-            }
-#pragma unroll
-            for (int k = 0; k < kG32Vpt; k++) {
-                if (pure[k]) {
-                    uint32_t o[8];
-                    realign32(A[k], B[k], C[k], sh[k], o);
-                    stg256(dst_tile + sub0 + k * 1024 + (int)lane * 32, o);
-                }
-            }
-        }
-
-        // ---- the 32-byte block that holds the last byte of entry j: its two halves
-        for (uint32_t j = tid; j < ne; j += NT) {
-            const int r1 = s_r1[j];
-            if (r1 <= 0 || (r1 & 31) == 0 || r1 > (int)tile_len) continue;
-            const bool has_nx = j + 1 < ne;
-#pragma unroll
-            for (int half = 0; half < 2; half++) {
-                const uint32_t b0 = ((uint32_t)r1 & ~31u) + 16u * half;
-                if (b0 >= tile_len) continue;
-                const int t = r1 - (int)b0;
-                uint4 o;
-                if (t >= 16) {
-                    o = ld16_any((uintptr_t)(s_adj[j] + b0), 16);
-                } else if (t <= 0) {
-                    if (!has_nx) continue;
-                    o = ld16_any((uintptr_t)(s_adj[j + 1] + b0), 16);
-                } else {
-                    o = ld16_any((uintptr_t)(s_adj[j] + b0), (uint32_t)t);
-                    if (b0 + 16 <= tile_len) {
-                        const uint4 H = ld16_any((uintptr_t)(s_adj[j + 1] + (unsigned long long)(long long)r1), 16);
-                        const uint4 HU = realign16_sel(make_uint4(0, 0, 0, 0), H, 16 - (uint32_t)t);
-                        const uint32_t wfull = (uint32_t)t >> 2, bits = ((uint32_t)t & 3) * 8;
-                        const uint32_t mmix = bits ? (0xFFFFFFFFu >> (32 - bits)) : 0u;
-                        uint32_t ow[4] = {o.x, o.y, o.z, o.w}, hw[4] = {HU.x, HU.y, HU.z, HU.w};
-#pragma unroll
-                        for (uint32_t qq = 0; qq < 4; qq++) {
-                            const uint32_t mk = qq < wfull ? 0xFFFFFFFFu : (qq == wfull ? mmix : 0u);
-                            ow[qq] = (ow[qq] & mk) | (hw[qq] & ~mk);
-                        }
-                        o = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-                    } else {
-                        const uint32_t ow[4] = {o.x, o.y, o.z, o.w};
-                        for (int b = 0; b < t; b++) dst_tile[b0 + b] = (uint8_t)(ow[b >> 2] >> ((b & 3) * 8));
-                        continue;
-                    }
-                }
-                reinterpret_cast<uint4 *>(dst_tile)[b0 >> 4] = o;
-            }
-        }
-
-        // ---- bloom (fused epilogue) unless it runs elsewhere
-        if (hash_here) {
-            for (uint32_t j = tid; j < ne; j += NT) {
-                const int r0 = s_r0[j];
-                if (r0 < 0 || r0 >= (int)kGatherTileBytes) continue;
-                const uint8_t *key = reinterpret_cast<const uint8_t *>((uintptr_t)(s_adj[j] + (unsigned long long)r0)) + 8;
-                const uint64_t klen = s_ks[j] - 8;
-                uint64_t h0, h1;
-                sip13_pair_vec_u8(p.bloom.sip, klen, [key](uint64_t qq) { return ld_u64_unaligned(key + 8 * qq); }, &h0, &h1);
-                uint32_t *words = p.bloom.words;
-                bloom_probe_all(h0, h1, p.bloom.k_num, p.bloom.bits, p.bloom.bits_magic,
-                                [words](uint64_t bit) { atomicOr(&words[bit >> 5], 1u << (bit & 31)); });
-            }
-        }
-
-        if (!has_next) break;
-        __syncthreads(); // s_adj / s_r0 / s_r1 and raw buffer `buf` are free again
-        tile += G;
-        lo0 = lo1; ne0 = ne1;
-        lo1 = lo2; ne1 = ne2;
-    }
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-}
-
 // Job header down / control block up without a copy engine: the pinned block is mapped into the GPU's address space.
 __global__ void __launch_bounds__(256) k_copy_words(uint32_t *dst, const uint32_t *src_host, uint32_t n) {
     pdl_trigger();
@@ -2501,25 +1392,6 @@ __global__ void k_bloom_frame(uint8_t *file, uint64_t n_words, BloomParams b) {
         put64(t + 16, 0);                         // ntail
         t += 18;
     }
-}
-
-// Single job, filter filled NEXT TO the gather instead of inside it: one thread per merged position, survivors only
-// (res[i].w != 0), key bytes from the entry's source (one 64-byte granule for ordinary keys).  Launched on the engine's
-// second stream right after k_resolve, so its random reads and SipHash rounds overlap k_emit and the payload copy -- the
-// gather is the kernel with no issue slot and no latency slack to spare, this one is all latency.
-__global__ void __launch_bounds__(256) k_bloom_res(Params p, const uint4 *res) {
-    pdl_trigger();
-    pdl_wait();
-    const uint32_t i = blockIdx.x * 256u + threadIdx.x;
-    if (i >= p.ctl->span) return;
-    const uint4 it = __ldg(&res[i]);
-    if (it.w == 0) return;
-    const uint8_t *key = reinterpret_cast<const uint8_t *>((uintptr_t)((unsigned long long)it.x | ((unsigned long long)it.y << 32))) + 8;
-    uint64_t h0, h1;
-    sip13_pair_vec_u8(p.bloom.sip, (uint64_t)(it.z - 8), [key](uint64_t q) { return ld_u64_unaligned_narrow(key + 8 * q); }, &h0, &h1);
-    uint32_t *words = p.bloom.words;
-    bloom_probe_all(h0, h1, p.bloom.k_num, p.bloom.bits, p.bloom.bits_magic,
-                    [words](uint64_t bit) { atomicOr(&words[bit >> 5], 1u << (bit & 31)); });
 }
 
 // compact-many: the filters are per job (own size, own seed), so they are filled by a pass of their own over the output

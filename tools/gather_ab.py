@@ -6,9 +6,9 @@
   2. the stage times of every spec, the specs alternated for --rounds rounds (spread = max - min over rounds);
   3. with --profile SPEC (repeatable), per-kernel device times from torch.profiler in a run of their own.
 
-A spec is tools/tune.py's: "DBEEL_GATHER=10,DBEEL_BLOOM_SIDE=1", "LIB=<variant>" (a build made by
+A spec is tools/tune.py's: "DBEEL_FUSED_FINAL=0,DBEEL_NARROW=0", "LIB=<variant>" (a build made by
 `python -m dbeel_b200._build --variant <name> -D...`), or "" for the default.
-Usage: tools/gather_ab.py --rounds 3 "" "DBEEL_GATHER=10" --profile "DBEEL_GATHER=10,DBEEL_BLOOM_SIDE=1"
+Usage: tools/gather_ab.py --rounds 3 "" "LIB=vpt2" --profile "LIB=vpt2"
 """
 import argparse
 import json

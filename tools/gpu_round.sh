@@ -30,7 +30,7 @@ from dbeel_b200 import capi, workloads as W
 import oracle
 runs = W.make_merge_runs(W.scaled(W.CFG2, 30000)); seed = bytes(range(32))
 exp = oracle.compact(runs, False, seed=seed)
-for env in ({}, {'DBEEL_FUSED_FINAL': '1'}, {'DBEEL_GATHER': '7'}):
+for env in ({}, {'DBEEL_FUSED_FINAL': '1'}):
     os.environ.update(env); e = capi.Engine(0); g = e.compact(runs, False, seed=seed); e.close()
     for k in env: del os.environ[k]
     print(env, all(np.array_equal(a, b) for a, b in zip(g[:3], exp[:3])))

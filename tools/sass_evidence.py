@@ -30,8 +30,8 @@ def main():
         elif cur and re.search(r"/\*[0-9a-f]{4}\*/", ln):
             kernels[cur].append(re.sub(r"/\* 0x[0-9a-f]+ \*/", "", ln).strip())
     print(f"# {os.path.relpath(LIB, ROOT)}: {len(kernels)} kernels, sm_90a SASS (cuobjdump -sass)\n")
-    want = sys.argv[1:] or ["k_gather32", "k_gather_p", "k_gather_tma", "k_gather", "k_merge_tma", "k_extract", "k_resolve", "k_emit",
-                            "k_bloom_res", "k_route_hash", "k_memtable_cuts"]
+    want = sys.argv[1:] or ["k_gather_h", "k_merge_final", "k_merge_tma", "k_extract", "k_resolve", "k_emit", "k_route_hash",
+                            "k_memtable_cuts"]
     for name, lines in kernels.items():
         short = name.split("::")[-1].split("<")[0]
         if short not in want:

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Kernel-variant sweep on one GPU: generates the cfg2 workload once, then times the device-resident
 pipeline for each environment configuration (variants are read from the environment when an engine
-is created; `LIB=<variant>` selects a compile-time variant built by dbeel_b200/_build.py).  Usage: tools/tune.py "DBEEL_GATHER_TUNE=6" "DBEEL_GATHER_TUNE=16,DBEEL_MERGE=2" ..."""
+is created; `LIB=<variant>` selects a compile-time variant built by dbeel_b200/_build.py).  Usage: tools/tune.py "" "DBEEL_FUSED_FINAL=0" "DBEEL_EXTRACT_PERSIST=0,DBEEL_NARROW=0" "LIB=<variant>" ..."""
 import os
 import sys
 
