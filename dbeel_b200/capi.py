@@ -45,7 +45,8 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_murmur3_32", "dbeel_ring_owner", "dbeel_shard_ring", "dbeel_route_device", "dbeel_flush_many_sparse_device",
            "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream",
            "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device", "dbeel_scan_stream", "dbeel_get_values",
-           "dbeel_get_values_device", "dbeel_get_values_stream"]
+           "dbeel_get_values_device", "dbeel_get_values_stream", "dbeel_reader_open", "dbeel_reader_get_values",
+           "dbeel_reader_close"]
 
 
 class Run(C.Structure):
@@ -216,6 +217,14 @@ def lib():
         L.dbeel_get_values_stream.restype = C.c_int
         L.dbeel_get_values_stream.argtypes = [C.c_void_p, C.POINTER(Table), C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint64,
                                               C.c_uint32, C.POINTER(ScanIO), C.POINTER(Out), C.c_void_p]
+        L.dbeel_reader_open.restype = C.c_int
+        L.dbeel_reader_open.argtypes = [C.c_void_p, C.POINTER(Table), C.c_uint32, C.POINTER(ScanIO), C.c_uint64,
+                                        C.POINTER(C.c_void_p)]
+        L.dbeel_reader_get_values.restype = C.c_int
+        L.dbeel_reader_get_values.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.POINTER(Out),
+                                              C.c_void_p]
+        L.dbeel_reader_close.restype = None
+        L.dbeel_reader_close.argtypes = [C.c_void_p]
         L.dbeel_scan_bound.restype = C.c_int
         L.dbeel_scan_bound.argtypes = [C.POINTER(Table), C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         for name in ("dbeel_scan", "dbeel_scan_device"):
@@ -321,6 +330,131 @@ class PinnedBuffer:
     def __del__(self):
         try:
             self.free()
+        except Exception:
+            pass
+
+
+READER_FRAME_CAP = 64                  # DBEEL_READER_FRAME_CAP: longest key a reader's cached fences serve
+DEFAULT_READER_FENCE_BYTES = 64 << 20  # DBEEL_READER_FENCE_BYTES_DEFAULT
+
+
+class _StreamTables:
+    """The tables and the read callback of a streamed read: (data, index, bloom | None) oldest first.  Without `read` the
+    callback serves data / index from memory; with it, data / index may be sizes, and read(table, kind, offset, size)
+    returns the bytes (kind 1 = .data, 2 = .index; called from several engine threads) or a nonzero int error code.
+    Every read is logged as (table, kind, offset, size); fail_read_at = n makes the n-th read of a call return 4242."""
+
+    def __init__(self, tables, read=None):
+        import threading
+
+        def size_of(x):
+            return int(x) if isinstance(x, (int, np.integer)) else _u8(x).size
+        self.keep = [(None if read else _u8(d), None if read else _u8(i), _u8(b) if b is not None and len(b) else None)
+                     for d, i, b in tables]
+        self.sizes = [(size_of(d), size_of(i)) for d, i, _ in tables]
+        self.arr = (Table * max(1, len(self.keep)))()
+        for j, ((_, _, b), (ds, isz)) in enumerate(zip(self.keep, self.sizes)):
+            self.arr[j] = Table(None, ds, None, isz, b.ctypes.data if b is not None else None, b.size if b is not None else 0)
+        self.fail_read_at = -1
+        self.log = []
+        self.last_reads = []
+        mu = threading.Lock()
+        keep = self.keep
+
+        def rd(_ctx, table, kind_, offset, size, dst):
+            with mu:
+                k = len(self.log)
+                self.log.append((int(table), int(kind_), int(offset), int(size)))
+            if k == self.fail_read_at:
+                return 4242
+            if read is None:
+                src = keep[table][0] if kind_ == 1 else keep[table][1]
+                if offset + size > src.size:
+                    return 4243
+                C.memmove(dst, src.ctypes.data + offset, size)
+                return 0
+            got = read(int(table), int(kind_), int(offset), int(size))
+            if isinstance(got, (int, np.integer)):
+                return int(got)
+            b = np.ascontiguousarray(np.frombuffer(got, np.uint8) if isinstance(got, (bytes, bytearray)) else _u8(got))
+            if b.size != size:
+                return 4243
+            C.memmove(dst, b.ctypes.data, size)
+            return 0
+
+        self.io = ScanIO(STREAM_READ_FN(rd), C.cast(None, SCAN_WRITE_FN), None)
+
+
+def _stream_values(call, name: str, h, n_keys: int, st: Optional[_StreamTables], caps, data_cap: int = 0):
+    """One streamed get_values: call(out, rows) -> rc, with caps (data_cap, index_cap) or by default at most 64 MiB of
+    .data (the tables' sizes when known, else data_cap) and 16 bytes per key, retried once with the sizes the engine
+    reports.  Returns (rows, data, index); st.last_reads = the reads of the last call."""
+    res = np.zeros(n_keys, dtype=LOOKUP_DTYPE)
+    dc0 = sum(d for d, _ in st.sizes) if st is not None else data_cap
+    dc, ic = caps if caps is not None else (min(dc0, 64 << 20), 16 * n_keys)
+    for attempt in range(2):
+        od, oi = np.empty(max(1, dc), np.uint8), np.empty(max(1, ic), np.uint8)
+        out = Out(od.ctypes.data, dc, 0, oi.ctypes.data, ic, 0, None, 0, 0, 0)
+        if st is not None:
+            st.log.clear()
+        rc = call(out, res)
+        if st is not None:
+            st.last_reads = list(st.log)
+        if rc == 0:
+            return res, od[:out.data_len], oi[:out.index_len]
+        err = DbeelError(rc, f"{name}: {lib().dbeel_last_error(h).decode()}")
+        if rc == ERR_CAPACITY:
+            err.needed = (int(out.data_len), int(out.index_len))
+        if caps is not None or attempt or rc != ERR_CAPACITY:
+            raise err
+        dc, ic = err.needed
+
+
+class Reader:
+    """dbeel_reader_*: get_values_stream's batches on a fixed set of tables, with the filters and fences kept on the
+    device between batches (Engine.open_reader, storage_engine.LSMTree.open_reader).  Use it as a context manager or
+    close() it; the engine closes readers still open when it is destroyed."""
+
+    def __init__(self, handle: C.c_void_p, engine: "Engine", st: Optional[_StreamTables] = None, data_cap: int = 0):
+        self._h = handle
+        self._engine = engine
+        self._st = st
+        self._data_cap = data_cap
+        self.last_stream_reads = None if st is None else []
+
+    def get_values(self, keys: Sequence[bytes], mode: int = LOOKUP_REFERENCE, caps: Optional[Tuple[int, int]] = None,
+                   fail_read_at: int = -1):
+        """What get_values_stream returns for the same tables, keys and mode: (rows, data, index).  last_stream_reads lists
+        this call's reads (readers of an engine's tables; None for a tree's); fail_read_at as in get_values_stream."""
+        if not self._h:
+            raise ValueError("reader is closed")
+        blob, off = pack_keys(keys)
+        if self._st is not None:
+            self._st.fail_read_at = fail_read_at
+
+        def call(out, res):
+            return lib().dbeel_reader_get_values(self._h, blob.ctypes.data if blob.size else None, off.ctypes.data, len(keys),
+                                                 mode, C.byref(out), res.ctypes.data)
+        try:
+            return _stream_values(call, "dbeel_reader_get_values", self._engine._h, len(keys), self._st, caps, self._data_cap)
+        finally:
+            if self._st is not None:
+                self.last_stream_reads = self._st.last_reads
+
+    def close(self):
+        if self._h and self._engine._h:  # an engine already destroyed has closed its readers
+            lib().dbeel_reader_close(self._h)
+        self._h = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
         except Exception:
             pass
 
@@ -667,58 +801,27 @@ class Engine:
         .data, 2 = .index; called from several engine threads) or a nonzero int error code.  fail_read_at = n makes the n-th
         read return 4242 (tests).  last_stream_reads lists every (table, kind, offset, size) read.  Returns (rows, data,
         index); caps as in get_values (by default at most 64 MiB of .data, retried once with the sizes needed)."""
-        def size_of(x):
-            return int(x) if isinstance(x, (int, np.integer)) else _u8(x).size
-        keep = [(None if read else _u8(d), None if read else _u8(i), _u8(b) if b is not None and len(b) else None)
-                for d, i, b in tables]
-        sizes = [(size_of(d), size_of(i)) for d, i, _ in tables]
-        arr = (Table * max(1, len(keep)))()
-        for j, ((_, _, b), (ds, isz)) in enumerate(zip(keep, sizes)):
-            arr[j] = Table(None, ds, None, isz, b.ctypes.data if b is not None else None, b.size if b is not None else 0)
+        st = _StreamTables(tables, read)
+        st.fail_read_at = fail_read_at
         blob, off = pack_keys(keys)
-        res = np.zeros(len(keys), dtype=LOOKUP_DTYPE)
-        import threading
-        mu = threading.Lock()
-        log = []
 
-        def rd(_ctx, table, kind_, offset, size, dst):
-            with mu:
-                k = len(log)
-                log.append((int(table), int(kind_), int(offset), int(size)))
-            if k == fail_read_at:
-                return 4242
-            if read is None:
-                src = keep[table][0] if kind_ == 1 else keep[table][1]
-                if offset + size > src.size:
-                    return 4243
-                C.memmove(dst, src.ctypes.data + offset, size)
-                return 0
-            got = read(int(table), int(kind_), int(offset), int(size))
-            if isinstance(got, (int, np.integer)):
-                return int(got)
-            b = np.ascontiguousarray(np.frombuffer(got, np.uint8) if isinstance(got, (bytes, bytearray)) else _u8(got))
-            if b.size != size:
-                return 4243
-            C.memmove(dst, b.ctypes.data, size)
-            return 0
+        def call(out, res):
+            return lib().dbeel_get_values_stream(self._h, st.arr, len(st.keep), blob.ctypes.data if blob.size else None,
+                                                 off.ctypes.data, len(keys), mode, C.byref(st.io), C.byref(out), res.ctypes.data)
+        try:
+            return _stream_values(call, "dbeel_get_values_stream", self._h, len(keys), st, caps)
+        finally:
+            self.last_stream_reads = st.last_reads
 
-        io = ScanIO(STREAM_READ_FN(rd), C.cast(None, SCAN_WRITE_FN), None)
-        dc, ic = caps if caps is not None else (min(sum(d for d, _ in sizes), 64 << 20), 16 * len(keys))
-        for attempt in range(2):
-            od, oi = np.empty(max(1, dc), np.uint8), np.empty(max(1, ic), np.uint8)
-            out = Out(od.ctypes.data, dc, 0, oi.ctypes.data, ic, 0, None, 0, 0, 0)
-            log.clear()
-            rc = lib().dbeel_get_values_stream(self._h, arr, len(keep), blob.ctypes.data if blob.size else None, off.ctypes.data,
-                                               len(keys), mode, C.byref(io), C.byref(out), res.ctypes.data)
-            self.last_stream_reads = list(log)
-            if rc == 0:
-                return res, od[:out.data_len], oi[:out.index_len]
-            err = DbeelError(rc, f"dbeel_get_values_stream: {lib().dbeel_last_error(self._h).decode()}")
-            if rc == ERR_CAPACITY:
-                err.needed = (int(out.data_len), int(out.index_len))
-            if caps is not None or attempt or rc != ERR_CAPACITY:
-                raise err
-            dc, ic = err.needed
+    def open_reader(self, tables: Sequence[Tuple[object, object, object]], read=None, fence_bytes: int = 0) -> "Reader":
+        """dbeel_reader_open: a Reader that answers get_values_stream's batches on these tables, with every .bloom on the
+        device from now on and each table's fences kept there after the first batch in a mode reaches it.  tables / read
+        as in get_values_stream; fence_bytes = device bytes for fences (0 = DEFAULT_READER_FENCE_BYTES)."""
+        st = _StreamTables(tables, read)
+        h = C.c_void_p()
+        self._check(lib().dbeel_reader_open(self._h, st.arr, len(st.keep), C.byref(st.io), fence_bytes, C.byref(h)),
+                    "dbeel_reader_open")
+        return Reader(h, self, st)
 
     def get_values_device(self, tables: Sequence[Tuple[int, int, int, int, int, int]], keys_ptr: int, offsets_ptr: int,
                           n_keys: int, results_ptr: int, out_ptrs: Tuple[int, int, int, int],

@@ -28,6 +28,7 @@
 #include "route.cuh"
 #include "scan.cuh"
 #include "wal.cuh"
+#include "host/reader_tables.h"
 #include "host/scan_plan.h"
 #include "host/stream_pump.h"
 
@@ -77,6 +78,7 @@ struct dbeel_engine {
     dbeel_stats stats = {};
     std::string err;
     bool busy = false;
+    std::vector<dbeel_reader *> readers; // open readers (dbeel_reader_open, dbeel_tree_reader_open): closed with the engine
     // asynchronous jobs (dbeel_compact_submit)
     std::thread worker;
     std::atomic<int> async_state{0}; // 0 idle, 1 running, 2 finished (status in async_status)
@@ -2217,13 +2219,126 @@ int gvs_read(dbeel_engine *e, const dbeel_scan_io *io, uint32_t t, uint32_t kind
     return parallel_pieces(ps.size(), [&](size_t k) { return io->read(io->ctx, t, kind, ps[k].off, ps[k].len, ps[k].dst); });
 }
 
+// The fences of the open internal nodes of pt, through the callback: their index records (runs closer than
+// kLookupMergeGap as one read) into fix[k], then their key frames of up to max_klen key bytes (runs that touch as one
+// read) into ring_in, staged from `base` on (sf).  has[k]: node k's record points inside .data and its frame is frame[k].
+struct GvsFenceReads {
+    std::vector<uint4> fix;
+    std::vector<ByteRange> frame;
+    std::vector<uint8_t> has;
+    GvsStaged sf;
+};
+
+int gvs_read_fences(dbeel_engine *e, const dbeel_scan_io *io, uint32_t ti, const ProbeTree &pt, uint64_t data_len, uint64_t max_klen,
+                    uint64_t base, GvsFenceReads *f) {
+    const uint32_t mode = pt.mode;
+    const uint64_t leaf0 = 1ull << pt.depth;
+    int rc;
+    std::vector<ByteRange> ir;
+    for (uint64_t k = 1; k < leaf0; k++)
+        if (pt.open[k]) { const uint64_t p = search_pos(mode, pt.state[k]); ir.push_back({16 * p, 16 * p + 16}); }
+    const GvsStaged si = gvs_stage(ir, kLookupMergeGap, 0);
+    if ((rc = ensure_host(e, &e->ring_out, &e->ring_out_cap, si.end))) return rc;
+    if ((rc = gvs_read(e, io, ti, DBEEL_STREAM_INDEX, si, e->ring_out))) return fail(e, rc, "stream read callback failed (.index, fences)");
+    f->fix.assign(leaf0, make_uint4(0, 0, 0, 0));
+    f->has.assign(leaf0, 0);
+    f->frame.assign(leaf0, ByteRange{0, 0});
+    std::vector<ByteRange> fr;
+    for (uint64_t k = 1; k < leaf0; k++) {
+        if (!pt.open[k]) continue;
+        memcpy(&f->fix[k], e->ring_out + si.at(16 * search_pos(mode, pt.state[k])), 16);
+        if (probe_frame(reinterpret_cast<const uint8_t *>(&f->fix[k]), data_len, max_klen, &f->frame[k])) { f->has[k] = 1; fr.push_back(f->frame[k]); }
+    }
+    f->sf = gvs_stage(fr, 0, base);
+    if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, f->sf.end))) return rc;
+    if ((rc = gvs_read(e, io, ti, DBEEL_STREAM_DATA, f->sf, e->ring_in))) return fail(e, rc, "stream read callback failed (.data, fences)");
+    return DBEEL_OK;
+}
+
+// node k's frame address: its staged frame at `frame` (host view `host`), or 0 when its length prefix runs past .data
+// (as probe(): the record is reported corrupt)
+inline unsigned long long gvs_frame_addr(const GvsFenceReads &f, uint64_t k, uint64_t data_len, const uint8_t *host, const uint8_t *dev) {
+    if (!f.has[k] || rd64(host) > data_len - f.frame[k].lo - 8) return 0;
+    return reinterpret_cast<unsigned long long>(dev);
+}
+
+} // namespace
+
+// ---- readers (dbeel_reader_*): what dbeel_get_values_stream would read again on every call, kept on the device
+// One table of a reader (a tree shares it between its readers): the filter, uploaded when the table is created, and per
+// mode the fences of the top `depth` levels (host/lookup_plan.h), read the first time a batch in that mode reaches it.
+struct dbeel_reader_table {
+    int device = 0;
+    TableDesc desc = {};      // data / index unset; words -> the resident filter, or nullptr
+    uint8_t *bloom_dev = nullptr;
+    int32_t depth = -1;       // D_t: chosen by the first reader that includes the table, kept after
+    struct Fences {
+        bool loaded = false;
+        ProbeTree pt;         // the leaves' intervals (the node states of the cached levels)
+        uint8_t *dev = nullptr; // fix[2^depth] | ffr[2^depth] | frame slots (kReaderFrameSlot bytes per node)
+    } fences[2];
+    ~dbeel_reader_table() {
+        cudaSetDevice(device);
+        if (bloom_dev) cudaFree(bloom_dev);
+        for (auto &f : fences)
+            if (f.dev) cudaFree(f.dev);
+    }
+};
+
+struct dbeel_reader {
+    dbeel_engine *e = nullptr;
+    std::vector<ReaderTableRef> tables;
+    dbeel_scan_io io = {};
+    std::shared_ptr<void> owner; // what io.ctx points at, when the reader owns it (tree readers)
+};
+
+namespace {
+
+// Reads the fences of reader table rt (table ti of the batch) in `mode` at its depth, into its own device block.  The
+// frames hold at most kReaderFrameCap key bytes.  The host image goes down from ring_out, which the leaf groups refill
+// only after the touched read-back has synchronised the stream.
+int reader_load_fences(dbeel_engine *e, const dbeel_scan_io *io, uint32_t ti, dbeel_reader_table *rt, uint32_t mode) {
+    dbeel_reader_table::Fences &c = rt->fences[mode];
+    plan_probe_tree(mode, rt->desc.n, (uint32_t)rt->depth, &c.pt);
+    const uint64_t leaf0 = 1ull << rt->depth, data_len = rt->desc.data_len;
+    if (rt->depth > 0) {
+        GvsFenceReads fr;
+        int rc = gvs_read_fences(e, io, ti, c.pt, data_len, kReaderFrameCap, 0, &fr);
+        if (rc) return rc;
+        const uint64_t o_ffr = 16 * leaf0, o_slot = o_ffr + 8 * leaf0, bytes = o_slot + kReaderFrameSlot * leaf0;
+        if ((rc = ensure_host(e, &e->ring_out, &e->ring_out_cap, bytes))) return rc;
+        if (c.dev) cudaFree(c.dev); // a load whose copy failed
+        if (cudaMalloc(reinterpret_cast<void **>(&c.dev), bytes) != cudaSuccess) {
+            cudaGetLastError();
+            c.dev = nullptr;
+            return fail(e, DBEEL_ERR_NOMEM, "cudaMalloc(reader fences)");
+        }
+        uint8_t *img = e->ring_out;
+        memset(img + o_slot, 0, kReaderFrameSlot * leaf0);
+        memcpy(img, fr.fix.data(), 16 * leaf0);
+        unsigned long long *ffr = reinterpret_cast<unsigned long long *>(img + o_ffr);
+        for (uint64_t k = 0; k < leaf0; k++) {
+            uint8_t *slot = img + o_slot + kReaderFrameSlot * k;
+            if (fr.has[k]) memcpy(slot, e->ring_in + fr.sf.at(fr.frame[k].lo), fr.frame[k].hi - fr.frame[k].lo);
+            ffr[k] = gvs_frame_addr(fr, k, data_len, slot, c.dev + o_slot + kReaderFrameSlot * k);
+        }
+        CU(cudaMemcpyAsync(c.dev, img, bytes, cudaMemcpyHostToDevice, e->stream));
+    }
+    c.loaded = true;
+    return DBEEL_OK;
+}
+
 // Per table, newest first: k_gvs_filter -> fences read, k_lookup_fence -> touched leaves read in groups under the partition
 // budget, k_lookup_leaf per group and k_gvs_copy for the group's hits (their entries leave the window for the hit heap).
 // Then the entries of hits at fences are read into the heap, k_gvs_hit decodes every hit and split_emit writes `out` in
 // query order, as dbeel_get_values does.  Every phase ends in a stream synchronise before its pinned
 // buffers are refilled.
+// With a reader, the filters are already on the device and a table whose cached fences serve the batch
+// (reader_uses_cache) descends them instead of reading its fences; when the depth the batch wants cannot exceed the cached
+// one for any number of open queries, k_gvs_filter and k_lookup_fence go back to back with no read-back between them.
 int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys, const uint64_t *key_off,
-                            uint64_t n_keys, uint32_t mode, const dbeel_scan_io *io, dbeel_out *out, dbeel_lookup_result *results) {
+                            uint64_t n_keys, uint32_t mode, const dbeel_scan_io *io, dbeel_out *out, dbeel_lookup_result *results,
+                            dbeel_reader *reader = nullptr) {
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!out || !io || !io->read) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     if (const int arc = lookup_args(e, tables, n_tables, key_off, n_keys, mode, results)) return arc;
@@ -2271,6 +2386,7 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
     for (uint32_t i = 0; i < n_tables; i++) {
         const dbeel_table &t = tables[i];
         td[i] = TableDesc{nullptr, t.data_len, nullptr, t.index_len / DBEEL_INDEX_ENTRY_SIZE, nullptr, 0, 0, 0, 0, {0, 0, 0, 0}};
+        if (reader) td[i] = reader->tables[i]->desc; // tables[] carries no filter: it is resident
         if (!t.bloom_len) continue;
         const uint8_t *b = static_cast<const uint8_t *>(t.bloom);
         if ((rc = parse_bloom(e, b, b + t.bloom_len - kBloomTrailer, t.bloom_len, &td[i]))) return rc;
@@ -2315,49 +2431,53 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
     for (uint32_t ti = n_tables; ti-- > 0;) { // sstables.iter().rev(): newest first
         const TableDesc &t = td[ti];
         const uint64_t data_len = t.data_len, nrec = t.n;
+        dbeel_reader_table *rt = reader ? reader->tables[ti].get() : nullptr;
+        dbeel_reader_table::Fences *cache = rt ? &rt->fences[mode] : nullptr;
+        const uint32_t cached_depth = rt ? (uint32_t)rt->depth : 0;
+        // whether the cached fences serve the batch, decided before the filter runs when no count of open queries can
+        // change it: the depth the batch wants grows with that count, which is at most n_keys
+        bool use_cache = cache && cache->loaded && cached_depth > 0 &&
+                         reader_uses_cache(max_klen, lookup_depth(n_keys, nrec, data_len, 8 + max_klen, budget), cached_depth);
         CU(cudaMemsetAsync(d_cnt, 0, 8, s));
         launch_k(e, k_gvs_filter, grid, 256, 0, s, gq, t, d_cnt);
-        CU(cudaMemcpyAsync(e->pin, d_cnt, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
         launches++;
-        const uint64_t m = rd64(e->pin);
-        if (m == 0) continue; // no query reaches the table: nothing of it is read
-        const uint32_t depth = lookup_depth(m, nrec, data_len, 8 + max_klen, budget);
-        ProbeTree pt;
-        plan_probe_tree(mode, nrec, depth, &pt);
+        uint32_t depth = cached_depth;
+        if (!use_cache) {
+            CU(cudaMemcpyAsync(e->pin, d_cnt, 8, cudaMemcpyDeviceToHost, s));
+            CU(cudaStreamSynchronize(s));
+            const uint64_t m = rd64(e->pin);
+            if (m == 0) continue; // no query reaches the table: nothing of it is read
+            depth = lookup_depth(m, nrec, data_len, 8 + max_klen, budget);
+            use_cache = cache && reader_uses_cache(max_klen, depth, cached_depth);
+            if (use_cache) {
+                depth = cached_depth;
+                if (!cache->loaded && (rc = reader_load_fences(e, io, ti, rt, mode))) return rc;
+            }
+        }
+        ProbeTree pt_call;
+        if (!use_cache) plan_probe_tree(mode, nrec, depth, &pt_call);
+        const ProbeTree &pt = use_cache ? cache->pt : pt_call;
         const uint64_t leaf0 = 1ull << depth;
         CU(cudaMemsetAsync(d_touched, 0, leaf0, s));
 
-        // ---- fences: the index records of the open internal nodes, then their key frames
-        if (depth > 0) {
-            std::vector<ByteRange> ir;
-            for (uint64_t k = 1; k < leaf0; k++)
-                if (pt.open[k]) { const uint64_t p = search_pos(mode, pt.state[k]); ir.push_back({16 * p, 16 * p + 16}); }
-            const GvsStaged si = gvs_stage(ir, kLookupMergeGap, 0);
-            if ((rc = ensure_host(e, &e->ring_out, &e->ring_out_cap, si.end))) return rc;
-            if ((rc = gvs_read(e, io, ti, DBEEL_STREAM_INDEX, si, e->ring_out))) return fail(e, rc, "stream read callback failed (.index, fences)");
-            std::vector<uint4> fix(leaf0, make_uint4(0, 0, 0, 0));
-            std::vector<ByteRange> fr;
-            std::vector<uint8_t> has(leaf0, 0);
-            std::vector<ByteRange> frame(leaf0);
-            for (uint64_t k = 1; k < leaf0; k++) {
-                if (!pt.open[k]) continue;
-                memcpy(&fix[k], e->ring_out + si.at(16 * search_pos(mode, pt.state[k])), 16);
-                if (probe_frame(reinterpret_cast<const uint8_t *>(&fix[k]), data_len, max_klen, &frame[k])) { has[k] = 1; fr.push_back(frame[k]); }
-            }
+        // ---- fences: the index records of the open internal nodes, then their key frames (or the reader's copies)
+        if (depth > 0 && use_cache) {
+            GvsFences gf{reinterpret_cast<const uint4 *>(cache->dev), reinterpret_cast<const unsigned long long *>(cache->dev + 16 * leaf0),
+                         depth, ti, nrec, d_touched};
+            launch_k(e, k_lookup_fence, grid, 256, 0, s, gq, gf);
+            launches++;
+        } else if (depth > 0) {
             const uint64_t o_fix = 0, o_ffr = align_up(16 * leaf0, kAlign);
-            const GvsStaged sf = gvs_stage(fr, 0, align_up(o_ffr + 8 * leaf0, kAlign));
-            if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, sf.end))) return rc;
+            GvsFenceReads fr;
+            if ((rc = gvs_read_fences(e, io, ti, pt, data_len, max_klen, align_up(o_ffr + 8 * leaf0, kAlign), &fr))) return rc;
+            const GvsStaged &sf = fr.sf;
             if ((rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, sf.end))) return rc;
-            if ((rc = gvs_read(e, io, ti, DBEEL_STREAM_DATA, sf, e->ring_in))) return fail(e, rc, "stream read callback failed (.data, fences)");
             uint8_t *img = e->ring_in;
-            memcpy(img + o_fix, fix.data(), 16 * leaf0);
+            memcpy(img + o_fix, fr.fix.data(), 16 * leaf0);
             unsigned long long *ffr = reinterpret_cast<unsigned long long *>(img + o_ffr);
             for (uint64_t k = 0; k < leaf0; k++) {
-                ffr[k] = 0;
-                if (!has[k]) continue;
-                const uint64_t p = sf.at(frame[k].lo), cur_klen = rd64(img + p);
-                if (cur_klen <= data_len - frame[k].lo - 8) ffr[k] = reinterpret_cast<unsigned long long>(e->stage_in + p); // else as probe(): corrupt
+                const uint64_t p = fr.has[k] ? sf.at(fr.frame[k].lo) : 0;
+                ffr[k] = gvs_frame_addr(fr, k, data_len, img + p, e->stage_in + p);
             }
             CU(cudaMemcpyAsync(e->stage_in, img, sf.end, cudaMemcpyHostToDevice, s));
             GvsFences gf{reinterpret_cast<const uint4 *>(e->stage_in + o_fix), reinterpret_cast<const unsigned long long *>(e->stage_in + o_ffr),
@@ -2801,6 +2921,66 @@ int scan_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tab
 
 } // namespace
 
+namespace dbeel {
+
+int reader_table_create(dbeel_engine *e, const dbeel_table &t, ReaderTableRef *out) {
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    // the table checks of dbeel_get_values_stream, and its filter parsed as there
+    if (t.index_len % DBEEL_INDEX_ENTRY_SIZE) return fail(e, DBEEL_ERR_INVALID_ARG, "index length is not a multiple of 16");
+    if (t.bloom_len && !t.bloom) return fail(e, DBEEL_ERR_INVALID_ARG, "null table buffer");
+    if (t.bloom_len && (t.bloom_len < 8 + kBloomTrailer || (t.bloom_len - 8 - kBloomTrailer) % 4))
+        return fail(e, DBEEL_ERR_BAD_BLOOM, "bloom file length is not 8 + 4 * words + 164");
+    auto rt = std::make_shared<dbeel_reader_table>();
+    rt->device = e->device;
+    rt->desc = TableDesc{nullptr, t.data_len, nullptr, t.index_len / DBEEL_INDEX_ENTRY_SIZE, nullptr, 0, 0, 0, 0, {0, 0, 0, 0}};
+    if (t.bloom_len) {
+        const uint8_t *b = static_cast<const uint8_t *>(t.bloom);
+        if (const int rc = parse_bloom(e, b, b + t.bloom_len - kBloomTrailer, t.bloom_len, &rt->desc)) return rc;
+        CU(cudaSetDevice(e->device));
+        if (cudaMalloc(reinterpret_cast<void **>(&rt->bloom_dev), t.bloom_len) != cudaSuccess) {
+            cudaGetLastError();
+            rt->bloom_dev = nullptr;
+            return fail(e, DBEEL_ERR_NOMEM, "cudaMalloc(reader filter)");
+        }
+        CU(cudaMemcpy(rt->bloom_dev, b, t.bloom_len, cudaMemcpyHostToDevice));
+        rt->desc.words = reinterpret_cast<const uint32_t *>(rt->bloom_dev + 8);
+    }
+    *out = std::move(rt);
+    return DBEEL_OK;
+}
+
+int reader_open_tables(dbeel_engine *e, std::vector<ReaderTableRef> tables, const dbeel_scan_io &io, uint64_t fence_bytes,
+                       std::shared_ptr<void> owner, dbeel_reader **out) {
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (!out || !io.read) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    if (tables.size() > 65536) return fail(e, DBEEL_ERR_TOO_MANY_RUNS, "more than 65536 tables");
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    const size_t nt = tables.size();
+    std::vector<uint64_t> n(nt), data_len(nt);
+    std::vector<int32_t> fixed(nt);
+    for (size_t i = 0; i < nt; i++) {
+        n[i] = tables[i]->desc.n;
+        data_len[i] = tables[i]->desc.data_len;
+        fixed[i] = tables[i]->depth;
+    }
+    const std::vector<uint32_t> d = reader_depths(n, data_len, fixed, fence_bytes);
+    for (size_t i = 0; i < nt; i++)
+        if (tables[i]->depth < 0) tables[i]->depth = (int32_t)d[i];
+    dbeel_reader *r = new (std::nothrow) dbeel_reader();
+    if (!r) return fail(e, DBEEL_ERR_NOMEM, "reader");
+    r->e = e;
+    r->tables = std::move(tables);
+    r->io = io;
+    r->owner = std::move(owner);
+    e->readers.push_back(r);
+    *out = r;
+    return DBEEL_OK;
+}
+
+} // namespace dbeel
+
 // ------------------------------------------------------------------------------------ C ABI
 
 extern "C" {
@@ -2865,6 +3045,8 @@ void dbeel_engine_destroy(dbeel_engine *e) {
     if (e->worker.joinable()) e->worker.join();
     cudaSetDevice(e->device);
     if (e->stream) cudaStreamSynchronize(e->stream);
+    for (dbeel_reader *r : e->readers) delete r; // the tables a tree still shares stay with the tree
+    e->readers.clear();
     for (int i = 0; i < EV_COUNT; i++)
         if (e->ev[i]) cudaEventDestroy(e->ev[i]);
     if (e->ws) cudaFree(e->ws);
@@ -3111,6 +3293,40 @@ int dbeel_get_values_stream(dbeel_engine *e, const dbeel_table *tables, uint32_t
                             dbeel_out *out, dbeel_lookup_result *results) {
     REFUSE_WHILE_ASYNC(e);
     return get_values_stream_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, io, out, results);
+}
+
+int dbeel_reader_open(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const dbeel_scan_io *io, uint64_t fence_bytes,
+                      dbeel_reader **out) {
+    REFUSE_WHILE_ASYNC(e);
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (!out || !io || !io->read) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    *out = nullptr;
+    if (const int arc = lookup_args(e, tables, n_tables, nullptr, 0, DBEEL_LOOKUP_REFERENCE, nullptr)) return arc;
+    e->err.clear();
+    std::vector<ReaderTableRef> rts(n_tables);
+    for (uint32_t i = 0; i < n_tables; i++)
+        if (const int rc = reader_table_create(e, tables[i], &rts[i])) return rc;
+    return reader_open_tables(e, std::move(rts), *io, fence_bytes, nullptr, out);
+}
+
+int dbeel_reader_get_values(dbeel_reader *r, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
+                            dbeel_out *out, dbeel_lookup_result *results) {
+    if (!r) return DBEEL_ERR_INVALID_ARG;
+    REFUSE_WHILE_ASYNC(r->e);
+    std::vector<dbeel_table> tables(r->tables.size());
+    for (size_t i = 0; i < tables.size(); i++) {
+        const TableDesc &d = r->tables[i]->desc;
+        tables[i] = dbeel_table{nullptr, d.data_len, nullptr, d.n * DBEEL_INDEX_ENTRY_SIZE, nullptr, 0};
+    }
+    return get_values_stream_entry(r->e, tables.data(), (uint32_t)tables.size(), keys, key_offsets, n_keys, mode, &r->io, out, results, r);
+}
+
+void dbeel_reader_close(dbeel_reader *r) {
+    if (!r) return;
+    auto &v = r->e->readers;
+    v.erase(std::remove(v.begin(), v.end(), r), v.end());
+    cudaSetDevice(r->e->device);
+    delete r;
 }
 
 int dbeel_scan_bound(const dbeel_table *tables, uint32_t n_tables, uint64_t *data_cap, uint64_t *index_cap) {

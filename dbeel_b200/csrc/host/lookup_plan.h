@@ -98,10 +98,15 @@ inline void plan_probe_tree(uint32_t mode, uint64_t n, uint32_t depth, ProbeTree
 // balances the fence reads against m leaf windows of data_len / 2^D bytes; at least deep enough that a leaf is a quarter
 // of the budget, never deeper than the tree (log2 n) or kLookupMaxDepth, and the fences (index record + key frame of up to
 // frame_bytes each) stay within half the budget.
+inline uint32_t lookup_max_depth(uint64_t n) { // floor(log2 n), at most kLookupMaxDepth
+    uint32_t d = 0;
+    while (d < kLookupMaxDepth && (2ull << d) <= n) d++;
+    return d;
+}
+
 inline uint32_t lookup_depth(uint64_t m, uint64_t n, uint64_t data_len, uint64_t frame_bytes, uint64_t budget) {
     if (n < 2 || m == 0) return 0;
-    uint32_t dmax = 0;
-    while (dmax < kLookupMaxDepth && (2ull << dmax) <= n) dmax++;
+    const uint32_t dmax = lookup_max_depth(n);
     const double want = 0.5 * std::log2(std::max(1.0, (double)m * (double)data_len / (double)kLookupFenceCost));
     uint32_t d = (uint32_t)std::min<double>(dmax, std::ceil(want));
     while (d < dmax && (data_len >> d) > budget / 4) d++;
@@ -165,6 +170,66 @@ inline bool leaf_window(const uint8_t *slice, uint64_t count, uint64_t data_len,
         out->hi = std::max(out->hi, f.hi);
     }
     return any;
+}
+
+// ---- readers (dbeel_reader_*): fences kept on the device across batches
+//
+// A reader keeps, per table and mode, the fences of the top D_t levels of the probe tree: for every node k < 2^D_t its
+// index record fix[k] (16 bytes), its frame address ffr[k] (8 bytes) and a frame slot of kReaderFrameSlot bytes.  Node
+// k's state depends only on k, the mode and n (plan_probe_tree), never on the batch, so the set is read once and serves
+// every later batch.  A cached frame holds the length prefix and at most kReaderFrameCap key bytes: cmp_key_bytes reads no
+// more than min(fence key length, query key length) key bytes, so for a query of at most kReaderFrameCap bytes the
+// truncated frame gives the comparison the whole key gives.  The "corrupt" decision (ffr = 0) depends only on the record
+// and the length prefix, so it is cached as is.
+constexpr uint64_t kReaderFrameCap = 64;
+constexpr uint64_t kReaderFrameSlot = (8 + kReaderFrameCap + 15) / 16 * 16;
+constexpr uint64_t kReaderNodeBytes = 16 + 8 + kReaderFrameSlot; // one node of one mode
+constexpr uint64_t kReaderFenceBytesDefault = 64ull << 20;
+
+// device bytes of one table's fences at depth d in both modes
+inline uint64_t reader_fence_bytes(uint32_t d) { return d ? (2 * kReaderNodeBytes) << d : 0; }
+
+// D_t for tables of n[t] records and data_len[t] bytes.  fixed[t] >= 0 is a depth chosen before (a table a reader shares
+// with another keeps its fences), counted against the budget.  The rest of fence_bytes (0 = kReaderFenceBytesDefault)
+// goes one level at a time to the table whose leaves are largest, (data_len + 16 n) >> D, ties to the lower position,
+// while its next level fits; no table goes deeper than lookup_max_depth(n).  So the tables' fences fit fence_bytes
+// whenever the fixed ones do.
+inline std::vector<uint32_t> reader_depths(const std::vector<uint64_t> &n, const std::vector<uint64_t> &data_len,
+                                           const std::vector<int32_t> &fixed, uint64_t fence_bytes) {
+    const size_t nt = n.size();
+    uint64_t left = fence_bytes ? fence_bytes : kReaderFenceBytesDefault;
+    std::vector<uint32_t> d(nt, 0);
+    std::vector<size_t> open;
+    for (size_t t = 0; t < nt; t++) {
+        if (fixed[t] >= 0) {
+            d[t] = (uint32_t)fixed[t];
+            left -= std::min(left, reader_fence_bytes(d[t]));
+        } else {
+            open.push_back(t);
+        }
+    }
+    auto leaf = [&](size_t t) { return (data_len[t] + 16 * n[t]) >> d[t]; };
+    auto later = [&](size_t a, size_t b) { return leaf(a) < leaf(b) || (leaf(a) == leaf(b) && a > b); };
+    std::make_heap(open.begin(), open.end(), later);
+    while (!open.empty()) {
+        std::pop_heap(open.begin(), open.end(), later);
+        const size_t t = open.back();
+        open.pop_back();
+        const uint64_t step = reader_fence_bytes(d[t] + 1) - reader_fence_bytes(d[t]);
+        if (d[t] >= lookup_max_depth(n[t]) || step > left) continue; // the budget only shrinks: it never fits later
+        left -= step;
+        d[t]++;
+        open.push_back(t);
+        std::push_heap(open.begin(), open.end(), later);
+    }
+    return d;
+}
+
+// A batch descends a table's cached fences when its longest key fits the cached frames and the depth it would read per
+// call (lookup_depth) is at most D_t; it then descends all D_t levels (deeper fences cost nothing once cached and make
+// the leaves smaller).  Otherwise that table's fences are read for this batch, as dbeel_get_values_stream reads them.
+inline bool reader_uses_cache(uint64_t max_klen, uint32_t want_depth, uint32_t cached_depth) {
+    return max_klen <= kReaderFrameCap && want_depth <= cached_depth;
 }
 
 } // namespace dbeel

@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../../include/dbeel_tree.h"
+#include "reader_tables.h"
 #include "../device_fns.cuh" // the scalar arithmetic the kernels use, compiled for the host here (murmur3_32, ring_owner)
 
 namespace fs = std::filesystem;
@@ -87,6 +88,21 @@ bool get_path(const std::string &b, size_t &pos, std::string *p) {
     return true;
 }
 
+// One SSTable as the tree's readers hold it: the engine's resident part (filter, fences) and the descriptors of its .data
+// and .index, opened when the first reader that includes it is opened.  The descriptors keep the files readable after a
+// compaction unlinks them, for as long as a reader holds the entry.
+struct ReaderEntry {
+    dbeel::ReaderTableRef dev;
+    int data_fd = -1, index_fd = -1;
+    ReaderEntry() = default;
+    ReaderEntry(const ReaderEntry &) = delete;
+    ReaderEntry &operator=(const ReaderEntry &) = delete;
+    ~ReaderEntry() {
+        if (data_fd >= 0) close(data_fd);
+        if (index_fd >= 0) close(index_fd);
+    }
+};
+
 } // namespace
 
 struct dbeel_tree {
@@ -98,6 +114,9 @@ struct dbeel_tree {
     std::string err;
     dbeel_page_sink page_sink = nullptr; // EntryWriter's page-cache write-through (entry_writer.rs:94-156), if the caller wants it
     void *page_ctx = nullptr;
+    // reader entries of the tables in `sstables`, by index; readers hold theirs by reference, so an entry whose table has
+    // left the tree lives exactly as long as the last reader that includes it
+    std::map<uint64_t, std::shared_ptr<ReaderEntry>> readers;
 };
 
 namespace {
@@ -105,6 +124,15 @@ namespace {
 int io_fail(dbeel_tree *t, const std::string &what) {
     t->err = what + ": " + strerror(errno);
     return DBEEL_ERR_IO;
+}
+
+// the tree lets go of the reader entries of tables that have left it (open readers keep theirs)
+void drop_left_tables(dbeel_tree *t) {
+    for (auto it = t->readers.begin(); it != t->readers.end();) {
+        const uint64_t idx = it->first;
+        const bool kept = std::any_of(t->sstables.begin(), t->sstables.end(), [idx](const SSTable &s) { return s.index == idx; });
+        it = kept ? std::next(it) : t->readers.erase(it);
+    }
 }
 
 // File <-> pinned memory in 32 MiB pieces spread over a few threads (pread / pwrite): one thread moves a RAM-resident
@@ -352,6 +380,7 @@ static int commit_written(dbeel_tree *t, const uint64_t *indices_to_compact, uin
     next.push_back({output_index, items_written});
     std::sort(next.begin(), next.end(), [](const SSTable &a, const SSTable &b) { return a.index < b.index; });
     t->sstables.swap(next);
+    drop_left_tables(t);
     // lsm_tree.rs:1147-1153: delete the inputs, then the journal
     for (auto &d : action.deletes)
         if (exists(d)) unlink(d.c_str());
@@ -738,6 +767,64 @@ int dbeel_tree_get_values_stream(dbeel_tree *t, const void *keys, const uint64_t
     const int rc = dbeel_get_values_stream(t->engine, tables.data(), (uint32_t)n, keys, key_offsets, n_keys, mode, &io, out, results);
     if (rc == DBEEL_ERR_IO && f.saved_errno.load()) { errno = f.saved_errno.load(); io_fail(t, "streamed read"); }
     else if (rc) t->err = dbeel_last_error(t->engine);
+    return rc;
+}
+
+namespace {
+struct ReaderFiles { // a tree reader's snapshot: the entries of its tables, in dbeel_tree_sstables() order
+    std::vector<std::shared_ptr<ReaderEntry>> tables;
+};
+int reader_read(void *ctx, uint32_t table, uint32_t kind, uint64_t off, uint64_t len, void *dst) {
+    const ReaderEntry &r = *static_cast<ReaderFiles *>(ctx)->tables[table];
+    const int fd = kind == DBEEL_STREAM_DATA ? r.data_fd : r.index_fd;
+    uint8_t *p = static_cast<uint8_t *>(dst);
+    while (len) {
+        const ssize_t got = pread(fd, p, len, (off_t)off);
+        if (got < 0 && errno == EINTR) continue;
+        if (got <= 0) return DBEEL_ERR_IO;
+        p += got; off += (uint64_t)got; len -= (uint64_t)got;
+    }
+    return 0;
+}
+} // namespace
+
+int dbeel_tree_reader_open(dbeel_tree *t, uint64_t fence_bytes, dbeel_reader **out) {
+    if (!t || !out) return DBEEL_ERR_INVALID_ARG;
+    *out = nullptr;
+    t->err.clear();
+    drop_left_tables(t);
+    auto files = std::make_shared<ReaderFiles>();
+    std::vector<dbeel::ReaderTableRef> dev;
+    for (const SSTable &s : t->sstables) {
+        std::shared_ptr<ReaderEntry> &slot = t->readers[s.index];
+        if (!slot) { // a table no live entry has: its descriptors and its filter, read whole as SSTable::new_with_bloom_read does
+            auto ent = std::make_shared<ReaderEntry>();
+            const std::string dp = file_path(t->dir, s.index, kData), ip = file_path(t->dir, s.index, kIndex),
+                              bp = file_path(t->dir, s.index, kBloom);
+            ent->data_fd = open(dp.c_str(), O_RDONLY);
+            ent->index_fd = open(ip.c_str(), O_RDONLY);
+            struct stat sd, si;
+            if (ent->data_fd < 0 || ent->index_fd < 0 || fstat(ent->data_fd, &sd) != 0 || fstat(ent->index_fd, &si) != 0) {
+                const int rc = io_fail(t, "open " + dp);
+                t->readers.erase(s.index);
+                return rc;
+            }
+            PinnedBuf bloom;
+            int rc = exists(bp) ? read_file(t, bp, &bloom) : DBEEL_OK;
+            const dbeel_table tab{nullptr, (uint64_t)sd.st_size, nullptr, (uint64_t)si.st_size, bloom.len ? bloom.p : nullptr, bloom.len};
+            if (!rc && (rc = dbeel::reader_table_create(t->engine, tab, &ent->dev))) t->err = dbeel_last_error(t->engine);
+            if (rc) {
+                t->readers.erase(s.index);
+                return rc;
+            }
+            slot = std::move(ent);
+        }
+        files->tables.push_back(slot);
+        dev.push_back(slot->dev);
+    }
+    const dbeel_scan_io io{reader_read, nullptr, files.get()};
+    const int rc = dbeel::reader_open_tables(t->engine, std::move(dev), io, fence_bytes, files, out);
+    if (rc) t->err = dbeel_last_error(t->engine);
     return rc;
 }
 

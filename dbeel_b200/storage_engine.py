@@ -55,6 +55,8 @@ def _lib():
         L.dbeel_tree_get_values_stream.restype = C.c_int
         L.dbeel_tree_get_values_stream.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32,
                                                    C.POINTER(capi.Out), C.c_void_p]
+        L.dbeel_tree_reader_open.restype = C.c_int
+        L.dbeel_tree_reader_open.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p)]
         L.dbeel_tree_scan.restype = C.c_int
         L.dbeel_tree_scan.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(capi.Out),
                                       C.POINTER(capi.JobResult), C.POINTER(capi.ScanStop)]
@@ -80,7 +82,7 @@ def _lib():
 
 
 TREE_EXPORTS = ["dbeel_tree_open", "dbeel_tree_close", "dbeel_tree_sstables", "dbeel_tree_write_sstable_index",
-                "dbeel_tree_compact", "dbeel_tree_compact_many", "dbeel_tree_flush", "dbeel_tree_recover_wal", "dbeel_tree_get_many", "dbeel_tree_get_values", "dbeel_tree_get_values_stream", "dbeel_tree_scan", "dbeel_tree_scan_stream", "dbeel_tree_last_error", "dbeel_memtable_cut",
+                "dbeel_tree_compact", "dbeel_tree_compact_many", "dbeel_tree_flush", "dbeel_tree_recover_wal", "dbeel_tree_get_many", "dbeel_tree_get_values", "dbeel_tree_get_values_stream", "dbeel_tree_reader_open", "dbeel_tree_scan", "dbeel_tree_scan_stream", "dbeel_tree_last_error", "dbeel_memtable_cut",
                 "dbeel_plan_compactions", "dbeel_out_pages", "dbeel_tree_set_page_sink"]
 
 
@@ -239,6 +241,17 @@ class LSMTree:
                 continue
             self._check(rc, "LSMTree.get_values_stream")
             return res, od[:out.data_len], oi[:out.index_len]
+
+    def open_reader(self, fence_bytes: int = 0) -> capi.Reader:
+        """dbeel_tree_reader_open: a capi.Reader over a snapshot of the tree's SSTables (get_values answers what
+        get_values_stream answered at open, table = a position in the snapshot), unaffected by later flushes and
+        compactions.  Readers share the tables they have in common: one opened after a flush loads only the new ones."""
+        from . import sstable
+        h = C.c_void_p()
+        self._check(_lib().dbeel_tree_reader_open(self._h, fence_bytes, C.byref(h)), "LSMTree.open_reader")
+        dc = sum(os.path.getsize(os.path.join(self.dir, sstable.file_name(idx, sstable.DATA_FILE_EXT)))
+                 for idx, _ in self.sstable_indices_and_sizes())
+        return capi.Reader(h, self._engine, data_cap=dc)
 
     def scan(self, ranges, kind: int = capi.SCAN_HASH):
         """The SSTable part of iter_filter (lsm_tree.rs:133-282) over the tree's files, oldest table first: every entry

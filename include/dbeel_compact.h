@@ -453,6 +453,37 @@ int dbeel_get_values_stream(dbeel_engine *e, const dbeel_table *tables, uint32_t
                             const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, const dbeel_scan_io *io,
                             dbeel_out *out, dbeel_lookup_result *results);
 
+/* Readers: dbeel_get_values_stream for a serving loop that sends many batches to the same tables.  The reference reads
+ * each table's .bloom once, when the table is opened or written (SSTable::new_with_bloom_read, lsm_tree.rs:94-101), and
+ * get_entry walks a snapshot of `sstables` (:686-688); a reader does the same for the GPU path:
+ *   - dbeel_reader_open validates every .bloom and uploads it once (a bad filter fails the open with the code
+ *     dbeel_get_values_stream returns for it); the caller may free its host copies afterwards.  tables / io mean what they
+ *     mean for dbeel_get_values_stream, with the same argument checks; io must stay valid until the reader is closed.
+ *   - The fences of each table (index record + key frame of the top D_t levels of the probe tree, per mode) are read the
+ *     first time a batch in that mode reaches the table, then kept on the device and never read again.  D_t is chosen
+ *     per table so that all the reader's fences, both modes, fit fence_bytes (0 = DBEEL_READER_FENCE_BYTES_DEFAULT): the
+ *     budget goes one level at a time to the table with the largest leaves, never deeper than 16 levels or log2 of the
+ *     table's records.  A cached key frame holds at most DBEEL_READER_FRAME_CAP key bytes.
+ *   - A batch descends a table's cached fences when its longest key is at most DBEEL_READER_FRAME_CAP bytes and the depth
+ *     dbeel_get_values_stream would read for it is at most D_t.  Otherwise it reads that table's fences for this batch
+ *     exactly as dbeel_get_values_stream does.
+ * dbeel_reader_get_values returns exactly what dbeel_get_values_stream(e, tables, ..., io, ...) returns for the same keys
+ * and mode: the rows (DBEEL_LOOKUP_CORRUPT and DBEEL_LOOKUP_BAD_ENTRY included, damaged tables included), out->data /
+ * out->index / items_written, DBEEL_ERR_CAPACITY with the sizes needed, and callback codes unchanged; the reader stays
+ * usable after any of them.  dbeel_last_stats: input_bytes = bytes read through the callback in this call (fences loaded
+ * on the way included), partitions = leaf groups run, the rest as dbeel_get_values_stream.
+ * The reader's device memory (the filters, plus the fences, at most fence_bytes) belongs to the engine.  Open and get
+ * take the engine as every entry point does (DBEEL_ERR_BUSY while another call runs).  dbeel_engine_destroy closes the
+ * readers still open. */
+#define DBEEL_READER_FRAME_CAP 64u
+#define DBEEL_READER_FENCE_BYTES_DEFAULT (64ull << 20)
+typedef struct dbeel_reader dbeel_reader;
+int dbeel_reader_open(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const dbeel_scan_io *io,
+                      uint64_t fence_bytes, dbeel_reader **out);
+int dbeel_reader_get_values(dbeel_reader *r, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
+                            dbeel_out *out, dbeel_lookup_result *results);
+void dbeel_reader_close(dbeel_reader *r);
+
 /* ---- N4: write-ahead-log replay + flush ------------------------------------------------------------------------
  * Replaces LSMTree::read_memtable_from_wal_file (lsm_tree.rs:552-574) followed by flush_memtable_to_disk, i.e. the
  * recovery of an unflushed memtable in open_or_create_ex (:478-513).  `wal` is the whole `.memtable` file: bincode

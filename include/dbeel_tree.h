@@ -90,6 +90,18 @@ int dbeel_tree_get_values(dbeel_tree *t, const void *keys, const uint64_t *key_o
 int dbeel_tree_get_values_stream(dbeel_tree *t, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
                                  dbeel_out *out, dbeel_lookup_result *results);
 
+/* A reader (dbeel_reader_open) over a snapshot of the tree's SSTables: dbeel_tree_sstables() at open, the `sstables` clone
+ * get_entry and AsyncIter take (lsm_tree.rs:177, 686).  dbeel_reader_get_values on it returns what
+ * dbeel_tree_get_values_stream returned at open, with results[i].table a position in the snapshot; close it with
+ * dbeel_reader_close.  The reader holds every table's .data / .index descriptors until it is closed, so a later compaction
+ * that unlinks its inputs does not disturb it (as the reference promises its iterators, :175-176).
+ * The tree keeps one entry per SSTable (device filter, fences per mode, descriptors), shared by reference count between
+ * the readers that include the table: a reader opened after a flush or a compaction loads only the tables no live entry
+ * has, and a table it shares keeps the fence depth it was loaded with (its fences count against fence_bytes first).  An
+ * entry is dropped when no reader holds it and its table has left the tree; dbeel_tree_close drops the tree's entries
+ * (open readers keep theirs until they are closed). */
+int dbeel_tree_reader_open(dbeel_tree *t, uint64_t fence_bytes, dbeel_reader **out);
+
 /* The SSTable part of LSMTree::iter_filter over the tree's files: every table's .data / .index in dbeel_tree_sstables()
  * order (oldest first, the iterator's order) through one dbeel_scan().  kind / ranges / results / stop as in dbeel_scan;
  * out holds host buffers (caps: the sums of the tables' .data and .index file sizes).  stop->table is a position in
