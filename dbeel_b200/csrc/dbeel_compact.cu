@@ -1131,7 +1131,9 @@ int run_job_host(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, const 
     if (sh.n_total) {
         cudaEventElapsedTime(&st.ms_h2d, e->ev[EV_H2D0], e->ev[EV_H2D1]);
         cudaEventElapsedTime(&st.ms_total, e->ev[EV_START], e->ev[EV_GATHER]);
-        cudaEventElapsedTime(&st.ms_extract, e->ev[EV_START], e->ev[EV_EXTRACT]);
+        // EV_EXTRACT is recorded only with stage events: on an event that was never recorded the call fails, and the error
+        // it leaves behind fails the next job's cudaGetLastError check
+        if (e->stage_events) cudaEventElapsedTime(&st.ms_extract, e->ev[EV_START], e->ev[EV_EXTRACT]);
     }
     CU(cudaEventRecord(e->ev[EV_D2H0], s));
     if (dout.data_len) CU(cudaMemcpyAsync(out->data, dout.data, dout.data_len, cudaMemcpyDeviceToHost, s));
