@@ -46,7 +46,7 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream",
            "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device", "dbeel_scan_stream", "dbeel_get_values",
            "dbeel_get_values_device", "dbeel_get_values_stream", "dbeel_reader_open", "dbeel_reader_get_values",
-           "dbeel_reader_close"]
+           "dbeel_reader_scan", "dbeel_reader_close"]
 
 
 class Run(C.Structure):
@@ -223,6 +223,9 @@ def lib():
         L.dbeel_reader_get_values.restype = C.c_int
         L.dbeel_reader_get_values.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.POINTER(Out),
                                               C.c_void_p]
+        L.dbeel_reader_scan.restype = C.c_int
+        L.dbeel_reader_scan.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, SCAN_WRITE_FN, C.c_void_p,
+                                        C.POINTER(JobResult), C.POINTER(ScanStop)]
         L.dbeel_reader_close.restype = None
         L.dbeel_reader_close.argtypes = [C.c_void_p]
         L.dbeel_scan_bound.restype = C.c_int
@@ -411,8 +414,8 @@ def _stream_values(call, name: str, h, n_keys: int, st: Optional[_StreamTables],
 
 
 class Reader:
-    """dbeel_reader_*: get_values_stream's batches on a fixed set of tables, with the filters and fences kept on the
-    device between batches (Engine.open_reader, storage_engine.LSMTree.open_reader).  Use it as a context manager or
+    """dbeel_reader_*: get_values_stream's batches and scan_stream's range scans on a fixed set of tables, with the
+    filters and fences kept on the device between calls (Engine.open_reader, storage_engine.LSMTree.open_reader).  Use it as a context manager or
     close() it; the engine closes readers still open when it is destroyed."""
 
     def __init__(self, handle: C.c_void_p, engine: "Engine", st: Optional[_StreamTables] = None, data_cap: int = 0):
@@ -440,6 +443,48 @@ class Reader:
         finally:
             if self._st is not None:
                 self.last_stream_reads = self._st.last_reads
+
+    def scan(self, ranges, kind: int = SCAN_KEY, write=None, fail_read_at: int = -1):
+        """dbeel_reader_scan: what LSMTree.scan_stream returns, on the reader's tables -- ([(data, index)] per range
+        collected in memory, or [(data_len, index_len, items)] per range when write(dest, kind, offset, src_address,
+        length) -> 0 or an error code receives the pieces), and (table, reason, record) of the stop, table = a position
+        in the reader's tables.  Key ranges read only the records from each bound's seek on; hash ranges read every
+        table.  last_stream_reads and fail_read_at as in get_values."""
+        import threading
+        if not self._h:
+            raise ValueError("reader is closed")
+        n = len(ranges)
+        files = [{1: bytearray(), 2: bytearray()} for _ in range(n)]
+        mu = threading.Lock()
+
+        def collect(dest, kind_, off, src, size):
+            with mu:
+                f = files[dest][kind_]
+                if len(f) < off + size:
+                    f.extend(bytes(off + size - len(f)))
+                f[off:off + size] = C.string_at(src, size)
+            return 0
+
+        cb = SCAN_WRITE_FN(lambda _ctx, dest, kind_, off, src, size: (write or collect)(dest, kind_, off, src, size))
+        rptr, _keep = pack_ranges(kind, ranges)
+        res = (JobResult * max(1, n))()
+        stop = ScanStop()
+        if self._st is not None:
+            self._st.fail_read_at = fail_read_at
+            self._st.log.clear()
+        try:
+            rc = lib().dbeel_reader_scan(self._h, kind, rptr, n, cb, None, res, C.byref(stop))
+        finally:
+            if self._st is not None:
+                self._st.last_reads = list(self._st.log)
+                self.last_stream_reads = self._st.last_reads
+                self._st.fail_read_at = -1
+        if rc:
+            raise DbeelError(rc, f"dbeel_reader_scan: {lib().dbeel_last_error(self._engine._h).decode()}")
+        if write is not None:
+            return [(int(r.data_len), int(r.index_len), int(r.items_written)) for r in res[:n]], stop.as_tuple()
+        return ([(np.frombuffer(bytes(f[1]), np.uint8).copy(), np.frombuffer(bytes(f[2]), np.uint8).copy()) for f in files],
+                stop.as_tuple())
 
     def close(self):
         if self._h and self._engine._h:  # an engine already destroyed has closed its readers

@@ -27,6 +27,7 @@
 #include "lookup_stream.cuh"
 #include "route.cuh"
 #include "scan.cuh"
+#include "scan_seek.cuh"
 #include "wal.cuh"
 #include "host/reader_tables.h"
 #include "host/scan_plan.h"
@@ -2631,34 +2632,14 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
 
 // ------------------------------------------------------------------------------------ N5 streamed: dbeel_scan_stream
 // The plan (host/scan_plan.h) cuts the record sequence into partitions; each goes file -> pinned ring slot -> device slot
-// c & 1 in ONE H2D copy of its slot image (table headers | per table: index slice, .data window), runs the scan chain with
+// c & 1 in ONE H2D copy of its slot image (table headers | per slice: index slice, .data window), runs the scan chain with
 // phase 2 sized from the plan's bound, and comes back with an exact D2H of what it selected.  H2D of c + 1, the kernels of c
 // and the D2H of c - 1 overlap; the engine thread enqueues partition c + 1's kernels before it waits for c's published sizes.
-int scan_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
-                      uint32_t n_ranges, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop) {
-    if (!e) return DBEEL_ERR_INVALID_ARG;
-    if (!io || !io->read || !io->write) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
-    uint64_t key_bytes = 0;
-    if (const int arc = scan_args(e, tables, n_tables, kind, ranges, n_ranges, results, stop, &key_bytes)) return arc;
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
-    for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
-    *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
-
-    // ---- 1. the plan, from the .index files read in pieces
-    std::vector<uint64_t> dlen(n_tables), ilen(n_tables);
-    for (uint32_t t = 0; t < n_tables; t++) {
-        dlen[t] = tables[t].data_len;
-        ilen[t] = tables[t].index_len;
-        e->stats.entries_in += ilen[t] / DBEEL_INDEX_ENTRY_SIZE;
-    }
-    ScanPlan plan;
-    int rc = plan_scan(dlen.data(), ilen.data(), n_tables, e->partition_bytes,
-                       [io](uint32_t t, uint64_t off, uint64_t len, void *dst) { return io->read(io->ctx, t, DBEEL_STREAM_INDEX, off, len, dst); },
-                       &plan);
-    if (rc) return fail(e, rc, "stream read callback failed (.index, planning)");
+// run_scan_plan runs a plan (steps 2 to the end) for dbeel_scan_stream (whole tables) and dbeel_reader_scan (spans): the
+// caller has checked the arguments, taken the engine, cleared results / stop / stats and set stats.entries_in.
+int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &plan, uint32_t kind, const void *ranges,
+                  uint32_t n_ranges, uint64_t key_bytes, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop) {
+    int rc = DBEEL_OK;
     const uint32_t np = (uint32_t)plan.parts.size();
     e->stats.partitions = np;
     auto host_stop = [&]() {
@@ -2919,6 +2900,363 @@ int scan_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tab
     e->stats.output_bytes = out_bytes;
     e->stats.entries_out = items;
     return DBEEL_OK;
+}
+
+// plan_scan over tables[0 .. n_tables) (spans: null = whole tables) through io->read, then run_scan_plan
+int plan_and_run_scan(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
+                      uint32_t n_ranges, uint64_t key_bytes, const dbeel_scan_io *io, dbeel_job_result *results,
+                      dbeel_scan_stop *stop, const std::vector<std::vector<ScanSpan>> *spans) {
+    std::vector<uint64_t> dlen(n_tables), ilen(n_tables);
+    for (uint32_t t = 0; t < n_tables; t++) {
+        dlen[t] = tables[t].data_len;
+        ilen[t] = tables[t].index_len;
+    }
+    ScanPlan plan;
+    const int rc = plan_scan(dlen.data(), ilen.data(), n_tables, e->partition_bytes,
+                             [io](uint32_t t, uint64_t off, uint64_t len, void *dst) { return io->read(io->ctx, t, DBEEL_STREAM_INDEX, off, len, dst); },
+                             &plan, spans);
+    if (rc) return fail(e, rc, "stream read callback failed (.index, planning)");
+    return run_scan_plan(e, tables, plan, kind, ranges, n_ranges, key_bytes, io, results, stop);
+}
+
+int scan_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
+                      uint32_t n_ranges, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop) {
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (!io || !io->read || !io->write) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    uint64_t key_bytes = 0;
+    if (const int arc = scan_args(e, tables, n_tables, kind, ranges, n_ranges, results, stop, &key_bytes)) return arc;
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    e->stats = dbeel_stats{};
+    for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+    *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+
+    // ---- 1. the plan, from the .index files read in pieces
+    for (uint32_t t = 0; t < n_tables; t++) e->stats.entries_in += tables[t].index_len / DBEEL_INDEX_ENTRY_SIZE;
+    return plan_and_run_scan(e, tables, n_tables, kind, ranges, n_ranges, key_bytes, io, results, stop, nullptr);
+}
+
+// ---- dbeel_reader_scan
+// The reader's read callback, counted (input_bytes), and the caller's write callback, behind one ctx.
+struct ReaderScanIo {
+    const dbeel_scan_io *rio;
+    int (*write)(void *, uint32_t, uint32_t, uint64_t, const void *, uint64_t);
+    void *wctx;
+    std::atomic<uint64_t> bytes{0};
+};
+
+int reader_scan_read(void *ctx, uint32_t t, uint32_t kind, uint64_t off, uint64_t len, void *dst) {
+    ReaderScanIo *x = static_cast<ReaderScanIo *>(ctx);
+    x->bytes += len;
+    return x->rio->read(x->rio->ctx, t, kind, off, len, dst);
+}
+
+int reader_scan_write(void *ctx, uint32_t d, uint32_t kind, uint64_t off, const void *src, uint64_t len) {
+    ReaderScanIo *x = static_cast<ReaderScanIo *>(ctx);
+    return x->write(x->wctx, d, kind, off, src, len);
+}
+
+// Vec<u8>::cmp(a, b) < 0
+inline bool key_less(const uint8_t *a, uint64_t al, const uint8_t *b, uint64_t bl) {
+    const int c = std::min(al, bl) ? memcmp(a, b, std::min(al, bl)) : 0;
+    return c < 0 || (c == 0 && al < bl);
+}
+
+// Key ranges (dbeel_compact.h, dbeel_reader_scan): 1. the bound searches of every table before the first one with no
+// index record, two per range with start < end -- fences (cached or read for this call) on the device in one pass
+// (k_seek_fence), then the touched leaves in groups of about the partition budget (k_seek_leaf); 2. the spans, merged per
+// table, up to the first table whose search failed; 3. plan_scan over the spans and run_scan_plan.  The first stop in
+// iteration order wins: a stop inside the spans lies before a failed search or an empty table.
+int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables, const void *ranges, uint32_t nd,
+                    uint64_t key_bytes, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop) {
+    const dbeel_key_ranges *kr = static_cast<const dbeel_key_ranges *>(ranges);
+    const uint8_t *kb = key_bytes ? static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0] : nullptr;
+    std::vector<uint64_t> ko(2 * nd + 1);
+    for (uint32_t k = 0; k <= 2 * nd; k++) ko[k] = kr->key_offsets[k] - kr->key_offsets[0];
+    std::vector<uint32_t> valid; // ranges that can take a record
+    uint64_t max_klen = 0;
+    for (uint32_t d = 0; d < nd; d++) {
+        if (!key_less(kb + ko[2 * d], ko[2 * d + 1] - ko[2 * d], kb + ko[2 * d + 1], ko[2 * d + 2] - ko[2 * d + 1])) continue;
+        valid.push_back(d);
+        max_klen = std::max({max_klen, ko[2 * d + 1] - ko[2 * d], ko[2 * d + 2] - ko[2 * d + 1]});
+    }
+    const uint32_t nt = (uint32_t)r->tables.size();
+    uint32_t nseek = nt; // the tables before the first one with no index record (a PANIC at its record 0)
+    for (uint32_t t = 0; t < nt; t++)
+        if (r->tables[t]->desc.n == 0) { nseek = t; break; }
+    dbeel_scan_stop host_stop = nseek < nt ? dbeel_scan_stop{(int32_t)nseek, DBEEL_SCAN_STOP_PANIC, 0}
+                                           : dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+    const uint64_t nv = valid.size(), Q = 2 * nv * nseek; // pair q: table q / (2 nv), range valid[(q / 2) % nv], end if q odd
+    uint32_t cutoff = nseek;
+    std::vector<std::vector<ScanSpan>> spans(nseek);
+    if (Q) {
+        cudaError_t ce = cudaSetDevice(e->device);
+        if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+        cudaStream_t s = e->stream;
+        const uint64_t budget = e->partition_bytes;
+        int rc;
+        // ---- fences per table: the reader's (loaded now if this is the first exact-mode call that reaches the table)
+        // or read for this call into one host image, staged to stage_out
+        std::vector<uint32_t> depth(nseek);
+        std::vector<ProbeTree> pt_call(nseek);
+        std::vector<const ProbeTree *> pts(nseek);
+        std::vector<GvsFences> gf(nseek);
+        std::vector<GvsFenceReads> frs(nseek);
+        std::vector<uint64_t> img_at(nseek, ~0ull), touched_at(nseek + 1, 0);
+        std::vector<uint8_t> img;
+        for (uint32_t t = 0; t < nseek; t++) {
+            dbeel_reader_table *rt = r->tables[t].get();
+            dbeel_reader_table::Fences &cache = rt->fences[DBEEL_LOOKUP_EXACT];
+            const uint64_t n = rt->desc.n, dl = rt->desc.data_len;
+            const uint32_t want = lookup_depth(2ull * nd, n, dl, 8 + max_klen, budget);
+            const bool use_cache = reader_uses_cache(max_klen, want, (uint32_t)rt->depth);
+            depth[t] = use_cache ? (uint32_t)rt->depth : want;
+            const uint64_t leaf0 = 1ull << depth[t];
+            touched_at[t + 1] = touched_at[t] + leaf0;
+            gf[t] = GvsFences{nullptr, nullptr, depth[t], t, n, nullptr};
+            if (use_cache) {
+                if (!cache.loaded) {
+                    if ((rc = reader_load_fences(e, io, t, rt, DBEEL_LOOKUP_EXACT))) return rc;
+                    CU(cudaStreamSynchronize(s)); // its image goes down from ring_out, which the next table refills
+                }
+                pts[t] = &cache.pt;
+                if (depth[t]) {
+                    gf[t].fix = reinterpret_cast<const uint4 *>(cache.dev);
+                    gf[t].ffr = reinterpret_cast<const unsigned long long *>(cache.dev + 16 * leaf0);
+                }
+                continue;
+            }
+            plan_probe_tree(DBEEL_LOOKUP_EXACT, n, depth[t], &pt_call[t]);
+            pts[t] = &pt_call[t];
+            if (!depth[t]) continue;
+            GvsFenceReads &fr = frs[t];
+            if ((rc = gvs_read_fences(e, io, t, pt_call[t], dl, max_klen, 0, &fr))) return rc;
+            img_at[t] = align_up(img.size(), kAlign);
+            img.resize(img_at[t] + 24 * leaf0 + fr.sf.end);
+            memcpy(img.data() + img_at[t], fr.fix.data(), 16 * leaf0);
+            memcpy(img.data() + img_at[t] + 24 * leaf0, e->ring_in, fr.sf.end);
+        }
+        if (!img.empty()) {
+            if ((rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, img.size()))) return rc;
+            for (uint32_t t = 0; t < nseek; t++) {
+                if (img_at[t] == ~0ull) continue;
+                const uint64_t leaf0 = 1ull << depth[t], o_frames = img_at[t] + 24 * leaf0;
+                unsigned long long *ffr = reinterpret_cast<unsigned long long *>(img.data() + img_at[t] + 16 * leaf0);
+                const GvsFenceReads &fr = frs[t];
+                for (uint64_t k = 0; k < leaf0; k++) {
+                    const uint64_t p = o_frames + (fr.has[k] ? fr.sf.at(fr.frame[k].lo) : 0);
+                    ffr[k] = gvs_frame_addr(fr, k, r->tables[t]->desc.data_len, img.data() + p, e->stage_out + p);
+                }
+                gf[t].fix = reinterpret_cast<const uint4 *>(e->stage_out + img_at[t]);
+                gf[t].ffr = reinterpret_cast<const unsigned long long *>(e->stage_out + img_at[t] + 16 * leaf0);
+            }
+        }
+
+        // ---- per-pair state in the workspace
+        uint64_t off = 0;
+        const uint64_t o_keys = carve_ws(&off, key_bytes + 16), o_koff = carve_ws(&off, 8 * Q), o_klen = carve_ws(&off, 8 * Q);
+        const uint64_t o_tab = carve_ws(&off, 4 * Q), o_state = carve_ws(&off, sizeof(SearchState) * Q), o_node = carve_ws(&off, 4 * Q);
+        const uint64_t o_res = carve_ws(&off, 8 * Q), o_bad = carve_ws(&off, 8 * Q), o_bix = carve_ws(&off, 16 * Q);
+        const uint64_t o_gf = carve_ws(&off, sizeof(GvsFences) * nseek), o_td = carve_ws(&off, sizeof(TableDesc) * nseek);
+        const uint64_t o_depth = carve_ws(&off, 4ull * nseek), o_touched = carve_ws(&off, touched_at[nseek]);
+        if ((rc = ensure_device(e, &e->ws, &e->ws_cap, off))) return rc;
+        uint8_t *ws = e->ws;
+        std::vector<uint64_t> qoff(Q), qlen(Q);
+        std::vector<uint32_t> qtab(Q);
+        std::vector<TableDesc> td(nseek);
+        for (uint64_t q = 0; q < Q; q++) {
+            const uint32_t k = 2 * valid[(q / 2) % nv] + (uint32_t)(q & 1);
+            qoff[q] = ko[k];
+            qlen[q] = ko[k + 1] - ko[k];
+            qtab[q] = (uint32_t)(q / (2 * nv));
+        }
+        for (uint32_t t = 0; t < nseek; t++) {
+            gf[t].touched = ws + o_touched + touched_at[t];
+            td[t] = r->tables[t]->desc;
+        }
+        if (key_bytes) CU(cudaMemcpyAsync(ws + o_keys, kb, key_bytes, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(ws + o_koff, qoff.data(), 8 * Q, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(ws + o_klen, qlen.data(), 8 * Q, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(ws + o_tab, qtab.data(), 4 * Q, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(ws + o_gf, gf.data(), sizeof(GvsFences) * nseek, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(ws + o_td, td.data(), sizeof(TableDesc) * nseek, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(ws + o_depth, depth.data(), 4ull * nseek, cudaMemcpyHostToDevice, s));
+        if (!img.empty()) CU(cudaMemcpyAsync(e->stage_out, img.data(), img.size(), cudaMemcpyHostToDevice, s));
+        CU(cudaMemsetAsync(ws + o_touched, 0, touched_at[nseek], s));
+        SeekQueries sq{ws + o_keys, reinterpret_cast<const uint64_t *>(ws + o_koff), reinterpret_cast<const uint64_t *>(ws + o_klen),
+                       reinterpret_cast<const uint32_t *>(ws + o_tab), Q, reinterpret_cast<SearchState *>(ws + o_state),
+                       reinterpret_cast<uint32_t *>(ws + o_node), reinterpret_cast<unsigned long long *>(ws + o_res),
+                       reinterpret_cast<unsigned long long *>(ws + o_bad), reinterpret_cast<uint4 *>(ws + o_bix)};
+        const uint32_t grid = (uint32_t)((Q + 255) / 256);
+        launch_k(e, k_seek_fence, grid, 256, 0, s, sq, reinterpret_cast<const GvsFences *>(ws + o_gf));
+        std::vector<uint8_t> touched(touched_at[nseek]);
+        CU(cudaMemcpyAsync(touched.data(), ws + o_touched, touched.size(), cudaMemcpyDeviceToHost, s));
+        CU(cudaGetLastError());
+        CU(cudaStreamSynchronize(s));
+
+        // ---- touched leaves, in groups of about `budget` bytes: per table its index slices, then their windows
+        struct Leaf { uint32_t t, leaf; };
+        std::vector<Leaf> group;
+        auto run_group = [&]() -> int {
+            const uint32_t nl = (uint32_t)group.size();
+            std::vector<ByteRange> sr(nl);
+            for (uint32_t k = 0; k < nl; k++) {
+                uint64_t a, b;
+                search_interval(DBEEL_LOOKUP_EXACT, pts[group[k].t]->state[(1ull << depth[group[k].t]) + group[k].leaf], &a, &b);
+                sr[k] = {16 * a, 16 * b};
+            }
+            // header: GvsLeaf[nl] | first[nseek + 1]; then the index slices, table after table
+            const uint64_t o_first = align_up(sizeof(GvsLeaf) * nl, 16);
+            std::vector<GvsStaged> ss(nseek), sw(nseek);
+            std::vector<uint32_t> first(nseek + 1, 0);
+            uint64_t end = align_up(o_first + 4ull * (nseek + 1), kAlign);
+            for (uint32_t k = 0, t = 0; t < nseek; t++) {
+                std::vector<ByteRange> x;
+                first[t] = k;
+                for (; k < nl && group[k].t == t; k++) x.push_back(sr[k]);
+                ss[t] = gvs_stage(std::move(x), kLookupMergeGap, end);
+                end = std::max(end, ss[t].end);
+                first[t + 1] = k;
+            }
+            int rc2 = ensure_host(e, &e->ring_in, &e->ring_in_cap, end);
+            if (!rc2) rc2 = ensure_device(e, &e->stage_in, &e->stage_in_cap, end);
+            if (rc2) return rc2;
+            for (uint32_t t = 0; t < nseek; t++)
+                if (!ss[t].runs.empty() && (rc2 = gvs_read(e, io, t, DBEEL_STREAM_INDEX, ss[t], e->ring_in)))
+                    return fail(e, rc2, "stream read callback failed (.index, leaves)");
+            std::vector<ByteRange> win(nl);
+            std::vector<uint8_t> has(nl, 0);
+            uint64_t wend = 0;
+            for (uint32_t t = 0; t < nseek; t++) {
+                std::vector<ByteRange> wr;
+                for (uint32_t k = first[t]; k < first[t + 1]; k++)
+                    if (leaf_window(e->ring_in + ss[t].at(sr[k].lo), (sr[k].hi - sr[k].lo) / 16, r->tables[t]->desc.data_len, max_klen, &win[k])) {
+                        has[k] = 1;
+                        wr.push_back(win[k]);
+                    }
+                sw[t] = gvs_stage(std::move(wr), 0, wend);
+                wend = std::max(wend, sw[t].end);
+            }
+            rc2 = ensure_host(e, &e->ring_out, &e->ring_out_cap, std::max<uint64_t>(wend, 256));
+            if (!rc2) rc2 = ensure_device(e, &e->stage_in2, &e->stage_in2_cap, std::max<uint64_t>(wend, 256));
+            if (rc2) return rc2;
+            for (uint32_t t = 0; t < nseek; t++)
+                if (!sw[t].runs.empty() && (rc2 = gvs_read(e, io, t, DBEEL_STREAM_DATA, sw[t], e->ring_out)))
+                    return fail(e, rc2, "stream read callback failed (.data, leaves)");
+            GvsLeaf *hl = reinterpret_cast<GvsLeaf *>(e->ring_in);
+            for (uint32_t t = 0; t < nseek; t++) {
+                for (uint32_t k = first[t]; k < first[t + 1]; k++) { // biased as in dbeel_get_values_stream's leaves
+                    const uintptr_t ib = reinterpret_cast<uintptr_t>(e->stage_in + ss[t].at(sr[k].lo)) - sr[k].lo;
+                    const uintptr_t db = has[k] ? reinterpret_cast<uintptr_t>(e->stage_in2 + sw[t].at(win[k].lo)) - win[k].lo
+                                                : reinterpret_cast<uintptr_t>(e->stage_in2);
+                    hl[k] = GvsLeaf{reinterpret_cast<const uint8_t *>(db), reinterpret_cast<const uint4 *>(ib), group[k].leaf, 0, 0};
+                }
+            }
+            memcpy(e->ring_in + o_first, first.data(), 4ull * (nseek + 1));
+            CU(cudaMemcpyAsync(e->stage_in, e->ring_in, end, cudaMemcpyHostToDevice, s));
+            if (wend) CU(cudaMemcpyAsync(e->stage_in2, e->ring_out, wend, cudaMemcpyHostToDevice, s));
+            launch_k(e, k_seek_leaf, grid, 256, 0, s, sq, reinterpret_cast<const TableDesc *>(ws + o_td),
+                     reinterpret_cast<const uint32_t *>(ws + o_depth), reinterpret_cast<const GvsLeaf *>(e->stage_in),
+                     reinterpret_cast<const uint32_t *>(e->stage_in + o_first));
+            CU(cudaGetLastError());
+            CU(cudaStreamSynchronize(s));
+            group.clear();
+            return DBEEL_OK;
+        };
+        uint64_t est = 0;
+        for (uint32_t t = 0; t < nseek; t++) {
+            const uint64_t n = r->tables[t]->desc.n, dl = r->tables[t]->desc.data_len;
+            const uint64_t leaf0 = 1ull << depth[t], per_rec = 16 + (dl + n - 1) / n;
+            for (uint64_t L = 0; L < leaf0; L++) {
+                if (!touched[touched_at[t] + L]) continue;
+                uint64_t a, b;
+                search_interval(DBEEL_LOOKUP_EXACT, pts[t]->state[leaf0 + L], &a, &b);
+                const uint64_t bytes = (b - a) * per_rec + 8 + max_klen;
+                if (!group.empty() && est + bytes > budget) {
+                    if ((rc = run_group())) return rc;
+                    est = 0;
+                }
+                group.push_back(Leaf{t, (uint32_t)L});
+                est += bytes;
+            }
+        }
+        if (!group.empty() && (rc = run_group())) return rc;
+
+        // ---- the bounds, the first failed search, the spans
+        std::vector<unsigned long long> res(Q), bad(Q);
+        std::vector<uint4> bix(Q);
+        CU(cudaMemcpyAsync(res.data(), ws + o_res, 8 * Q, cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(bad.data(), ws + o_bad, 8 * Q, cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(bix.data(), ws + o_bix, 16 * Q, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        for (uint32_t t = 0; t < nseek && cutoff == nseek; t++) {
+            uint64_t worst = ~0ull;
+            uint4 ix = make_uint4(0, 0, 0, 0);
+            std::vector<ScanSpan> sp;
+            for (uint64_t q = 2 * nv * t; q < 2 * nv * (t + 1); q += 2) {
+                for (uint64_t j = q; j < q + 2; j++)
+                    if (bad[j] < worst) { worst = bad[j]; ix = bix[j]; }
+                if (res[q] < res[q + 1] && res[q + 1] != ~0ull) sp.push_back(ScanSpan{res[q], res[q + 1]});
+            }
+            if (worst != ~0ull) { // as dbeel_scan on reaching the record: PANIC when its index record alone shows it
+                const uint64_t o = (uint64_t)ix.x | ((uint64_t)ix.y << 32), dl = r->tables[t]->desc.data_len;
+                const bool panic = ix.w == 0 || o > dl || ix.w > dl - o;
+                host_stop = dbeel_scan_stop{(int32_t)t, panic ? DBEEL_SCAN_STOP_PANIC : DBEEL_SCAN_STOP_ERR, worst};
+                cutoff = t;
+                break;
+            }
+            std::sort(sp.begin(), sp.end(), [](const ScanSpan &a, const ScanSpan &b) { return a.lo < b.lo; });
+            for (const ScanSpan &x : sp) {
+                if (!spans[t].empty() && x.lo <= spans[t].back().hi) spans[t].back().hi = std::max(spans[t].back().hi, x.hi);
+                else spans[t].push_back(x);
+            }
+        }
+    }
+    spans.resize(cutoff);
+    for (uint32_t t = 0; t < cutoff; t++)
+        for (const ScanSpan &x : spans[t]) e->stats.entries_in += x.hi - x.lo;
+    const int rc = plan_and_run_scan(e, tables, cutoff, DBEEL_SCAN_KEY, ranges, nd, key_bytes, io, results, stop, &spans);
+    if (!rc && stop->table < 0) *stop = host_stop;
+    return rc;
+}
+
+int reader_scan_entry(dbeel_reader *r, uint32_t kind, const void *ranges, uint32_t n_ranges,
+                      int (*write)(void *, uint32_t, uint32_t, uint64_t, const void *, uint64_t), void *ctx,
+                      dbeel_job_result *results, dbeel_scan_stop *stop) {
+    dbeel_engine *e = r->e;
+    if (!write) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    std::vector<dbeel_table> tables(r->tables.size());
+    for (size_t i = 0; i < tables.size(); i++) {
+        const TableDesc &d = r->tables[i]->desc;
+        tables[i] = dbeel_table{nullptr, d.data_len, nullptr, d.n * DBEEL_INDEX_ENTRY_SIZE, nullptr, 0};
+    }
+    const uint32_t nt = (uint32_t)tables.size();
+    uint64_t key_bytes = 0;
+    if (const int arc = scan_args(e, tables.data(), nt, kind, ranges, n_ranges, results, stop, &key_bytes)) return arc;
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    e->stats = dbeel_stats{};
+    for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+    *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+    ReaderScanIo x;
+    x.rio = &r->io;
+    x.write = write;
+    x.wctx = ctx;
+    const dbeel_scan_io io{reader_scan_read, reader_scan_write, &x};
+    if (kind == DBEEL_SCAN_HASH) { // dbeel_scan_stream on the snapshot
+        for (uint32_t t = 0; t < nt; t++) e->stats.entries_in += tables[t].index_len / DBEEL_INDEX_ENTRY_SIZE;
+        return plan_and_run_scan(e, tables.data(), nt, kind, ranges, n_ranges, key_bytes, &io, results, stop, nullptr);
+    }
+    const int rc = reader_scan_key(e, r, tables.data(), ranges, n_ranges, key_bytes, &io, results, stop);
+    if (rc) {
+        cudaStreamSynchronize(e->stream); // nothing of this call may touch the engine's buffers after it returns
+        for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+        *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+    }
+    e->stats.input_bytes = x.bytes;
+    return rc;
 }
 
 } // namespace
@@ -3321,6 +3659,14 @@ int dbeel_reader_get_values(dbeel_reader *r, const void *keys, const uint64_t *k
         tables[i] = dbeel_table{nullptr, d.data_len, nullptr, d.n * DBEEL_INDEX_ENTRY_SIZE, nullptr, 0};
     }
     return get_values_stream_entry(r->e, tables.data(), (uint32_t)tables.size(), keys, key_offsets, n_keys, mode, &r->io, out, results, r);
+}
+
+int dbeel_reader_scan(dbeel_reader *r, uint32_t kind, const void *ranges, uint32_t n_ranges,
+                      int (*write)(void *ctx, uint32_t dest, uint32_t kind, uint64_t offset, const void *src, uint64_t len),
+                      void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop) {
+    if (!r) return DBEEL_ERR_INVALID_ARG;
+    REFUSE_WHILE_ASYNC(r->e);
+    return reader_scan_entry(r, kind, ranges, n_ranges, write, ctx, results, stop);
 }
 
 void dbeel_reader_close(dbeel_reader *r) {

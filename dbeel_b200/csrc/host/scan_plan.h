@@ -13,6 +13,13 @@
 // The index is read in pieces through the caller's read callback and only the plan rows are kept, so the planner's memory
 // is O(partitions), not O(records).  Every stop the reference would PANIC on is visible in the index alone -- full_size == 0,
 // bytes past the end of .data, a table with no index record -- so the plan ends there and no partition carries such a record.
+//
+// Spans (dbeel_reader_scan's key ranges): per table ascending, disjoint record intervals; only they are read and planned.
+// The plan is then the plan of the tables cut down to their spans (each .index = its span records back to back, .data
+// whole; a table with records but an empty span dropped), with record numbers mapped back: the partitions cut at the same
+// records, and a slice that runs across a span boundary in the cut table becomes one slice per span, each with the window
+// of its own records.  The budget is charged with the cut table's window, which covers them all.  One more cut keeps a
+// partition at kScanPartMaxSlices slices (k_scan_classify's table limit); whole-table plans never reach it.
 #pragma once
 #include <stdint.h>
 
@@ -45,9 +52,15 @@ using ScanIndexRead = std::function<int(uint32_t, uint64_t, uint64_t, void *)>;
 
 constexpr uint64_t kScanPlanPiece = 1ull << 20;          // .index bytes per read while planning
 constexpr uint64_t kScanPartMaxRecords = 0xFFFFFFF0ull - 1; // the whole-buffer scan's record limit, per partition
+constexpr uint32_t kScanPartMaxSlices = 1024;               // = kScanMaxTables
 
+struct ScanSpan { // index records [lo, hi) of one table
+    uint64_t lo, hi;
+};
+
+// spans: null = every table whole (dbeel_scan_stream's plan), else (*spans)[t] = table t's spans.
 inline int plan_scan(const uint64_t *data_len, const uint64_t *index_len, uint32_t n_tables, uint64_t budget,
-                     const ScanIndexRead &read, ScanPlan *plan) {
+                     const ScanIndexRead &read, ScanPlan *plan, const std::vector<std::vector<ScanSpan>> *spans = nullptr) {
     plan->parts.clear();
     plan->slices.clear();
     plan->panic_table = -1;
@@ -55,20 +68,27 @@ inline int plan_scan(const uint64_t *data_len, const uint64_t *index_len, uint32
     std::vector<uint8_t> buf(kScanPlanPiece);
     bool open = false;        // a partition is being filled
     ScanPart part = {};
-    ScanSlice sl = {};        // the open partition's last slice (its table is the current one once a record is in)
+    ScanSlice run = {};       // the open partition's records of the current table: the cut table's slice (budget)
+    bool run_open = false;
+    ScanSlice sl = {};        // the open slice: contiguous records of one span
     bool slice_open = false;
-    uint64_t closed_win = 0;  // windows of the open partition's earlier slices
+    uint64_t closed_win = 0;  // windows of the open partition's earlier tables
     uint64_t out_bound = 0;   // sum of (full_size + 16) in the open partition
     auto close_slice = [&]() {
         if (!slice_open) return;
         plan->slices.push_back(sl);
         part.n_slices++;
-        closed_win += sl.win_hi - sl.win_lo;
         slice_open = false;
+    };
+    auto close_run = [&]() {
+        close_slice();
+        if (!run_open) return;
+        closed_win += run.win_hi - run.win_lo;
+        run_open = false;
     };
     auto close_part = [&]() {
         if (!open) return;
-        close_slice();
+        close_run();
         plan->parts.push_back(part);
         open = false;
     };
@@ -79,46 +99,62 @@ inline int plan_scan(const uint64_t *data_len, const uint64_t *index_len, uint32
             close_part();
             return 0;
         }
-        for (uint64_t r0 = 0; r0 < n; r0 += kScanPlanPiece / 16) {
-            const uint64_t m = n - r0 < kScanPlanPiece / 16 ? n - r0 : kScanPlanPiece / 16;
-            const int rc = read(t, 16 * r0, 16 * m, buf.data());
-            if (rc) return rc;
-            for (uint64_t k = 0; k < m; k++) {
-                const uint8_t *q = buf.data() + 16 * k;
-                uint64_t off = 0;
-                uint32_t fs = 0;
-                for (int b = 7; b >= 0; b--) off = (off << 8) | q[b];
-                for (int b = 15; b >= 12; b--) fs = (fs << 8) | q[b];
-                if (fs == 0 || off > data_len[t] || fs > data_len[t] - off) { // cached_file_reader.rs:68,82
-                    plan->panic_table = (int32_t)t;
-                    plan->panic_record = r0 + k;
-                    close_part();
-                    return 0;
+        const std::vector<ScanSpan> whole = {ScanSpan{0, n}};
+        for (const ScanSpan &span : spans ? (*spans)[t] : whole) {
+            const uint64_t s_hi = span.hi < n ? span.hi : n;
+            for (uint64_t r0 = span.lo; r0 < s_hi; r0 += kScanPlanPiece / 16) {
+                const uint64_t m = s_hi - r0 < kScanPlanPiece / 16 ? s_hi - r0 : kScanPlanPiece / 16;
+                const int rc = read(t, 16 * r0, 16 * m, buf.data());
+                if (rc) return rc;
+                for (uint64_t k = 0; k < m; k++) {
+                    const uint8_t *q = buf.data() + 16 * k;
+                    const uint64_t r = r0 + k;
+                    uint64_t off = 0;
+                    uint32_t fs = 0;
+                    for (int b = 7; b >= 0; b--) off = (off << 8) | q[b];
+                    for (int b = 15; b >= 12; b--) fs = (fs << 8) | q[b];
+                    if (fs == 0 || off > data_len[t] || fs > data_len[t] - off) { // cached_file_reader.rs:68,82
+                        plan->panic_table = (int32_t)t;
+                        plan->panic_record = r;
+                        close_part();
+                        return 0;
+                    }
+                    const uint64_t lo = off, hi = off + fs;
+                    const bool same = run_open && run.table == t;
+                    const bool joins = slice_open && sl.table == t && sl.rec_hi == r; // extends the open slice
+                    if (open) { // would this record push the partition past the budget?
+                        const uint64_t w = same ? (hi > run.win_hi ? hi : run.win_hi) - (lo < run.win_lo ? lo : run.win_lo)
+                                                : (run_open ? run.win_hi - run.win_lo : 0) + fs;
+                        const uint32_t slices = part.n_slices + (slice_open ? 1u : 0u) + (joins ? 0u : 1u);
+                        if (closed_win + w > budget || out_bound + fs + 16 > budget || part.n_rec + 1 > kScanPartMaxRecords ||
+                            slices > kScanPartMaxSlices)
+                            close_part();
+                    }
+                    if (!open) {
+                        part = ScanPart{(uint32_t)plan->slices.size(), 0, 0, 0};
+                        closed_win = 0;
+                        out_bound = 0;
+                        open = true;
+                    }
+                    if (run_open && run.table != t) close_run();
+                    if (!run_open) {
+                        run = ScanSlice{t, r, r, lo, hi};
+                        run_open = true;
+                    }
+                    if (slice_open && (sl.table != t || sl.rec_hi != r)) close_slice();
+                    if (!slice_open) {
+                        sl = ScanSlice{t, r, r, lo, hi};
+                        slice_open = true;
+                    }
+                    if (lo < run.win_lo) run.win_lo = lo;
+                    if (hi > run.win_hi) run.win_hi = hi;
+                    if (lo < sl.win_lo) sl.win_lo = lo;
+                    if (hi > sl.win_hi) sl.win_hi = hi;
+                    run.rec_hi = sl.rec_hi = r + 1;
+                    part.n_rec++;
+                    part.data_bound += fs;
+                    out_bound += fs + 16;
                 }
-                const uint64_t lo = off, hi = off + fs;
-                if (open) { // would this record push the partition past the budget?
-                    const bool same = slice_open && sl.table == t;
-                    const uint64_t w = same ? (hi > sl.win_hi ? hi : sl.win_hi) - (lo < sl.win_lo ? lo : sl.win_lo)
-                                            : (slice_open ? sl.win_hi - sl.win_lo : 0) + fs;
-                    if (closed_win + w > budget || out_bound + fs + 16 > budget || part.n_rec + 1 > kScanPartMaxRecords) close_part();
-                }
-                if (!open) {
-                    part = ScanPart{(uint32_t)plan->slices.size(), 0, 0, 0};
-                    closed_win = 0;
-                    out_bound = 0;
-                    open = true;
-                }
-                if (slice_open && sl.table != t) close_slice();
-                if (!slice_open) {
-                    sl = ScanSlice{t, r0 + k, r0 + k, lo, hi};
-                    slice_open = true;
-                }
-                if (lo < sl.win_lo) sl.win_lo = lo;
-                if (hi > sl.win_hi) sl.win_hi = hi;
-                sl.rec_hi = r0 + k + 1;
-                part.n_rec++;
-                part.data_bound += fs;
-                out_bound += fs + 16;
             }
         }
     }

@@ -244,8 +244,9 @@ class LSMTree:
 
     def open_reader(self, fence_bytes: int = 0) -> capi.Reader:
         """dbeel_tree_reader_open: a capi.Reader over a snapshot of the tree's SSTables (get_values answers what
-        get_values_stream answered at open, table = a position in the snapshot), unaffected by later flushes and
-        compactions.  Readers share the tables they have in common: one opened after a flush loads only the new ones."""
+        get_values_stream answered at open, scan what scan_stream returned at open, table = a position in the snapshot),
+        unaffected by later flushes and compactions.  Readers share the tables they have in common: one opened after a
+        flush loads only the new ones."""
         from . import sstable
         h = C.c_void_p()
         self._check(_lib().dbeel_tree_reader_open(self._h, fence_bytes, C.byref(h)), "LSMTree.open_reader")

@@ -482,6 +482,45 @@ int dbeel_reader_open(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tab
                       uint64_t fence_bytes, dbeel_reader **out);
 int dbeel_reader_get_values(dbeel_reader *r, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
                             dbeel_out *out, dbeel_lookup_result *results);
+
+/* Range scans on a reader: dbeel_scan_stream's call on the reader's tables (a snapshot: a tree reader keeps its tables'
+ * files open while the tree flushes and compacts).  kind / ranges / n_ranges / results / stop mean what they mean for
+ * dbeel_scan_stream, with its argument checks and limits (kind, 1 <= n_ranges <= DBEEL_MAX_SCAN_RANGES, a non-null write,
+ * the record limit per partition); ranges, results and stop in host memory.  Output pieces go to write(ctx, ...) as to
+ * dbeel_scan_io.write: destination d's .data / .index start at offset 0, pieces arrive in any order and from several
+ * threads.  The reader's io.read reads the files; its io.write is not used.  stop->table is a position in the reader's
+ * tables.
+ *   DBEEL_SCAN_HASH  a hash range cannot seek: exactly what dbeel_scan_stream returns on the reader's tables through the
+ *                    reader's io -- the same files, results and stop.
+ *   DBEEL_SCAN_KEY   a seek.  For table t of n_t records and each range d with start_d < end_d (byte order), lo = seek_t(start_d)
+ *                    and hi = seek_t(end_d); a range with start_d >= end_d takes no record and is not searched.  seek_t(k):
+ *                    a = 0, b = n_t; while a < b: mid = a + (b - a) / 2, compare the key of record mid with k (c), a = mid + 1
+ *                    if c < 0 else b = mid; the result is a -- the exact-mode search of DBEEL_LOOKUP_EXACT without its exit
+ *                    on equality, so the reader's exact-mode fences serve it.  On keys that strictly ascend, seek_t(k) is the
+ *                    first record whose key is >= k.  Table t's span is the union of the [lo, hi), merged into ascending
+ *                    disjoint record intervals.  The output and *stop are exactly what dbeel_scan_stream (= dbeel_scan)
+ *                    returns on the same ranges over the tables cut down to their spans (each .index = its span records back
+ *                    to back, .data whole; a table whose span is empty contributes nothing), with record numbers mapped back
+ *                    to the original tables.  On the tables the writer produces (keys strictly ascending) with no stop, that
+ *                    is plain dbeel_scan_stream(DBEEL_SCAN_KEY) on the same tables, byte for byte.  A table with no index
+ *                    record is a DBEEL_SCAN_STOP_PANIC at (t, 0), as in dbeel_scan; nothing is read for it.
+ *                    A search that probes a record the lookup reports corrupt (offset or length prefix past the end of .data)
+ *                    fails: table t contributes nothing and the scan ends before it, with *stop = (t, reason, r), r the
+ *                    smallest such record of t and reason what dbeel_scan reports on reaching r (PANIC when the index record
+ *                    alone shows it, ERR otherwise).  Every search finishes before the first record is scanned, so the stop
+ *                    is the first, in iteration order, of the failed searches, the empty tables and the stops in the spans.
+ *                    Reads: the fences, from the reader's cache under dbeel_reader_get_values' rule (range keys of at most
+ *                    DBEEL_READER_FRAME_CAP bytes, the depth for 2 * n_ranges queries at most D_t; a first scan loads the
+ *                    exact-mode fences, which get_values shares) or read for this call; the leaves the searches end in (index
+ *                    slice and key frames); then the span slices and .data windows, planned and pumped as dbeel_scan_stream
+ *                    plans and pumps whole tables.  No other .index or .data byte is read.
+ * dbeel_last_stats: input_bytes = bytes read through the callback in this call (fences loaded on the way included; for
+ * DBEEL_SCAN_HASH as dbeel_scan_stream), output_bytes as dbeel_scan_stream, entries_in = records in the spans (all records
+ * for DBEEL_SCAN_HASH), partitions = span partitions run.  A callback's nonzero return comes back unchanged; the reader
+ * stays usable after it, after any stop and after an argument error.  DBEEL_ERR_BUSY while another call runs. */
+int dbeel_reader_scan(dbeel_reader *r, uint32_t kind, const void *ranges, uint32_t n_ranges,
+                      int (*write)(void *ctx, uint32_t dest, uint32_t kind, uint64_t offset, const void *src, uint64_t len),
+                      void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop);
 void dbeel_reader_close(dbeel_reader *r);
 
 /* ---- N4: write-ahead-log replay + flush ------------------------------------------------------------------------
