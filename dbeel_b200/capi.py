@@ -46,7 +46,8 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream",
            "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device", "dbeel_scan_stream", "dbeel_get_values",
            "dbeel_get_values_device", "dbeel_get_values_stream", "dbeel_reader_open", "dbeel_reader_get_values",
-           "dbeel_reader_scan", "dbeel_reader_close"]
+           "dbeel_reader_scan", "dbeel_reader_close", "dbeel_page_cache_create", "dbeel_page_cache_destroy",
+           "dbeel_reader_attach_page_cache", "dbeel_page_cache_stats"]
 
 
 class Run(C.Structure):
@@ -228,6 +229,14 @@ def lib():
                                         C.POINTER(JobResult), C.POINTER(ScanStop)]
         L.dbeel_reader_close.restype = None
         L.dbeel_reader_close.argtypes = [C.c_void_p]
+        L.dbeel_page_cache_create.restype = C.c_int
+        L.dbeel_page_cache_create.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p)]
+        L.dbeel_page_cache_destroy.restype = None
+        L.dbeel_page_cache_destroy.argtypes = [C.c_void_p]
+        L.dbeel_reader_attach_page_cache.restype = C.c_int
+        L.dbeel_reader_attach_page_cache.argtypes = [C.c_void_p, C.c_void_p]
+        L.dbeel_page_cache_stats.restype = C.c_int
+        L.dbeel_page_cache_stats.argtypes = [C.c_void_p, C.POINTER(PageCacheStats)]
         L.dbeel_scan_bound.restype = C.c_int
         L.dbeel_scan_bound.argtypes = [C.POINTER(Table), C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
         for name in ("dbeel_scan", "dbeel_scan_device"):
@@ -413,6 +422,44 @@ def _stream_values(call, name: str, h, n_keys: int, st: Optional[_StreamTables],
         dc, ic = err.needed
 
 
+class PageCacheStats(C.Structure):
+    _fields_ = [("capacity_pages", C.c_uint64), ("resident_pages", C.c_uint64), ("hits", C.c_uint64), ("misses", C.c_uint64),
+                ("evictions", C.c_uint64)]
+
+
+class PageCache:
+    """dbeel_page_cache_*: 4096-byte pages of readers' .data / .index files kept on the device across batches and across
+    the readers attached to it (Reader.attach_page_cache, LSMTree.open_reader(page_cache=...)), made by
+    Engine.open_page_cache.  Not LSMTree.set_page_cache, which mirrors the reference's write-through into a Python dict.
+    Use it as a context manager or close() it; closing detaches it from its readers, which go on uncached, and the engine
+    destroys caches still open when it is destroyed."""
+
+    def __init__(self, handle: C.c_void_p, engine: "Engine"):
+        self._h = handle
+        self._engine = engine
+
+    def stats(self) -> dict:
+        """capacity_pages, resident_pages; hits, misses and evictions in pages since the cache was made."""
+        if not self._h:
+            raise ValueError("page cache is closed")
+        st = PageCacheStats()
+        rc = lib().dbeel_page_cache_stats(self._h, C.byref(st))
+        if rc:
+            raise DbeelError(rc, "dbeel_page_cache_stats")
+        return {name: int(getattr(st, name)) for name, _ in PageCacheStats._fields_}
+
+    def close(self):
+        if self._h and self._engine._h:  # an engine already destroyed has destroyed its caches
+            lib().dbeel_page_cache_destroy(self._h)
+        self._h = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
 class Reader:
     """dbeel_reader_*: get_values_stream's batches and scan_stream's range scans on a fixed set of tables, with the
     filters and fences kept on the device between calls (Engine.open_reader, storage_engine.LSMTree.open_reader).  Use it as a context manager or
@@ -424,6 +471,20 @@ class Reader:
         self._st = st
         self._data_cap = data_cap
         self.last_stream_reads = None if st is None else []
+        self._cache = None
+
+    def attach_page_cache(self, cache: Optional[PageCache]):
+        """dbeel_reader_attach_page_cache: read leaf slices, windows and entries through `cache` from the next call on
+        (None detaches).  Results stay exactly what they are uncached; only the reads through the callback change."""
+        if not self._h:
+            raise ValueError("reader is closed")
+        h = cache._h if cache is not None else None
+        if cache is not None and not h:
+            raise ValueError("page cache is closed")
+        rc = lib().dbeel_reader_attach_page_cache(self._h, h)
+        if rc:
+            raise DbeelError(rc, f"dbeel_reader_attach_page_cache: {lib().dbeel_last_error(self._engine._h).decode()}")
+        self._cache = cache
 
     def get_values(self, keys: Sequence[bytes], mode: int = LOOKUP_REFERENCE, caps: Optional[Tuple[int, int]] = None,
                    fail_read_at: int = -1):
@@ -867,6 +928,12 @@ class Engine:
         self._check(lib().dbeel_reader_open(self._h, st.arr, len(st.keep), C.byref(st.io), fence_bytes, C.byref(h)),
                     "dbeel_reader_open")
         return Reader(h, self, st)
+
+    def open_page_cache(self, nbytes: int) -> PageCache:
+        """dbeel_page_cache_create: a PageCache of nbytes // 4096 page slots in one device allocation made now."""
+        h = C.c_void_p()
+        self._check(lib().dbeel_page_cache_create(self._h, nbytes, C.byref(h)), "dbeel_page_cache_create")
+        return PageCache(h, self)
 
     def get_values_device(self, tables: Sequence[Tuple[int, int, int, int, int, int]], keys_ptr: int, offsets_ptr: int,
                           n_keys: int, results_ptr: int, out_ptrs: Tuple[int, int, int, int],

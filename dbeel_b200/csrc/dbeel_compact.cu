@@ -29,6 +29,7 @@
 #include "scan.cuh"
 #include "scan_seek.cuh"
 #include "wal.cuh"
+#include "host/page_cache.h"
 #include "host/reader_tables.h"
 #include "host/scan_plan.h"
 #include "host/stream_pump.h"
@@ -80,6 +81,7 @@ struct dbeel_engine {
     std::string err;
     bool busy = false;
     std::vector<dbeel_reader *> readers; // open readers (dbeel_reader_open, dbeel_tree_reader_open): closed with the engine
+    std::vector<dbeel_page_cache *> page_caches; // open page caches (dbeel_page_cache_create): destroyed with the engine
     // asynchronous jobs (dbeel_compact_submit)
     std::thread worker;
     std::atomic<int> async_state{0}; // 0 idle, 1 running, 2 finished (status in async_status)
@@ -2272,6 +2274,7 @@ inline unsigned long long gvs_frame_addr(const GvsFenceReads &f, uint64_t k, uin
 // mode the fences of the top `depth` levels (host/lookup_plan.h), read the first time a batch in that mode reaches it.
 struct dbeel_reader_table {
     int device = 0;
+    uint64_t id = next_id(); // the page cache's key for the table's files: process-wide, never reused
     TableDesc desc = {};      // data / index unset; words -> the resident filter, or nullptr
     uint8_t *bloom_dev = nullptr;
     int32_t depth = -1;       // D_t: chosen by the first reader that includes the table, kept after
@@ -2286,6 +2289,10 @@ struct dbeel_reader_table {
         for (auto &f : fences)
             if (f.dev) cudaFree(f.dev);
     }
+    static uint64_t next_id() {
+        static std::atomic<uint64_t> n{1};
+        return n.fetch_add(1);
+    }
 };
 
 struct dbeel_reader {
@@ -2293,6 +2300,21 @@ struct dbeel_reader {
     std::vector<ReaderTableRef> tables;
     dbeel_scan_io io = {};
     std::shared_ptr<void> owner; // what io.ctx points at, when the reader owns it (tree readers)
+    dbeel_page_cache *cache = nullptr; // dbeel_reader_attach_page_cache
+};
+
+// The readers' page cache: its slots in one device allocation, the page table and CLOCK on the host (host/page_cache.h).
+struct dbeel_page_cache {
+    dbeel_engine *e = nullptr;
+    uint8_t *pool = nullptr; // pc.capacity() slots of kPageBytes
+    PageCache pc;
+    uint8_t *host = nullptr; // page-locked staging of one request: its miss image, then its copy list (grow-only)
+    uint64_t host_cap = 0;
+    explicit dbeel_page_cache(uint64_t slots) : pc(slots) {}
+    ~dbeel_page_cache() {
+        if (pool) cudaFree(pool);
+        if (host) cudaFreeHost(host);
+    }
 };
 
 namespace {
@@ -2328,6 +2350,72 @@ int reader_load_fences(dbeel_engine *e, const dbeel_scan_io *io, uint32_t ti, db
         CU(cudaMemcpyAsync(c.dev, img, bytes, cudaMemcpyHostToDevice, e->stream));
     }
     c.loaded = true;
+    return DBEEL_OK;
+}
+
+// One staged image of file `kind`: the runs of every part's GvsStaged (table t of the batch) at their positions, which lie
+// in [from, to) of `host` (page-locked) and `dev`.  Without a page cache, or when the request needs more pages than the
+// cache has slots, that is gvs_read into host and one H2D of [from, to).  With a cache attached to reader r, the pages it
+// holds are copied on the device, and the missing ones are read through the callback into the cache's staging (page-aligned
+// runs clipped to the file's length, host/page_cache.h), go down with the copy list to stage_out, and one k_page_copy fills
+// their slots and the image from them; host_too brings the image back to host (the .index slices, whose records the host
+// reads).  The pages become resident only once their reads have succeeded.  The caller has synchronised the stream since
+// its last use of stage_out and of the cache's staging.  The callback's code comes back unchanged, with `what`.
+struct GvsPart { uint32_t t; const GvsStaged *s; };
+
+int gvs_load(dbeel_engine *e, const dbeel_scan_io *io, const dbeel_reader *r, uint32_t kind, const std::vector<GvsPart> &parts,
+             uint8_t *host, uint8_t *dev, uint64_t from, uint64_t to, bool host_too, const char *what) {
+    dbeel_page_cache *c = r ? r->cache : nullptr;
+    cudaStream_t s = e->stream;
+    int rc;
+    PagePlan p;
+    if (c) {
+        std::vector<PagePart> pp;
+        for (const GvsPart &g : parts) {
+            const TableDesc &d = r->tables[g.t]->desc;
+            pp.push_back(PagePart{r->tables[g.t]->id, kind, kind == DBEEL_STREAM_DATA ? d.data_len : 16 * d.n, {}});
+            for (size_t k = 0; k < g.s->runs.size(); k++) pp.back().ranges.push_back(PageRange{g.s->runs[k].lo, g.s->runs[k].hi, g.s->pos[k]});
+        }
+        p = c->pc.plan(pp, StreamPump::kPiece);
+    }
+    if (!c || p.bypass) {
+        for (const GvsPart &g : parts)
+            if ((rc = gvs_read(e, io, g.t, kind, *g.s, host))) return fail(e, rc, what);
+        if (to > from) CU(cudaMemcpyAsync(dev + from, host + from, to - from, cudaMemcpyHostToDevice, s));
+        return DBEEL_OK;
+    }
+    const uint64_t o_copy = align_up(p.img_bytes, kAlign), bytes = o_copy + sizeof(PageCopy) * p.moves.size();
+    rc = ensure_host(e, &c->host, &c->host_cap, std::max<uint64_t>(bytes, 256));
+    if (!rc) rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, std::max<uint64_t>(bytes, 256));
+    if (rc) { c->pc.commit(p, false); return rc; }
+    for (const PageRead &x : p.reads) e->stats.input_bytes += x.len;
+    rc = parallel_pieces(p.reads.size(), [&](size_t k) {
+        const PageRead &x = p.reads[k];
+        return io->read(io->ctx, parts[x.part].t, kind, x.off, x.len, c->host + x.img);
+    });
+    if (rc) { c->pc.commit(p, false); return fail(e, rc, what); }
+    const uint64_t src[3] = {(uint64_t)e->stage_out, (uint64_t)e->stage_out, (uint64_t)c->pool}; // by PageMove::how
+    const uint64_t dst[3] = {(uint64_t)c->pool, (uint64_t)dev, (uint64_t)dev};
+    PageCopy *pc = reinterpret_cast<PageCopy *>(c->host + o_copy);
+    for (size_t k = 0; k < p.moves.size(); k++) {
+        const PageMove &m = p.moves[k];
+        pc[k] = PageCopy{src[m.how] + m.src, dst[m.how] + m.dst, m.len, 0};
+    }
+    cudaError_t ce = cudaSuccess;
+    if (!p.moves.empty()) {
+        ce = cudaMemcpyAsync(e->stage_out, c->host, bytes, cudaMemcpyHostToDevice, s);
+        if (ce == cudaSuccess) {
+            launch_k(e, k_page_copy, (uint32_t)((32 * p.moves.size() + 255) / 256), 256, 0, s, reinterpret_cast<const PageCopy *>(e->stage_out + o_copy),
+                     (uint64_t)p.moves.size());
+            ce = cudaGetLastError();
+        }
+    }
+    c->pc.commit(p, ce == cudaSuccess); // the copies that read a slot are enqueued before any later fill of it
+    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "k_page_copy", ce);
+    if (host_too && to > from) {
+        CU(cudaMemcpyAsync(host + from, dev + from, to - from, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+    }
     return DBEEL_OK;
 }
 
@@ -2495,8 +2583,11 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
         CU(cudaStreamSynchronize(s));
         touched.assign(e->pin, e->pin + leaf0);
 
-        // ---- leaves, in groups of about `budget` bytes: index slices, then the windows their records point at
+        // ---- leaves, in groups of about `budget` bytes (with a page cache, at most its capacity): index slices, then the
+        // windows their records point at
         const uint64_t per_rec = 16 + (nrec ? (data_len + nrec - 1) / nrec : 0);
+        const bool paged = reader && reader->cache; // a leaf's slice and window each end in pages of their own
+        const uint64_t group_bytes = paged ? std::min(budget, kPageBytes * reader->cache->pc.capacity()) : budget;
         std::vector<uint32_t> group;
         auto run_group = [&]() -> int {
             const uint32_t nl = (uint32_t)group.size();
@@ -2506,12 +2597,14 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
                 search_interval(mode, pt.state[leaf0 + group[k]], &a, &b);
                 sr[k] = {16 * a, 16 * b};
             }
-            const uint64_t o_hdr = 0;
-            const GvsStaged ss = gvs_stage(sr, kLookupMergeGap, align_up(sizeof(GvsLeaf) * nl, kAlign));
+            const uint64_t o_hdr = 0, hdr = align_up(sizeof(GvsLeaf) * nl, kAlign);
+            const GvsStaged ss = gvs_stage(sr, kLookupMergeGap, hdr);
             int rc2 = ensure_host(e, &e->ring_in, &e->ring_in_cap, ss.end);
             if (!rc2) rc2 = ensure_device(e, &e->stage_in, &e->stage_in_cap, ss.end);
             if (rc2) return rc2;
-            if ((rc2 = gvs_read(e, io, ti, DBEEL_STREAM_INDEX, ss, e->ring_in))) return fail(e, rc2, "stream read callback failed (.index, leaves)");
+            if ((rc2 = gvs_load(e, io, reader, DBEEL_STREAM_INDEX, {GvsPart{ti, &ss}}, e->ring_in, e->stage_in, hdr, ss.end, true,
+                                "stream read callback failed (.index, leaves)")))
+                return rc2;
             std::vector<ByteRange> win(nl);
             std::vector<uint8_t> has(nl, 0);
             std::vector<ByteRange> wr;
@@ -2521,7 +2614,9 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
             rc2 = ensure_host(e, &e->ring_out, &e->ring_out_cap, sw.end);
             if (!rc2) rc2 = ensure_device(e, &e->stage_in2, &e->stage_in2_cap, sw.end);
             if (rc2) return rc2;
-            if ((rc2 = gvs_read(e, io, ti, DBEEL_STREAM_DATA, sw, e->ring_out))) return fail(e, rc2, "stream read callback failed (.data, leaves)");
+            if ((rc2 = gvs_load(e, io, reader, DBEEL_STREAM_DATA, {GvsPart{ti, &sw}}, e->ring_out, e->stage_in2, 0, sw.end, false,
+                                "stream read callback failed (.data, leaves)")))
+                return rc2;
             GvsLeaf *hl = reinterpret_cast<GvsLeaf *>(e->ring_in + o_hdr);
             for (uint32_t k = 0; k < nl; k++) {
                 // biased: record r of the table at index + r, file offset o at data + o (a leaf whose records all point past
@@ -2531,8 +2626,7 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
                                             : reinterpret_cast<uintptr_t>(e->stage_in2);
                 hl[k] = GvsLeaf{reinterpret_cast<const uint8_t *>(db), reinterpret_cast<const uint4 *>(ib), group[k], 0, 0};
             }
-            CU(cudaMemcpyAsync(e->stage_in, e->ring_in, ss.end, cudaMemcpyHostToDevice, s));
-            if (sw.end) CU(cudaMemcpyAsync(e->stage_in2, e->ring_out, sw.end, cudaMemcpyHostToDevice, s));
+            CU(cudaMemcpyAsync(e->stage_in, e->ring_in, hdr, cudaMemcpyHostToDevice, s));
             CU(cudaMemsetAsync(d_need, 0, 8, s));
             launch_k(e, k_lookup_leaf, grid, 256, 0, s, gq, t, reinterpret_cast<const GvsLeaf *>(e->stage_in + o_hdr), nl, depth, ti, d_need);
             CU(cudaMemcpyAsync(e->pin, d_need, 8, cudaMemcpyDeviceToHost, s));
@@ -2556,8 +2650,8 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
             if (!touched[L]) continue;
             uint64_t a, b;
             search_interval(mode, pt.state[leaf0 + L], &a, &b);
-            const uint64_t bytes = (b - a) * per_rec + 8 + max_klen;
-            if (!group.empty() && est + bytes > budget) {
+            const uint64_t bytes = (b - a) * per_rec + 8 + max_klen + (paged ? 2 * kPageBytes : 0);
+            if (!group.empty() && est + bytes > group_bytes) {
                 if ((rc = run_group())) return rc;
                 est = 0;
             }
@@ -2599,9 +2693,12 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
         }
         if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, std::max<uint64_t>(staged, 256)))) return rc;
         if ((rc = heap_reserve(base + staged + 256))) return rc;
+        std::vector<GvsPart> parts;
         for (uint32_t i = 0; i < n_tables; i++)
-            if ((rc = gvs_read(e, io, i, DBEEL_STREAM_DATA, sh[i], e->ring_in))) return fail(e, rc, "stream read callback failed (.data, entries)");
-        if (staged) CU(cudaMemcpyAsync(e->stage_out2 + base, e->ring_in, staged, cudaMemcpyHostToDevice, s));
+            if (!sh[i].runs.empty()) parts.push_back(GvsPart{i, &sh[i]});
+        if ((rc = gvs_load(e, io, reader, DBEEL_STREAM_DATA, parts, e->ring_in, e->stage_out2 + base, 0, staged, false,
+                           "stream read callback failed (.data, entries)")))
+            return rc;
         for (uint64_t q = 0; q < n_keys; q++) {
             ByteRange r;
             if (hoff[q] != kGvsFenceHit) continue;
@@ -3095,7 +3192,10 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
         CU(cudaGetLastError());
         CU(cudaStreamSynchronize(s));
 
-        // ---- touched leaves, in groups of about `budget` bytes: per table its index slices, then their windows
+        // ---- touched leaves, in groups of about `budget` bytes (with a page cache, at most its capacity): per table its
+        // index slices, then their windows
+        const bool paged = r->cache != nullptr; // a leaf's slice and window each end in pages of their own
+        const uint64_t group_bytes = paged ? std::min(budget, kPageBytes * r->cache->pc.capacity()) : budget;
         struct Leaf { uint32_t t, leaf; };
         std::vector<Leaf> group;
         auto run_group = [&]() -> int {
@@ -3110,7 +3210,8 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
             const uint64_t o_first = align_up(sizeof(GvsLeaf) * nl, 16);
             std::vector<GvsStaged> ss(nseek), sw(nseek);
             std::vector<uint32_t> first(nseek + 1, 0);
-            uint64_t end = align_up(o_first + 4ull * (nseek + 1), kAlign);
+            const uint64_t hdr = align_up(o_first + 4ull * (nseek + 1), kAlign);
+            uint64_t end = hdr;
             for (uint32_t k = 0, t = 0; t < nseek; t++) {
                 std::vector<ByteRange> x;
                 first[t] = k;
@@ -3122,9 +3223,12 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
             int rc2 = ensure_host(e, &e->ring_in, &e->ring_in_cap, end);
             if (!rc2) rc2 = ensure_device(e, &e->stage_in, &e->stage_in_cap, end);
             if (rc2) return rc2;
+            std::vector<GvsPart> parts;
             for (uint32_t t = 0; t < nseek; t++)
-                if (!ss[t].runs.empty() && (rc2 = gvs_read(e, io, t, DBEEL_STREAM_INDEX, ss[t], e->ring_in)))
-                    return fail(e, rc2, "stream read callback failed (.index, leaves)");
+                if (!ss[t].runs.empty()) parts.push_back(GvsPart{t, &ss[t]});
+            if ((rc2 = gvs_load(e, io, r, DBEEL_STREAM_INDEX, parts, e->ring_in, e->stage_in, hdr, end, true,
+                                "stream read callback failed (.index, leaves)")))
+                return rc2;
             std::vector<ByteRange> win(nl);
             std::vector<uint8_t> has(nl, 0);
             uint64_t wend = 0;
@@ -3141,9 +3245,12 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
             rc2 = ensure_host(e, &e->ring_out, &e->ring_out_cap, std::max<uint64_t>(wend, 256));
             if (!rc2) rc2 = ensure_device(e, &e->stage_in2, &e->stage_in2_cap, std::max<uint64_t>(wend, 256));
             if (rc2) return rc2;
+            parts.clear();
             for (uint32_t t = 0; t < nseek; t++)
-                if (!sw[t].runs.empty() && (rc2 = gvs_read(e, io, t, DBEEL_STREAM_DATA, sw[t], e->ring_out)))
-                    return fail(e, rc2, "stream read callback failed (.data, leaves)");
+                if (!sw[t].runs.empty()) parts.push_back(GvsPart{t, &sw[t]});
+            if ((rc2 = gvs_load(e, io, r, DBEEL_STREAM_DATA, parts, e->ring_out, e->stage_in2, 0, wend, false,
+                                "stream read callback failed (.data, leaves)")))
+                return rc2;
             GvsLeaf *hl = reinterpret_cast<GvsLeaf *>(e->ring_in);
             for (uint32_t t = 0; t < nseek; t++) {
                 for (uint32_t k = first[t]; k < first[t + 1]; k++) { // biased as in dbeel_get_values_stream's leaves
@@ -3154,8 +3261,7 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
                 }
             }
             memcpy(e->ring_in + o_first, first.data(), 4ull * (nseek + 1));
-            CU(cudaMemcpyAsync(e->stage_in, e->ring_in, end, cudaMemcpyHostToDevice, s));
-            if (wend) CU(cudaMemcpyAsync(e->stage_in2, e->ring_out, wend, cudaMemcpyHostToDevice, s));
+            CU(cudaMemcpyAsync(e->stage_in, e->ring_in, hdr, cudaMemcpyHostToDevice, s));
             launch_k(e, k_seek_leaf, grid, 256, 0, s, sq, reinterpret_cast<const TableDesc *>(ws + o_td),
                      reinterpret_cast<const uint32_t *>(ws + o_depth), reinterpret_cast<const GvsLeaf *>(e->stage_in),
                      reinterpret_cast<const uint32_t *>(e->stage_in + o_first));
@@ -3172,8 +3278,8 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
                 if (!touched[touched_at[t] + L]) continue;
                 uint64_t a, b;
                 search_interval(DBEEL_LOOKUP_EXACT, pts[t]->state[leaf0 + L], &a, &b);
-                const uint64_t bytes = (b - a) * per_rec + 8 + max_klen;
-                if (!group.empty() && est + bytes > budget) {
+                const uint64_t bytes = (b - a) * per_rec + 8 + max_klen + (paged ? 2 * kPageBytes : 0);
+                if (!group.empty() && est + bytes > group_bytes) {
                     if ((rc = run_group())) return rc;
                     est = 0;
                 }
@@ -3387,6 +3493,8 @@ void dbeel_engine_destroy(dbeel_engine *e) {
     if (e->stream) cudaStreamSynchronize(e->stream);
     for (dbeel_reader *r : e->readers) delete r; // the tables a tree still shares stay with the tree
     e->readers.clear();
+    for (dbeel_page_cache *c : e->page_caches) delete c;
+    e->page_caches.clear();
     for (int i = 0; i < EV_COUNT; i++)
         if (e->ev[i]) cudaEventDestroy(e->ev[i]);
     if (e->ws) cudaFree(e->ws);
@@ -3675,6 +3783,64 @@ void dbeel_reader_close(dbeel_reader *r) {
     v.erase(std::remove(v.begin(), v.end(), r), v.end());
     cudaSetDevice(r->e->device);
     delete r;
+}
+
+int dbeel_page_cache_create(dbeel_engine *e, uint64_t bytes, dbeel_page_cache **out) {
+    REFUSE_WHILE_ASYNC(e);
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (!out) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    *out = nullptr;
+    const uint64_t slots = bytes / kPageBytes;
+    if (slots == 0) return fail(e, DBEEL_ERR_INVALID_ARG, "a page cache needs at least one 4096-byte page");
+    if (slots > 0xFFFFFFFFull) return fail(e, DBEEL_ERR_INVALID_ARG, "a page cache holds at most 2^32 - 1 pages");
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    CU(cudaSetDevice(e->device));
+    uint8_t *pool = nullptr;
+    cudaError_t ce = cudaMalloc(reinterpret_cast<void **>(&pool), slots * kPageBytes);
+    if (ce != cudaSuccess) { cudaGetLastError(); return fail(e, DBEEL_ERR_NOMEM, "cudaMalloc(page cache)", ce); }
+    dbeel_page_cache *c = new (std::nothrow) dbeel_page_cache(slots);
+    if (!c) { cudaFree(pool); return fail(e, DBEEL_ERR_NOMEM, "page cache"); }
+    c->e = e;
+    c->pool = pool;
+    e->page_caches.push_back(c);
+    *out = c;
+    return DBEEL_OK;
+}
+
+void dbeel_page_cache_destroy(dbeel_page_cache *c) {
+    if (!c) return;
+    dbeel_engine *e = c->e;
+    for (dbeel_reader *r : e->readers)
+        if (r->cache == c) r->cache = nullptr;
+    auto &v = e->page_caches;
+    v.erase(std::remove(v.begin(), v.end(), c), v.end());
+    cudaSetDevice(e->device);
+    cudaStreamSynchronize(e->stream); // copies still reading its slots
+    delete c;
+}
+
+int dbeel_reader_attach_page_cache(dbeel_reader *r, dbeel_page_cache *c) {
+    if (!r) return DBEEL_ERR_INVALID_ARG;
+    dbeel_engine *e = r->e;
+    REFUSE_WHILE_ASYNC(e);
+    if (c && c->e != e) return fail(e, DBEEL_ERR_INVALID_ARG, "the page cache belongs to another engine");
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    r->cache = c;
+    return DBEEL_OK;
+}
+
+int dbeel_page_cache_stats(const dbeel_page_cache *c, struct dbeel_page_cache_stats *out) {
+    if (!c || !out) return DBEEL_ERR_INVALID_ARG;
+    REFUSE_WHILE_ASYNC(c->e);
+    if (c->e->busy) return DBEEL_ERR_BUSY;
+    out->capacity_pages = c->pc.capacity();
+    out->resident_pages = c->pc.resident();
+    out->hits = c->pc.hits;
+    out->misses = c->pc.misses;
+    out->evictions = c->pc.evictions;
+    return DBEEL_OK;
 }
 
 int dbeel_scan_bound(const dbeel_table *tables, uint32_t n_tables, uint64_t *data_cap, uint64_t *index_cap) {

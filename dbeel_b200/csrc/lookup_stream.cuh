@@ -7,6 +7,7 @@
 //   k_lookup_leaf  resumes the search inside a staged leaf: the table's TableDesc with .index / .data biased to the slice and
 //                  the window, so probe() checks the same bounds against the file's data_len as k_lookup does
 //   k_gvs_copy     copies the entries of the group's hits out of the window into the hit heap before the window is reused
+//   k_page_copy    with a page cache attached to a reader: assembles the staged slices, windows and entries from its pages
 //
 // Hits at fences have no window: their entries are read one record each after the last table.  Then k_gvs_hit decodes
 // every hit's entry from the heap the way k_lookup_emit decodes it.
@@ -184,8 +185,19 @@ __global__ void __launch_bounds__(256) k_lookup_leaf(GvsQueries g, TableDesc t, 
     g.node[q] = 0;
 }
 
+// n bytes from s to d by the 32 lanes of a warp, d congruent to s modulo 16: bytes up to s's first 16-byte boundary,
+// 16-byte copies in the middle, bytes at the end.
+__device__ __forceinline__ void warp_copy_congruent(const uint8_t *s, uint8_t *d, uint64_t n, uint32_t lane) {
+    const uint64_t a = reinterpret_cast<uintptr_t>(s) & 15;
+    const uint64_t head = ((16 - a) & 15) < n ? ((16 - a) & 15) : n;
+    const uint64_t body = (n - head) / 16, tail0 = head + 16 * body;
+    for (uint64_t i = lane; i < head; i += 32) d[i] = s[i];
+    for (uint64_t i = lane; i < body; i += 32) reinterpret_cast<uint4 *>(d + head)[i] = reinterpret_cast<const uint4 *>(s + head)[i];
+    for (uint64_t i = tail0 + lane; i < n; i += 32) d[i] = s[i];
+}
+
 // One warp per query: a leaf hit's entry from its window into the hit heap, at a position congruent to the source modulo
-// 16 (16-byte copies in the middle, bytes at the ends), so entries of any size, multi-megabyte ones included, move at once.
+// 16, so entries of any size, multi-megabyte ones included, move at once.
 __global__ void __launch_bounds__(256) k_gvs_copy(GvsQueries g, uint8_t *heap, unsigned long long *cursor) {
     pdl_trigger();
     pdl_wait();
@@ -198,17 +210,27 @@ __global__ void __launch_bounds__(256) k_gvs_copy(GvsQueries g, uint8_t *heap, u
     unsigned long long pos = 0;
     if (lane == 0) pos = atomicAdd(cursor, (unsigned long long)((fs + 15) / 16 * 16 + 16));
     pos = __shfl_sync(0xFFFFFFFFu, pos, 0) + (src & 15);
-    const uint8_t *s = reinterpret_cast<const uint8_t *>(src);
-    uint8_t *d = heap + pos;
-    const uint64_t head = ((16 - (src & 15)) & 15) < fs ? ((16 - (src & 15)) & 15) : fs;
-    const uint64_t body = (fs - head) / 16, tail0 = head + 16 * body;
-    for (uint64_t i = lane; i < head; i += 32) d[i] = s[i];
-    for (uint64_t i = lane; i < body; i += 32) reinterpret_cast<uint4 *>(d + head)[i] = reinterpret_cast<const uint4 *>(s + head)[i];
-    for (uint64_t i = tail0 + lane; i < fs; i += 32) d[i] = s[i];
+    warp_copy_congruent(reinterpret_cast<const uint8_t *>(src), heap + pos, fs, lane);
     if (lane == 0) {
         g.hit_off[q] = pos;
         g.hit_src[q] = 0;
     }
+}
+
+// The page cache's copies of one request (host/page_cache.h): miss image -> slot, miss image -> destination image and
+// slot -> destination image, every source congruent to its destination modulo 16.  One warp per copy.  (Under plain
+// __launch_bounds__(256) ptxas holds it to 40 registers and spills 16 bytes; a minimum of 4 CTAs per SM leaves it 44 and
+// no spill.)
+struct PageCopy {
+    unsigned long long src, dst, len, pad;
+};
+
+__global__ void __launch_bounds__(256, 4) k_page_copy(const PageCopy *c, uint64_t n) {
+    pdl_trigger();
+    pdl_wait();
+    const uint64_t k = ((uint64_t)blockIdx.x * 256u + threadIdx.x) / 32;
+    if (k >= n) return;
+    warp_copy_congruent(reinterpret_cast<const uint8_t *>(c[k].src), reinterpret_cast<uint8_t *>(c[k].dst), c[k].len, threadIdx.x & 31);
 }
 
 // After the last table: every hit's entry as k_lookup_emit decodes it, from the heap (hit_off: its offset there, or

@@ -133,7 +133,9 @@ class LSMTree:
 
     def set_page_cache(self, cache: Optional[dict]):
         """Mirror EntryWriter's write-through: every SSTable this tree writes from now on is also `set` page by page into
-        `cache` under the reference's key ((FileTypeKind, files_index), address) (entry_writer.rs:100-156).  None = off."""
+        `cache` under the reference's key ((FileTypeKind, files_index), address) (entry_writer.rs:100-156).  None = off.
+        This is a host-side mirror of the reference's cache; the device page cache that readers read through is
+        capi.PageCache (open_reader(page_cache=...)), which this does not fill."""
         if cache is None:
             self._sink = PAGE_SINK(0)
         else:
@@ -242,17 +244,22 @@ class LSMTree:
             self._check(rc, "LSMTree.get_values_stream")
             return res, od[:out.data_len], oi[:out.index_len]
 
-    def open_reader(self, fence_bytes: int = 0) -> capi.Reader:
+    def open_reader(self, fence_bytes: int = 0, page_cache: Optional[capi.PageCache] = None) -> capi.Reader:
         """dbeel_tree_reader_open: a capi.Reader over a snapshot of the tree's SSTables (get_values answers what
         get_values_stream answered at open, scan what scan_stream returned at open, table = a position in the snapshot),
         unaffected by later flushes and compactions.  Readers share the tables they have in common: one opened after a
-        flush loads only the new ones."""
+        flush loads only the new ones.  page_cache: a capi.PageCache (Engine.open_page_cache) the reader reads its leaves
+        and entries through; pages of the tables it shares with earlier readers of the same cache are hits.  (Not
+        set_page_cache, the host-side mirror of the reference's write-through.)"""
         from . import sstable
         h = C.c_void_p()
         self._check(_lib().dbeel_tree_reader_open(self._h, fence_bytes, C.byref(h)), "LSMTree.open_reader")
         dc = sum(os.path.getsize(os.path.join(self.dir, sstable.file_name(idx, sstable.DATA_FILE_EXT)))
                  for idx, _ in self.sstable_indices_and_sizes())
-        return capi.Reader(h, self._engine, data_cap=dc)
+        r = capi.Reader(h, self._engine, data_cap=dc)
+        if page_cache is not None:
+            r.attach_page_cache(page_cache)
+        return r
 
     def scan(self, ranges, kind: int = capi.SCAN_HASH):
         """The SSTable part of iter_filter (lsm_tree.rs:133-282) over the tree's files, oldest table first: every entry

@@ -523,6 +523,46 @@ int dbeel_reader_scan(dbeel_reader *r, uint32_t kind, const void *ranges, uint32
                       void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop);
 void dbeel_reader_close(dbeel_reader *r);
 
+/* Page cache for readers: the reference reads every .data / .index byte of a lookup or seek through a per-shard cache of
+ * 4096-byte pages (CachedFileReader::read_at_into over PartitionPageCache, cached_file_reader.rs:28-79); this one keeps such
+ * pages on the device, across batches and across the readers attached to it.
+ *   - dbeel_page_cache_create: bytes / 4096 page slots in one device allocation on the engine's device, made now; the page
+ *     table lives on the host, and no other device memory is taken.  Fewer than one slot is DBEEL_ERR_INVALID_ARG, a failed
+ *     allocation DBEEL_ERR_NOMEM.
+ *   - A page is the 4096 bytes at a page-aligned offset of one reader table's .data or .index; a file's last page holds only
+ *     the bytes up to the file's length (never anything past EOF).  It is keyed by (table, file kind, page), where a table
+ *     is what a tree's readers share (a reader opened after a flush hits on every table it shares with the reader before
+ *     it), and a table that is gone is never hit again: its pages age out.
+ *   - Contract: a reader's table files do not change while it is open (SSTables are immutable; cached fences assume it too).
+ *   - dbeel_reader_attach_page_cache(r, c) makes r read through c from its next call; NULL detaches.  A cache of another
+ *     engine is DBEEL_ERR_INVALID_ARG.  Any number of readers may share one cache.
+ *   - Through the cache go the leaf .index slices and .data windows of dbeel_reader_get_values and the entries of its hits
+ *     at fences, and the leaf slices and windows of dbeel_reader_scan's seeks (DBEEL_SCAN_KEY).  Resident pages are copied
+ *     on the device; the missing ones are read through io.read as page-aligned ranges clipped to the file's length (the
+ *     consecutive missing pages of a file as one read, in pieces of at most 8 MiB), and become resident only once their
+ *     read has returned 0.  Eviction is CLOCK (second chance); the pages one step of a call needs are never evicted by it.
+ *     A step that needs more pages than the cache has slots (a leaf larger than the cache) reads uncached.
+ *   - Not through the cache: fence loads and per-call fences (a reader keeps its fences itself), hash scans, and the span
+ *     partitions of key scans, which stream whole ranges once and would evict the point-read working set.
+ *   - A cached reader returns exactly what it returns uncached (rows and flags, out, items_written, DBEEL_ERR_CAPACITY with
+ *     the sizes needed, stops, callback codes unchanged); only what goes through the callback changes, and
+ *     dbeel_last_stats' input_bytes still counts it.  After a callback error the cache holds only good pages, and both the
+ *     reader and the cache stay usable.
+ *   - dbeel_page_cache_stats: capacity / resident in pages; hits, misses and evictions in pages since create.
+ *   - dbeel_page_cache_destroy detaches the cache from every reader that has it (they go on uncached);
+ *     dbeel_engine_destroy destroys the caches still open.  Create, attach and stats take the engine as every entry point
+ *     does (DBEEL_ERR_BUSY while another call runs). */
+typedef struct dbeel_page_cache dbeel_page_cache;
+/* a struct tag only, as POSIX's struct stat beside stat(): the function takes the plain name */
+struct dbeel_page_cache_stats {
+    uint64_t capacity_pages, resident_pages;
+    uint64_t hits, misses, evictions; /* pages, since create */
+};
+int dbeel_page_cache_create(dbeel_engine *e, uint64_t bytes, dbeel_page_cache **out);
+void dbeel_page_cache_destroy(dbeel_page_cache *c);
+int dbeel_reader_attach_page_cache(dbeel_reader *r, dbeel_page_cache *c /* NULL detaches */);
+int dbeel_page_cache_stats(const dbeel_page_cache *c, struct dbeel_page_cache_stats *out);
+
 /* ---- N4: write-ahead-log replay + flush ------------------------------------------------------------------------
  * Replaces LSMTree::read_memtable_from_wal_file (lsm_tree.rs:552-574) followed by flush_memtable_to_disk, i.e. the
  * recovery of an unflushed memtable in open_or_create_ex (:478-513).  `wal` is the whole `.memtable` file: bincode

@@ -99,7 +99,10 @@ int dbeel_tree_get_values_stream(dbeel_tree *t, const void *keys, const uint64_t
  * the readers that include the table: a reader opened after a flush or a compaction loads only the tables no live entry
  * has, and a table it shares keeps the fence depth it was loaded with (its fences count against fence_bytes first).  An
  * entry is dropped when no reader holds it and its table has left the tree; dbeel_tree_close drops the tree's entries
- * (open readers keep theirs until they are closed). */
+ * (open readers keep theirs until they are closed).
+ * A device page cache (dbeel_page_cache_create, dbeel_reader_attach_page_cache) keys its pages by that shared entry, so a
+ * reader opened after a flush and attached to the same cache hits on every table it shares with the readers before it.
+ * The tree's own page sink (dbeel_tree_set_page_sink) is a separate, host-side mirror and does not fill it. */
 int dbeel_tree_reader_open(dbeel_tree *t, uint64_t fence_bytes, dbeel_reader **out);
 
 /* The SSTable part of LSMTree::iter_filter over the tree's files: every table's .data / .index in dbeel_tree_sstables()
