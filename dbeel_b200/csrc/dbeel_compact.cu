@@ -2226,16 +2226,18 @@ int gvs_read(dbeel_engine *e, const dbeel_scan_io *io, uint32_t t, uint32_t kind
 
 // The fences of the open internal nodes of pt, through the callback: their index records (runs closer than
 // kLookupMergeGap as one read) into fix[k], then their key frames of up to max_klen key bytes (runs that touch as one
-// read) into ring_in, staged from `base` on (sf).  has[k]: node k's record points inside .data and its frame is frame[k].
+// read) into frames, staged by sf.  has[k]: node k's record points inside .data and its frame is frame[k].
 struct GvsFenceReads {
     std::vector<uint4> fix;
     std::vector<ByteRange> frame;
     std::vector<uint8_t> has;
     GvsStaged sf;
+    std::vector<uint8_t> frames;
+    uint64_t image_bytes() const { return 24 * fix.size() + sf.end; } // gvs_fence_image
 };
 
 int gvs_read_fences(dbeel_engine *e, const dbeel_scan_io *io, uint32_t ti, const ProbeTree &pt, uint64_t data_len, uint64_t max_klen,
-                    uint64_t base, GvsFenceReads *f) {
+                    GvsFenceReads *f) {
     const uint32_t mode = pt.mode;
     const uint64_t leaf0 = 1ull << pt.depth;
     int rc;
@@ -2254,9 +2256,9 @@ int gvs_read_fences(dbeel_engine *e, const dbeel_scan_io *io, uint32_t ti, const
         memcpy(&f->fix[k], e->ring_out + si.at(16 * search_pos(mode, pt.state[k])), 16);
         if (probe_frame(reinterpret_cast<const uint8_t *>(&f->fix[k]), data_len, max_klen, &f->frame[k])) { f->has[k] = 1; fr.push_back(f->frame[k]); }
     }
-    f->sf = gvs_stage(fr, 0, base);
-    if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, f->sf.end))) return rc;
-    if ((rc = gvs_read(e, io, ti, DBEEL_STREAM_DATA, f->sf, e->ring_in))) return fail(e, rc, "stream read callback failed (.data, fences)");
+    f->sf = gvs_stage(fr, 0, 0);
+    f->frames.resize(f->sf.end);
+    if ((rc = gvs_read(e, io, ti, DBEEL_STREAM_DATA, f->sf, f->frames.data()))) return fail(e, rc, "stream read callback failed (.data, fences)");
     return DBEEL_OK;
 }
 
@@ -2265,6 +2267,20 @@ int gvs_read_fences(dbeel_engine *e, const dbeel_scan_io *io, uint32_t ti, const
 inline unsigned long long gvs_frame_addr(const GvsFenceReads &f, uint64_t k, uint64_t data_len, const uint8_t *host, const uint8_t *dev) {
     if (!f.has[k] || rd64(host) > data_len - f.frame[k].lo - 8) return 0;
     return reinterpret_cast<unsigned long long>(dev);
+}
+
+// The fences of one table read for one call, as GvsFences descends them: fix[2^depth] | ffr[2^depth] | frames, written
+// at img (host, image_bytes()) for a device copy at dev, which ffr points into.  With dev 16-aligned and depth >= 1, every
+// frame stays congruent to its file offset modulo 16.
+void gvs_fence_image(const GvsFenceReads &f, uint64_t data_len, uint8_t *img, uint8_t *dev) {
+    const uint64_t leaf0 = f.fix.size(), o_frames = 24 * leaf0;
+    memcpy(img, f.fix.data(), 16 * leaf0);
+    memcpy(img + o_frames, f.frames.data(), f.sf.end);
+    unsigned long long *ffr = reinterpret_cast<unsigned long long *>(img + 16 * leaf0);
+    for (uint64_t k = 0; k < leaf0; k++) {
+        const uint64_t p = o_frames + (f.has[k] ? f.sf.at(f.frame[k].lo) : 0);
+        ffr[k] = gvs_frame_addr(f, k, data_len, img + p, dev + p);
+    }
 }
 
 } // namespace
@@ -2328,7 +2344,7 @@ int reader_load_fences(dbeel_engine *e, const dbeel_scan_io *io, uint32_t ti, db
     const uint64_t leaf0 = 1ull << rt->depth, data_len = rt->desc.data_len;
     if (rt->depth > 0) {
         GvsFenceReads fr;
-        int rc = gvs_read_fences(e, io, ti, c.pt, data_len, kReaderFrameCap, 0, &fr);
+        int rc = gvs_read_fences(e, io, ti, c.pt, data_len, kReaderFrameCap, &fr);
         if (rc) return rc;
         const uint64_t o_ffr = 16 * leaf0, o_slot = o_ffr + 8 * leaf0, bytes = o_slot + kReaderFrameSlot * leaf0;
         if ((rc = ensure_host(e, &e->ring_out, &e->ring_out_cap, bytes))) return rc;
@@ -2344,7 +2360,7 @@ int reader_load_fences(dbeel_engine *e, const dbeel_scan_io *io, uint32_t ti, db
         unsigned long long *ffr = reinterpret_cast<unsigned long long *>(img + o_ffr);
         for (uint64_t k = 0; k < leaf0; k++) {
             uint8_t *slot = img + o_slot + kReaderFrameSlot * k;
-            if (fr.has[k]) memcpy(slot, e->ring_in + fr.sf.at(fr.frame[k].lo), fr.frame[k].hi - fr.frame[k].lo);
+            if (fr.has[k]) memcpy(slot, fr.frames.data() + fr.sf.at(fr.frame[k].lo), fr.frame[k].hi - fr.frame[k].lo);
             ffr[k] = gvs_frame_addr(fr, k, data_len, slot, c.dev + o_slot + kReaderFrameSlot * k);
         }
         CU(cudaMemcpyAsync(c.dev, img, bytes, cudaMemcpyHostToDevice, e->stream));
@@ -2419,6 +2435,71 @@ int gvs_load(dbeel_engine *e, const dbeel_scan_io *io, const dbeel_reader *r, ui
     return DBEEL_OK;
 }
 
+// One group of touched leaves (group_leaves), ascending (table, leaf), on the device for k_lookup_leaf / k_seek_leaf: per
+// table its index slices into stage_in behind the header (through ring_in, and back to it), then the .data windows of
+// those slices (leaf_window) into stage_in2 (through ring_out).  The header at stage_in is GvsLeaf[nl] | first[nt + 1]
+// (nt = data_len.size()): table t's leaves are [first[t], first[t + 1]), each biased so that record r of the table lies
+// at index + r and file offset o at data + o (a leaf whose records all point past the file never dereferences data:
+// probe() reports them corrupt first).  Through gvs_load, so with a page cache this writes stage_out: reader_scan_key's
+// per-call fences live there, and its k_seek_fence has completed (a synchronise) before the first group is loaded.
+int gvs_load_leaves(dbeel_engine *e, const dbeel_scan_io *io, const dbeel_reader *r, const TouchedLeaf *lv, uint32_t nl,
+                    const std::vector<uint64_t> &data_len, uint64_t max_klen) {
+    const uint32_t nt = (uint32_t)data_len.size();
+    std::vector<uint32_t> first(nt + 1, 0);
+    for (uint32_t k = 0; k < nl; k++) first[lv[k].t + 1]++;
+    for (uint32_t t = 0; t < nt; t++) first[t + 1] += first[t];
+    const uint64_t o_first = sizeof(GvsLeaf) * nl, hdr = align_up(o_first + 4ull * (nt + 1), kAlign);
+    std::vector<GvsStaged> ss(nt), sw(nt);
+    std::vector<GvsPart> parts;
+    uint64_t end = hdr;
+    for (uint32_t t = 0; t < nt; t++) {
+        if (first[t] == first[t + 1]) continue;
+        std::vector<ByteRange> x;
+        for (uint32_t k = first[t]; k < first[t + 1]; k++) x.push_back({16 * lv[k].a, 16 * lv[k].b});
+        ss[t] = gvs_stage(std::move(x), kLookupMergeGap, end);
+        end = ss[t].end;
+        parts.push_back(GvsPart{t, &ss[t]});
+    }
+    int rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, end);
+    if (!rc) rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, end);
+    if (rc) return rc;
+    if ((rc = gvs_load(e, io, r, DBEEL_STREAM_INDEX, parts, e->ring_in, e->stage_in, hdr, end, true, "stream read callback failed (.index, leaves)")))
+        return rc;
+    std::vector<ByteRange> win(nl);
+    std::vector<uint8_t> has(nl, 0);
+    uint64_t wend = 0;
+    parts.clear();
+    for (uint32_t t = 0; t < nt; t++) {
+        if (first[t] == first[t + 1]) continue;
+        std::vector<ByteRange> wr;
+        for (uint32_t k = first[t]; k < first[t + 1]; k++)
+            if (leaf_window(e->ring_in + ss[t].at(16 * lv[k].a), lv[k].b - lv[k].a, data_len[t], max_klen, &win[k])) {
+                has[k] = 1;
+                wr.push_back(win[k]);
+            }
+        sw[t] = gvs_stage(std::move(wr), 0, wend);
+        wend = sw[t].end;
+        if (!sw[t].runs.empty()) parts.push_back(GvsPart{t, &sw[t]});
+    }
+    rc = ensure_host(e, &e->ring_out, &e->ring_out_cap, std::max<uint64_t>(wend, 256));
+    if (!rc) rc = ensure_device(e, &e->stage_in2, &e->stage_in2_cap, std::max<uint64_t>(wend, 256));
+    if (rc) return rc;
+    if ((rc = gvs_load(e, io, r, DBEEL_STREAM_DATA, parts, e->ring_out, e->stage_in2, 0, wend, false, "stream read callback failed (.data, leaves)")))
+        return rc;
+    GvsLeaf *hl = reinterpret_cast<GvsLeaf *>(e->ring_in);
+    for (uint32_t k = 0; k < nl; k++) {
+        const uint32_t t = lv[k].t;
+        const uint64_t lo = 16 * lv[k].a;
+        const uintptr_t ib = reinterpret_cast<uintptr_t>(e->stage_in + ss[t].at(lo)) - lo;
+        const uintptr_t db = has[k] ? reinterpret_cast<uintptr_t>(e->stage_in2 + sw[t].at(win[k].lo)) - win[k].lo
+                                    : reinterpret_cast<uintptr_t>(e->stage_in2);
+        hl[k] = GvsLeaf{reinterpret_cast<const uint8_t *>(db), reinterpret_cast<const uint4 *>(ib), lv[k].leaf, 0, 0};
+    }
+    memcpy(e->ring_in + o_first, first.data(), 4ull * (nt + 1));
+    CU(cudaMemcpyAsync(e->stage_in, e->ring_in, hdr, cudaMemcpyHostToDevice, e->stream));
+    return DBEEL_OK;
+}
+
 // Per table, newest first: k_gvs_filter -> fences read, k_lookup_fence -> touched leaves read in groups under the partition
 // budget, k_lookup_leaf per group and k_gvs_copy for the group's hits (their entries leave the window for the hit heap).
 // Then the entries of hits at fences are read into the heap, k_gvs_hit decodes every hit and split_emit writes `out` in
@@ -2473,11 +2554,14 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
     if ((rc = ensure_device(e, &e->bloom_dev, &e->bloom_dev_cap, std::max<uint64_t>(bloom_bytes, 256)))) return rc;
     uint8_t *ws = e->ws;
     std::vector<TableDesc> td(n_tables);
+    std::vector<uint64_t> nrecs(n_tables), data_lens(n_tables);
     uint64_t bpos = 0;
     for (uint32_t i = 0; i < n_tables; i++) {
         const dbeel_table &t = tables[i];
         td[i] = TableDesc{nullptr, t.data_len, nullptr, t.index_len / DBEEL_INDEX_ENTRY_SIZE, nullptr, 0, 0, 0, 0, {0, 0, 0, 0}};
         if (reader) td[i] = reader->tables[i]->desc; // tables[] carries no filter: it is resident
+        nrecs[i] = td[i].n;
+        data_lens[i] = td[i].data_len;
         if (!t.bloom_len) continue;
         const uint8_t *b = static_cast<const uint8_t *>(t.bloom);
         if ((rc = parse_bloom(e, b, b + t.bloom_len - kBloomTrailer, t.bloom_len, &td[i]))) return rc;
@@ -2517,7 +2601,8 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
     const uint32_t grid = (n + 255) / 256;
     uint32_t launches = 0, groups = 0;
     const uint64_t budget = e->partition_bytes;
-    std::vector<uint8_t> touched;
+    const bool paged = reader && reader->cache;
+    const uint64_t group_bytes = paged ? std::min(budget, kPageBytes * reader->cache->pc.capacity()) : budget;
 
     for (uint32_t ti = n_tables; ti-- > 0;) { // sstables.iter().rev(): newest first
         const TableDesc &t = td[ti];
@@ -2552,27 +2637,18 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
         CU(cudaMemsetAsync(d_touched, 0, leaf0, s));
 
         // ---- fences: the index records of the open internal nodes, then their key frames (or the reader's copies)
-        if (depth > 0 && use_cache) {
-            GvsFences gf{reinterpret_cast<const uint4 *>(cache->dev), reinterpret_cast<const unsigned long long *>(cache->dev + 16 * leaf0),
-                         depth, ti, nrec, d_touched};
-            launch_k(e, k_lookup_fence, grid, 256, 0, s, gq, gf);
-            launches++;
-        } else if (depth > 0) {
-            const uint64_t o_fix = 0, o_ffr = align_up(16 * leaf0, kAlign);
-            GvsFenceReads fr;
-            if ((rc = gvs_read_fences(e, io, ti, pt, data_len, max_klen, align_up(o_ffr + 8 * leaf0, kAlign), &fr))) return rc;
-            const GvsStaged &sf = fr.sf;
-            if ((rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, sf.end))) return rc;
-            uint8_t *img = e->ring_in;
-            memcpy(img + o_fix, fr.fix.data(), 16 * leaf0);
-            unsigned long long *ffr = reinterpret_cast<unsigned long long *>(img + o_ffr);
-            for (uint64_t k = 0; k < leaf0; k++) {
-                const uint64_t p = fr.has[k] ? sf.at(fr.frame[k].lo) : 0;
-                ffr[k] = gvs_frame_addr(fr, k, data_len, img + p, e->stage_in + p);
+        if (depth > 0) {
+            if (!use_cache) {
+                GvsFenceReads fr;
+                if ((rc = gvs_read_fences(e, io, ti, pt, data_len, max_klen, &fr))) return rc;
+                const uint64_t bytes = fr.image_bytes();
+                if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, bytes))) return rc;
+                if ((rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, bytes))) return rc;
+                gvs_fence_image(fr, data_len, e->ring_in, e->stage_in);
+                CU(cudaMemcpyAsync(e->stage_in, e->ring_in, bytes, cudaMemcpyHostToDevice, s));
             }
-            CU(cudaMemcpyAsync(e->stage_in, img, sf.end, cudaMemcpyHostToDevice, s));
-            GvsFences gf{reinterpret_cast<const uint4 *>(e->stage_in + o_fix), reinterpret_cast<const unsigned long long *>(e->stage_in + o_ffr),
-                         depth, ti, nrec, d_touched};
+            const uint8_t *f = use_cache ? cache->dev : e->stage_in; // fix[leaf0] | ffr[leaf0] | ...
+            GvsFences gf{reinterpret_cast<const uint4 *>(f), reinterpret_cast<const unsigned long long *>(f + 16 * leaf0), depth, ti, nrec, d_touched};
             launch_k(e, k_lookup_fence, grid, 256, 0, s, gq, gf);
             launches++;
         } else {
@@ -2581,60 +2657,22 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
         CU(cudaMemcpyAsync(e->pin, d_touched, leaf0, cudaMemcpyDeviceToHost, s));
         CU(cudaGetLastError());
         CU(cudaStreamSynchronize(s));
-        touched.assign(e->pin, e->pin + leaf0);
 
-        // ---- leaves, in groups of about `budget` bytes (with a page cache, at most its capacity): index slices, then the
-        // windows their records point at
-        const uint64_t per_rec = 16 + (nrec ? (data_len + nrec - 1) / nrec : 0);
-        const bool paged = reader && reader->cache; // a leaf's slice and window each end in pages of their own
-        const uint64_t group_bytes = paged ? std::min(budget, kPageBytes * reader->cache->pc.capacity()) : budget;
-        std::vector<uint32_t> group;
-        auto run_group = [&]() -> int {
-            const uint32_t nl = (uint32_t)group.size();
-            std::vector<ByteRange> sr(nl);
-            for (uint32_t k = 0; k < nl; k++) {
-                uint64_t a, b;
-                search_interval(mode, pt.state[leaf0 + group[k]], &a, &b);
-                sr[k] = {16 * a, 16 * b};
-            }
-            const uint64_t o_hdr = 0, hdr = align_up(sizeof(GvsLeaf) * nl, kAlign);
-            const GvsStaged ss = gvs_stage(sr, kLookupMergeGap, hdr);
-            int rc2 = ensure_host(e, &e->ring_in, &e->ring_in_cap, ss.end);
-            if (!rc2) rc2 = ensure_device(e, &e->stage_in, &e->stage_in_cap, ss.end);
-            if (rc2) return rc2;
-            if ((rc2 = gvs_load(e, io, reader, DBEEL_STREAM_INDEX, {GvsPart{ti, &ss}}, e->ring_in, e->stage_in, hdr, ss.end, true,
-                                "stream read callback failed (.index, leaves)")))
-                return rc2;
-            std::vector<ByteRange> win(nl);
-            std::vector<uint8_t> has(nl, 0);
-            std::vector<ByteRange> wr;
-            for (uint32_t k = 0; k < nl; k++)
-                if (leaf_window(e->ring_in + ss.at(sr[k].lo), (sr[k].hi - sr[k].lo) / 16, data_len, max_klen, &win[k])) { has[k] = 1; wr.push_back(win[k]); }
-            const GvsStaged sw = gvs_stage(wr, 0, 0);
-            rc2 = ensure_host(e, &e->ring_out, &e->ring_out_cap, sw.end);
-            if (!rc2) rc2 = ensure_device(e, &e->stage_in2, &e->stage_in2_cap, sw.end);
-            if (rc2) return rc2;
-            if ((rc2 = gvs_load(e, io, reader, DBEEL_STREAM_DATA, {GvsPart{ti, &sw}}, e->ring_out, e->stage_in2, 0, sw.end, false,
-                                "stream read callback failed (.data, leaves)")))
-                return rc2;
-            GvsLeaf *hl = reinterpret_cast<GvsLeaf *>(e->ring_in + o_hdr);
-            for (uint32_t k = 0; k < nl; k++) {
-                // biased: record r of the table at index + r, file offset o at data + o (a leaf whose records all point past
-                // the file never dereferences data: probe() reports them corrupt first)
-                const uintptr_t ib = reinterpret_cast<uintptr_t>(e->stage_in + ss.at(sr[k].lo)) - sr[k].lo;
-                const uintptr_t db = has[k] ? reinterpret_cast<uintptr_t>(e->stage_in2 + sw.at(win[k].lo)) - win[k].lo
-                                            : reinterpret_cast<uintptr_t>(e->stage_in2);
-                hl[k] = GvsLeaf{reinterpret_cast<const uint8_t *>(db), reinterpret_cast<const uint4 *>(ib), group[k], 0, 0};
-            }
-            CU(cudaMemcpyAsync(e->stage_in, e->ring_in, hdr, cudaMemcpyHostToDevice, s));
+        // ---- leaves, in groups of about `budget` bytes (with a page cache, at most its capacity)
+        std::vector<TouchedLeaf> lv;
+        touched_leaves(pt, ti, e->pin, &lv);
+        const std::vector<size_t> cut = group_leaves(lv, nrecs, data_lens, max_klen, group_bytes, paged);
+        for (size_t gi = 0; gi + 1 < cut.size(); gi++) {
+            const uint32_t nl = (uint32_t)(cut[gi + 1] - cut[gi]);
+            if ((rc = gvs_load_leaves(e, io, reader, lv.data() + cut[gi], nl, data_lens, max_klen))) return rc;
             CU(cudaMemsetAsync(d_need, 0, 8, s));
-            launch_k(e, k_lookup_leaf, grid, 256, 0, s, gq, t, reinterpret_cast<const GvsLeaf *>(e->stage_in + o_hdr), nl, depth, ti, d_need);
+            launch_k(e, k_lookup_leaf, grid, 256, 0, s, gq, t, reinterpret_cast<const GvsLeaf *>(e->stage_in), nl, depth, ti, d_need);
             CU(cudaMemcpyAsync(e->pin, d_need, 8, cudaMemcpyDeviceToHost, s));
             CU(cudaGetLastError());
             CU(cudaStreamSynchronize(s));
             launches++;
             if (const uint64_t need = rd64(e->pin)) { // the group's hits leave the window for the heap before it is reused
-                if ((rc2 = heap_reserve(heap_bound + need))) return rc2;
+                if ((rc = heap_reserve(heap_bound + need))) return rc;
                 heap_bound += need;
                 launch_k(e, k_gvs_copy, (uint32_t)((32 * n_keys + 255) / 256), 256, 0, s, gq, e->stage_out2, d_cursor);
                 CU(cudaGetLastError());
@@ -2642,23 +2680,7 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
                 launches++;
             }
             groups++;
-            group.clear();
-            return DBEEL_OK;
-        };
-        uint64_t est = 0;
-        for (uint64_t L = 0; L < leaf0; L++) {
-            if (!touched[L]) continue;
-            uint64_t a, b;
-            search_interval(mode, pt.state[leaf0 + L], &a, &b);
-            const uint64_t bytes = (b - a) * per_rec + 8 + max_klen + (paged ? 2 * kPageBytes : 0);
-            if (!group.empty() && est + bytes > group_bytes) {
-                if ((rc = run_group())) return rc;
-                est = 0;
-            }
-            group.push_back((uint32_t)L);
-            est += bytes;
         }
-        if (!group.empty() && (rc = run_group())) return rc;
     }
 
     // ---- hits at fences: their entries, one record each (runs that touch as one read), into the heap behind the copies
@@ -3100,12 +3122,14 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
         std::vector<const ProbeTree *> pts(nseek);
         std::vector<GvsFences> gf(nseek);
         std::vector<GvsFenceReads> frs(nseek);
-        std::vector<uint64_t> img_at(nseek, ~0ull), touched_at(nseek + 1, 0);
-        std::vector<uint8_t> img;
+        std::vector<uint64_t> img_at(nseek, ~0ull), touched_at(nseek + 1, 0), nrecs(nseek), data_lens(nseek);
+        uint64_t img_bytes = 0;
         for (uint32_t t = 0; t < nseek; t++) {
             dbeel_reader_table *rt = r->tables[t].get();
             dbeel_reader_table::Fences &cache = rt->fences[DBEEL_LOOKUP_EXACT];
             const uint64_t n = rt->desc.n, dl = rt->desc.data_len;
+            nrecs[t] = n;
+            data_lens[t] = dl;
             const uint32_t want = lookup_depth(2ull * nd, n, dl, 8 + max_klen, budget);
             const bool use_cache = reader_uses_cache(max_klen, want, (uint32_t)rt->depth);
             depth[t] = use_cache ? (uint32_t)rt->depth : want;
@@ -3127,26 +3151,18 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
             plan_probe_tree(DBEEL_LOOKUP_EXACT, n, depth[t], &pt_call[t]);
             pts[t] = &pt_call[t];
             if (!depth[t]) continue;
-            GvsFenceReads &fr = frs[t];
-            if ((rc = gvs_read_fences(e, io, t, pt_call[t], dl, max_klen, 0, &fr))) return rc;
-            img_at[t] = align_up(img.size(), kAlign);
-            img.resize(img_at[t] + 24 * leaf0 + fr.sf.end);
-            memcpy(img.data() + img_at[t], fr.fix.data(), 16 * leaf0);
-            memcpy(img.data() + img_at[t] + 24 * leaf0, e->ring_in, fr.sf.end);
+            if ((rc = gvs_read_fences(e, io, t, pt_call[t], dl, max_klen, &frs[t]))) return rc;
+            img_at[t] = align_up(img_bytes, kAlign);
+            img_bytes = img_at[t] + frs[t].image_bytes();
         }
-        if (!img.empty()) {
-            if ((rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, img.size()))) return rc;
+        std::vector<uint8_t> img(img_bytes);
+        if (img_bytes) {
+            if ((rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, img_bytes))) return rc;
             for (uint32_t t = 0; t < nseek; t++) {
                 if (img_at[t] == ~0ull) continue;
-                const uint64_t leaf0 = 1ull << depth[t], o_frames = img_at[t] + 24 * leaf0;
-                unsigned long long *ffr = reinterpret_cast<unsigned long long *>(img.data() + img_at[t] + 16 * leaf0);
-                const GvsFenceReads &fr = frs[t];
-                for (uint64_t k = 0; k < leaf0; k++) {
-                    const uint64_t p = o_frames + (fr.has[k] ? fr.sf.at(fr.frame[k].lo) : 0);
-                    ffr[k] = gvs_frame_addr(fr, k, r->tables[t]->desc.data_len, img.data() + p, e->stage_out + p);
-                }
+                gvs_fence_image(frs[t], data_lens[t], img.data() + img_at[t], e->stage_out + img_at[t]);
                 gf[t].fix = reinterpret_cast<const uint4 *>(e->stage_out + img_at[t]);
-                gf[t].ffr = reinterpret_cast<const unsigned long long *>(e->stage_out + img_at[t] + 16 * leaf0);
+                gf[t].ffr = reinterpret_cast<const unsigned long long *>(e->stage_out + img_at[t] + 16 * (1ull << depth[t]));
             }
         }
 
@@ -3192,102 +3208,21 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
         CU(cudaGetLastError());
         CU(cudaStreamSynchronize(s));
 
-        // ---- touched leaves, in groups of about `budget` bytes (with a page cache, at most its capacity): per table its
-        // index slices, then their windows
-        const bool paged = r->cache != nullptr; // a leaf's slice and window each end in pages of their own
+        // ---- touched leaves, in groups of about `budget` bytes (with a page cache, at most its capacity)
+        const bool paged = r->cache != nullptr;
         const uint64_t group_bytes = paged ? std::min(budget, kPageBytes * r->cache->pc.capacity()) : budget;
-        struct Leaf { uint32_t t, leaf; };
-        std::vector<Leaf> group;
-        auto run_group = [&]() -> int {
-            const uint32_t nl = (uint32_t)group.size();
-            std::vector<ByteRange> sr(nl);
-            for (uint32_t k = 0; k < nl; k++) {
-                uint64_t a, b;
-                search_interval(DBEEL_LOOKUP_EXACT, pts[group[k].t]->state[(1ull << depth[group[k].t]) + group[k].leaf], &a, &b);
-                sr[k] = {16 * a, 16 * b};
-            }
-            // header: GvsLeaf[nl] | first[nseek + 1]; then the index slices, table after table
-            const uint64_t o_first = align_up(sizeof(GvsLeaf) * nl, 16);
-            std::vector<GvsStaged> ss(nseek), sw(nseek);
-            std::vector<uint32_t> first(nseek + 1, 0);
-            const uint64_t hdr = align_up(o_first + 4ull * (nseek + 1), kAlign);
-            uint64_t end = hdr;
-            for (uint32_t k = 0, t = 0; t < nseek; t++) {
-                std::vector<ByteRange> x;
-                first[t] = k;
-                for (; k < nl && group[k].t == t; k++) x.push_back(sr[k]);
-                ss[t] = gvs_stage(std::move(x), kLookupMergeGap, end);
-                end = std::max(end, ss[t].end);
-                first[t + 1] = k;
-            }
-            int rc2 = ensure_host(e, &e->ring_in, &e->ring_in_cap, end);
-            if (!rc2) rc2 = ensure_device(e, &e->stage_in, &e->stage_in_cap, end);
-            if (rc2) return rc2;
-            std::vector<GvsPart> parts;
-            for (uint32_t t = 0; t < nseek; t++)
-                if (!ss[t].runs.empty()) parts.push_back(GvsPart{t, &ss[t]});
-            if ((rc2 = gvs_load(e, io, r, DBEEL_STREAM_INDEX, parts, e->ring_in, e->stage_in, hdr, end, true,
-                                "stream read callback failed (.index, leaves)")))
-                return rc2;
-            std::vector<ByteRange> win(nl);
-            std::vector<uint8_t> has(nl, 0);
-            uint64_t wend = 0;
-            for (uint32_t t = 0; t < nseek; t++) {
-                std::vector<ByteRange> wr;
-                for (uint32_t k = first[t]; k < first[t + 1]; k++)
-                    if (leaf_window(e->ring_in + ss[t].at(sr[k].lo), (sr[k].hi - sr[k].lo) / 16, r->tables[t]->desc.data_len, max_klen, &win[k])) {
-                        has[k] = 1;
-                        wr.push_back(win[k]);
-                    }
-                sw[t] = gvs_stage(std::move(wr), 0, wend);
-                wend = std::max(wend, sw[t].end);
-            }
-            rc2 = ensure_host(e, &e->ring_out, &e->ring_out_cap, std::max<uint64_t>(wend, 256));
-            if (!rc2) rc2 = ensure_device(e, &e->stage_in2, &e->stage_in2_cap, std::max<uint64_t>(wend, 256));
-            if (rc2) return rc2;
-            parts.clear();
-            for (uint32_t t = 0; t < nseek; t++)
-                if (!sw[t].runs.empty()) parts.push_back(GvsPart{t, &sw[t]});
-            if ((rc2 = gvs_load(e, io, r, DBEEL_STREAM_DATA, parts, e->ring_out, e->stage_in2, 0, wend, false,
-                                "stream read callback failed (.data, leaves)")))
-                return rc2;
-            GvsLeaf *hl = reinterpret_cast<GvsLeaf *>(e->ring_in);
-            for (uint32_t t = 0; t < nseek; t++) {
-                for (uint32_t k = first[t]; k < first[t + 1]; k++) { // biased as in dbeel_get_values_stream's leaves
-                    const uintptr_t ib = reinterpret_cast<uintptr_t>(e->stage_in + ss[t].at(sr[k].lo)) - sr[k].lo;
-                    const uintptr_t db = has[k] ? reinterpret_cast<uintptr_t>(e->stage_in2 + sw[t].at(win[k].lo)) - win[k].lo
-                                                : reinterpret_cast<uintptr_t>(e->stage_in2);
-                    hl[k] = GvsLeaf{reinterpret_cast<const uint8_t *>(db), reinterpret_cast<const uint4 *>(ib), group[k].leaf, 0, 0};
-                }
-            }
-            memcpy(e->ring_in + o_first, first.data(), 4ull * (nseek + 1));
-            CU(cudaMemcpyAsync(e->stage_in, e->ring_in, hdr, cudaMemcpyHostToDevice, s));
+        std::vector<TouchedLeaf> lv;
+        for (uint32_t t = 0; t < nseek; t++) touched_leaves(*pts[t], t, touched.data() + touched_at[t], &lv);
+        const std::vector<size_t> cut = group_leaves(lv, nrecs, data_lens, max_klen, group_bytes, paged);
+        for (size_t g = 0; g + 1 < cut.size(); g++) {
+            const uint32_t nl = (uint32_t)(cut[g + 1] - cut[g]);
+            if ((rc = gvs_load_leaves(e, io, r, lv.data() + cut[g], nl, data_lens, max_klen))) return rc;
             launch_k(e, k_seek_leaf, grid, 256, 0, s, sq, reinterpret_cast<const TableDesc *>(ws + o_td),
                      reinterpret_cast<const uint32_t *>(ws + o_depth), reinterpret_cast<const GvsLeaf *>(e->stage_in),
-                     reinterpret_cast<const uint32_t *>(e->stage_in + o_first));
+                     reinterpret_cast<const uint32_t *>(e->stage_in + sizeof(GvsLeaf) * nl));
             CU(cudaGetLastError());
             CU(cudaStreamSynchronize(s));
-            group.clear();
-            return DBEEL_OK;
-        };
-        uint64_t est = 0;
-        for (uint32_t t = 0; t < nseek; t++) {
-            const uint64_t n = r->tables[t]->desc.n, dl = r->tables[t]->desc.data_len;
-            const uint64_t leaf0 = 1ull << depth[t], per_rec = 16 + (dl + n - 1) / n;
-            for (uint64_t L = 0; L < leaf0; L++) {
-                if (!touched[touched_at[t] + L]) continue;
-                uint64_t a, b;
-                search_interval(DBEEL_LOOKUP_EXACT, pts[t]->state[leaf0 + L], &a, &b);
-                const uint64_t bytes = (b - a) * per_rec + 8 + max_klen + (paged ? 2 * kPageBytes : 0);
-                if (!group.empty() && est + bytes > group_bytes) {
-                    if ((rc = run_group())) return rc;
-                    est = 0;
-                }
-                group.push_back(Leaf{t, (uint32_t)L});
-                est += bytes;
-            }
         }
-        if (!group.empty() && (rc = run_group())) return rc;
 
         // ---- the bounds, the first failed search, the spans
         std::vector<unsigned long long> res(Q), bad(Q);

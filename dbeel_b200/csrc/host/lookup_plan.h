@@ -14,6 +14,8 @@
 #include <cmath>
 #include <vector>
 
+#include "page_cache.h"
+
 #ifdef __CUDACC__
 #define DBEEL_HD __host__ __device__ __forceinline__
 #else
@@ -170,6 +172,45 @@ inline bool leaf_window(const uint8_t *slice, uint64_t count, uint64_t data_len,
         out->hi = std::max(out->hi, f.hi);
     }
     return any;
+}
+
+// A leaf the fence descent touched: leaf `leaf` of table t of the batch, whose open searches resume in records [a, b).
+struct TouchedLeaf {
+    uint32_t t, leaf;
+    uint64_t a, b;
+};
+
+// Appends the leaves L of pt (table t) with touched[L] set, ascending.
+inline void touched_leaves(const ProbeTree &pt, uint32_t t, const uint8_t *touched, std::vector<TouchedLeaf> *out) {
+    const uint64_t leaf0 = 1ull << pt.depth;
+    for (uint64_t L = 0; L < leaf0; L++) {
+        if (!touched[L]) continue;
+        uint64_t a, b;
+        search_interval(pt.mode, pt.state[leaf0 + L], &a, &b);
+        out->push_back(TouchedLeaf{t, (uint32_t)L, a, b});
+    }
+}
+
+// Cuts touched leaves, in the order they are loaded, into groups of about group_bytes.  A leaf costs its records at 16
+// index bytes plus table t's mean entry (ceil(data_len[t] / n[t]), 0 for an empty table), and 8 + max_klen for a probe
+// frame; with a page cache (paged), two more pages, as its slice and window each end in pages of their own.  A group
+// holds at least one leaf.  Group g is leaves [cut[g], cut[g + 1]) of the returned cut.
+inline std::vector<size_t> group_leaves(const std::vector<TouchedLeaf> &leaves, const std::vector<uint64_t> &n,
+                                        const std::vector<uint64_t> &data_len, uint64_t max_klen, uint64_t group_bytes, bool paged) {
+    std::vector<size_t> cut = {0};
+    uint64_t est = 0;
+    for (size_t k = 0; k < leaves.size(); k++) {
+        const TouchedLeaf &l = leaves[k];
+        const uint64_t per_rec = 16 + (n[l.t] ? (data_len[l.t] + n[l.t] - 1) / n[l.t] : 0);
+        const uint64_t bytes = (l.b - l.a) * per_rec + 8 + max_klen + (paged ? 2 * kPageBytes : 0);
+        if (k > cut.back() && est + bytes > group_bytes) {
+            cut.push_back(k);
+            est = 0;
+        }
+        est += bytes;
+    }
+    if (!leaves.empty()) cut.push_back(leaves.size());
+    return cut;
 }
 
 // ---- readers (dbeel_reader_*): fences kept on the device across batches

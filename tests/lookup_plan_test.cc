@@ -7,6 +7,7 @@
 //            linked in) on real tables of n = 0..300 records, for every present key and every gap
 //   windows  leaf windows on damaged index slices: lying key_size / offset / full_size, overlapping records, full_size < 8
 //   merge    merging of read ranges
+//   groups   touched leaves cut into groups: the cut points, a leaf larger than the budget, the paged bound, n == 0
 // Prints "ok" or the first mismatch.  Table key of record r: 2r + 2, queries are integers (absent: odd or out of range).
 #include <stdio.h>
 #include <string.h>
@@ -200,6 +201,34 @@ static int merge() {
     return 0;
 }
 
+// Table 0: 10 records, 95 bytes of .data (16 + ceil(9.5) = 26 bytes a record); table 1: no records (16 bytes a record).
+// With max_klen 4 every leaf adds 12, so the leaves below cost 64, 38, 194, 28 and 44 bytes (+ 8192 when paged).
+static int groups() {
+    const std::vector<TouchedLeaf> lv = {{0, 0, 0, 2}, {0, 1, 2, 3}, {0, 3, 3, 10}, {1, 0, 0, 1}, {1, 2, 1, 3}};
+    const std::vector<uint64_t> n = {10, 0}, dl = {95, 0};
+    struct Case { uint64_t budget; bool paged; std::vector<size_t> want; const char *what; };
+    const std::vector<Case> cases = {
+        {100, false, {0, 1, 2, 3, 5}, "cut where the next leaf overflows; a 194-byte leaf alone; the empty table's 28 + 44"},
+        {102, false, {0, 2, 3, 5}, "64 + 38 fills the budget exactly"},
+        {71, false, {0, 1, 2, 3, 4, 5}, "28 + 44 = 72 overflows 71"},
+        {72, false, {0, 1, 2, 3, 5}, "28 + 44 = 72 fits 72"},
+        {1, false, {0, 1, 2, 3, 4, 5}, "every leaf larger than the budget: one a group"},
+        {8192 + 368, false, {0, 5}, "unpaged: all 368 bytes in one group"},
+        {8192 + 368, true, {0, 1, 2, 3, 4, 5}, "paged: two pages a leaf"},
+        {2 * 8192 + 102, true, {0, 2, 3, 5}, "paged: 64 + 38 and their pages fit exactly, as do 28 + 44"},
+    };
+    for (const Case &c : cases) {
+        const std::vector<size_t> got = group_leaves(lv, n, dl, 4, c.budget, c.paged);
+        if (got != c.want) {
+            printf("groups: budget %llu paged %d (%s): got", (unsigned long long)c.budget, (int)c.paged, c.what);
+            for (size_t x : got) printf(" %zu", x);
+            return printf("\n"), 1;
+        }
+    }
+    if (group_leaves({}, n, dl, 4, 100, false) != std::vector<size_t>{0}) return printf("groups: no leaves\n"), 1;
+    return 0;
+}
+
 int main(int argc, char **argv) {
     const char *what = argc > 1 ? argv[1] : "";
     if (!strcmp(what, "descent")) {
@@ -220,6 +249,8 @@ int main(int argc, char **argv) {
         if (windows()) return 1;
     } else if (!strcmp(what, "merge")) {
         if (merge()) return 1;
+    } else if (!strcmp(what, "groups")) {
+        if (groups()) return 1;
     } else if (!strcmp(what, "depth")) {
         // the depth stays inside its clamps
         for (uint64_t n : {0ull, 1ull, 2ull, 3ull, 1000ull, 1ull << 30})
@@ -231,7 +262,7 @@ int main(int argc, char **argv) {
         if (lookup_depth(1, 1ull << 20, 1ull << 28, 24, 1ull << 30) >= lookup_depth(1ull << 20, 1ull << 20, 1ull << 28, 24, 1ull << 30))
             return printf("depth: does not grow with the batch\n"), 1;
     } else {
-        return printf("usage: descent | oracle | windows | merge | depth\n"), 2;
+        return printf("usage: descent | oracle | windows | merge | groups | depth\n"), 2;
     }
     printf("ok\n");
     return 0;

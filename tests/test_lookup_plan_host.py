@@ -1,7 +1,7 @@
 """The read plan of dbeel_get_values_stream on a box without a GPU (tests/lookup_plan_test.cc): the fence descent plus the
 resume from a leaf probes exactly what the whole-table search probes, in both modes and at every depth; that search
 against the oracle's orc_sstable_lookup on real tables; leaf windows on
-damaged index slices; merging of read ranges; the depth's clamps."""
+damaged index slices; merging of read ranges; the grouping of touched leaves; the depth's clamps."""
 import os
 import shutil
 import subprocess
@@ -21,7 +21,7 @@ def exe(tmp_path_factory):
     return out
 
 
-@pytest.mark.parametrize("what", ["descent", "oracle", "windows", "merge", "depth"])
+@pytest.mark.parametrize("what", ["descent", "oracle", "windows", "merge", "groups", "depth"])
 def test_lookup_plan(exe, what):
     out = subprocess.run([exe, what], capture_output=True, text=True, timeout=600)
     assert out.returncode == 0, out.stdout + out.stderr
