@@ -26,6 +26,7 @@ LOOKUP_BAD_ENTRY = 0x40000000  # get_values: the hit's entry does not decode (th
 SCAN_HASH = 0  # ranges: (start, end) u32 pairs, murmur3_32(key) tested with migration.rs's between_cmp
 SCAN_KEY = 1   # ranges: (start, end) byte strings, start <= key < end
 SCAN_STOP_NONE, SCAN_STOP_ERR, SCAN_STOP_PANIC = 0, 1, 2
+RANGE_KEEP_TOMBSTONES = 0x1  # dbeel_reader_get_range: keep entries with dlen == 0
 ERR_UNSORTED_RUN = 8
 ERR_CAPACITY = 2
 ERR_INVALID_ARG = 1
@@ -46,7 +47,7 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream",
            "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device", "dbeel_scan_stream", "dbeel_get_values",
            "dbeel_get_values_device", "dbeel_get_values_stream", "dbeel_reader_open", "dbeel_reader_get_values",
-           "dbeel_reader_scan", "dbeel_reader_close", "dbeel_page_cache_create", "dbeel_page_cache_destroy",
+           "dbeel_reader_scan", "dbeel_reader_get_range", "dbeel_reader_close", "dbeel_page_cache_create", "dbeel_page_cache_destroy",
            "dbeel_reader_attach_page_cache", "dbeel_page_cache_stats"]
 
 
@@ -227,6 +228,9 @@ def lib():
         L.dbeel_reader_scan.restype = C.c_int
         L.dbeel_reader_scan.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, SCAN_WRITE_FN, C.c_void_p,
                                         C.POINTER(JobResult), C.POINTER(ScanStop)]
+        L.dbeel_reader_get_range.restype = C.c_int
+        L.dbeel_reader_get_range.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, SCAN_WRITE_FN, C.c_void_p,
+                                             C.POINTER(JobResult), C.POINTER(ScanStop)]
         L.dbeel_reader_close.restype = None
         L.dbeel_reader_close.argtypes = [C.c_void_p]
         L.dbeel_page_cache_create.restype = C.c_int
@@ -511,10 +515,24 @@ class Reader:
         length) -> 0 or an error code receives the pieces), and (table, reason, record) of the stop, table = a position
         in the reader's tables.  Key ranges read only the records from each bound's seek on; hash ranges read every
         table.  last_stream_reads and fail_read_at as in get_values."""
+        rptr, _keep = pack_ranges(kind, ranges)
+        return self._ranges_call("dbeel_reader_scan", lambda cb, res, stop: lib().dbeel_reader_scan(
+            self._h, kind, rptr, len(ranges), cb, None, res, stop), len(ranges), write, fail_read_at)
+
+    def get_range(self, ranges, keep_tombstones: bool = False, write=None, fail_read_at: int = -1):
+        """dbeel_reader_get_range: per key range, the newest version of every key in it (get_entry's answer), in key
+        order, tombstones dropped unless keep_tombstones -- one SSTable (data, index) per range, or (data_len, index_len,
+        items) per range when write(dest, kind, offset, src_address, length) receives the pieces; and the stop, which is
+        Reader.scan's for the same ranges (results are then empty).  last_stream_reads and fail_read_at as in get_values."""
+        rptr, _keep = pack_ranges(SCAN_KEY, ranges)
+        flags = RANGE_KEEP_TOMBSTONES if keep_tombstones else 0
+        return self._ranges_call("dbeel_reader_get_range", lambda cb, res, stop: lib().dbeel_reader_get_range(
+            self._h, rptr, len(ranges), flags, cb, None, res, stop), len(ranges), write, fail_read_at, void_on_stop=True)
+
+    def _ranges_call(self, name: str, call, n: int, write, fail_read_at: int, void_on_stop: bool = False):
         import threading
         if not self._h:
             raise ValueError("reader is closed")
-        n = len(ranges)
         files = [{1: bytearray(), 2: bytearray()} for _ in range(n)]
         mu = threading.Lock()
 
@@ -527,23 +545,24 @@ class Reader:
             return 0
 
         cb = SCAN_WRITE_FN(lambda _ctx, dest, kind_, off, src, size: (write or collect)(dest, kind_, off, src, size))
-        rptr, _keep = pack_ranges(kind, ranges)
         res = (JobResult * max(1, n))()
         stop = ScanStop()
         if self._st is not None:
             self._st.fail_read_at = fail_read_at
             self._st.log.clear()
         try:
-            rc = lib().dbeel_reader_scan(self._h, kind, rptr, n, cb, None, res, C.byref(stop))
+            rc = call(cb, res, C.byref(stop))
         finally:
             if self._st is not None:
                 self._st.last_reads = list(self._st.log)
                 self.last_stream_reads = self._st.last_reads
                 self._st.fail_read_at = -1
         if rc:
-            raise DbeelError(rc, f"dbeel_reader_scan: {lib().dbeel_last_error(self._engine._h).decode()}")
+            raise DbeelError(rc, f"{name}: {lib().dbeel_last_error(self._engine._h).decode()}")
         if write is not None:
             return [(int(r.data_len), int(r.index_len), int(r.items_written)) for r in res[:n]], stop.as_tuple()
+        if void_on_stop and stop.table >= 0:  # the bytes written before the stop are void
+            files = [{1: b"", 2: b""} for _ in range(n)]
         return ([(np.frombuffer(bytes(f[1]), np.uint8).copy(), np.frombuffer(bytes(f[2]), np.uint8).copy()) for f in files],
                 stop.as_tuple())
 

@@ -22,6 +22,7 @@
 #include "../../include/dbeel_compact.h"
 #include "kernels.cuh"
 #include "merge_final.cuh"
+#include "merge_range.cuh"
 #include "gather_h.cuh"
 #include "lookup.cuh"
 #include "lookup_stream.cuh"
@@ -2756,8 +2757,17 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
 // and the D2H of c - 1 overlap; the engine thread enqueues partition c + 1's kernels before it waits for c's published sizes.
 // run_scan_plan runs a plan (steps 2 to the end) for dbeel_scan_stream (whole tables) and dbeel_reader_scan (spans): the
 // caller has checked the arguments, taken the engine, cleared results / stop / stats and set stats.entries_in.
+// dbeel_reader_get_range passes `merge` (a key-aligned plan, plan_merge): every partition runs the merge stage of
+// merge_range.cuh between the split and phase 2, and merge->unsorted reports a table whose span records do not ascend.
+struct RangeMerge {
+    const std::vector<std::vector<uint8_t>> *cuts; // plan.parts.size() - 1 ascending splitters (MergePlan::cuts)
+    bool keep_tombstones;
+    bool unsorted; // out
+};
+
 int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &plan, uint32_t kind, const void *ranges,
-                  uint32_t n_ranges, uint64_t key_bytes, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop) {
+                  uint32_t n_ranges, uint64_t key_bytes, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop,
+                  RangeMerge *merge = nullptr) {
     int rc = DBEEL_OK;
     const uint32_t np = (uint32_t)plan.parts.size();
     e->stats.partitions = np;
@@ -2809,6 +2819,27 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
     const uint64_t o_cbytes = carve(8 * res_chunks), o_ccount = carve(4 * res_chunks);
     const uint64_t o_src = carve(8ull * n_max), o_tf = carve(4ull * (gather_tiles_max + 2));
     const uint64_t pub_words = 5ull * nd + 2, pub_stride = align_up(8 * pub_words, 64), pin_pub = align_up(header_bytes, 64);
+    // the merge stage: per split record its table, key prefix and keep flag / prefix sum; per destination its surviving
+    // bytes; the error word; every slice's table and every splitter, uploaded once
+    std::vector<uint32_t> m_slt;
+    std::vector<uint64_t> m_koff(1, 0);
+    std::vector<uint8_t> m_keys;
+    uint64_t o_mtab = 0, o_mpfx = 0, o_mpre = 0, o_mtile = 0, o_mbytes = 0, o_merr = 0, o_mslt = 0, o_mkeys = 0;
+    if (merge) {
+        for (const ScanSlice &sl : plan.slices) m_slt.push_back(sl.table);
+        for (const std::vector<uint8_t> &k : *merge->cuts) {
+            m_keys.insert(m_keys.end(), k.begin(), k.end());
+            m_koff.push_back(m_keys.size());
+        }
+        o_mtab = carve(4ull * n_max);
+        o_mpfx = carve(8ull * n_max);
+        o_mpre = carve(4ull * n_max + 4);
+        o_mtile = carve(4ull * ((n_max + kRangeTile - 1) / kRangeTile + 1));
+        o_mbytes = carve(8ull * nd);
+        o_merr = carve(8);
+        o_mslt = carve(4ull * m_slt.size());
+        o_mkeys = carve(m_keys.size() + 16);
+    }
     const uint32_t R = (uint32_t)std::max(2, e->stream_ring);
     rc = ensure_device(e, &e->ws, &e->ws_cap, off);
     if (!rc) rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, max_in);
@@ -2878,6 +2909,25 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
              reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(header_bytes / 4));
     CU(cudaMemsetAsync(carry, 0, 8ull * (2 * nd + 1), s));
     CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
+    RangeMergeParams mp = {};
+    if (merge) {
+        CU(cudaMemsetAsync(ws + o_mbytes, 0, 8ull * nd, s));
+        CU(cudaMemsetAsync(ws + o_merr, 0, 8, s));
+        CU(cudaMemcpyAsync(ws + o_mslt, m_slt.data(), 4ull * m_slt.size(), cudaMemcpyHostToDevice, s));
+        if (!m_keys.empty()) CU(cudaMemcpyAsync(ws + o_mkeys, m_keys.data(), m_keys.size(), cudaMemcpyHostToDevice, s));
+        mp.n_ranges = nd;
+        mp.keep_tombstones = merge->keep_tombstones ? 1u : 0u;
+        mp.flat = sp.flat;
+        mp.split = rp.out_index;
+        mp.out = sp.flat;
+        mp.totals = rp.totals;
+        mp.tab = reinterpret_cast<uint32_t *>(ws + o_mtab);
+        mp.pfx = reinterpret_cast<unsigned long long *>(ws + o_mpfx);
+        mp.pre = reinterpret_cast<uint32_t *>(ws + o_mpre);
+        mp.tile = reinterpret_cast<uint32_t *>(ws + o_mtile);
+        mp.dbytes = reinterpret_cast<unsigned long long *>(ws + o_mbytes);
+        mp.err = reinterpret_cast<uint32_t *>(ws + o_merr);
+    }
 
     // ---- 5. the pipeline
     auto enqueue_h2d = [&](uint32_t c) -> int {
@@ -2924,8 +2974,35 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
         launch_k(e, k_route_scan, nd, 1024, 0, s, rpc);
         launch_k(e, k_route_starts, 1, 256, 0, s, rpc, pub);
         launch_k(e, k_route_scatter, nb, kRouteThreads, 0, s, rpc);
-        launch_k(e, k_scan_stream_carry, 1, 32, 0, s, rpc, pc, carry, pub);
         const uint4 *split = rpc.out_index;
+        if (merge) { // the merged split replaces the split, in flat
+            RangeMergeParams mpc = mp;
+            mpc.tables = spc.tables;
+            mpc.slice_table = reinterpret_cast<const uint32_t *>(ws + o_mslt) + pt.first_slice;
+            mpc.n_slices = pt.n_slices;
+            mpc.n = n;
+            mpc.pub = pub;
+            if (c > 0) {
+                mpc.lo = ws + o_mkeys + m_koff[c - 1];
+                mpc.lo_len = (uint32_t)(m_koff[c] - m_koff[c - 1]);
+            }
+            if (c + 1 < np) {
+                mpc.hi = ws + o_mkeys + m_koff[c];
+                mpc.hi_len = (uint32_t)(m_koff[c + 1] - m_koff[c]);
+            }
+            const uint32_t g = (n + 255) / 256, gt = (n + kRangeTile - 1) / kRangeTile;
+            launch_k(e, k_range_keys, g, 256, 0, s, mpc);
+            launch_k(e, k_range_check, g, 256, 0, s, mpc);
+            launch_k(e, k_range_flag, g, 256, 0, s, mpc);
+            launch_k(e, k_range_tile_sums, gt, kRangeTile, 0, s, mpc);
+            launch_k(e, k_range_tile_scan, 1, kRangeTile, 0, s, mpc);
+            launch_k(e, k_range_prefix, gt, kRangeTile, 0, s, mpc);
+            launch_k(e, k_range_rank, g, 256, 0, s, mpc);
+            launch_k(e, k_range_totals, 1, 256, 0, s, mpc);
+            launches += 8;
+            split = sp.flat;
+        }
+        launch_k(e, k_scan_stream_carry, 1, 32, 0, s, rpc, pc, carry, pub);
         launch_k(e, k_scan_tile_sums, tiles, kResolveThreads, 0, s, pc, split);
         launch_k(e, k_scan_tiles, (tiles + 1023) / 1024, 1024, 0, s, pc);
         launch_k(e, k_scan_chunks, 1, 1024, 0, s, pc);
@@ -3008,6 +3085,11 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
         return fail(e, frc, "stream write callback failed");
     }
     if (!stopped) host_stop();
+    if (merge) {
+        uint32_t err = 0;
+        CU(cudaMemcpy(&err, ws + o_merr, 4, cudaMemcpyDeviceToHost));
+        merge->unsorted = err != 0;
+    }
     uint64_t items = 0;
     for (uint32_t d = 0; d < nd; d++) {
         results[d].index_len = 16 * results[d].items_written;
@@ -3082,160 +3164,176 @@ inline bool key_less(const uint8_t *a, uint64_t al, const uint8_t *b, uint64_t b
     return c < 0 || (c == 0 && al < bl);
 }
 
-// Key ranges (dbeel_compact.h, dbeel_reader_scan): 1. the bound searches of every table before the first one with no
-// index record, two per range with start < end -- fences (cached or read for this call) on the device in one pass
-// (k_seek_fence), then the touched leaves in groups of about the partition budget (k_seek_leaf); 2. the spans, merged per
-// table, up to the first table whose search failed; 3. plan_scan over the spans and run_scan_plan.  The first stop in
-// iteration order wins: a stop inside the spans lies before a failed search or an empty table.
-int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables, const void *ranges, uint32_t nd,
-                    uint64_t key_bytes, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop) {
+// seek_t(bound) of dbeel_reader_scan (dbeel_compact.h) for every table t < nseek and every bound b of kb[boff[b] ..
+// + blen[b]): res / bad / bix[t * nb + b] = k_seek_leaf's result, its smallest corrupt probe (~0: none) and that probe's
+// index record.  Fences (cached or read for this call) on the device in one pass (k_seek_fence), then the touched leaves in
+// groups of about the partition budget (k_seek_leaf).  depth_queries sizes per-call fences (lookup_depth).
+int reader_seek(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, uint32_t nseek, const uint8_t *kb, uint64_t key_bytes,
+                const std::vector<uint64_t> &boff, const std::vector<uint64_t> &blen, uint64_t depth_queries,
+                std::vector<unsigned long long> *res_out, std::vector<unsigned long long> *bad_out, std::vector<uint4> *bix_out) {
+    const uint64_t nb = boff.size(), Q = nb * nseek; // pair q: table q / nb, bound q % nb
+    uint64_t max_klen = 0;
+    for (uint64_t b = 0; b < nb; b++) max_klen = std::max(max_klen, blen[b]);
+    if (!Q) return DBEEL_OK;
+    cudaError_t ce = cudaSetDevice(e->device);
+    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    cudaStream_t s = e->stream;
+    const uint64_t budget = e->partition_bytes;
+    int rc;
+    // ---- fences per table: the reader's (loaded now if this is the first exact-mode call that reaches the table)
+    // or read for this call into one host image, staged to stage_out
+    std::vector<uint32_t> depth(nseek);
+    std::vector<ProbeTree> pt_call(nseek);
+    std::vector<const ProbeTree *> pts(nseek);
+    std::vector<GvsFences> gf(nseek);
+    std::vector<GvsFenceReads> frs(nseek);
+    std::vector<uint64_t> img_at(nseek, ~0ull), touched_at(nseek + 1, 0), nrecs(nseek), data_lens(nseek);
+    uint64_t img_bytes = 0;
+    for (uint32_t t = 0; t < nseek; t++) {
+        dbeel_reader_table *rt = r->tables[t].get();
+        dbeel_reader_table::Fences &cache = rt->fences[DBEEL_LOOKUP_EXACT];
+        const uint64_t n = rt->desc.n, dl = rt->desc.data_len;
+        nrecs[t] = n;
+        data_lens[t] = dl;
+        const uint32_t want = lookup_depth(depth_queries, n, dl, 8 + max_klen, budget);
+        const bool use_cache = reader_uses_cache(max_klen, want, (uint32_t)rt->depth);
+        depth[t] = use_cache ? (uint32_t)rt->depth : want;
+        const uint64_t leaf0 = 1ull << depth[t];
+        touched_at[t + 1] = touched_at[t] + leaf0;
+        gf[t] = GvsFences{nullptr, nullptr, depth[t], t, n, nullptr};
+        if (use_cache) {
+            if (!cache.loaded) {
+                if ((rc = reader_load_fences(e, io, t, rt, DBEEL_LOOKUP_EXACT))) return rc;
+                CU(cudaStreamSynchronize(s)); // its image goes down from ring_out, which the next table refills
+            }
+            pts[t] = &cache.pt;
+            if (depth[t]) {
+                gf[t].fix = reinterpret_cast<const uint4 *>(cache.dev);
+                gf[t].ffr = reinterpret_cast<const unsigned long long *>(cache.dev + 16 * leaf0);
+            }
+            continue;
+        }
+        plan_probe_tree(DBEEL_LOOKUP_EXACT, n, depth[t], &pt_call[t]);
+        pts[t] = &pt_call[t];
+        if (!depth[t]) continue;
+        if ((rc = gvs_read_fences(e, io, t, pt_call[t], dl, max_klen, &frs[t]))) return rc;
+        img_at[t] = align_up(img_bytes, kAlign);
+        img_bytes = img_at[t] + frs[t].image_bytes();
+    }
+    std::vector<uint8_t> img(img_bytes);
+    if (img_bytes) {
+        if ((rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, img_bytes))) return rc;
+        for (uint32_t t = 0; t < nseek; t++) {
+            if (img_at[t] == ~0ull) continue;
+            gvs_fence_image(frs[t], data_lens[t], img.data() + img_at[t], e->stage_out + img_at[t]);
+            gf[t].fix = reinterpret_cast<const uint4 *>(e->stage_out + img_at[t]);
+            gf[t].ffr = reinterpret_cast<const unsigned long long *>(e->stage_out + img_at[t] + 16 * (1ull << depth[t]));
+        }
+    }
+
+    // ---- per-pair state in the workspace
+    uint64_t off = 0;
+    const uint64_t o_keys = carve_ws(&off, key_bytes + 16), o_koff = carve_ws(&off, 8 * Q), o_klen = carve_ws(&off, 8 * Q);
+    const uint64_t o_tab = carve_ws(&off, 4 * Q), o_state = carve_ws(&off, sizeof(SearchState) * Q), o_node = carve_ws(&off, 4 * Q);
+    const uint64_t o_res = carve_ws(&off, 8 * Q), o_bad = carve_ws(&off, 8 * Q), o_bix = carve_ws(&off, 16 * Q);
+    const uint64_t o_gf = carve_ws(&off, sizeof(GvsFences) * nseek), o_td = carve_ws(&off, sizeof(TableDesc) * nseek);
+    const uint64_t o_depth = carve_ws(&off, 4ull * nseek), o_touched = carve_ws(&off, touched_at[nseek]);
+    if ((rc = ensure_device(e, &e->ws, &e->ws_cap, off))) return rc;
+    uint8_t *ws = e->ws;
+    std::vector<uint64_t> qoff(Q), qlen(Q);
+    std::vector<uint32_t> qtab(Q);
+    std::vector<TableDesc> td(nseek);
+    for (uint64_t q = 0; q < Q; q++) {
+        qoff[q] = boff[q % nb];
+        qlen[q] = blen[q % nb];
+        qtab[q] = (uint32_t)(q / nb);
+    }
+    for (uint32_t t = 0; t < nseek; t++) {
+        gf[t].touched = ws + o_touched + touched_at[t];
+        td[t] = r->tables[t]->desc;
+    }
+    if (key_bytes) CU(cudaMemcpyAsync(ws + o_keys, kb, key_bytes, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_koff, qoff.data(), 8 * Q, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_klen, qlen.data(), 8 * Q, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_tab, qtab.data(), 4 * Q, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_gf, gf.data(), sizeof(GvsFences) * nseek, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_td, td.data(), sizeof(TableDesc) * nseek, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_depth, depth.data(), 4ull * nseek, cudaMemcpyHostToDevice, s));
+    if (!img.empty()) CU(cudaMemcpyAsync(e->stage_out, img.data(), img.size(), cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(ws + o_touched, 0, touched_at[nseek], s));
+    SeekQueries sq{ws + o_keys, reinterpret_cast<const uint64_t *>(ws + o_koff), reinterpret_cast<const uint64_t *>(ws + o_klen),
+                   reinterpret_cast<const uint32_t *>(ws + o_tab), Q, reinterpret_cast<SearchState *>(ws + o_state),
+                   reinterpret_cast<uint32_t *>(ws + o_node), reinterpret_cast<unsigned long long *>(ws + o_res),
+                   reinterpret_cast<unsigned long long *>(ws + o_bad), reinterpret_cast<uint4 *>(ws + o_bix)};
+    const uint32_t grid = (uint32_t)((Q + 255) / 256);
+    launch_k(e, k_seek_fence, grid, 256, 0, s, sq, reinterpret_cast<const GvsFences *>(ws + o_gf));
+    std::vector<uint8_t> touched(touched_at[nseek]);
+    CU(cudaMemcpyAsync(touched.data(), ws + o_touched, touched.size(), cudaMemcpyDeviceToHost, s));
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(s));
+
+    // ---- touched leaves, in groups of about `budget` bytes (with a page cache, at most its capacity)
+    const bool paged = r->cache != nullptr;
+    const uint64_t group_bytes = paged ? std::min(budget, kPageBytes * r->cache->pc.capacity()) : budget;
+    std::vector<TouchedLeaf> lv;
+    for (uint32_t t = 0; t < nseek; t++) touched_leaves(*pts[t], t, touched.data() + touched_at[t], &lv);
+    const std::vector<size_t> cut = group_leaves(lv, nrecs, data_lens, max_klen, group_bytes, paged);
+    for (size_t g = 0; g + 1 < cut.size(); g++) {
+        const uint32_t nl = (uint32_t)(cut[g + 1] - cut[g]);
+        if ((rc = gvs_load_leaves(e, io, r, lv.data() + cut[g], nl, data_lens, max_klen))) return rc;
+        launch_k(e, k_seek_leaf, grid, 256, 0, s, sq, reinterpret_cast<const TableDesc *>(ws + o_td),
+                 reinterpret_cast<const uint32_t *>(ws + o_depth), reinterpret_cast<const GvsLeaf *>(e->stage_in),
+                 reinterpret_cast<const uint32_t *>(e->stage_in + sizeof(GvsLeaf) * nl));
+        CU(cudaGetLastError());
+        CU(cudaStreamSynchronize(s));
+    }
+
+    // ---- the bounds and the failed searches
+    res_out->assign(Q, 0);
+    bad_out->assign(Q, 0);
+    bix_out->assign(Q, make_uint4(0, 0, 0, 0));
+    CU(cudaMemcpyAsync(res_out->data(), ws + o_res, 8 * Q, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(bad_out->data(), ws + o_bad, 8 * Q, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(bix_out->data(), ws + o_bix, 16 * Q, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    return DBEEL_OK;
+}
+
+// Steps 1-2 of a key-range read on a reader (dbeel_reader_scan, dbeel_reader_get_range): the bound searches of every table
+// before the first one with no index record, two per range with start < end; then the spans, merged per table, up to the
+// first table whose search failed (spans->size() = that table).  *host_stop = the stop of that search or of the first empty
+// table (none: table -1); a stop inside the spans lies before it in iteration order.
+int reader_spans(dbeel_engine *e, dbeel_reader *r, const void *ranges, uint32_t nd, uint64_t key_bytes, const dbeel_scan_io *io,
+                 std::vector<std::vector<ScanSpan>> *spans, dbeel_scan_stop *host_stop) {
     const dbeel_key_ranges *kr = static_cast<const dbeel_key_ranges *>(ranges);
     const uint8_t *kb = key_bytes ? static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0] : nullptr;
     std::vector<uint64_t> ko(2 * nd + 1);
     for (uint32_t k = 0; k <= 2 * nd; k++) ko[k] = kr->key_offsets[k] - kr->key_offsets[0];
-    std::vector<uint32_t> valid; // ranges that can take a record
-    uint64_t max_klen = 0;
+    std::vector<uint64_t> boff, blen; // the bounds of the ranges that can take a record: start, end, start, end, ...
     for (uint32_t d = 0; d < nd; d++) {
         if (!key_less(kb + ko[2 * d], ko[2 * d + 1] - ko[2 * d], kb + ko[2 * d + 1], ko[2 * d + 2] - ko[2 * d + 1])) continue;
-        valid.push_back(d);
-        max_klen = std::max({max_klen, ko[2 * d + 1] - ko[2 * d], ko[2 * d + 2] - ko[2 * d + 1]});
+        for (uint32_t k = 2 * d; k < 2 * d + 2; k++) {
+            boff.push_back(ko[k]);
+            blen.push_back(ko[k + 1] - ko[k]);
+        }
     }
     const uint32_t nt = (uint32_t)r->tables.size();
     uint32_t nseek = nt; // the tables before the first one with no index record (a PANIC at its record 0)
     for (uint32_t t = 0; t < nt; t++)
         if (r->tables[t]->desc.n == 0) { nseek = t; break; }
-    dbeel_scan_stop host_stop = nseek < nt ? dbeel_scan_stop{(int32_t)nseek, DBEEL_SCAN_STOP_PANIC, 0}
-                                           : dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
-    const uint64_t nv = valid.size(), Q = 2 * nv * nseek; // pair q: table q / (2 nv), range valid[(q / 2) % nv], end if q odd
+    *host_stop = nseek < nt ? dbeel_scan_stop{(int32_t)nseek, DBEEL_SCAN_STOP_PANIC, 0} : dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+    const uint64_t nb = boff.size();
     uint32_t cutoff = nseek;
-    std::vector<std::vector<ScanSpan>> spans(nseek);
-    if (Q) {
-        cudaError_t ce = cudaSetDevice(e->device);
-        if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
-        cudaStream_t s = e->stream;
-        const uint64_t budget = e->partition_bytes;
-        int rc;
-        // ---- fences per table: the reader's (loaded now if this is the first exact-mode call that reaches the table)
-        // or read for this call into one host image, staged to stage_out
-        std::vector<uint32_t> depth(nseek);
-        std::vector<ProbeTree> pt_call(nseek);
-        std::vector<const ProbeTree *> pts(nseek);
-        std::vector<GvsFences> gf(nseek);
-        std::vector<GvsFenceReads> frs(nseek);
-        std::vector<uint64_t> img_at(nseek, ~0ull), touched_at(nseek + 1, 0), nrecs(nseek), data_lens(nseek);
-        uint64_t img_bytes = 0;
-        for (uint32_t t = 0; t < nseek; t++) {
-            dbeel_reader_table *rt = r->tables[t].get();
-            dbeel_reader_table::Fences &cache = rt->fences[DBEEL_LOOKUP_EXACT];
-            const uint64_t n = rt->desc.n, dl = rt->desc.data_len;
-            nrecs[t] = n;
-            data_lens[t] = dl;
-            const uint32_t want = lookup_depth(2ull * nd, n, dl, 8 + max_klen, budget);
-            const bool use_cache = reader_uses_cache(max_klen, want, (uint32_t)rt->depth);
-            depth[t] = use_cache ? (uint32_t)rt->depth : want;
-            const uint64_t leaf0 = 1ull << depth[t];
-            touched_at[t + 1] = touched_at[t] + leaf0;
-            gf[t] = GvsFences{nullptr, nullptr, depth[t], t, n, nullptr};
-            if (use_cache) {
-                if (!cache.loaded) {
-                    if ((rc = reader_load_fences(e, io, t, rt, DBEEL_LOOKUP_EXACT))) return rc;
-                    CU(cudaStreamSynchronize(s)); // its image goes down from ring_out, which the next table refills
-                }
-                pts[t] = &cache.pt;
-                if (depth[t]) {
-                    gf[t].fix = reinterpret_cast<const uint4 *>(cache.dev);
-                    gf[t].ffr = reinterpret_cast<const unsigned long long *>(cache.dev + 16 * leaf0);
-                }
-                continue;
-            }
-            plan_probe_tree(DBEEL_LOOKUP_EXACT, n, depth[t], &pt_call[t]);
-            pts[t] = &pt_call[t];
-            if (!depth[t]) continue;
-            if ((rc = gvs_read_fences(e, io, t, pt_call[t], dl, max_klen, &frs[t]))) return rc;
-            img_at[t] = align_up(img_bytes, kAlign);
-            img_bytes = img_at[t] + frs[t].image_bytes();
-        }
-        std::vector<uint8_t> img(img_bytes);
-        if (img_bytes) {
-            if ((rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, img_bytes))) return rc;
-            for (uint32_t t = 0; t < nseek; t++) {
-                if (img_at[t] == ~0ull) continue;
-                gvs_fence_image(frs[t], data_lens[t], img.data() + img_at[t], e->stage_out + img_at[t]);
-                gf[t].fix = reinterpret_cast<const uint4 *>(e->stage_out + img_at[t]);
-                gf[t].ffr = reinterpret_cast<const unsigned long long *>(e->stage_out + img_at[t] + 16 * (1ull << depth[t]));
-            }
-        }
-
-        // ---- per-pair state in the workspace
-        uint64_t off = 0;
-        const uint64_t o_keys = carve_ws(&off, key_bytes + 16), o_koff = carve_ws(&off, 8 * Q), o_klen = carve_ws(&off, 8 * Q);
-        const uint64_t o_tab = carve_ws(&off, 4 * Q), o_state = carve_ws(&off, sizeof(SearchState) * Q), o_node = carve_ws(&off, 4 * Q);
-        const uint64_t o_res = carve_ws(&off, 8 * Q), o_bad = carve_ws(&off, 8 * Q), o_bix = carve_ws(&off, 16 * Q);
-        const uint64_t o_gf = carve_ws(&off, sizeof(GvsFences) * nseek), o_td = carve_ws(&off, sizeof(TableDesc) * nseek);
-        const uint64_t o_depth = carve_ws(&off, 4ull * nseek), o_touched = carve_ws(&off, touched_at[nseek]);
-        if ((rc = ensure_device(e, &e->ws, &e->ws_cap, off))) return rc;
-        uint8_t *ws = e->ws;
-        std::vector<uint64_t> qoff(Q), qlen(Q);
-        std::vector<uint32_t> qtab(Q);
-        std::vector<TableDesc> td(nseek);
-        for (uint64_t q = 0; q < Q; q++) {
-            const uint32_t k = 2 * valid[(q / 2) % nv] + (uint32_t)(q & 1);
-            qoff[q] = ko[k];
-            qlen[q] = ko[k + 1] - ko[k];
-            qtab[q] = (uint32_t)(q / (2 * nv));
-        }
-        for (uint32_t t = 0; t < nseek; t++) {
-            gf[t].touched = ws + o_touched + touched_at[t];
-            td[t] = r->tables[t]->desc;
-        }
-        if (key_bytes) CU(cudaMemcpyAsync(ws + o_keys, kb, key_bytes, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(ws + o_koff, qoff.data(), 8 * Q, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(ws + o_klen, qlen.data(), 8 * Q, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(ws + o_tab, qtab.data(), 4 * Q, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(ws + o_gf, gf.data(), sizeof(GvsFences) * nseek, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(ws + o_td, td.data(), sizeof(TableDesc) * nseek, cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(ws + o_depth, depth.data(), 4ull * nseek, cudaMemcpyHostToDevice, s));
-        if (!img.empty()) CU(cudaMemcpyAsync(e->stage_out, img.data(), img.size(), cudaMemcpyHostToDevice, s));
-        CU(cudaMemsetAsync(ws + o_touched, 0, touched_at[nseek], s));
-        SeekQueries sq{ws + o_keys, reinterpret_cast<const uint64_t *>(ws + o_koff), reinterpret_cast<const uint64_t *>(ws + o_klen),
-                       reinterpret_cast<const uint32_t *>(ws + o_tab), Q, reinterpret_cast<SearchState *>(ws + o_state),
-                       reinterpret_cast<uint32_t *>(ws + o_node), reinterpret_cast<unsigned long long *>(ws + o_res),
-                       reinterpret_cast<unsigned long long *>(ws + o_bad), reinterpret_cast<uint4 *>(ws + o_bix)};
-        const uint32_t grid = (uint32_t)((Q + 255) / 256);
-        launch_k(e, k_seek_fence, grid, 256, 0, s, sq, reinterpret_cast<const GvsFences *>(ws + o_gf));
-        std::vector<uint8_t> touched(touched_at[nseek]);
-        CU(cudaMemcpyAsync(touched.data(), ws + o_touched, touched.size(), cudaMemcpyDeviceToHost, s));
-        CU(cudaGetLastError());
-        CU(cudaStreamSynchronize(s));
-
-        // ---- touched leaves, in groups of about `budget` bytes (with a page cache, at most its capacity)
-        const bool paged = r->cache != nullptr;
-        const uint64_t group_bytes = paged ? std::min(budget, kPageBytes * r->cache->pc.capacity()) : budget;
-        std::vector<TouchedLeaf> lv;
-        for (uint32_t t = 0; t < nseek; t++) touched_leaves(*pts[t], t, touched.data() + touched_at[t], &lv);
-        const std::vector<size_t> cut = group_leaves(lv, nrecs, data_lens, max_klen, group_bytes, paged);
-        for (size_t g = 0; g + 1 < cut.size(); g++) {
-            const uint32_t nl = (uint32_t)(cut[g + 1] - cut[g]);
-            if ((rc = gvs_load_leaves(e, io, r, lv.data() + cut[g], nl, data_lens, max_klen))) return rc;
-            launch_k(e, k_seek_leaf, grid, 256, 0, s, sq, reinterpret_cast<const TableDesc *>(ws + o_td),
-                     reinterpret_cast<const uint32_t *>(ws + o_depth), reinterpret_cast<const GvsLeaf *>(e->stage_in),
-                     reinterpret_cast<const uint32_t *>(e->stage_in + sizeof(GvsLeaf) * nl));
-            CU(cudaGetLastError());
-            CU(cudaStreamSynchronize(s));
-        }
-
-        // ---- the bounds, the first failed search, the spans
-        std::vector<unsigned long long> res(Q), bad(Q);
-        std::vector<uint4> bix(Q);
-        CU(cudaMemcpyAsync(res.data(), ws + o_res, 8 * Q, cudaMemcpyDeviceToHost, s));
-        CU(cudaMemcpyAsync(bad.data(), ws + o_bad, 8 * Q, cudaMemcpyDeviceToHost, s));
-        CU(cudaMemcpyAsync(bix.data(), ws + o_bix, 16 * Q, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
+    spans->assign(nseek, {});
+    if (nb && nseek) {
+        std::vector<unsigned long long> res, bad;
+        std::vector<uint4> bix;
+        if (const int rc = reader_seek(e, r, io, nseek, kb, key_bytes, boff, blen, 2ull * nd, &res, &bad, &bix)) return rc;
         for (uint32_t t = 0; t < nseek && cutoff == nseek; t++) {
             uint64_t worst = ~0ull;
             uint4 ix = make_uint4(0, 0, 0, 0);
             std::vector<ScanSpan> sp;
-            for (uint64_t q = 2 * nv * t; q < 2 * nv * (t + 1); q += 2) {
+            for (uint64_t q = nb * t; q < nb * (t + 1); q += 2) {
                 for (uint64_t j = q; j < q + 2; j++)
                     if (bad[j] < worst) { worst = bad[j]; ix = bix[j]; }
                 if (res[q] < res[q + 1] && res[q + 1] != ~0ull) sp.push_back(ScanSpan{res[q], res[q + 1]});
@@ -3243,21 +3341,31 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
             if (worst != ~0ull) { // as dbeel_scan on reaching the record: PANIC when its index record alone shows it
                 const uint64_t o = (uint64_t)ix.x | ((uint64_t)ix.y << 32), dl = r->tables[t]->desc.data_len;
                 const bool panic = ix.w == 0 || o > dl || ix.w > dl - o;
-                host_stop = dbeel_scan_stop{(int32_t)t, panic ? DBEEL_SCAN_STOP_PANIC : DBEEL_SCAN_STOP_ERR, worst};
+                *host_stop = dbeel_scan_stop{(int32_t)t, panic ? DBEEL_SCAN_STOP_PANIC : DBEEL_SCAN_STOP_ERR, worst};
                 cutoff = t;
                 break;
             }
             std::sort(sp.begin(), sp.end(), [](const ScanSpan &a, const ScanSpan &b) { return a.lo < b.lo; });
             for (const ScanSpan &x : sp) {
-                if (!spans[t].empty() && x.lo <= spans[t].back().hi) spans[t].back().hi = std::max(spans[t].back().hi, x.hi);
-                else spans[t].push_back(x);
+                if (!(*spans)[t].empty() && x.lo <= (*spans)[t].back().hi) (*spans)[t].back().hi = std::max((*spans)[t].back().hi, x.hi);
+                else (*spans)[t].push_back(x);
             }
         }
     }
-    spans.resize(cutoff);
+    spans->resize(cutoff);
     for (uint32_t t = 0; t < cutoff; t++)
-        for (const ScanSpan &x : spans[t]) e->stats.entries_in += x.hi - x.lo;
-    const int rc = plan_and_run_scan(e, tables, cutoff, DBEEL_SCAN_KEY, ranges, nd, key_bytes, io, results, stop, &spans);
+        for (const ScanSpan &x : (*spans)[t]) e->stats.entries_in += x.hi - x.lo;
+    return DBEEL_OK;
+}
+
+// Key ranges (dbeel_compact.h, dbeel_reader_scan): 1-2. reader_spans; 3. plan_scan over the spans and run_scan_plan.  The
+// first stop in iteration order wins: a stop inside the spans lies before a failed search or an empty table.
+int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables, const void *ranges, uint32_t nd,
+                    uint64_t key_bytes, const dbeel_scan_io *io, dbeel_job_result *results, dbeel_scan_stop *stop) {
+    std::vector<std::vector<ScanSpan>> spans;
+    dbeel_scan_stop host_stop;
+    if (const int rc = reader_spans(e, r, ranges, nd, key_bytes, io, &spans, &host_stop)) return rc;
+    const int rc = plan_and_run_scan(e, tables, (uint32_t)spans.size(), DBEEL_SCAN_KEY, ranges, nd, key_bytes, io, results, stop, &spans);
     if (!rc && stop->table < 0) *stop = host_stop;
     return rc;
 }
@@ -3291,6 +3399,145 @@ int reader_scan_entry(dbeel_reader *r, uint32_t kind, const void *ranges, uint32
         return plan_and_run_scan(e, tables.data(), nt, kind, ranges, n_ranges, key_bytes, &io, results, stop, nullptr);
     }
     const int rc = reader_scan_key(e, r, tables.data(), ranges, n_ranges, key_bytes, &io, results, stop);
+    if (rc) {
+        cudaStreamSynchronize(e->stream); // nothing of this call may touch the engine's buffers after it returns
+        for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+        *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+    }
+    e->stats.input_bytes = x.bytes;
+    return rc;
+}
+
+// ---- dbeel_reader_get_range
+int discard_write(void *, uint32_t, uint32_t, uint64_t, const void *, uint64_t) { return 0; }
+
+// Key ranges merged (dbeel_compact.h, dbeel_reader_get_range): 1-2. reader_spans; 3. plan_merge over the spans (its seek is
+// reader_seek with the splitters as bounds, its key reads go through io); 4. run_scan_plan with the merge stage.  A stop --
+// a failed search, an empty table, a PANIC record the planner met or a stop in a partition -- is dbeel_reader_scan's stop:
+// the raw scan of the same spans is run with a discarding writer, since partitions are not in iteration order.
+int reader_get_range_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables, const void *ranges, uint32_t nd,
+                         uint64_t key_bytes, bool keep_tombstones, const dbeel_scan_io *io, dbeel_job_result *results,
+                         dbeel_scan_stop *stop) {
+    std::vector<std::vector<ScanSpan>> spans;
+    dbeel_scan_stop host_stop;
+    int rc = reader_spans(e, r, ranges, nd, key_bytes, io, &spans, &host_stop);
+    if (rc) return rc;
+    const uint32_t nt = (uint32_t)spans.size();
+    auto void_results = [&]() {
+        for (uint32_t d = 0; d < nd; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+    };
+    auto raw_stop = [&]() -> int { // *stop = dbeel_reader_scan's; partitions stays the key partitions run (0: none)
+        const dbeel_scan_io dio{io->read, discard_write, io->ctx};
+        std::vector<dbeel_job_result> scratch(nd);
+        const uint32_t parts = e->stats.partitions;
+        *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+        const int src = plan_and_run_scan(e, tables, nt, DBEEL_SCAN_KEY, ranges, nd, key_bytes, &dio, scratch.data(), stop, &spans);
+        if (!src && stop->table < 0) *stop = host_stop;
+        void_results();
+        e->stats.output_bytes = e->stats.entries_out = 0; // nothing that was written stands
+        e->stats.partitions = parts;
+        return src;
+    };
+    if (host_stop.table >= 0) return raw_stop();
+    std::vector<uint64_t> dlen(nt), ilen(nt);
+    for (uint32_t t = 0; t < nt; t++) {
+        dlen[t] = tables[t].data_len;
+        ilen[t] = tables[t].index_len;
+    }
+    const ScanIndexRead read_index = [io](uint32_t t, uint64_t off, uint64_t len, void *dst) {
+        return io->read(io->ctx, t, DBEEL_STREAM_INDEX, off, len, dst);
+    };
+    const MergeKeyRead read_key = [io](uint32_t t, uint64_t off, uint32_t fs, std::vector<uint8_t> *key, bool *ok) {
+        constexpr uint64_t kHead = 8 + DBEEL_READER_FRAME_CAP; // most keys come with their length prefix in one read
+        std::vector<uint8_t> b(std::min<uint64_t>(fs, kHead));
+        *ok = false;
+        if (b.size() < 8) return 0;
+        if (const int krc = io->read(io->ctx, t, DBEEL_STREAM_DATA, off, b.size(), b.data())) return krc;
+        uint64_t klen = 0;
+        memcpy(&klen, b.data(), 8);
+        if (klen > fs - 8) return 0;
+        key->assign(b.begin() + 8, b.begin() + 8 + std::min<uint64_t>(klen, b.size() - 8));
+        if (8 + klen > b.size()) {
+            const uint64_t have = key->size();
+            key->resize(klen);
+            if (const int krc = io->read(io->ctx, t, DBEEL_STREAM_DATA, off + 8 + have, klen - have, key->data() + have)) return krc;
+        }
+        *ok = true;
+        return 0;
+    };
+    // The splitters in batches whose search state (kSeekPairBytes per table and key, plus the keys) fits the budget.
+    constexpr uint64_t kSeekPairBytes = 128;
+    const MergeSeek seek = [&](const std::vector<std::vector<uint8_t>> &keys, std::vector<uint64_t> *pos) {
+        pos->assign((uint64_t)nt * keys.size(), ~0ull);
+        for (size_t j0 = 0; j0 < keys.size();) {
+            std::vector<uint8_t> blob;
+            std::vector<uint64_t> boff, blen;
+            size_t j1 = j0;
+            uint64_t bytes = 0;
+            while (j1 < keys.size() && (j1 == j0 || bytes + keys[j1].size() + kSeekPairBytes * nt <= e->partition_bytes)) {
+                bytes += keys[j1].size() + kSeekPairBytes * nt;
+                boff.push_back(blob.size());
+                blen.push_back(keys[j1].size());
+                blob.insert(blob.end(), keys[j1].begin(), keys[j1].end());
+                j1++;
+            }
+            std::vector<unsigned long long> res, bad;
+            std::vector<uint4> bix;
+            const int src = reader_seek(e, r, io, nt, blob.data(), blob.size(), boff, blen, j1 - j0, &res, &bad, &bix);
+            if (src) return src;
+            const uint64_t nb = j1 - j0;
+            for (uint64_t q = 0; q < res.size(); q++)
+                (*pos)[(q / nb) * keys.size() + j0 + q % nb] = bad[q] != ~0ull ? ~0ull : res[q];
+            j0 = j1;
+        }
+        return 0;
+    };
+    MergePlan mplan;
+    rc = plan_merge(dlen.data(), ilen.data(), nt, e->partition_bytes, spans, read_index, read_key, seek, &mplan);
+    if (rc) return e->err.empty() ? fail(e, rc, "stream read callback failed (planning)") : rc;
+    if (mplan.refused) { // nothing past the budget is staged: the raw scan's stop, else keys that do not ascend
+        if ((rc = raw_stop()) || stop->table >= 0) return rc;
+        return fail(e, DBEEL_ERR_UNSORTED_RUN, "a key interval passes the partition budget: span records do not strictly ascend");
+    }
+    if (mplan.plan.panic_table >= 0) return raw_stop();
+    RangeMerge m{&mplan.cuts, keep_tombstones, false};
+    rc = run_scan_plan(e, tables, mplan.plan, DBEEL_SCAN_KEY, ranges, nd, key_bytes, io, results, stop, &m);
+    if (rc) return rc;
+    if (stop->table >= 0) return raw_stop();
+    if (m.unsorted) {
+        void_results();
+        return fail(e, DBEEL_ERR_UNSORTED_RUN, "a table's span records do not strictly ascend by key");
+    }
+    return DBEEL_OK;
+}
+
+int reader_get_range_entry(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, uint32_t flags,
+                           int (*write)(void *, uint32_t, uint32_t, uint64_t, const void *, uint64_t), void *ctx,
+                           dbeel_job_result *results, dbeel_scan_stop *stop) {
+    dbeel_engine *e = r->e;
+    if (!write) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    if (flags & ~DBEEL_RANGE_KEEP_TOMBSTONES) return fail(e, DBEEL_ERR_INVALID_ARG, "unknown flag");
+    std::vector<dbeel_table> tables(r->tables.size());
+    for (size_t i = 0; i < tables.size(); i++) {
+        const TableDesc &d = r->tables[i]->desc;
+        tables[i] = dbeel_table{nullptr, d.data_len, nullptr, d.n * DBEEL_INDEX_ENTRY_SIZE, nullptr, 0};
+    }
+    uint64_t key_bytes = 0;
+    if (const int arc = scan_args(e, tables.data(), (uint32_t)tables.size(), DBEEL_SCAN_KEY, ranges, n_ranges, results, stop, &key_bytes))
+        return arc;
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    e->stats = dbeel_stats{};
+    for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+    *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+    ReaderScanIo x;
+    x.rio = &r->io;
+    x.write = write;
+    x.wctx = ctx;
+    const dbeel_scan_io io{reader_scan_read, reader_scan_write, &x};
+    const int rc = reader_get_range_key(e, r, tables.data(), ranges, n_ranges, key_bytes, (flags & DBEEL_RANGE_KEEP_TOMBSTONES) != 0,
+                                        &io, results, stop);
     if (rc) {
         cudaStreamSynchronize(e->stream); // nothing of this call may touch the engine's buffers after it returns
         for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
@@ -3718,6 +3965,14 @@ void dbeel_reader_close(dbeel_reader *r) {
     v.erase(std::remove(v.begin(), v.end(), r), v.end());
     cudaSetDevice(r->e->device);
     delete r;
+}
+
+int dbeel_reader_get_range(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, uint32_t flags,
+                           int (*write)(void *ctx, uint32_t dest, uint32_t kind, uint64_t offset, const void *src, uint64_t len),
+                           void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop) {
+    if (!r) return DBEEL_ERR_INVALID_ARG;
+    REFUSE_WHILE_ASYNC(r->e);
+    return reader_get_range_entry(r, ranges, n_ranges, flags, write, ctx, results, stop);
 }
 
 int dbeel_page_cache_create(dbeel_engine *e, uint64_t bytes, dbeel_page_cache **out) {

@@ -521,6 +521,47 @@ int dbeel_reader_get_values(dbeel_reader *r, const void *keys, const uint64_t *k
 int dbeel_reader_scan(dbeel_reader *r, uint32_t kind, const void *ranges, uint32_t n_ranges,
                       int (*write)(void *ctx, uint32_t dest, uint32_t kind, uint64_t offset, const void *src, uint64_t len),
                       void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop);
+
+/* Range reads on a reader: what get_entry / dbeel_reader_get_values(DBEEL_LOOKUP_EXACT) return for every key of the
+ * ranges, merged on the device.  Let S_d be the entries dbeel_reader_scan(r, DBEEL_SCAN_KEY, ranges, n_ranges, ...)
+ * writes to destination d, in its order.
+ *   Output.  Destination d receives one SSTable pair: for every distinct key of S_d, in ascending byte order, the LAST
+ *            entry of S_d with that key -- on sorted tables the newest table's version, the one get_entry returns.  An
+ *            entry with dlen == 0 (a tombstone) is left out unless flags has DBEEL_RANGE_KEEP_TOMBSTONES.  Entries keep
+ *            their stored bytes; .index offsets run from 0 and key_size is 8 + klen.  With the flag, destination d is
+ *            byte for byte what dbeel_flush writes for S_d taken as one arrival batch.  Every destination is a valid
+ *            SSTable (keys strictly ascending), usable as a compaction input or a reader table.
+ *   Ranges.  As dbeel_reader_scan(DBEEL_SCAN_KEY): the first range that accepts a key takes it, start >= end takes
+ *            nothing, same limits.  DBEEL_ERR_INVALID_ARG for a null write, n_ranges of 0 or more than
+ *            DBEEL_MAX_SCAN_RANGES, or an unknown bit in flags.
+ *   Stops.   *stop is exactly dbeel_reader_scan's for the same ranges (a failed search, a table with no record, a PANIC or
+ *            ERR inside the spans).  With a stop the call returns DBEEL_OK, every results[d] is zero and the bytes already
+ *            passed to write are void: a damaged tree's result is its stop, never a merged prefix.
+ *   Sorted.  With no stop, a table whose span records (the union of its spans, in record order) do not strictly ascend by
+ *            key gives DBEEL_ERR_UNSORTED_RUN, results zero and the bytes written void.  Only tables the writer did not
+ *            produce can do that.
+ *   Delivery as dbeel_reader_scan: destination d's .data and .index start at offset 0, pieces arrive in any order and
+ *            from several threads, the reader's io.write is not used.
+ *   Reads.   The bound searches of dbeel_reader_scan (fences cached or read for this call, touched leaves through the page
+ *            cache when one is attached); the span .index slices, for planning and again for the partitions; the key-aligned
+ *            planner's reads -- a second pass over the span .index slices, the keys of sampled records (.data) and the
+ *            searches for those keys, as the bound searches; and the partitions' .data windows (not through the page
+ *            cache).  When the span slices and windows fit one partition, the call makes exactly dbeel_reader_scan's reads.
+ *   Memory.  Device and page-locked memory are bounded by the partition budget (DBEEL_PARTITION_MB / _KB): a partition's
+ *            index slices and windows, and its output bound, are at most the budget plus one record per table, on any
+ *            tables.  A partition is a key interval of every table, cut at sampled keys, and a window never spans more
+ *            bytes than its records hold.  A key interval that would pass that bound -- possible only when some table's
+ *            span keys do not ascend, or when a sampled key's search met a corrupt record -- is not staged: the call
+ *            returns dbeel_reader_scan's stop if there is one, else DBEEL_ERR_UNSORTED_RUN.  The searches of the sampled
+ *            keys run in batches whose search state fits the budget.
+ * dbeel_last_stats: input_bytes = every byte read through the callback in this call, output_bytes / entries_out = what
+ * was written (0 with a stop), entries_in = records in the spans, partitions = key partitions run.  A callback's nonzero return comes back
+ * unchanged; the reader, the engine and an attached page cache stay usable after every error, stop and argument failure.
+ * DBEEL_ERR_BUSY while another call runs. */
+#define DBEEL_RANGE_KEEP_TOMBSTONES 0x1u
+int dbeel_reader_get_range(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, uint32_t flags,
+                           int (*write)(void *ctx, uint32_t dest, uint32_t kind, uint64_t offset, const void *src, uint64_t len),
+                           void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop);
 void dbeel_reader_close(dbeel_reader *r);
 
 /* Page cache for readers: the reference reads every .data / .index byte of a lookup or seek through a per-shard cache of
