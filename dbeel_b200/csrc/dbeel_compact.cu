@@ -1831,34 +1831,64 @@ int scan_args(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uin
     return DBEEL_OK;
 }
 
-// The ranges as the kernels read them (ScanParams.hash_ranges / key_off / keys), written into the pinned header block.
-void scan_range_header(uint32_t kind, const void *ranges, uint32_t nd, uint64_t key_bytes, uint8_t *rng, uint8_t *keys) {
-    if (kind == DBEEL_SCAN_KEY) {
-        const dbeel_key_ranges *kr = static_cast<const dbeel_key_ranges *>(ranges);
-        uint64_t *ko = reinterpret_cast<uint64_t *>(rng);
-        for (uint32_t k = 0; k <= 2 * nd; k++) ko[k] = kr->key_offsets[k] - kr->key_offsets[0];
-        if (key_bytes) memcpy(keys, static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0], key_bytes);
-    } else {
-        memcpy(rng, ranges, 8ull * nd);
-    }
+// results and stop as a scan that delivered nothing leaves them
+void clear_scan(dbeel_job_result *results, uint32_t nd, dbeel_scan_stop *stop) {
+    for (uint32_t d = 0; d < nd; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+    *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
 }
-
-// ---- the split and phase 2 of a scan, shared with dbeel_get_values*
-// Input: n 16-byte records {source address, 8 + klen, full_size} (ScanParams.flat) and a destination per record
-// (ScanParams.dest, kScanNone = not delivered).  Output: the nd streams back to back in out->data / out->index, in record
-// order inside each stream, every stream's .index offsets relative to its own first byte -- nd arrival batches.  The
-// output can be larger than the inputs (records may share .data bytes), so it is sized from a read-back.
-struct SplitLayout {
-    uint64_t o_ctl, o_memtab, header2_bytes; // second header, after the split is known: control block | (bytes, entries) before each stream
-    uint64_t o_tot, o_dest, o_flat, o_split, o_hist, o_tbytes, o_tcount, o_cbytes, o_ccount, o_src;
-    uint32_t n, nd, n_blocks;
-};
 
 uint64_t carve_ws(uint64_t *off, uint64_t b) {
     const uint64_t o = *off;
     *off = align_up(*off + b, kAlign);
     return o;
 }
+
+// ---- the ranges as the kernels read them (ScanParams.hash_ranges / key_off / keys), carved behind what the caller put
+// at the front of the workspace.  land_ranges writes them into the pinned block at the same offsets and lands ws[0, bytes)
+// -- the caller's front block included -- with one k_copy_words.
+struct RangeHeader {
+    uint64_t o_rng, o_keys, bytes;
+};
+
+RangeHeader carve_ranges(uint64_t *off, uint32_t kind, uint32_t nd, uint64_t key_bytes) {
+    RangeHeader rh;
+    rh.o_rng = carve_ws(off, kind == DBEEL_SCAN_KEY ? 8ull * (2 * nd + 1) : 8ull * nd);
+    rh.o_keys = carve_ws(off, key_bytes + 16);
+    rh.bytes = *off;
+    return rh;
+}
+
+void land_ranges(dbeel_engine *e, const RangeHeader &rh, uint32_t kind, const void *ranges, uint32_t nd, uint64_t key_bytes,
+                 ScanParams *sp) {
+    uint8_t *ws = e->ws, *h = e->pin;
+    if (kind == DBEEL_SCAN_KEY) {
+        const dbeel_key_ranges *kr = static_cast<const dbeel_key_ranges *>(ranges);
+        uint64_t *ko = reinterpret_cast<uint64_t *>(h + rh.o_rng);
+        for (uint32_t k = 0; k <= 2 * nd; k++) ko[k] = kr->key_offsets[k] - kr->key_offsets[0];
+        if (key_bytes) memcpy(h + rh.o_keys, static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0], key_bytes);
+    } else {
+        memcpy(h + rh.o_rng, ranges, 8ull * nd);
+    }
+    sp->key_kind = kind == DBEEL_SCAN_KEY ? 1u : 0u;
+    sp->n_ranges = nd;
+    sp->hash_ranges = reinterpret_cast<const uint32_t *>(ws + rh.o_rng);
+    sp->key_off = reinterpret_cast<const unsigned long long *>(ws + rh.o_rng);
+    sp->keys = ws + rh.o_keys;
+    launch_k(e, k_copy_words, (uint32_t)((rh.bytes / 4 + 255) / 256), 256, 0, e->stream, reinterpret_cast<uint32_t *>(ws),
+             reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(rh.bytes / 4));
+}
+
+// ---- the split and phase 2 of a scan, shared by every call that returns entries
+// Input: n 16-byte records {source address, 8 + klen, full_size} (ScanParams.flat) and a destination per record
+// (ScanParams.dest, kScanNone = not delivered).  Output: the nd streams back to back, in record order inside each stream,
+// every stream's .index offsets relative to its own first byte -- nd arrival batches.  split_emit runs it once, sized
+// from a read-back (records may share .data bytes, so the output can be larger than the inputs); run_scan_plan runs it
+// per partition, sized from the plan's bound.
+struct SplitLayout {
+    uint64_t o_ctl, o_memtab, header2_bytes; // second header, after the split is known: control block | (bytes, entries) before each stream
+    uint64_t o_tot, o_dest, o_flat, o_split, o_hist, o_tbytes, o_tcount, o_cbytes, o_ccount, o_src;
+    uint32_t n, nd, n_blocks;
+};
 
 SplitLayout carve_split(uint64_t *off, uint32_t n, uint32_t nd) {
     SplitLayout w;
@@ -1882,40 +1912,71 @@ SplitLayout carve_split(uint64_t *off, uint32_t n, uint32_t nd) {
     return w;
 }
 
-// ScanParams fields the split reads: records, destinations, the stop word (totals[3 nd], stop0 = none)
-void split_params(const SplitLayout &w, uint8_t *ws, ScanParams *sp) {
+// The split's workspace bound into the kernels' parameters: ScanParams' records, destinations and stop word (totals[3 nd],
+// stop0 = none), the split's RouteParams and phase 2's workspace in Params.  n / n_blocks, tile_first, data_bound and the
+// outputs are the caller's.
+void split_bind(const SplitLayout &w, uint8_t *ws, ScanParams *sp, RouteParams *rp, Params *p) {
     sp->dest = reinterpret_cast<uint32_t *>(ws + w.o_dest);
     sp->flat = reinterpret_cast<uint4 *>(ws + w.o_flat);
     sp->stop = reinterpret_cast<unsigned long long *>(ws + w.o_tot) + 3ull * w.nd;
     sp->stop0 = ~0ull;
+    *rp = RouteParams{};
+    rp->index = sp->flat;
+    rp->n_shards = w.nd;
+    rp->shard_of = sp->dest;
+    rp->hist = reinterpret_cast<uint32_t *>(ws + w.o_hist);
+    rp->totals = reinterpret_cast<unsigned long long *>(ws + w.o_tot);
+    rp->out_index = reinterpret_cast<uint4 *>(ws + w.o_split);
+    memset(p, 0, sizeof *p);
+    p->ctl = reinterpret_cast<Ctl *>(ws + w.o_ctl);
+    p->tile_bytes = reinterpret_cast<unsigned long long *>(ws + w.o_tbytes);
+    p->tile_count = reinterpret_cast<uint32_t *>(ws + w.o_tcount);
+    p->chunk_bytes = reinterpret_cast<unsigned long long *>(ws + w.o_cbytes);
+    p->chunk_count = reinterpret_cast<uint32_t *>(ws + w.o_ccount);
+    p->src_ptr = reinterpret_cast<unsigned long long *>(ws + w.o_src);
+    p->n_groups = w.nd;
+    p->mem_table = reinterpret_cast<unsigned long long *>(ws + w.o_memtab);
 }
 
-// Enqueued behind the kernels that wrote sp.flat / sp.dest (totals zeroed, the stop word set).  k_scan_hist drops what lies
-// at or past the stop, k_route_scan / k_route_starts / k_route_scatter split the records stably, and k_route_starts publishes
-// the totals (counts | bytes | starts | stop, nd each + 1) to the mapped pinned block at pin_tot.  `sized(totals)` runs on
-// them before the caps are checked: DBEEL_ERR_CAPACITY (nothing written, *items / *bytes = the required sizes) is the
-// caller's to report.  Then k_scan_tile_sums .. k_rebase_index write the output; ms_total runs from EV_START.
+// k_scan_hist drops what lies at or past the stop, k_route_scan / k_route_starts / k_route_scatter split the records
+// stably into rp.out_index, and k_route_starts publishes the totals (counts | bytes | starts | stop, nd each + 1) to pub.
+void launch_split(dbeel_engine *e, const ScanParams &sp, const RouteParams &rp, unsigned long long *pub) {
+    cudaStream_t s = e->stream;
+    launch_k(e, k_scan_hist, rp.n_blocks, kRouteThreads, 0, s, sp, rp);
+    launch_k(e, k_route_scan, rp.n_shards, 1024, 0, s, rp);
+    launch_k(e, k_route_starts, 1, 256, 0, s, rp, pub);
+    launch_k(e, k_route_scatter, rp.n_blocks, kRouteThreads, 0, s, rp);
+}
+
+// Phase 2 over n split records (a bound: tiles past Ctl.span return at once): k_emit's .index offsets scan, the payload
+// gather over gather_tiles 8 KB output tiles (past Ctl.out_data_len they return at once; no filter: Params.bloom.words is
+// null), per-destination file offsets.
+void launch_phase2(dbeel_engine *e, const Params &p, const uint4 *split, uint64_t n, uint64_t gather_tiles) {
+    cudaStream_t s = e->stream;
+    const uint32_t tiles = (uint32_t)((n + kResolveThreads - 1) / kResolveThreads);
+    launch_k(e, k_scan_tile_sums, tiles, kResolveThreads, 0, s, p, split);
+    launch_k(e, k_scan_tiles, (tiles + 1023) / 1024, 1024, 0, s, p);
+    launch_k(e, k_scan_chunks, 1, 1024, 0, s, p);
+    launch_k(e, k_emit, tiles, kResolveThreads, 0, s, p, split);
+    launch_k(e, k_gather_h, (uint32_t)gather_tiles, kGhThreads, 0, s, p);
+    launch_k(e, k_rebase_index, (uint32_t)((n + 255) / 256), 256, 0, s, p);
+}
+
+// Enqueued behind the kernels that wrote sp.flat / sp.dest (totals zeroed, the stop word set); sp, rp and p come from
+// split_bind.  The split publishes to the mapped pinned block at pin_tot.  `sized(totals)` runs on them before the caps are
+// checked: DBEEL_ERR_CAPACITY (nothing written, *items / *bytes = the required sizes) is the caller's to report.  Then
+// phase 2 writes the output; ms_total runs from EV_START.
 template <class F>
-int split_emit(dbeel_engine *e, const SplitLayout &w, const ScanParams &sp, uint64_t pin_tot, bool device, dbeel_out *out,
-               uint32_t *launches, uint64_t *items_out, uint64_t *bytes_out, F &&sized) {
+int split_emit(dbeel_engine *e, const SplitLayout &w, const ScanParams &sp, RouteParams rp, Params p, uint64_t pin_tot, bool device,
+               dbeel_out *out, uint32_t *launches, uint64_t *items_out, uint64_t *bytes_out, F &&sized) {
     cudaStream_t s = e->stream;
     uint8_t *ws = e->ws, *h = e->pin;
-    const uint32_t n = w.n, nd = w.nd;
-    RouteParams rp = {};
-    rp.index = sp.flat;
-    rp.n = n;
-    rp.n_shards = nd;
+    const uint32_t nd = w.nd;
+    rp.n = w.n;
     rp.n_blocks = w.n_blocks;
-    rp.shard_of = sp.dest;
-    rp.hist = reinterpret_cast<uint32_t *>(ws + w.o_hist);
-    rp.totals = reinterpret_cast<unsigned long long *>(ws + w.o_tot);
-    rp.out_index = reinterpret_cast<uint4 *>(ws + w.o_split);
-    launch_k(e, k_scan_hist, w.n_blocks, kRouteThreads, 0, s, sp, rp);
-    launch_k(e, k_route_scan, nd, 1024, 0, s, rp);
-    unsigned long long *host_tot = reinterpret_cast<unsigned long long *>(e->pin + pin_tot);
-    launch_k(e, k_route_starts, 1, 256, 0, s, rp, reinterpret_cast<unsigned long long *>(e->pin_dev + pin_tot));
-    launch_k(e, k_route_scatter, w.n_blocks, kRouteThreads, 0, s, rp);
+    launch_split(e, sp, rp, reinterpret_cast<unsigned long long *>(e->pin_dev + pin_tot));
     *launches += 4;
+    unsigned long long *host_tot = reinterpret_cast<unsigned long long *>(e->pin + pin_tot);
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(s));
     sized(static_cast<const unsigned long long *>(host_tot));
@@ -1953,31 +2014,14 @@ int split_emit(dbeel_engine *e, const SplitLayout &w, const ScanParams &sp, uint
             hm[2 * d + 1] = before_i;
             if (d < nd) { before_b += host_tot[nd + d]; before_i += host_tot[d]; }
         }
-        Params p;
-        memset(&p, 0, sizeof p);
-        p.ctl = reinterpret_cast<Ctl *>(ws + w.o_ctl);
-        p.tile_bytes = reinterpret_cast<unsigned long long *>(ws + w.o_tbytes);
-        p.tile_count = reinterpret_cast<uint32_t *>(ws + w.o_tcount);
-        p.chunk_bytes = reinterpret_cast<unsigned long long *>(ws + w.o_cbytes);
-        p.chunk_count = reinterpret_cast<uint32_t *>(ws + w.o_ccount);
-        p.src_ptr = reinterpret_cast<unsigned long long *>(ws + w.o_src);
         p.tile_first = tile_first;
         p.tile_first_n = (uint32_t)(gather_tiles + 2);
         p.data_bound = bytes;
-        p.n_groups = nd;
-        p.mem_table = reinterpret_cast<unsigned long long *>(ws + w.o_memtab);
         p.out_data = o_data;
         p.out_index = reinterpret_cast<uint4 *>(o_index);
-        const uint4 *split = rp.out_index;
-        const uint32_t tiles = (uint32_t)((items + kResolveThreads - 1) / kResolveThreads);
         launch_k(e, k_copy_words, (uint32_t)((w.header2_bytes / 4 + 255) / 256), 256, 0, s, reinterpret_cast<uint32_t *>(ws + w.o_ctl),
                  reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(w.header2_bytes / 4));
-        launch_k(e, k_scan_tile_sums, tiles, kResolveThreads, 0, s, p, split);
-        launch_k(e, k_scan_tiles, (tiles + 1023) / 1024, 1024, 0, s, p);
-        launch_k(e, k_scan_chunks, 1, 1024, 0, s, p);
-        launch_k(e, k_emit, tiles, kResolveThreads, 0, s, p, split);
-        launch_k(e, k_gather_h, (uint32_t)gather_tiles, kGhThreads, 0, s, p); // no filter: Params.bloom.words is null
-        launch_k(e, k_rebase_index, (uint32_t)((items + 255) / 256), 256, 0, s, p);
+        launch_phase2(e, p, rp.out_index, items, gather_tiles);
         *launches += 7;
     }
     CU(cudaEventRecord(e->ev[EV_GATHER], s));
@@ -2009,8 +2053,7 @@ int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
     e->err.clear();
     e->stats = dbeel_stats{};
     out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
-    for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
-    *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+    clear_scan(results, n_ranges, stop);
     uint64_t n64 = 0, data_total = 0, index_total = 0;
     unsigned long long stop0 = ~0ull; // an empty table: its first index read runs past EOF
     for (uint32_t t = 0; t < n_tables; t++) {
@@ -2069,41 +2112,34 @@ int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
     uint64_t off = 0;
     // header block, one copy through the mapped pinned block: tables | hash ranges or key offsets | range keys
     const uint64_t o_tab = carve_ws(&off, sizeof(ScanTable) * n_tables);
-    const uint64_t o_rng = carve_ws(&off, kind == DBEEL_SCAN_KEY ? 8ull * (2 * nd + 1) : 8ull * nd);
-    const uint64_t o_keys = carve_ws(&off, key_bytes + 16);
-    const uint64_t header_bytes = off;
+    const RangeHeader rh = carve_ranges(&off, kind, nd, key_bytes);
     const SplitLayout w = carve_split(&off, n, nd);
     int rc = ensure_device(e, &e->ws, &e->ws_cap, off);
-    const uint64_t pin_tot = align_up(std::max(header_bytes, w.header2_bytes), 64);
+    const uint64_t pin_tot = align_up(std::max(rh.bytes, w.header2_bytes), 64);
     if (!rc) rc = ensure_pinned(e, pin_tot + 8ull * (3 * nd + 1));
     if (rc) return rc;
-    uint8_t *ws = e->ws, *h = e->pin;
-    memcpy(h + o_tab, td.data(), sizeof(ScanTable) * n_tables);
-    scan_range_header(kind, ranges, nd, key_bytes, h + o_rng, h + o_keys);
+    uint8_t *ws = e->ws;
+    memcpy(e->pin + o_tab, td.data(), sizeof(ScanTable) * n_tables);
 
     ScanParams sp = {};
+    RouteParams rp;
+    Params p;
     sp.tables = reinterpret_cast<const ScanTable *>(ws + o_tab);
     sp.n_tables = n_tables;
     sp.n = n;
-    sp.key_kind = kind == DBEEL_SCAN_KEY ? 1u : 0u;
-    sp.n_ranges = nd;
-    sp.hash_ranges = reinterpret_cast<const uint32_t *>(ws + o_rng);
-    sp.key_off = reinterpret_cast<const unsigned long long *>(ws + o_rng);
-    sp.keys = ws + o_keys;
-    split_params(w, ws, &sp);
+    split_bind(w, ws, &sp, &rp, &p);
     sp.stop0 = stop0;
 
     // ---- phase 1: classify; the split and phase 2 (split_emit) size the output from what it selected
     uint32_t launches = 0;
     CU(cudaEventRecord(e->ev[EV_START], s));
-    launch_k(e, k_copy_words, (uint32_t)((header_bytes / 4 + 255) / 256), 256, 0, s, reinterpret_cast<uint32_t *>(ws),
-             reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(header_bytes / 4));
+    land_ranges(e, rh, kind, ranges, nd, key_bytes, &sp);
     CU(cudaMemsetAsync(ws + w.o_tot, 0, 8ull * 3 * nd, s));
     CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
     launch_k(e, k_scan_classify, (n + 255) / 256, 256, 0, s, sp);
     launches += 2;
     uint64_t items = 0, bytes = 0;
-    rc = split_emit(e, w, sp, pin_tot, device, out, &launches, &items, &bytes, [&](const unsigned long long *host_tot) {
+    rc = split_emit(e, w, sp, rp, p, pin_tot, device, out, &launches, &items, &bytes, [&](const unsigned long long *host_tot) {
         const unsigned long long stop_key = std::min<unsigned long long>(host_tot[3 * nd], stop0);
         set_stop(stop_key);
         e->stats.entries_valid = stop_key == ~0ull ? n : (stop_key >> 12);
@@ -2120,7 +2156,7 @@ int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
         }
     });
     if (rc == DBEEL_ERR_CAPACITY) {
-        for (uint32_t d = 0; d < nd; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
+        std::fill_n(results, nd, dbeel_job_result{});
         return fail(e, DBEEL_ERR_CAPACITY, "scan output larger than the buffers (index records that overlap in .data)");
     }
     return rc;
@@ -2162,7 +2198,9 @@ int get_values_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tabl
     if (rc) return rc;
     uint8_t *ws = e->ws;
     ScanParams sp = {};
-    split_params(w, ws, &sp);
+    RouteParams rp;
+    Params p;
+    split_bind(w, ws, &sp, &rp, &p);
     uint4 *d_res = device ? reinterpret_cast<uint4 *>(results) : reinterpret_cast<uint4 *>(ws + o_rows);
     LookupParams lp{reinterpret_cast<const TableDesc *>(ws + o_desc), n_tables, mode, d_keys, d_off, n_keys, d_res};
     e->stats.entries_in = n_keys;
@@ -2173,7 +2211,7 @@ int get_values_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tabl
     launch_k(e, k_lookup_emit, (n + 255) / 256, 256, 0, s, lp, LookupEmit{sp.dest, sp.flat});
     if (!device) CU(cudaMemcpyAsync(results, d_res, 16ull * n, cudaMemcpyDeviceToHost, s)); // back with the sizes: filled on ERR_CAPACITY too
     uint64_t items = 0, bytes = 0;
-    rc = split_emit(e, w, sp, pin_tot, device, out, &launches, &items, &bytes, [](const unsigned long long *) {});
+    rc = split_emit(e, w, sp, rp, p, pin_tot, device, out, &launches, &items, &bytes, [](const unsigned long long *) {});
     if (rc == DBEEL_ERR_CAPACITY) {
         out->data_len = bytes;
         out->index_len = 16 * items;
@@ -2731,7 +2769,9 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
         CU(cudaStreamSynchronize(s));
     }
     ScanParams sp = {};
-    split_params(w, ws, &sp);
+    RouteParams rp;
+    Params p;
+    split_bind(w, ws, &sp, &rp, &p);
     CU(cudaMemsetAsync(ws + w.o_tot, 0, 8ull * 3, s));
     CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
     launch_k(e, k_gvs_hit, grid, 256, 0, s, gq, static_cast<const uint8_t *>(e->stage_out2), LookupEmit{sp.dest, sp.flat});
@@ -2740,7 +2780,7 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
     e->stats.entries_in = n_keys;
     e->stats.partitions = groups;
     uint64_t items = 0, bytes = 0;
-    rc = split_emit(e, w, sp, pin_tot, false, out, &launches, &items, &bytes, [](const unsigned long long *) {});
+    rc = split_emit(e, w, sp, rp, p, pin_tot, false, out, &launches, &items, &bytes, [](const unsigned long long *) {});
     if (rc == DBEEL_ERR_CAPACITY) {
         out->data_len = bytes;
         out->index_len = 16 * items;
@@ -2752,8 +2792,9 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
 
 // ------------------------------------------------------------------------------------ N5 streamed: dbeel_scan_stream
 // The plan (host/scan_plan.h) cuts the record sequence into partitions; each goes file -> pinned ring slot -> device slot
-// c & 1 in ONE H2D copy of its slot image (table headers | per slice: index slice, .data window), runs the scan chain with
-// phase 2 sized from the plan's bound, and comes back with an exact D2H of what it selected.  H2D of c + 1, the kernels of c
+// c & 1 in ONE H2D copy of its slot image (table headers | per slice: index slice, .data window), runs k_scan_classify,
+// launch_split, k_scan_stream_carry and launch_phase2 with phase 2 sized from the plan's bound (the split's workspace from
+// split_bind, as split_emit's), and comes back with an exact D2H of what it selected.  H2D of c + 1, the kernels of c
 // and the D2H of c - 1 overlap; the engine thread enqueues partition c + 1's kernels before it waits for c's published sizes.
 // run_scan_plan runs a plan (steps 2 to the end) for dbeel_scan_stream (whole tables) and dbeel_reader_scan (spans): the
 // caller has checked the arguments, taken the engine, cleared results / stop / stats and set stats.entries_in.
@@ -2802,23 +2843,12 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
         h2d_bytes += in;
     }
     const uint64_t out_index_at = align_up(max_bound + 16, kAlign), max_out = out_index_at + align_up(16 * max_rec + 16, kAlign);
-    const uint32_t n_max = (uint32_t)max_rec;
-    const uint32_t n_blocks = (n_max + kRouteThreads - 1) / kRouteThreads;
-    const uint64_t res_tiles = (max_rec + kResolveThreads - 1) / kResolveThreads, res_chunks = (res_tiles + 1023) / 1024;
     const uint64_t gather_tiles_max = (max_bound + kGatherTileBytes - 1) / kGatherTileBytes;
     uint64_t off = 0;
-    auto carve = [&](uint64_t b) { uint64_t o2 = off; off = align_up(off + b, kAlign); return o2; };
-    const uint64_t o_rng = carve(kind == DBEEL_SCAN_KEY ? 8ull * (2 * nd + 1) : 8ull * nd);
-    const uint64_t o_keys = carve(key_bytes + 16);
-    const uint64_t header_bytes = off;
-    const uint64_t o_ctl = carve(sizeof(Ctl)), o_memtab = carve(16ull * (nd + 1));
-    const uint64_t o_tot = carve(8ull * (3 * nd + 1)), o_carry = carve(8ull * (2 * nd + 1));
-    const uint64_t o_dest = carve(4ull * n_max), o_flat = carve(16ull * n_max), o_split = carve(16ull * n_max);
-    const uint64_t o_hist = carve(4ull * n_blocks * nd);
-    const uint64_t o_tbytes = carve(8 * res_tiles), o_tcount = carve(4 * res_tiles);
-    const uint64_t o_cbytes = carve(8 * res_chunks), o_ccount = carve(4 * res_chunks);
-    const uint64_t o_src = carve(8ull * n_max), o_tf = carve(4ull * (gather_tiles_max + 2));
-    const uint64_t pub_words = 5ull * nd + 2, pub_stride = align_up(8 * pub_words, 64), pin_pub = align_up(header_bytes, 64);
+    const RangeHeader rh = carve_ranges(&off, kind, nd, key_bytes);
+    const SplitLayout w = carve_split(&off, (uint32_t)max_rec, nd);
+    const uint64_t o_carry = carve_ws(&off, 8ull * (2 * nd + 1)), o_tf = carve_ws(&off, 4ull * (gather_tiles_max + 2));
+    const uint64_t pub_words = 5ull * nd + 2, pub_stride = align_up(8 * pub_words, 64), pin_pub = align_up(rh.bytes, 64);
     // the merge stage: per split record its table, key prefix and keep flag / prefix sum; per destination its surviving
     // bytes; the error word; every slice's table and every splitter, uploaded once
     std::vector<uint32_t> m_slt;
@@ -2831,14 +2861,14 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
             m_keys.insert(m_keys.end(), k.begin(), k.end());
             m_koff.push_back(m_keys.size());
         }
-        o_mtab = carve(4ull * n_max);
-        o_mpfx = carve(8ull * n_max);
-        o_mpre = carve(4ull * n_max + 4);
-        o_mtile = carve(4ull * ((n_max + kRangeTile - 1) / kRangeTile + 1));
-        o_mbytes = carve(8ull * nd);
-        o_merr = carve(8);
-        o_mslt = carve(4ull * m_slt.size());
-        o_mkeys = carve(m_keys.size() + 16);
+        o_mtab = carve_ws(&off, 4ull * w.n);
+        o_mpfx = carve_ws(&off, 8ull * w.n);
+        o_mpre = carve_ws(&off, 4ull * w.n + 4);
+        o_mtile = carve_ws(&off, 4ull * ((w.n + kRangeTile - 1) / kRangeTile + 1));
+        o_mbytes = carve_ws(&off, 8ull * nd);
+        o_merr = carve_ws(&off, 8);
+        o_mslt = carve_ws(&off, 4ull * m_slt.size());
+        o_mkeys = carve_ws(&off, m_keys.size() + 16);
     }
     const uint32_t R = (uint32_t)std::max(2, e->stream_ring);
     rc = ensure_device(e, &e->ws, &e->ws_cap, off);
@@ -2873,40 +2903,16 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
     }
     pump.start();
 
-    // ---- 4. per-scan state on the device: ranges (once), carry, stop word
-    scan_range_header(kind, ranges, nd, key_bytes, e->pin + o_rng, e->pin + o_keys);
+    // ---- 4. per-scan state on the device: ranges (once), carry, stop word.  stop0 stays none: the plan ends before every
+    // stop the index shows (empty tables included).
     ScanParams sp = {};
-    sp.n_ranges = nd;
-    sp.key_kind = kind == DBEEL_SCAN_KEY ? 1u : 0u;
-    sp.hash_ranges = reinterpret_cast<const uint32_t *>(ws + o_rng);
-    sp.key_off = reinterpret_cast<const unsigned long long *>(ws + o_rng);
-    sp.keys = ws + o_keys;
-    sp.dest = reinterpret_cast<uint32_t *>(ws + o_dest);
-    sp.flat = reinterpret_cast<uint4 *>(ws + o_flat);
-    sp.stop = reinterpret_cast<unsigned long long *>(ws + o_tot) + 3ull * nd;
-    sp.stop0 = ~0ull; // the plan ends before every stop the index shows (empty tables included)
-    RouteParams rp = {};
-    rp.index = sp.flat;
-    rp.n_shards = nd;
-    rp.shard_of = sp.dest;
-    rp.hist = reinterpret_cast<uint32_t *>(ws + o_hist);
-    rp.totals = reinterpret_cast<unsigned long long *>(ws + o_tot);
-    rp.out_index = reinterpret_cast<uint4 *>(ws + o_split);
+    RouteParams rp;
     Params p;
-    memset(&p, 0, sizeof p);
-    p.ctl = reinterpret_cast<Ctl *>(ws + o_ctl);
-    p.tile_bytes = reinterpret_cast<unsigned long long *>(ws + o_tbytes);
-    p.tile_count = reinterpret_cast<uint32_t *>(ws + o_tcount);
-    p.chunk_bytes = reinterpret_cast<unsigned long long *>(ws + o_cbytes);
-    p.chunk_count = reinterpret_cast<uint32_t *>(ws + o_ccount);
-    p.src_ptr = reinterpret_cast<unsigned long long *>(ws + o_src);
+    split_bind(w, ws, &sp, &rp, &p);
     p.tile_first = reinterpret_cast<uint32_t *>(ws + o_tf);
-    p.n_groups = nd;
-    p.mem_table = reinterpret_cast<unsigned long long *>(ws + o_memtab);
     unsigned long long *carry = reinterpret_cast<unsigned long long *>(ws + o_carry);
     CU(cudaEventRecord(e->ev[EV_START], s));
-    launch_k(e, k_copy_words, (uint32_t)((header_bytes / 4 + 255) / 256), 256, 0, s, reinterpret_cast<uint32_t *>(ws),
-             reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(header_bytes / 4));
+    land_ranges(e, rh, kind, ranges, nd, key_bytes, &sp);
     CU(cudaMemsetAsync(carry, 0, 8ull * (2 * nd + 1), s));
     CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
     RangeMergeParams mp = {};
@@ -2951,7 +2957,6 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
     auto enqueue_kernels = [&](uint32_t c) -> int {
         const ScanPart &pt = plan.parts[c];
         const uint32_t n = (uint32_t)pt.n_rec, nb = (n + kRouteThreads - 1) / kRouteThreads;
-        const uint32_t tiles = (n + kResolveThreads - 1) / kResolveThreads;
         const uint64_t gtiles = (pt.data_bound + kGatherTileBytes - 1) / kGatherTileBytes;
         CU(cudaStreamWaitEvent(s, e->ev_h2d[c & 1], 0));
         if (c >= 2) CU(cudaStreamWaitEvent(s, e->ev_d2h[c & 1], 0)); // output slot c & 1 has gone back to the host
@@ -2970,10 +2975,7 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
         unsigned long long *pub = reinterpret_cast<unsigned long long *>(e->pin_dev + pin_pub + (c & 1) * pub_stride);
         CU(cudaMemsetAsync(rp.totals, 0, 8ull * 3 * nd, s));
         launch_k(e, k_scan_classify, (n + 255) / 256, 256, 0, s, spc);
-        launch_k(e, k_scan_hist, nb, kRouteThreads, 0, s, spc, rpc);
-        launch_k(e, k_route_scan, nd, 1024, 0, s, rpc);
-        launch_k(e, k_route_starts, 1, 256, 0, s, rpc, pub);
-        launch_k(e, k_route_scatter, nb, kRouteThreads, 0, s, rpc);
+        launch_split(e, spc, rpc, pub);
         const uint4 *split = rpc.out_index;
         if (merge) { // the merged split replaces the split, in flat
             RangeMergeParams mpc = mp;
@@ -3003,12 +3005,7 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
             split = sp.flat;
         }
         launch_k(e, k_scan_stream_carry, 1, 32, 0, s, rpc, pc, carry, pub);
-        launch_k(e, k_scan_tile_sums, tiles, kResolveThreads, 0, s, pc, split);
-        launch_k(e, k_scan_tiles, (tiles + 1023) / 1024, 1024, 0, s, pc);
-        launch_k(e, k_scan_chunks, 1, 1024, 0, s, pc);
-        launch_k(e, k_emit, tiles, kResolveThreads, 0, s, pc, split);
-        launch_k(e, k_gather_h, (uint32_t)gtiles, kGhThreads, 0, s, pc); // tiles past Ctl.out_data_len return at once
-        launch_k(e, k_rebase_index, (n + 255) / 256, 256, 0, s, pc);
+        launch_phase2(e, pc, split, n, gtiles);
         launches += 12;
         CU(cudaGetLastError());
         CU(cudaEventRecord(e->ev_comp[c & 1], s));
@@ -3071,8 +3068,7 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
         cudaStreamSynchronize(s);
         cudaStreamSynchronize(e->s_d2h);
         pump.abort(rc);
-        for (uint32_t d = 0; d < nd; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
-        *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+        clear_scan(results, nd, stop);
         return rc;
     }
     CU(cudaEventRecord(e->ev[EV_GATHER], s));
@@ -3080,8 +3076,7 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
     CU(cudaStreamSynchronize(e->s_d2h));
     const int frc = pump.finish(); // every destination's bytes have gone through the write callback
     if (frc) {
-        for (uint32_t d = 0; d < nd; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
-        *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+        clear_scan(results, nd, stop);
         return fail(e, frc, "stream write callback failed");
     }
     if (!stopped) host_stop();
@@ -3103,19 +3098,32 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
     return DBEEL_OK;
 }
 
-// plan_scan over tables[0 .. n_tables) (spans: null = whole tables) through io->read, then run_scan_plan
+// The tables as plan_scan / plan_merge take them: their lengths, and their .index files read through io->read.
+struct PlanTables {
+    std::vector<uint64_t> dlen, ilen;
+    ScanIndexRead read_index;
+};
+
+PlanTables plan_tables(const dbeel_table *tables, uint32_t n_tables, const dbeel_scan_io *io) {
+    PlanTables pt{std::vector<uint64_t>(n_tables), std::vector<uint64_t>(n_tables),
+                  [io](uint32_t t, uint64_t off, uint64_t len, void *dst) { return io->read(io->ctx, t, DBEEL_STREAM_INDEX, off, len, dst); }};
+    for (uint32_t t = 0; t < n_tables; t++) {
+        pt.dlen[t] = tables[t].data_len;
+        pt.ilen[t] = tables[t].index_len;
+    }
+    return pt;
+}
+
+// 1. plan_scan over tables[0 .. n_tables) through io->read, from the .index files read in pieces; then run_scan_plan.
+// spans: null = whole tables, whose index records all count in stats.entries_in (reader_spans counts the spans').
 int plan_and_run_scan(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
                       uint32_t n_ranges, uint64_t key_bytes, const dbeel_scan_io *io, dbeel_job_result *results,
                       dbeel_scan_stop *stop, const std::vector<std::vector<ScanSpan>> *spans) {
-    std::vector<uint64_t> dlen(n_tables), ilen(n_tables);
-    for (uint32_t t = 0; t < n_tables; t++) {
-        dlen[t] = tables[t].data_len;
-        ilen[t] = tables[t].index_len;
-    }
+    if (!spans)
+        for (uint32_t t = 0; t < n_tables; t++) e->stats.entries_in += tables[t].index_len / DBEEL_INDEX_ENTRY_SIZE;
+    const PlanTables pt = plan_tables(tables, n_tables, io);
     ScanPlan plan;
-    const int rc = plan_scan(dlen.data(), ilen.data(), n_tables, e->partition_bytes,
-                             [io](uint32_t t, uint64_t off, uint64_t len, void *dst) { return io->read(io->ctx, t, DBEEL_STREAM_INDEX, off, len, dst); },
-                             &plan, spans);
+    const int rc = plan_scan(pt.dlen.data(), pt.ilen.data(), n_tables, e->partition_bytes, pt.read_index, &plan, spans);
     if (rc) return fail(e, rc, "stream read callback failed (.index, planning)");
     return run_scan_plan(e, tables, plan, kind, ranges, n_ranges, key_bytes, io, results, stop);
 }
@@ -3130,11 +3138,7 @@ int scan_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tab
     BusyGuard g(e);
     e->err.clear();
     e->stats = dbeel_stats{};
-    for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
-    *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
-
-    // ---- 1. the plan, from the .index files read in pieces
-    for (uint32_t t = 0; t < n_tables; t++) e->stats.entries_in += tables[t].index_len / DBEEL_INDEX_ENTRY_SIZE;
+    clear_scan(results, n_ranges, stop);
     return plan_and_run_scan(e, tables, n_tables, kind, ranges, n_ranges, key_bytes, io, results, stop, nullptr);
 }
 
@@ -3156,6 +3160,16 @@ int reader_scan_read(void *ctx, uint32_t t, uint32_t kind, uint64_t off, uint64_
 int reader_scan_write(void *ctx, uint32_t d, uint32_t kind, uint64_t off, const void *src, uint64_t len) {
     ReaderScanIo *x = static_cast<ReaderScanIo *>(ctx);
     return x->write(x->wctx, d, kind, off, src, len);
+}
+
+// The reader's tables as the entry points take them: lengths only, their bytes come through the reader's callback.
+std::vector<dbeel_table> reader_tables(const dbeel_reader *r) {
+    std::vector<dbeel_table> tables(r->tables.size());
+    for (size_t i = 0; i < tables.size(); i++) {
+        const TableDesc &d = r->tables[i]->desc;
+        tables[i] = dbeel_table{nullptr, d.data_len, nullptr, d.n * DBEEL_INDEX_ENTRY_SIZE, nullptr, 0};
+    }
+    return tables;
 }
 
 // Vec<u8>::cmp(a, b) < 0
@@ -3370,44 +3384,6 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
     return rc;
 }
 
-int reader_scan_entry(dbeel_reader *r, uint32_t kind, const void *ranges, uint32_t n_ranges,
-                      int (*write)(void *, uint32_t, uint32_t, uint64_t, const void *, uint64_t), void *ctx,
-                      dbeel_job_result *results, dbeel_scan_stop *stop) {
-    dbeel_engine *e = r->e;
-    if (!write) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
-    std::vector<dbeel_table> tables(r->tables.size());
-    for (size_t i = 0; i < tables.size(); i++) {
-        const TableDesc &d = r->tables[i]->desc;
-        tables[i] = dbeel_table{nullptr, d.data_len, nullptr, d.n * DBEEL_INDEX_ENTRY_SIZE, nullptr, 0};
-    }
-    const uint32_t nt = (uint32_t)tables.size();
-    uint64_t key_bytes = 0;
-    if (const int arc = scan_args(e, tables.data(), nt, kind, ranges, n_ranges, results, stop, &key_bytes)) return arc;
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
-    for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
-    *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
-    ReaderScanIo x;
-    x.rio = &r->io;
-    x.write = write;
-    x.wctx = ctx;
-    const dbeel_scan_io io{reader_scan_read, reader_scan_write, &x};
-    if (kind == DBEEL_SCAN_HASH) { // dbeel_scan_stream on the snapshot
-        for (uint32_t t = 0; t < nt; t++) e->stats.entries_in += tables[t].index_len / DBEEL_INDEX_ENTRY_SIZE;
-        return plan_and_run_scan(e, tables.data(), nt, kind, ranges, n_ranges, key_bytes, &io, results, stop, nullptr);
-    }
-    const int rc = reader_scan_key(e, r, tables.data(), ranges, n_ranges, key_bytes, &io, results, stop);
-    if (rc) {
-        cudaStreamSynchronize(e->stream); // nothing of this call may touch the engine's buffers after it returns
-        for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
-        *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
-    }
-    e->stats.input_bytes = x.bytes;
-    return rc;
-}
-
 // ---- dbeel_reader_get_range
 int discard_write(void *, uint32_t, uint32_t, uint64_t, const void *, uint64_t) { return 0; }
 
@@ -3423,30 +3399,18 @@ int reader_get_range_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *ta
     int rc = reader_spans(e, r, ranges, nd, key_bytes, io, &spans, &host_stop);
     if (rc) return rc;
     const uint32_t nt = (uint32_t)spans.size();
-    auto void_results = [&]() {
-        for (uint32_t d = 0; d < nd; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
-    };
     auto raw_stop = [&]() -> int { // *stop = dbeel_reader_scan's; partitions stays the key partitions run (0: none)
         const dbeel_scan_io dio{io->read, discard_write, io->ctx};
         std::vector<dbeel_job_result> scratch(nd);
         const uint32_t parts = e->stats.partitions;
-        *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+        clear_scan(results, nd, stop);
         const int src = plan_and_run_scan(e, tables, nt, DBEEL_SCAN_KEY, ranges, nd, key_bytes, &dio, scratch.data(), stop, &spans);
         if (!src && stop->table < 0) *stop = host_stop;
-        void_results();
         e->stats.output_bytes = e->stats.entries_out = 0; // nothing that was written stands
         e->stats.partitions = parts;
         return src;
     };
     if (host_stop.table >= 0) return raw_stop();
-    std::vector<uint64_t> dlen(nt), ilen(nt);
-    for (uint32_t t = 0; t < nt; t++) {
-        dlen[t] = tables[t].data_len;
-        ilen[t] = tables[t].index_len;
-    }
-    const ScanIndexRead read_index = [io](uint32_t t, uint64_t off, uint64_t len, void *dst) {
-        return io->read(io->ctx, t, DBEEL_STREAM_INDEX, off, len, dst);
-    };
     const MergeKeyRead read_key = [io](uint32_t t, uint64_t off, uint32_t fs, std::vector<uint8_t> *key, bool *ok) {
         constexpr uint64_t kHead = 8 + DBEEL_READER_FRAME_CAP; // most keys come with their length prefix in one read
         std::vector<uint8_t> b(std::min<uint64_t>(fs, kHead));
@@ -3492,8 +3456,9 @@ int reader_get_range_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *ta
         }
         return 0;
     };
+    const PlanTables pt = plan_tables(tables, nt, io);
     MergePlan mplan;
-    rc = plan_merge(dlen.data(), ilen.data(), nt, e->partition_bytes, spans, read_index, read_key, seek, &mplan);
+    rc = plan_merge(pt.dlen.data(), pt.ilen.data(), nt, e->partition_bytes, spans, pt.read_index, read_key, seek, &mplan);
     if (rc) return e->err.empty() ? fail(e, rc, "stream read callback failed (planning)") : rc;
     if (mplan.refused) { // nothing past the budget is staged: the raw scan's stop, else keys that do not ascend
         if ((rc = raw_stop()) || stop->table >= 0) return rc;
@@ -3504,44 +3469,39 @@ int reader_get_range_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *ta
     rc = run_scan_plan(e, tables, mplan.plan, DBEEL_SCAN_KEY, ranges, nd, key_bytes, io, results, stop, &m);
     if (rc) return rc;
     if (stop->table >= 0) return raw_stop();
-    if (m.unsorted) {
-        void_results();
-        return fail(e, DBEEL_ERR_UNSORTED_RUN, "a table's span records do not strictly ascend by key");
-    }
+    if (m.unsorted) return fail(e, DBEEL_ERR_UNSORTED_RUN, "a table's span records do not strictly ascend by key");
     return DBEEL_OK;
 }
 
-int reader_get_range_entry(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, uint32_t flags,
-                           int (*write)(void *, uint32_t, uint32_t, uint64_t, const void *, uint64_t), void *ctx,
-                           dbeel_job_result *results, dbeel_scan_stop *stop) {
+// dbeel_reader_scan, or dbeel_reader_get_range when `get_range` (kind DBEEL_SCAN_KEY), on the reader's tables through its
+// read callback, counted in input_bytes.  Hash ranges read every table as dbeel_scan_stream does.
+int reader_range_entry(dbeel_reader *r, bool get_range, uint32_t kind, const void *ranges, uint32_t n_ranges, uint32_t flags,
+                       int (*write)(void *, uint32_t, uint32_t, uint64_t, const void *, uint64_t), void *ctx,
+                       dbeel_job_result *results, dbeel_scan_stop *stop) {
     dbeel_engine *e = r->e;
     if (!write) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     if (flags & ~DBEEL_RANGE_KEEP_TOMBSTONES) return fail(e, DBEEL_ERR_INVALID_ARG, "unknown flag");
-    std::vector<dbeel_table> tables(r->tables.size());
-    for (size_t i = 0; i < tables.size(); i++) {
-        const TableDesc &d = r->tables[i]->desc;
-        tables[i] = dbeel_table{nullptr, d.data_len, nullptr, d.n * DBEEL_INDEX_ENTRY_SIZE, nullptr, 0};
-    }
+    const std::vector<dbeel_table> tables = reader_tables(r);
+    const uint32_t nt = (uint32_t)tables.size();
     uint64_t key_bytes = 0;
-    if (const int arc = scan_args(e, tables.data(), (uint32_t)tables.size(), DBEEL_SCAN_KEY, ranges, n_ranges, results, stop, &key_bytes))
-        return arc;
+    if (const int arc = scan_args(e, tables.data(), nt, kind, ranges, n_ranges, results, stop, &key_bytes)) return arc;
     if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
     BusyGuard g(e);
     e->err.clear();
     e->stats = dbeel_stats{};
-    for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
-    *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+    clear_scan(results, n_ranges, stop);
     ReaderScanIo x;
     x.rio = &r->io;
     x.write = write;
     x.wctx = ctx;
     const dbeel_scan_io io{reader_scan_read, reader_scan_write, &x};
-    const int rc = reader_get_range_key(e, r, tables.data(), ranges, n_ranges, key_bytes, (flags & DBEEL_RANGE_KEEP_TOMBSTONES) != 0,
-                                        &io, results, stop);
+    if (kind == DBEEL_SCAN_HASH) return plan_and_run_scan(e, tables.data(), nt, kind, ranges, n_ranges, key_bytes, &io, results, stop, nullptr);
+    const int rc = get_range ? reader_get_range_key(e, r, tables.data(), ranges, n_ranges, key_bytes,
+                                                    (flags & DBEEL_RANGE_KEEP_TOMBSTONES) != 0, &io, results, stop)
+                             : reader_scan_key(e, r, tables.data(), ranges, n_ranges, key_bytes, &io, results, stop);
     if (rc) {
         cudaStreamSynchronize(e->stream); // nothing of this call may touch the engine's buffers after it returns
-        for (uint32_t d = 0; d < n_ranges; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
-        *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+        clear_scan(results, n_ranges, stop);
     }
     e->stats.input_bytes = x.bytes;
     return rc;
@@ -3943,11 +3903,7 @@ int dbeel_reader_get_values(dbeel_reader *r, const void *keys, const uint64_t *k
                             dbeel_out *out, dbeel_lookup_result *results) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
     REFUSE_WHILE_ASYNC(r->e);
-    std::vector<dbeel_table> tables(r->tables.size());
-    for (size_t i = 0; i < tables.size(); i++) {
-        const TableDesc &d = r->tables[i]->desc;
-        tables[i] = dbeel_table{nullptr, d.data_len, nullptr, d.n * DBEEL_INDEX_ENTRY_SIZE, nullptr, 0};
-    }
+    const std::vector<dbeel_table> tables = reader_tables(r);
     return get_values_stream_entry(r->e, tables.data(), (uint32_t)tables.size(), keys, key_offsets, n_keys, mode, &r->io, out, results, r);
 }
 
@@ -3956,7 +3912,7 @@ int dbeel_reader_scan(dbeel_reader *r, uint32_t kind, const void *ranges, uint32
                       void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
     REFUSE_WHILE_ASYNC(r->e);
-    return reader_scan_entry(r, kind, ranges, n_ranges, write, ctx, results, stop);
+    return reader_range_entry(r, false, kind, ranges, n_ranges, 0, write, ctx, results, stop);
 }
 
 void dbeel_reader_close(dbeel_reader *r) {
@@ -3972,7 +3928,7 @@ int dbeel_reader_get_range(dbeel_reader *r, const dbeel_key_ranges *ranges, uint
                            void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
     REFUSE_WHILE_ASYNC(r->e);
-    return reader_get_range_entry(r, ranges, n_ranges, flags, write, ctx, results, stop);
+    return reader_range_entry(r, true, DBEEL_SCAN_KEY, ranges, n_ranges, flags, write, ctx, results, stop);
 }
 
 int dbeel_page_cache_create(dbeel_engine *e, uint64_t bytes, dbeel_page_cache **out) {

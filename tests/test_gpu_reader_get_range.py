@@ -86,6 +86,8 @@ def check(e, reader, tables, ranges, keep=False):
     assert st["input_bytes"] == sum(r[3] for r in reads)
     assert st["output_bytes"] == sum(g[0].size + g[1].size for g in out)
     assert st["entries_out"] == sum(g[1].size // 16 for g in out)
+    if stop[0] < 0 and st["partitions"]:  # the range header copy, then the scan chain + the merge stage per partition
+        assert st["kernel_launches"] == 1 + 20 * st["partitions"]
     for t, kind, off, size in reads:
         f = tables[t][0] if kind == 1 else tables[t][1]
         assert kind in (1, 2) and off + size <= len(f)

@@ -27,6 +27,9 @@ def _check(got, exp, what):
 def _both(engine, tables, ranges, kind, what):
     exp = scan_oracle.scan(tables, ranges, kind)
     _check(engine.scan(tables, ranges, kind), exp, what)
+    st = engine.stats()
+    if st["entries_in"]:  # header copy + classify, the split, then the second header copy + phase 2 if anything was selected
+        assert st["kernel_launches"] == (13 if st["entries_out"] else 6), what
     return exp
 
 

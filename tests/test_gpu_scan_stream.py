@@ -43,6 +43,9 @@ def _all(stream_engine, tables, ranges, kind, what, engine=None):
     exp = scan_oracle.scan(tables, ranges, kind)
     got = stream_engine.scan_stream(tables, ranges, kind)
     _check(got, exp, what)
+    st = stream_engine.stats()
+    if st["partitions"]:  # the range header copy, then classify + split + carry + phase 2 per partition
+        assert st["kernel_launches"] == 1 + 12 * st["partitions"], what
     if engine is not None:
         _check(engine.scan(tables, ranges, kind), exp, what + " (dbeel_scan)")
     return exp
