@@ -27,6 +27,8 @@ SCAN_HASH = 0  # ranges: (start, end) u32 pairs, murmur3_32(key) tested with mig
 SCAN_KEY = 1   # ranges: (start, end) byte strings, start <= key < end
 SCAN_STOP_NONE, SCAN_STOP_ERR, SCAN_STOP_PANIC = 0, 1, 2
 RANGE_KEEP_TOMBSTONES = 0x1  # dbeel_reader_get_range: keep entries with dlen == 0
+RANGE_LIMIT_MAX = 65536  # dbeel_reader_get_ranges: the largest limit of one query
+RANGE_MORE, RANGE_STOPPED, RANGE_UNSORTED = 0x1, 0x2, 0x4  # dbeel_range_row.flags
 ERR_UNSORTED_RUN = 8
 ERR_CAPACITY = 2
 ERR_INVALID_ARG = 1
@@ -47,7 +49,7 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream",
            "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device", "dbeel_scan_stream", "dbeel_get_values",
            "dbeel_get_values_device", "dbeel_get_values_stream", "dbeel_reader_open", "dbeel_reader_get_values",
-           "dbeel_reader_scan", "dbeel_reader_get_range", "dbeel_reader_close", "dbeel_page_cache_create", "dbeel_page_cache_destroy",
+           "dbeel_reader_scan", "dbeel_reader_get_range", "dbeel_reader_get_ranges", "dbeel_reader_close", "dbeel_page_cache_create", "dbeel_page_cache_destroy",
            "dbeel_reader_attach_page_cache", "dbeel_page_cache_stats"]
 
 
@@ -106,6 +108,11 @@ class ScanStop(C.Structure):
     def as_tuple(self):
         """(table, reason, record); (-1, SCAN_STOP_NONE, 0) when every record was read."""
         return int(self.table), int(self.reason), int(self.record)
+
+
+# dbeel_range_row: the query's first entry number in out, its entry count, DBEEL_RANGE_* flags and its stop
+RANGE_ROW_DTYPE = np.dtype([("first", "<u8"), ("count", "<u4"), ("flags", "<u4"), ("table", "<i4"), ("reason", "<u4"),
+                            ("record", "<u8")])
 
 
 def pack_ranges(kind: int, ranges):
@@ -231,6 +238,9 @@ def lib():
         L.dbeel_reader_get_range.restype = C.c_int
         L.dbeel_reader_get_range.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, SCAN_WRITE_FN, C.c_void_p,
                                              C.POINTER(JobResult), C.POINTER(ScanStop)]
+        L.dbeel_reader_get_ranges.restype = C.c_int
+        L.dbeel_reader_get_ranges.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(Out),
+                                              C.c_void_p]
         L.dbeel_reader_close.restype = None
         L.dbeel_reader_close.argtypes = [C.c_void_p]
         L.dbeel_page_cache_create.restype = C.c_int
@@ -528,6 +538,50 @@ class Reader:
         flags = RANGE_KEEP_TOMBSTONES if keep_tombstones else 0
         return self._ranges_call("dbeel_reader_get_range", lambda cb, res, stop: lib().dbeel_reader_get_range(
             self._h, rptr, len(ranges), flags, cb, None, res, stop), len(ranges), write, fail_read_at, void_on_stop=True)
+
+    def get_ranges(self, ranges, limits, keep_tombstones: bool = False, caps: Optional[Tuple[int, int]] = None,
+                   fail_read_at: int = -1):
+        """dbeel_reader_get_ranges: per key range, its first `limit` entries as get_range returns them, for many ranges in
+        one call.  limits is an int (every range) or one per range.  Returns (rows, data, index): rows a RANGE_ROW_DTYPE
+        array (first, count, flags, table, reason, record), the entries of every range packed in range order.  Capacity is
+        retried once with the sizes the engine reports unless caps is given; last_stream_reads and fail_read_at as in
+        get_values."""
+        if not self._h:
+            raise ValueError("reader is closed")
+        n = len(ranges)
+        lim = np.ascontiguousarray(np.full(n, limits, np.uint32) if isinstance(limits, (int, np.integer))
+                                   else np.array([int(x) for x in limits], np.uint32))
+        if lim.size != n:
+            raise ValueError("one limit per range")
+        rptr, _keep = pack_ranges(SCAN_KEY, ranges)
+        flags = RANGE_KEEP_TOMBSTONES if keep_tombstones else 0
+        if self._st is not None:
+            self._st.fail_read_at = fail_read_at
+        rows = np.zeros(max(1, n), RANGE_ROW_DTYPE)
+        dc0 = sum(d for d, _ in self._st.sizes) if self._st is not None else self._data_cap
+        dc, ic = caps if caps is not None else (min(dc0, 64 << 20), min(16 * int(lim.sum()), 16 << 20))
+        try:
+            for attempt in range(2):
+                od, oi = np.empty(max(1, dc), np.uint8), np.empty(max(1, ic), np.uint8)
+                out = Out(od.ctypes.data, dc, 0, oi.ctypes.data, ic, 0, None, 0, 0, 0)
+                if self._st is not None:
+                    self._st.log.clear()
+                rc = lib().dbeel_reader_get_ranges(self._h, rptr, n, lim.ctypes.data, flags, C.byref(out), rows.ctypes.data)
+                if self._st is not None:
+                    self._st.last_reads = list(self._st.log)
+                if rc == 0:
+                    return rows[:n], od[:out.data_len], oi[:out.index_len]
+                err = DbeelError(rc, f"dbeel_reader_get_ranges: {lib().dbeel_last_error(self._engine._h).decode()}")
+                if rc == ERR_CAPACITY:
+                    err.needed = (int(out.data_len), int(out.index_len))
+                    err.rows = rows[:n].copy()
+                if caps is not None or attempt or rc != ERR_CAPACITY:
+                    raise err
+                dc, ic = err.needed
+        finally:
+            if self._st is not None:
+                self._st.fail_read_at = -1
+                self.last_stream_reads = self._st.last_reads
 
     def _ranges_call(self, name: str, call, n: int, write, fail_read_at: int, void_on_stop: bool = False):
         import threading

@@ -23,6 +23,7 @@
 #include "kernels.cuh"
 #include "merge_final.cuh"
 #include "merge_range.cuh"
+#include "range_limit.cuh"
 #include "gather_h.cuh"
 #include "lookup.cuh"
 #include "lookup_stream.cuh"
@@ -3384,6 +3385,42 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
     return rc;
 }
 
+// reader_seek for many bounds (kb[boff[b] .. + blen[b])) in batches whose search state (kSeekPairBytes per table and
+// bound, plus the bound's bytes) fits the partition budget: res / bad / bix[t * nb + b] as one reader_seek would give them.
+int reader_seek_batched(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, uint32_t nt, const uint8_t *kb,
+                        const std::vector<uint64_t> &boff, const std::vector<uint64_t> &blen, std::vector<unsigned long long> *res,
+                        std::vector<unsigned long long> *bad, std::vector<uint4> *bix) {
+    constexpr uint64_t kSeekPairBytes = 128;
+    const uint64_t nb = boff.size();
+    res->assign(nt * nb, ~0ull);
+    bad->assign(nt * nb, ~0ull);
+    bix->assign(nt * nb, make_uint4(0, 0, 0, 0));
+    for (uint64_t j0 = 0; j0 < nb;) {
+        std::vector<uint8_t> blob;
+        std::vector<uint64_t> bo, bl;
+        uint64_t j1 = j0, bytes = 0;
+        while (j1 < nb && (j1 == j0 || bytes + blen[j1] + kSeekPairBytes * nt <= e->partition_bytes)) {
+            bytes += blen[j1] + kSeekPairBytes * nt;
+            bo.push_back(blob.size());
+            bl.push_back(blen[j1]);
+            blob.insert(blob.end(), kb + boff[j1], kb + boff[j1] + blen[j1]);
+            j1++;
+        }
+        std::vector<unsigned long long> rs, bd;
+        std::vector<uint4> bx;
+        if (const int rc = reader_seek(e, r, io, nt, blob.data(), blob.size(), bo, bl, j1 - j0, &rs, &bd, &bx)) return rc;
+        const uint64_t m = j1 - j0;
+        for (uint64_t q = 0; q < rs.size(); q++) {
+            const uint64_t at = (q / m) * nb + j0 + q % m;
+            (*res)[at] = rs[q];
+            (*bad)[at] = bd[q];
+            (*bix)[at] = bx[q];
+        }
+        j0 = j1;
+    }
+    return DBEEL_OK;
+}
+
 // ---- dbeel_reader_get_range
 int discard_write(void *, uint32_t, uint32_t, uint64_t, const void *, uint64_t) { return 0; }
 
@@ -3429,31 +3466,19 @@ int reader_get_range_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *ta
         *ok = true;
         return 0;
     };
-    // The splitters in batches whose search state (kSeekPairBytes per table and key, plus the keys) fits the budget.
-    constexpr uint64_t kSeekPairBytes = 128;
     const MergeSeek seek = [&](const std::vector<std::vector<uint8_t>> &keys, std::vector<uint64_t> *pos) {
-        pos->assign((uint64_t)nt * keys.size(), ~0ull);
-        for (size_t j0 = 0; j0 < keys.size();) {
-            std::vector<uint8_t> blob;
-            std::vector<uint64_t> boff, blen;
-            size_t j1 = j0;
-            uint64_t bytes = 0;
-            while (j1 < keys.size() && (j1 == j0 || bytes + keys[j1].size() + kSeekPairBytes * nt <= e->partition_bytes)) {
-                bytes += keys[j1].size() + kSeekPairBytes * nt;
-                boff.push_back(blob.size());
-                blen.push_back(keys[j1].size());
-                blob.insert(blob.end(), keys[j1].begin(), keys[j1].end());
-                j1++;
-            }
-            std::vector<unsigned long long> res, bad;
-            std::vector<uint4> bix;
-            const int src = reader_seek(e, r, io, nt, blob.data(), blob.size(), boff, blen, j1 - j0, &res, &bad, &bix);
-            if (src) return src;
-            const uint64_t nb = j1 - j0;
-            for (uint64_t q = 0; q < res.size(); q++)
-                (*pos)[(q / nb) * keys.size() + j0 + q % nb] = bad[q] != ~0ull ? ~0ull : res[q];
-            j0 = j1;
+        std::vector<uint8_t> blob;
+        std::vector<uint64_t> boff, blen;
+        for (const std::vector<uint8_t> &k : keys) {
+            boff.push_back(blob.size());
+            blen.push_back(k.size());
+            blob.insert(blob.end(), k.begin(), k.end());
         }
+        std::vector<unsigned long long> res, bad;
+        std::vector<uint4> bix;
+        if (const int src = reader_seek_batched(e, r, io, nt, blob.data(), boff, blen, &res, &bad, &bix)) return src;
+        pos->assign(res.size(), ~0ull);
+        for (uint64_t q = 0; q < res.size(); q++) (*pos)[q] = bad[q] != ~0ull ? ~0ull : res[q];
         return 0;
     };
     const PlanTables pt = plan_tables(tables, nt, io);
@@ -3502,6 +3527,387 @@ int reader_range_entry(dbeel_reader *r, bool get_range, uint32_t kind, const voi
     if (rc) {
         cudaStreamSynchronize(e->stream); // nothing of this call may touch the engine's buffers after it returns
         clear_scan(results, n_ranges, stop);
+    }
+    e->stats.input_bytes = x.bytes;
+    return rc;
+}
+
+// ---- dbeel_reader_get_ranges
+// One query of a call: its span [lo, hi) per searched table, the chunk width per table, and where its entries went.
+struct LimitState {
+    std::vector<uint64_t> lo, hi, w;
+    int32_t em = -1; // emission that holds its entries
+    uint32_t at = 0; // its first entry there
+};
+
+// One merge round of a group of live queries (range_limit.cuh): per (query, table) pair the records [lo, lo + w) cut at hi
+// -- their .index slices, then the .data windows of the records whose index record stays inside .data, both through
+// gvs_load -- decoded, merged and ranked on the device.  A query is finished when it is damaged, when it has limit + 1
+// survivors at or below its frontier, or when every pair reached its span's end; the entries of the finished ones go
+// through the split and phase 2 into emission `em` (host memory).  The pairs that set an unfinished query's frontier
+// double their width; that query goes to *next.
+int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const uint32_t *qs, uint32_t gq, const uint32_t *limits,
+                bool keep_tombstones, std::vector<LimitState> &st, dbeel_range_row *rows, std::vector<std::vector<uint8_t>> *em,
+                std::vector<uint32_t> *next, uint32_t *launches, uint64_t *gather_bytes) {
+    const uint32_t nseek = (uint32_t)st[qs[0]].lo.size();
+    cudaStream_t s = e->stream;
+    int rc;
+    std::vector<LimitPair> pairs;
+    std::vector<uint32_t> ptab;
+    std::vector<LimitQuery> lq(gq);
+    std::vector<std::vector<ByteRange>> ir(nseek);
+    uint32_t n = 0;
+    for (uint32_t g = 0; g < gq; g++) {
+        const LimitState &q = st[qs[g]];
+        lq[g] = LimitQuery{(uint32_t)pairs.size(), 0, n, 0, limits[qs[g]], 0};
+        for (uint32_t t = 0; t < nseek; t++) {
+            if (q.hi[t] <= q.lo[t]) continue;
+            const uint64_t c = std::min(q.w[t], q.hi[t] - q.lo[t]);
+            pairs.push_back(LimitPair{n, (uint32_t)c, g, q.lo[t] + c < q.hi[t] ? 1u : 0u});
+            ptab.push_back(t);
+            ir[t].push_back({16 * q.lo[t], 16 * (q.lo[t] + c)});
+            n += (uint32_t)c;
+        }
+        lq[g].pair1 = (uint32_t)pairs.size();
+        lq[g].last = n;
+    }
+    const uint32_t np = (uint32_t)pairs.size();
+    e->stats.entries_in += n;
+    // ---- the .index slices (back to host too), then the windows of the records
+    std::vector<GvsStaged> ss(nseek), sw(nseek);
+    std::vector<GvsPart> parts;
+    uint64_t end = 0;
+    for (uint32_t t = 0; t < nseek; t++) {
+        if (ir[t].empty()) continue;
+        ss[t] = gvs_stage(std::move(ir[t]), 0, end);
+        end = ss[t].end;
+        parts.push_back(GvsPart{t, &ss[t]});
+    }
+    rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, end);
+    if (!rc) rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, end);
+    if (rc) return rc;
+    if ((rc = gvs_load(e, io, r, DBEEL_STREAM_INDEX, parts, e->ring_in, e->stage_in, 0, end, true, "stream read callback failed (.index, ranges)")))
+        return rc;
+    std::vector<uint4> rec(n);
+    std::vector<uint32_t> rpair(n);
+    std::vector<std::vector<ByteRange>> wr(nseek);
+    for (uint32_t k = 0; k < np; k++) {
+        const uint32_t t = ptab[k];
+        const LimitState &q = st[qs[pairs[k].query]];
+        const uint64_t dl = r->tables[t]->desc.data_len;
+        for (uint32_t j = 0; j < pairs[k].count; j++) {
+            const uint8_t *ix = e->ring_in + ss[t].at(16 * (q.lo[t] + j));
+            const uint64_t off = rd_le(ix, 8), fs = rd_le(ix + 12, 4);
+            const bool panic = fs == 0 || off > dl || fs > dl - off; // as k_scan_classify: the index record alone shows it
+            rec[pairs[k].first + j] = make_uint4(0, 0, panic ? kScanStopPanic : 0u, (uint32_t)fs);
+            rpair[pairs[k].first + j] = k;
+            if (!panic) wr[t].push_back({off, off + fs});
+        }
+    }
+    uint64_t wend = 0;
+    parts.clear();
+    for (uint32_t t = 0; t < nseek; t++) {
+        sw[t] = gvs_stage(std::move(wr[t]), 0, wend);
+        wend = sw[t].end;
+        if (!sw[t].runs.empty()) parts.push_back(GvsPart{t, &sw[t]});
+    }
+    rc = ensure_host(e, &e->ring_out, &e->ring_out_cap, std::max<uint64_t>(wend, 256));
+    if (!rc) rc = ensure_device(e, &e->stage_in2, &e->stage_in2_cap, std::max<uint64_t>(wend, 256));
+    if (rc) return rc;
+    if ((rc = gvs_load(e, io, r, DBEEL_STREAM_DATA, parts, e->ring_out, e->stage_in2, 0, wend, false, "stream read callback failed (.data, ranges)")))
+        return rc;
+    for (uint32_t k = 0; k < np; k++) {
+        const uint32_t t = ptab[k];
+        const LimitState &q = st[qs[pairs[k].query]];
+        for (uint32_t j = 0; j < pairs[k].count; j++) {
+            uint4 &x = rec[pairs[k].first + j];
+            if (x.z) continue;
+            const uint64_t a = reinterpret_cast<uint64_t>(e->stage_in2 + sw[t].at(rd_le(e->ring_in + ss[t].at(16 * (q.lo[t] + j)), 8)));
+            x.x = (uint32_t)a;
+            x.y = (uint32_t)(a >> 32);
+        }
+    }
+
+    // ---- workspace: the round's arrays, then the split of the selected records
+    const uint32_t tiles = (n + kRangeTile - 1) / kRangeTile;
+    uint64_t off = 0;
+    const uint64_t o_pairs = carve_ws(&off, sizeof(LimitPair) * np), o_q = carve_ws(&off, sizeof(LimitQuery) * gq);
+    const uint64_t o_rec = carve_ws(&off, 16ull * n), o_rpair = carve_ws(&off, 4ull * n), o_flat = carve_ws(&off, 16ull * n);
+    const uint64_t o_pfx = carve_ws(&off, 8ull * n), o_code = carve_ws(&off, 4ull * n), o_pbad = carve_ws(&off, 4ull * np);
+    const uint64_t o_setter = carve_ws(&off, 4ull * np), o_front = carve_ws(&off, 4ull * gq), o_qout = carve_ws(&off, 16ull * gq);
+    const uint64_t o_pre = carve_ws(&off, 4ull * (n + 1)), o_rank = carve_ws(&off, 4ull * n), o_tile = carve_ws(&off, 4ull * (tiles + 1));
+    const uint64_t o_tot = carve_ws(&off, 32), o_qsel = carve_ws(&off, 4ull * gq);
+    SplitLayout w = carve_split(&off, n, 1);
+    if ((rc = ensure_device(e, &e->ws, &e->ws_cap, off))) return rc;
+    const uint64_t pin_tot = align_up(w.header2_bytes, 64);
+    if ((rc = ensure_pinned(e, pin_tot + 8ull * 4))) return rc;
+    uint8_t *ws = e->ws;
+    const unsigned long long tot[4] = {n, 0, 0, ~0ull}; // one segment of n records for k_range_tile_sums .. k_range_prefix
+    CU(cudaMemcpyAsync(ws + o_pairs, pairs.data(), sizeof(LimitPair) * np, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_q, lq.data(), sizeof(LimitQuery) * gq, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_rec, rec.data(), 16ull * n, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_rpair, rpair.data(), 4ull * n, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_tot, tot, 32, cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(ws + o_pbad, 0xFF, 4ull * np, s));
+    ScanParams sp = {};
+    RouteParams rp;
+    Params p;
+    split_bind(w, ws, &sp, &rp, &p);
+    LimitParams lp{reinterpret_cast<const LimitPair *>(ws + o_pairs), reinterpret_cast<const LimitQuery *>(ws + o_q),
+                   reinterpret_cast<const uint4 *>(ws + o_rec), reinterpret_cast<const uint32_t *>(ws + o_rpair), n, gq,
+                   keep_tombstones ? 1u : 0u, 0, reinterpret_cast<uint4 *>(ws + o_flat), reinterpret_cast<unsigned long long *>(ws + o_pfx),
+                   reinterpret_cast<uint32_t *>(ws + o_code), reinterpret_cast<uint32_t *>(ws + o_pbad), reinterpret_cast<uint32_t *>(ws + o_setter),
+                   reinterpret_cast<uint32_t *>(ws + o_front), reinterpret_cast<uint4 *>(ws + o_qout), reinterpret_cast<const uint32_t *>(ws + o_pre),
+                   reinterpret_cast<uint32_t *>(ws + o_pre), reinterpret_cast<uint32_t *>(ws + o_rank), reinterpret_cast<const uint32_t *>(ws + o_qsel),
+                   sp.flat, sp.dest};
+    RangeMergeParams mp = {};
+    mp.n_ranges = 1;
+    mp.totals = reinterpret_cast<unsigned long long *>(ws + o_tot);
+    mp.pre = reinterpret_cast<uint32_t *>(ws + o_pre);
+    mp.tile = reinterpret_cast<uint32_t *>(ws + o_tile);
+    const uint32_t gn = (n + 255) / 256, gqn = (gq + 255) / 256;
+    launch_k(e, k_limit_decode, gn, 256, 0, s, lp);
+    launch_k(e, k_limit_query, gqn, 256, 0, s, lp);
+    launch_k(e, k_limit_flag, gn, 256, 0, s, lp);
+    launch_k(e, k_range_tile_sums, tiles, kRangeTile, 0, s, mp);
+    launch_k(e, k_range_tile_scan, 1, kRangeTile, 0, s, mp);
+    launch_k(e, k_range_prefix, tiles, kRangeTile, 0, s, mp);
+    launch_k(e, k_limit_rank, std::max(gn, gqn), 256, 0, s, lp);
+    *launches += 7;
+    std::vector<uint4> qout(gq);
+    std::vector<uint32_t> setter(np);
+    CU(cudaMemcpyAsync(qout.data(), ws + o_qout, 16ull * gq, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(setter.data(), ws + o_setter, 4ull * np, cudaMemcpyDeviceToHost, s));
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(s));
+    e->stats.partitions++;
+
+    // ---- finished queries: their rows and out slots; the others widen the pairs that hold their frontier back
+    std::vector<uint32_t> qsel(gq, ~0u), done;
+    uint32_t n_sel = 0;
+    for (uint32_t g = 0; g < gq; g++) {
+        const uint32_t qi = qs[g], lim = limits[qi];
+        dbeel_range_row &row = rows[qi];
+        LimitState &q = st[qi];
+        const uint4 o = qout[g];
+        if (o.z != ~0u) {
+            const uint32_t t = ptab[o.z];
+            row.flags = o.y == kLimitUnsorted ? DBEEL_RANGE_UNSORTED : DBEEL_RANGE_STOPPED;
+            row.stop = dbeel_scan_stop{(int32_t)t, o.y == kLimitUnsorted ? DBEEL_SCAN_STOP_NONE : o.y, q.lo[t] + o.w};
+            continue;
+        }
+        bool truncated = false;
+        for (uint32_t k = lq[g].pair0; k < lq[g].pair1; k++) truncated |= pairs[k].truncated != 0;
+        if (o.x > lim || !truncated) {
+            row.count = std::min(o.x, lim);
+            row.flags = o.x > lim ? DBEEL_RANGE_MORE : 0u;
+            if (row.count) {
+                qsel[g] = n_sel;
+                q.at = n_sel;
+                q.em = (int32_t)(em->size() / 2);
+                n_sel += row.count;
+            }
+            continue;
+        }
+        for (uint32_t k = lq[g].pair0; k < lq[g].pair1; k++)
+            if (setter[k]) q.w[ptab[k]] *= 2;
+        next->push_back(qi);
+    }
+    if (!n_sel) return DBEEL_OK;
+    CU(cudaMemcpyAsync(ws + o_qsel, qsel.data(), 4ull * gq, cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(ws + w.o_tot, 0, 8ull * 3, s));
+    CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
+    launch_k(e, k_limit_select, gn, 256, 0, s, lp);
+    *launches += 1;
+    w.n = n_sel;
+    w.n_blocks = (n_sel + kRouteThreads - 1) / kRouteThreads;
+    em->emplace_back();
+    em->emplace_back();
+    std::vector<uint8_t> &ed = (*em)[em->size() - 2], &ei = (*em)[em->size() - 1];
+    dbeel_out tmp = {};
+    uint64_t items = 0, bytes = 0;
+    rc = split_emit(e, w, sp, rp, p, pin_tot, false, &tmp, launches, &items, &bytes, [&](const unsigned long long *host_tot) {
+        ed.resize(std::max<uint64_t>(host_tot[1], 1));
+        ei.resize(16 * host_tot[0] + 16);
+        tmp.data = ed.data();
+        tmp.data_cap = host_tot[1];
+        tmp.index = ei.data();
+        tmp.index_cap = 16 * host_tot[0];
+    });
+    if (rc) return rc;
+    *gather_bytes += e->stats.gather_bytes;
+    ed.resize(bytes);
+    ei.resize(16 * items);
+    return DBEEL_OK;
+}
+
+// dbeel_reader_get_ranges (dbeel_compact.h): the bound searches (reader_seek_batched), the spans and seek stops per query,
+// then merge rounds over groups of the live queries of about the partition budget (limit_round) until every query is
+// finished, then the rows and `out` from the emissions, in query order.
+int reader_get_ranges(dbeel_engine *e, dbeel_reader *r, const uint8_t *kb, const std::vector<uint64_t> &ko, uint32_t nq,
+                      const uint32_t *limits, bool keep_tombstones, const dbeel_scan_io *io, dbeel_out *out, dbeel_range_row *rows) {
+    const uint32_t nt = (uint32_t)r->tables.size();
+    uint32_t nseek = nt; // the tables before the first one with no index record
+    for (uint32_t t = 0; t < nt; t++)
+        if (r->tables[t]->desc.n == 0) { nseek = t; break; }
+    std::vector<uint32_t> vq; // the queries with start < end
+    std::vector<uint64_t> boff, blen;
+    for (uint32_t q = 0; q < nq; q++) {
+        if (!key_less(kb + ko[2 * q], ko[2 * q + 1] - ko[2 * q], kb + ko[2 * q + 1], ko[2 * q + 2] - ko[2 * q + 1])) continue;
+        vq.push_back(q);
+        for (uint32_t k = 2 * q; k < 2 * q + 2; k++) {
+            boff.push_back(ko[k]);
+            blen.push_back(ko[k + 1] - ko[k]);
+        }
+    }
+    const dbeel_scan_stop empty_stop{(int32_t)nseek, DBEEL_SCAN_STOP_PANIC, 0};
+    if (nseek < nt)
+        for (uint32_t q = 0; q < nq; q++) { rows[q].flags = DBEEL_RANGE_STOPPED; rows[q].stop = empty_stop; }
+    std::vector<unsigned long long> res, bad;
+    std::vector<uint4> bix;
+    int rc;
+    if (!vq.empty() && nseek)
+        if ((rc = reader_seek_batched(e, r, io, nseek, kb, boff, blen, &res, &bad, &bix))) return rc;
+    cudaError_t ce = cudaSetDevice(e->device);
+    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    CU(cudaEventRecord(e->ev[EV_START], e->stream));
+    const uint64_t nb = boff.size();
+    std::vector<LimitState> st(nq);
+    std::vector<uint32_t> live;
+    for (uint64_t j = 0; j < vq.size(); j++) {
+        const uint32_t q = vq[j];
+        LimitState &x = st[q];
+        x.lo.assign(nseek, 0);
+        x.hi.assign(nseek, 0);
+        x.w.assign(nseek, (uint64_t)limits[q] + 1);
+        bool any = false;
+        for (uint32_t t = 0; t < nseek; t++) {
+            const uint64_t a = t * nb + 2 * j, b = a + 1;
+            if (bad[a] != ~0ull || bad[b] != ~0ull) { // as reader_spans: the smallest corrupt probe, PANIC when its index record shows it
+                const uint64_t c = bad[a] <= bad[b] ? a : b;
+                const uint4 ix = bix[c];
+                const uint64_t o = (uint64_t)ix.x | ((uint64_t)ix.y << 32), dl = r->tables[t]->desc.data_len;
+                const bool panic = ix.w == 0 || o > dl || ix.w > dl - o;
+                rows[q].flags = DBEEL_RANGE_STOPPED;
+                rows[q].stop = dbeel_scan_stop{(int32_t)t, panic ? DBEEL_SCAN_STOP_PANIC : DBEEL_SCAN_STOP_ERR, bad[c]};
+                any = false;
+                break;
+            }
+            if (res[a] < res[b] && res[b] != ~0ull) {
+                x.lo[t] = res[a];
+                x.hi[t] = res[b];
+                any = true;
+            }
+        }
+        if (any && !rows[q].flags) live.push_back(q);
+    }
+
+    // ---- rounds: the live queries in groups of about the budget (their chunks' index records and mean entries)
+    std::vector<uint64_t> mean(nseek);
+    for (uint32_t t = 0; t < nseek; t++) mean[t] = (r->tables[t]->desc.data_len + r->tables[t]->desc.n - 1) / r->tables[t]->desc.n;
+    // per staged record: its .index record, its mean entry and the round's workspace (LimitParams' arrays, the split)
+    constexpr uint64_t kLimitRecordBytes = 16 + 128;
+    const uint64_t page_bytes = r->cache ? 2 * kPageBytes : 0;
+    std::vector<std::vector<uint8_t>> em; // emission k: data at 2k, index at 2k + 1
+    uint32_t launches = 0;
+    uint64_t gather_bytes = 0;
+    while (!live.empty()) {
+        std::vector<uint32_t> next;
+        for (size_t g0 = 0; g0 < live.size();) {
+            size_t g1 = g0;
+            uint64_t bytes = 0;
+            while (g1 < live.size()) {
+                const LimitState &x = st[live[g1]];
+                uint64_t cost = 0;
+                for (uint32_t t = 0; t < nseek; t++)
+                    if (x.hi[t] > x.lo[t]) cost += std::min(x.w[t], x.hi[t] - x.lo[t]) * (kLimitRecordBytes + mean[t]) + page_bytes;
+                if (g1 > g0 && bytes + cost > e->partition_bytes) break;
+                bytes += cost;
+                g1++;
+            }
+            if ((rc = limit_round(e, r, io, live.data() + g0, (uint32_t)(g1 - g0), limits, keep_tombstones, st, rows, &em, &next,
+                                  &launches, &gather_bytes)))
+                return rc;
+            g0 = g1;
+        }
+        live.swap(next);
+    }
+
+    // ---- out: every query's entries, in query order, offsets rebased
+    uint64_t items = 0, bytes = 0;
+    for (uint32_t q = 0; q < nq; q++) {
+        rows[q].first = items;
+        items += rows[q].count;
+        if (!rows[q].count) continue;
+        const uint8_t *ix = em[2 * st[q].em + 1].data() + 16ull * st[q].at;
+        const uint64_t last = 16ull * (rows[q].count - 1);
+        bytes += rd_le(ix + last, 8) + rd_le(ix + last + 12, 4) - rd_le(ix, 8);
+    }
+    if (bytes > out->data_cap || 16 * items > out->index_cap) {
+        out->data_len = bytes;
+        out->index_len = 16 * items;
+        return fail(e, DBEEL_ERR_CAPACITY, "the entries found are larger than the output buffers (data_len / index_len: the sizes needed)");
+    }
+    if ((bytes && !out->data) || (items && !out->index)) return fail(e, DBEEL_ERR_INVALID_ARG, "null output buffer");
+    uint8_t *od = static_cast<uint8_t *>(out->data), *oi = static_cast<uint8_t *>(out->index);
+    uint64_t at = 0;
+    for (uint32_t q = 0; q < nq; q++) {
+        if (!rows[q].count) continue;
+        const uint8_t *ix = em[2 * st[q].em + 1].data() + 16ull * st[q].at;
+        const uint64_t base = rd_le(ix, 8), last = 16ull * (rows[q].count - 1);
+        const uint64_t len = rd_le(ix + last, 8) + rd_le(ix + last + 12, 4) - base;
+        memcpy(od + at, em[2 * st[q].em].data() + base, len);
+        for (uint32_t k = 0; k < rows[q].count; k++) {
+            uint8_t *dst = oi + 16ull * (rows[q].first + k);
+            memcpy(dst, ix + 16ull * k, 16);
+            const uint64_t o = rd_le(ix + 16ull * k, 8) - base + at;
+            memcpy(dst, &o, 8);
+        }
+        at += len;
+    }
+    out->data_len = bytes;
+    out->index_len = 16 * items;
+    out->items_written = items;
+    e->stats.kernel_launches = launches;
+    e->stats.gather_bytes = gather_bytes;
+    e->stats.entries_out = items;
+    e->stats.output_bytes = bytes + 16 * items;
+    return DBEEL_OK;
+}
+
+int reader_get_ranges_entry(dbeel_reader *r, const dbeel_key_ranges *kr, uint32_t nq, const uint32_t *limits, uint32_t flags,
+                            dbeel_out *out, dbeel_range_row *rows) {
+    if (!r) return DBEEL_ERR_INVALID_ARG;
+    dbeel_engine *e = r->e;
+    if (!kr || !kr->key_offsets || !limits || !out || !rows) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    if (nq == 0) return fail(e, DBEEL_ERR_INVALID_ARG, "n_ranges must be at least 1");
+    if (flags & ~DBEEL_RANGE_KEEP_TOMBSTONES) return fail(e, DBEEL_ERR_INVALID_ARG, "unknown flag");
+    uint64_t total = 0;
+    for (uint32_t q = 0; q < nq; q++) {
+        if (limits[q] == 0 || limits[q] > DBEEL_RANGE_LIMIT_MAX) return fail(e, DBEEL_ERR_INVALID_ARG, "a limit must be 1 .. DBEEL_RANGE_LIMIT_MAX");
+        total += limits[q];
+    }
+    if (total >= 0xFFFFFFF0ull) return fail(e, DBEEL_ERR_INVALID_ARG, "the limits sum to 2^32 - 16 or more");
+    std::vector<uint64_t> ko(2ull * nq + 1);
+    for (uint64_t k = 0; k <= 2ull * nq; k++) {
+        if (k && kr->key_offsets[k] < kr->key_offsets[k - 1]) return fail(e, DBEEL_ERR_INVALID_ARG, "key_offsets must not decrease");
+        ko[k] = kr->key_offsets[k] - kr->key_offsets[0];
+    }
+    if (ko[2ull * nq] && !kr->keys) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    e->stats = dbeel_stats{};
+    out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
+    for (uint32_t q = 0; q < nq; q++) rows[q] = dbeel_range_row{0, 0, 0, dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0}};
+    ReaderScanIo x;
+    x.rio = &r->io;
+    const dbeel_scan_io io{reader_scan_read, nullptr, &x};
+    const uint8_t *kb = ko[2ull * nq] ? static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0] : nullptr;
+    const int rc = reader_get_ranges(e, r, kb, ko, nq, limits, (flags & DBEEL_RANGE_KEEP_TOMBSTONES) != 0, &io, out, rows);
+    if (rc && rc != DBEEL_ERR_CAPACITY) {
+        cudaStreamSynchronize(e->stream); // nothing of this call may touch the engine's buffers after it returns
+        for (uint32_t q = 0; q < nq; q++) rows[q] = dbeel_range_row{0, 0, 0, dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0}};
     }
     e->stats.input_bytes = x.bytes;
     return rc;
@@ -3929,6 +4335,13 @@ int dbeel_reader_get_range(dbeel_reader *r, const dbeel_key_ranges *ranges, uint
     if (!r) return DBEEL_ERR_INVALID_ARG;
     REFUSE_WHILE_ASYNC(r->e);
     return reader_range_entry(r, true, DBEEL_SCAN_KEY, ranges, n_ranges, flags, write, ctx, results, stop);
+}
+
+int dbeel_reader_get_ranges(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, const uint32_t *limits,
+                            uint32_t flags, dbeel_out *out, dbeel_range_row *rows) {
+    if (!r) return DBEEL_ERR_INVALID_ARG;
+    REFUSE_WHILE_ASYNC(r->e);
+    return reader_get_ranges_entry(r, ranges, n_ranges, limits, flags, out, rows);
 }
 
 int dbeel_page_cache_create(dbeel_engine *e, uint64_t bytes, dbeel_page_cache **out) {

@@ -562,6 +562,57 @@ int dbeel_reader_scan(dbeel_reader *r, uint32_t kind, const void *ranges, uint32
 int dbeel_reader_get_range(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, uint32_t flags,
                            int (*write)(void *ctx, uint32_t dest, uint32_t kind, uint64_t offset, const void *src, uint64_t len),
                            void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop);
+
+/* Range reads with a limit, batched: the first entries of many key ranges in one call, for a serving loop (a page of a
+ * listing, the next page from a cursor).  Query q is the range [start_q, end_q), laid out as in dbeel_reader_get_range
+ * (key_offsets has 2 * n_ranges + 1 entries), with the limit limits[q].  Let G_q be destination 0 of
+ * dbeel_reader_get_range(r, &range_q, 1, flags, ...) for that range alone.
+ *   Clean.   A query whose range makes that call return no stop and not DBEEL_ERR_UNSORTED_RUN gets the first
+ *            min(limits[q], |G_q|) entries of G_q, byte for byte; DBEEL_RANGE_MORE is set iff |G_q| > limits[q].  A query
+ *            with start >= end gets count 0, reads nothing and is never stopped, except by an empty table.
+ *   Output.  Entries packed as dbeel_get_values packs them: query order, ascending keys within a query, bytes as stored;
+ *            the .index offsets start at 0 in out->data, key_size = 8 + klen, out->items_written = the total.  Row q's
+ *            entries are entry numbers [first, first + count).  A caller pages on with start = last key + "\x00".
+ *   Stops.   A failed bound search or a table with no index record, as seek_t meets them for the query's range alone (the
+ *            stop of dbeel_reader_scan's searches): the row is DBEEL_RANGE_STOPPED with that stop and nothing is read for
+ *            the query's records.
+ *   Damage.  Only a prefix of every span is read.  Let A_q be the merge, under G_q's rule, of every table's span records
+ *            for q, each cut just before its first record that fails dbeel_scan's decode (ERR / PANIC as the scan
+ *            classifies it) or is not strictly above its predecessor.  The row is then either the first min(limit, |A_q|)
+ *            entries of A_q (MORE iff |A_q| > limit), or DBEEL_RANGE_STOPPED with stop = (table, ERR / PANIC, record) of a
+ *            record that fails the decode, or DBEEL_RANGE_UNSORTED with stop = (table, DBEEL_SCAN_STOP_NONE, record) of a
+ *            record not above its predecessor.  The first record of every non-empty span is always read.  One query's
+ *            damage never changes another query's row.
+ *   Reads.   The bound searches of the queries with start < end (dbeel_reader_scan's: fences cached or read for this
+ *            call, the touched leaves); per query and table, index records from seek_t(start) on, never past
+ *            seek_t(end), in chunks that start at seek_t(start) and double for the tables that hold back the merge; the
+ *            .data windows of exactly the records staged, each never wider than its records.  Leaf slices, staged index
+ *            slices and windows go through an attached page cache.  Nothing else is read.
+ *   Memory.  Device and page-locked memory follow the partition budget (DBEEL_PARTITION_MB / _KB): each round runs the
+ *            live queries in groups whose staged records (index record, mean entry and workspace) fit it, and a group
+ *            holds at least one query.  A query's chunks double without a cap, so one query whose merge a long run of
+ *            tombstones or superseded versions holds back can stage past the budget, up to about twice that run.
+ *   Errors.  DBEEL_ERR_CAPACITY as dbeel_get_values: the rows filled, out->data_len / index_len = the sizes needed, nothing
+ *            written.  DBEEL_ERR_INVALID_ARG for a null pointer, n_ranges == 0, a limit of 0 or above
+ *            DBEEL_RANGE_LIMIT_MAX, a sum of limits >= 2^32 - 16, or a flag other than DBEEL_RANGE_KEEP_TOMBSTONES.  A
+ *            callback's nonzero return comes back unchanged; the reader, the engine and an attached page cache stay usable
+ *            after every error.  DBEEL_ERR_BUSY while another call runs.  out->bloom is not used.
+ * dbeel_last_stats: input_bytes = every byte read through the callback in this call, entries_in = index records staged,
+ * output_bytes / entries_out = what was returned, partitions = merge rounds run, summed over groups; kernel_launches and
+ * gather_bytes summed over the rounds, ms_total from the first round to the last output copy. */
+#define DBEEL_RANGE_LIMIT_MAX 65536u
+#define DBEEL_RANGE_MORE 0x1u     /* the range holds more entries than were returned */
+#define DBEEL_RANGE_STOPPED 0x2u  /* stop says where; no entries */
+#define DBEEL_RANGE_UNSORTED 0x4u /* stop.table's records read for it do not strictly ascend; stop.record = the first one
+                                     not above its predecessor; no entries */
+typedef struct dbeel_range_row {
+    uint64_t first;       /* entry number in out of the query's first entry */
+    uint32_t count;       /* entries returned */
+    uint32_t flags;       /* DBEEL_RANGE_* */
+    dbeel_scan_stop stop; /* {-1, DBEEL_SCAN_STOP_NONE, 0} unless STOPPED / UNSORTED */
+} dbeel_range_row;
+int dbeel_reader_get_ranges(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, const uint32_t *limits,
+                            uint32_t flags, dbeel_out *out, dbeel_range_row *rows);
 void dbeel_reader_close(dbeel_reader *r);
 
 /* Page cache for readers: the reference reads every .data / .index byte of a lookup or seek through a per-shard cache of
