@@ -49,7 +49,8 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream",
            "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device", "dbeel_scan_stream", "dbeel_get_values",
            "dbeel_get_values_device", "dbeel_get_values_stream", "dbeel_reader_open", "dbeel_reader_get_values",
-           "dbeel_reader_scan", "dbeel_reader_get_range", "dbeel_reader_get_ranges", "dbeel_reader_close", "dbeel_page_cache_create", "dbeel_page_cache_destroy",
+           "dbeel_reader_scan", "dbeel_reader_get_range", "dbeel_reader_get_ranges",
+           "dbeel_reader_get_ranges_reverse", "dbeel_reader_close", "dbeel_page_cache_create", "dbeel_page_cache_destroy",
            "dbeel_reader_attach_page_cache", "dbeel_page_cache_stats"]
 
 
@@ -241,6 +242,9 @@ def lib():
         L.dbeel_reader_get_ranges.restype = C.c_int
         L.dbeel_reader_get_ranges.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(Out),
                                               C.c_void_p]
+        L.dbeel_reader_get_ranges_reverse.restype = C.c_int
+        L.dbeel_reader_get_ranges_reverse.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32,
+                                                      C.POINTER(Out), C.c_void_p]
         L.dbeel_reader_close.restype = None
         L.dbeel_reader_close.argtypes = [C.c_void_p]
         L.dbeel_page_cache_create.restype = C.c_int
@@ -540,10 +544,11 @@ class Reader:
             self._h, rptr, len(ranges), flags, cb, None, res, stop), len(ranges), write, fail_read_at, void_on_stop=True)
 
     def get_ranges(self, ranges, limits, keep_tombstones: bool = False, caps: Optional[Tuple[int, int]] = None,
-                   fail_read_at: int = -1):
+                   fail_read_at: int = -1, reverse: bool = False):
         """dbeel_reader_get_ranges: per key range, its first `limit` entries as get_range returns them, for many ranges in
-        one call.  limits is an int (every range) or one per range.  Returns (rows, data, index): rows a RANGE_ROW_DTYPE
-        array (first, count, flags, table, reason, record), the entries of every range packed in range order.  Capacity is
+        one call; with reverse, dbeel_reader_get_ranges_reverse: its last `limit` entries, in descending key order.
+        limits is an int (every range) or one per range.  Returns (rows, data, index): rows a RANGE_ROW_DTYPE array
+        (first, count, flags, table, reason, record), the entries of every range packed in range order.  Capacity is
         retried once with the sizes the engine reports unless caps is given; last_stream_reads and fail_read_at as in
         get_values."""
         if not self._h:
@@ -558,6 +563,8 @@ class Reader:
         if self._st is not None:
             self._st.fail_read_at = fail_read_at
         rows = np.zeros(max(1, n), RANGE_ROW_DTYPE)
+        name = "dbeel_reader_get_ranges_reverse" if reverse else "dbeel_reader_get_ranges"
+        fn = getattr(lib(), name)
         dc0 = sum(d for d, _ in self._st.sizes) if self._st is not None else self._data_cap
         dc, ic = caps if caps is not None else (min(dc0, 64 << 20), min(16 * int(lim.sum()), 16 << 20))
         try:
@@ -566,12 +573,12 @@ class Reader:
                 out = Out(od.ctypes.data, dc, 0, oi.ctypes.data, ic, 0, None, 0, 0, 0)
                 if self._st is not None:
                     self._st.log.clear()
-                rc = lib().dbeel_reader_get_ranges(self._h, rptr, n, lim.ctypes.data, flags, C.byref(out), rows.ctypes.data)
+                rc = fn(self._h, rptr, n, lim.ctypes.data, flags, C.byref(out), rows.ctypes.data)
                 if self._st is not None:
                     self._st.last_reads = list(self._st.log)
                 if rc == 0:
                     return rows[:n], od[:out.data_len], oi[:out.index_len]
-                err = DbeelError(rc, f"dbeel_reader_get_ranges: {lib().dbeel_last_error(self._engine._h).decode()}")
+                err = DbeelError(rc, f"{name}: {lib().dbeel_last_error(self._engine._h).decode()}")
                 if rc == ERR_CAPACITY:
                     err.needed = (int(out.data_len), int(out.index_len))
                     err.rows = rows[:n].copy()

@@ -3541,19 +3541,20 @@ struct LimitState {
 };
 
 // One merge round of a group of live queries (range_limit.cuh): per (query, table) pair the records [lo, lo + w) cut at hi
-// -- their .index slices, then the .data windows of the records whose index record stays inside .data, both through
-// gvs_load -- decoded, merged and ranked on the device.  A query is finished when it is damaged, when it has limit + 1
-// survivors at or below its frontier, or when every pair reached its span's end; the entries of the finished ones go
-// through the split and phase 2 into emission `em` (host memory).  The pairs that set an unfinished query's frontier
-// double their width; that query goes to *next.
+// -- desc: [hi - w, hi) cut at lo -- their .index slices, then the .data windows of the records whose index record stays
+// inside .data, both through gvs_load -- decoded, merged and ranked on the device.  A query is finished when it is damaged,
+// when it has limit + 1 survivors on the complete side of its frontier, or when every pair reached its span's far end; the
+// entries of the finished ones go through the split and phase 2 into emission `em` (host memory).  The pairs that set an
+// unfinished query's frontier double their width; that query goes to *next.
 int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const uint32_t *qs, uint32_t gq, const uint32_t *limits,
-                bool keep_tombstones, std::vector<LimitState> &st, dbeel_range_row *rows, std::vector<std::vector<uint8_t>> *em,
-                std::vector<uint32_t> *next, uint32_t *launches, uint64_t *gather_bytes) {
+                bool keep_tombstones, bool desc, std::vector<LimitState> &st, dbeel_range_row *rows,
+                std::vector<std::vector<uint8_t>> *em, std::vector<uint32_t> *next, uint32_t *launches, uint64_t *gather_bytes) {
     const uint32_t nseek = (uint32_t)st[qs[0]].lo.size();
     cudaStream_t s = e->stream;
     int rc;
     std::vector<LimitPair> pairs;
     std::vector<uint32_t> ptab;
+    std::vector<uint64_t> pbase; // the table's record number of the pair's first staged record
     std::vector<LimitQuery> lq(gq);
     std::vector<std::vector<ByteRange>> ir(nseek);
     uint32_t n = 0;
@@ -3562,10 +3563,11 @@ int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const
         lq[g] = LimitQuery{(uint32_t)pairs.size(), 0, n, 0, limits[qs[g]], 0};
         for (uint32_t t = 0; t < nseek; t++) {
             if (q.hi[t] <= q.lo[t]) continue;
-            const uint64_t c = std::min(q.w[t], q.hi[t] - q.lo[t]);
-            pairs.push_back(LimitPair{n, (uint32_t)c, g, q.lo[t] + c < q.hi[t] ? 1u : 0u});
+            const uint64_t c = std::min(q.w[t], q.hi[t] - q.lo[t]), b = desc ? q.hi[t] - c : q.lo[t];
+            pairs.push_back(LimitPair{n, (uint32_t)c, g, (desc ? b > q.lo[t] : b + c < q.hi[t]) ? 1u : 0u});
             ptab.push_back(t);
-            ir[t].push_back({16 * q.lo[t], 16 * (q.lo[t] + c)});
+            pbase.push_back(b);
+            ir[t].push_back({16 * b, 16 * (b + c)});
             n += (uint32_t)c;
         }
         lq[g].pair1 = (uint32_t)pairs.size();
@@ -3593,10 +3595,9 @@ int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const
     std::vector<std::vector<ByteRange>> wr(nseek);
     for (uint32_t k = 0; k < np; k++) {
         const uint32_t t = ptab[k];
-        const LimitState &q = st[qs[pairs[k].query]];
         const uint64_t dl = r->tables[t]->desc.data_len;
         for (uint32_t j = 0; j < pairs[k].count; j++) {
-            const uint8_t *ix = e->ring_in + ss[t].at(16 * (q.lo[t] + j));
+            const uint8_t *ix = e->ring_in + ss[t].at(16 * (pbase[k] + j));
             const uint64_t off = rd_le(ix, 8), fs = rd_le(ix + 12, 4);
             const bool panic = fs == 0 || off > dl || fs > dl - off; // as k_scan_classify: the index record alone shows it
             rec[pairs[k].first + j] = make_uint4(0, 0, panic ? kScanStopPanic : 0u, (uint32_t)fs);
@@ -3618,11 +3619,10 @@ int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const
         return rc;
     for (uint32_t k = 0; k < np; k++) {
         const uint32_t t = ptab[k];
-        const LimitState &q = st[qs[pairs[k].query]];
         for (uint32_t j = 0; j < pairs[k].count; j++) {
             uint4 &x = rec[pairs[k].first + j];
             if (x.z) continue;
-            const uint64_t a = reinterpret_cast<uint64_t>(e->stage_in2 + sw[t].at(rd_le(e->ring_in + ss[t].at(16 * (q.lo[t] + j)), 8)));
+            const uint64_t a = reinterpret_cast<uint64_t>(e->stage_in2 + sw[t].at(rd_le(e->ring_in + ss[t].at(16 * (pbase[k] + j)), 8)));
             x.x = (uint32_t)a;
             x.y = (uint32_t)(a >> 32);
         }
@@ -3655,7 +3655,7 @@ int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const
     split_bind(w, ws, &sp, &rp, &p);
     LimitParams lp{reinterpret_cast<const LimitPair *>(ws + o_pairs), reinterpret_cast<const LimitQuery *>(ws + o_q),
                    reinterpret_cast<const uint4 *>(ws + o_rec), reinterpret_cast<const uint32_t *>(ws + o_rpair), n, gq,
-                   keep_tombstones ? 1u : 0u, 0, reinterpret_cast<uint4 *>(ws + o_flat), reinterpret_cast<unsigned long long *>(ws + o_pfx),
+                   keep_tombstones ? 1u : 0u, desc ? 1u : 0u, reinterpret_cast<uint4 *>(ws + o_flat), reinterpret_cast<unsigned long long *>(ws + o_pfx),
                    reinterpret_cast<uint32_t *>(ws + o_code), reinterpret_cast<uint32_t *>(ws + o_pbad), reinterpret_cast<uint32_t *>(ws + o_setter),
                    reinterpret_cast<uint32_t *>(ws + o_front), reinterpret_cast<uint4 *>(ws + o_qout), reinterpret_cast<const uint32_t *>(ws + o_pre),
                    reinterpret_cast<uint32_t *>(ws + o_pre), reinterpret_cast<uint32_t *>(ws + o_rank), reinterpret_cast<const uint32_t *>(ws + o_qsel),
@@ -3692,8 +3692,9 @@ int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const
         const uint4 o = qout[g];
         if (o.z != ~0u) {
             const uint32_t t = ptab[o.z];
+            const uint64_t rec_no = pbase[o.z] + (desc ? pairs[o.z].count - 1 - o.w : o.w); // o.w: from the chunk's fixed end
             row.flags = o.y == kLimitUnsorted ? DBEEL_RANGE_UNSORTED : DBEEL_RANGE_STOPPED;
-            row.stop = dbeel_scan_stop{(int32_t)t, o.y == kLimitUnsorted ? DBEEL_SCAN_STOP_NONE : o.y, q.lo[t] + o.w};
+            row.stop = dbeel_scan_stop{(int32_t)t, o.y == kLimitUnsorted ? DBEEL_SCAN_STOP_NONE : o.y, rec_no};
             continue;
         }
         bool truncated = false;
@@ -3741,11 +3742,12 @@ int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const
     return DBEEL_OK;
 }
 
-// dbeel_reader_get_ranges (dbeel_compact.h): the bound searches (reader_seek_batched), the spans and seek stops per query,
-// then merge rounds over groups of the live queries of about the partition budget (limit_round) until every query is
-// finished, then the rows and `out` from the emissions, in query order.
+// dbeel_reader_get_ranges, or dbeel_reader_get_ranges_reverse when `desc` (dbeel_compact.h): the bound searches
+// (reader_seek_batched), the spans and seek stops per query, then merge rounds over groups of the live queries of about the
+// partition budget (limit_round) until every query is finished, then the rows and `out` from the emissions, in query order.
 int reader_get_ranges(dbeel_engine *e, dbeel_reader *r, const uint8_t *kb, const std::vector<uint64_t> &ko, uint32_t nq,
-                      const uint32_t *limits, bool keep_tombstones, const dbeel_scan_io *io, dbeel_out *out, dbeel_range_row *rows) {
+                      const uint32_t *limits, bool keep_tombstones, bool desc, const dbeel_scan_io *io, dbeel_out *out,
+                      dbeel_range_row *rows) {
     const uint32_t nt = (uint32_t)r->tables.size();
     uint32_t nseek = nt; // the tables before the first one with no index record
     for (uint32_t t = 0; t < nt; t++)
@@ -3825,8 +3827,8 @@ int reader_get_ranges(dbeel_engine *e, dbeel_reader *r, const uint8_t *kb, const
                 bytes += cost;
                 g1++;
             }
-            if ((rc = limit_round(e, r, io, live.data() + g0, (uint32_t)(g1 - g0), limits, keep_tombstones, st, rows, &em, &next,
-                                  &launches, &gather_bytes)))
+            if ((rc = limit_round(e, r, io, live.data() + g0, (uint32_t)(g1 - g0), limits, keep_tombstones, desc, st, rows, &em,
+                                  &next, &launches, &gather_bytes)))
                 return rc;
             g0 = g1;
         }
@@ -3876,7 +3878,7 @@ int reader_get_ranges(dbeel_engine *e, dbeel_reader *r, const uint8_t *kb, const
 }
 
 int reader_get_ranges_entry(dbeel_reader *r, const dbeel_key_ranges *kr, uint32_t nq, const uint32_t *limits, uint32_t flags,
-                            dbeel_out *out, dbeel_range_row *rows) {
+                            bool desc, dbeel_out *out, dbeel_range_row *rows) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
     dbeel_engine *e = r->e;
     if (!kr || !kr->key_offsets || !limits || !out || !rows) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
@@ -3904,7 +3906,7 @@ int reader_get_ranges_entry(dbeel_reader *r, const dbeel_key_ranges *kr, uint32_
     x.rio = &r->io;
     const dbeel_scan_io io{reader_scan_read, nullptr, &x};
     const uint8_t *kb = ko[2ull * nq] ? static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0] : nullptr;
-    const int rc = reader_get_ranges(e, r, kb, ko, nq, limits, (flags & DBEEL_RANGE_KEEP_TOMBSTONES) != 0, &io, out, rows);
+    const int rc = reader_get_ranges(e, r, kb, ko, nq, limits, (flags & DBEEL_RANGE_KEEP_TOMBSTONES) != 0, desc, &io, out, rows);
     if (rc && rc != DBEEL_ERR_CAPACITY) {
         cudaStreamSynchronize(e->stream); // nothing of this call may touch the engine's buffers after it returns
         for (uint32_t q = 0; q < nq; q++) rows[q] = dbeel_range_row{0, 0, 0, dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0}};
@@ -4341,7 +4343,14 @@ int dbeel_reader_get_ranges(dbeel_reader *r, const dbeel_key_ranges *ranges, uin
                             uint32_t flags, dbeel_out *out, dbeel_range_row *rows) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
     REFUSE_WHILE_ASYNC(r->e);
-    return reader_get_ranges_entry(r, ranges, n_ranges, limits, flags, out, rows);
+    return reader_get_ranges_entry(r, ranges, n_ranges, limits, flags, false, out, rows);
+}
+
+int dbeel_reader_get_ranges_reverse(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, const uint32_t *limits,
+                                    uint32_t flags, dbeel_out *out, dbeel_range_row *rows) {
+    if (!r) return DBEEL_ERR_INVALID_ARG;
+    REFUSE_WHILE_ASYNC(r->e);
+    return reader_get_ranges_entry(r, ranges, n_ranges, limits, flags, true, out, rows);
 }
 
 int dbeel_page_cache_create(dbeel_engine *e, uint64_t bytes, dbeel_page_cache **out) {

@@ -1,19 +1,24 @@
-// range_limit.cuh -- one merge round of dbeel_reader_get_ranges: per query, a prefix of every table's span records (a
-// "pair" = one query and one table, its chunk staged as {entry address, index status, full_size} records), merged into the
-// query's first entries under dbeel_reader_get_range's rule -- the newest table's version of a key wins, tombstones dropped
-// unless asked for.  Pairs of a query lie together, tables ascending; a pair's records lie in record order.
+// range_limit.cuh -- one merge round of dbeel_reader_get_ranges / _reverse: per query, a prefix (forward) or a suffix
+// (reverse, LimitParams.desc) of every table's span records (a "pair" = one query and one table, its chunk staged as
+// {entry address, index status, full_size} records), merged into the query's first (forward) or last (reverse) entries
+// under dbeel_reader_get_range's rule -- the newest table's version of a key wins, tombstones dropped unless asked for.
+// Pairs of a query lie together, tables ascending; a pair's records lie in record order in both directions.
 //
 //   k_limit_decode  per record: the scan's decode (PANIC / ERR), the flat split record {address, 8 + klen, full_size},
-//                   the big-endian 8-byte key prefix, and strict ascent over the pair's previous record; the first damaged
-//                   record of every pair (atomicMin)
-//   k_limit_query   per query: the first damaged pair, else the frontier F_q = the smallest last staged key over the pairs
-//                   whose chunk ended before the span's end (every key <= F_q is complete), and the pairs that set it
-//   k_limit_flag    per record: keep = the query is clean, key <= F_q, no newer pair staged the key, tombstone rule
+//                   the big-endian 8-byte key prefix, and strict ascent over the pair's neighbour record -- forward the
+//                   previous one (a violation flags the higher record), reverse the next one (it flags the lower); per
+//                   pair the damaged record met first from the chunk's fixed end (atomicMin of its distance from there)
+//   k_limit_query   per query: the first damaged pair, else the frontier F_q over the pairs whose chunk stopped short of
+//                   the span's far end -- forward the smallest last staged key (every key <= F_q is complete), reverse
+//                   the largest first staged key (every key >= F_q is) -- and the pairs that set it
+//   k_limit_flag    per record: keep = the query is clean, key on the complete side of F_q, no newer pair staged the key,
+//                   tombstone rule
 //   k_range_tile_sums / k_range_tile_scan / k_range_prefix (merge_range.cuh) on one segment: exclusive prefix sum of keep
-//   k_limit_rank    per survivor: its merged position in the query (own pair's survivors before it + every other pair's
-//                   survivors below its key); per query: its survivors
+//   k_limit_rank    per survivor: its merged position in the query's output order (own pair's survivors before it --
+//                   after it, reverse -- + every other pair's survivors below its key -- above it, reverse); per query:
+//                   its survivors
 //   k_limit_select  per survivor of a finished query with rank < limit: its split record to out slot base + rank
-// The selected records then go through the split and phase 2 (split_emit) unchanged.
+// The selected records then go through the split and phase 2 (split_emit) unchanged, in rank order.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -28,7 +33,7 @@ constexpr uint32_t kLimitUnsorted = 4u; // damage code of a record not above its
 
 struct LimitPair {
     uint32_t first, count; // its records [first, first + count) of the round
-    uint32_t query, truncated; // truncated: the chunk ended before the span's end
+    uint32_t query, truncated; // truncated: the chunk stopped short of the span's far end (its end; reverse: its start)
 };
 
 struct LimitQuery {
@@ -42,14 +47,16 @@ struct LimitParams {
     const LimitQuery *queries;
     const uint4 *rec;              // [n] {entry address (x, y), kScanStopPanic when the index record alone shows it, full_size}
     const uint32_t *rpair;         // [n] pair of every record
-    uint32_t n, n_queries, keep_tombstones, pad;
+    uint32_t n, n_queries, keep_tombstones;
+    uint32_t desc;                 // 1: reverse -- chunks end at the span's end, the last entries in descending key order
     uint4 *flat;                   // [n] {entry address, 8 + klen, full_size}
     unsigned long long *pfx;       // [n]
     uint32_t *code;                // [n] 0 or the record's damage (kScanStopErr, kScanStopPanic, kLimitUnsorted)
-    uint32_t *pair_bad;            // [pairs] first damaged record of the pair (pair-local), ~0 = none
-    uint32_t *setter;              // [pairs] 1: the pair's last staged key is F_q
+    uint32_t *pair_bad;            // [pairs] the pair's damaged record nearest its chunk's fixed end, as its distance from
+                                   // there (forward: from the first record, reverse: from the last), ~0 = none
+    uint32_t *setter;              // [pairs] 1: the pair's last (reverse: first) staged key is F_q
     uint32_t *front;               // [queries] the record that holds F_q, ~0 = every pair read to its span's end
-    uint4 *qout;                   // [queries] {survivors <= F_q, damage code, damaged pair, its pair-local record}
+    uint4 *qout;                   // [queries] {survivors on F_q's complete side, damage code, damaged pair, its pair_bad}
     const uint32_t *pre;           // [n + 1] keep, then its exclusive prefix sum (k_range_prefix)
     uint32_t *keep;                // the same array, written by k_limit_flag
     uint32_t *rank;                // [n]
@@ -106,12 +113,15 @@ __global__ void __launch_bounds__(256) k_limit_decode(LimitParams p) {
     p.flat[i] = make_uint4(r.x, r.y, (uint32_t)(8 + kl), r.w);
     p.pfx[i] = ok ? range_prefix(key, (uint32_t)kl) : 0ull;
     const uint32_t pr = p.rpair[i];
-    uint64_t pkl = 0;
-    if (ok && i > p.pairs[pr].first && limit_decode(p.rec[i - 1], &pkl) &&
-        scan_key_cmp(range_entry(p.rec[i - 1]) + 8, pkl, key, kl) >= 0)
-        code = kLimitUnsorted;
+    const LimitPair pp = p.pairs[pr];
+    const uint32_t j = p.desc ? i + 1 : i - 1; // the neighbour: previous record (forward), next record (reverse)
+    uint64_t nkl = 0;
+    if (ok && (p.desc ? j < pp.first + pp.count : i > pp.first) && limit_decode(p.rec[j], &nkl)) {
+        const int c = scan_key_cmp(range_entry(p.rec[j]) + 8, nkl, key, kl);
+        if (p.desc ? c <= 0 : c >= 0) code = kLimitUnsorted;
+    }
     p.code[i] = code;
-    if (code) atomicMin(&p.pair_bad[pr], i - p.pairs[pr].first);
+    if (code) atomicMin(&p.pair_bad[pr], p.desc ? pp.first + pp.count - 1 - i : i - pp.first);
 }
 
 __global__ void __launch_bounds__(256) k_limit_query(LimitParams p) {
@@ -123,7 +133,8 @@ __global__ void __launch_bounds__(256) k_limit_query(LimitParams p) {
     for (uint32_t k = Q.pair0; k < Q.pair1; k++) {
         const uint32_t b = p.pair_bad[k];
         if (b != ~0u) {
-            p.qout[q] = make_uint4(0, p.code[p.pairs[k].first + b], k, b);
+            const LimitPair pp = p.pairs[k];
+            p.qout[q] = make_uint4(0, p.code[p.desc ? pp.first + pp.count - 1 - b : pp.first + b], k, b);
             p.front[q] = ~0u;
             return;
         }
@@ -132,16 +143,18 @@ __global__ void __launch_bounds__(256) k_limit_query(LimitParams p) {
     for (uint32_t k = Q.pair0; k < Q.pair1; k++) {
         const LimitPair pp = p.pairs[k];
         if (!pp.truncated || !pp.count) continue;
-        const uint32_t j = pp.first + pp.count - 1;
+        const uint32_t j = p.desc ? pp.first : pp.first + pp.count - 1; // the staged record nearest the span's far end
         const uint4 r = p.flat[j];
-        if (best == ~0u || limit_cmp(p, j, p.pfx[j], range_entry(r) + 8, r.z - 8, best) < 0) best = j;
+        if (best == ~0u) { best = j; continue; }
+        const int c = limit_cmp(p, j, p.pfx[j], range_entry(r) + 8, r.z - 8, best);
+        if (p.desc ? c > 0 : c < 0) best = j;
     }
     for (uint32_t k = Q.pair0; k < Q.pair1; k++) {
         const LimitPair pp = p.pairs[k];
         bool set = false;
         if (best != ~0u && pp.truncated && pp.count) {
             const uint4 r = p.flat[best];
-            set = limit_cmp(p, best, p.pfx[best], range_entry(r) + 8, r.z - 8, pp.first + pp.count - 1) == 0;
+            set = limit_cmp(p, best, p.pfx[best], range_entry(r) + 8, r.z - 8, p.desc ? pp.first : pp.first + pp.count - 1) == 0;
         }
         p.setter[k] = set ? 1u : 0u;
     }
@@ -162,7 +175,10 @@ __global__ void __launch_bounds__(256) k_limit_flag(LimitParams p) {
     const uint32_t kl = r.z - 8;
     const unsigned long long pk = p.pfx[i];
     const uint32_t f = p.front[q];
-    if (keep && f != ~0u) keep = limit_cmp(p, i, pk, k, kl, f) <= 0;
+    if (keep && f != ~0u) {
+        const int c = limit_cmp(p, i, pk, k, kl, f);
+        keep = p.desc ? c >= 0 : c <= 0;
+    }
     if (keep) keep = p.keep_tombstones || ld_u64_unaligned_narrow(k + kl) != 0;
     const uint32_t pair1 = p.queries[q].pair1;
     for (uint32_t x = pr + 1; keep && x < pair1; x++) { // a newer table staged the key
@@ -189,11 +205,13 @@ __global__ void __launch_bounds__(256) k_limit_rank(LimitParams p) {
     const uint8_t *k = range_entry(r) + 8;
     const uint32_t kl = r.z - 8;
     const unsigned long long pk = p.pfx[i];
-    uint32_t rank = p.pre[i] - p.pre[mine.first];
+    // reverse: survivors after it in its pair, and every other pair's at or above its key (none there equals it)
+    uint32_t rank = p.desc ? p.pre[mine.first + mine.count] - p.pre[i + 1] : p.pre[i] - p.pre[mine.first];
     for (uint32_t x = Q.pair0; x < Q.pair1; x++) {
         if (x == pr) continue;
         const LimitPair pp = p.pairs[x];
-        rank += p.pre[limit_lower_bound(p, pp, pk, k, kl)] - p.pre[pp.first];
+        const uint32_t at = limit_lower_bound(p, pp, pk, k, kl);
+        rank += p.desc ? p.pre[pp.first + pp.count] - p.pre[at] : p.pre[at] - p.pre[pp.first];
     }
     p.rank[i] = rank;
 }

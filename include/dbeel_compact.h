@@ -613,6 +613,37 @@ typedef struct dbeel_range_row {
 } dbeel_range_row;
 int dbeel_reader_get_ranges(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, const uint32_t *limits,
                             uint32_t flags, dbeel_out *out, dbeel_range_row *rows);
+
+/* Range reads from the end, batched: the LAST entries of many key ranges, in descending key order (the last page of a
+ * listing, the previous page from a cursor, the newest events when keys end in a timestamp).  Arguments, ranges, limits
+ * and flags as dbeel_reader_get_ranges; G_q as there (destination 0 of dbeel_reader_get_range for range q alone, in
+ * ascending key order).
+ *   Clean.   A query whose range makes that call return no stop and not DBEEL_ERR_UNSORTED_RUN gets the last
+ *            min(limits[q], |G_q|) entries of G_q, in descending key order, byte for byte; DBEEL_RANGE_MORE is set iff
+ *            |G_q| > limits[q].  A query with start >= end gets count 0, reads nothing and is never stopped, except by an
+ *            empty table.
+ *   Output.  Entries packed as dbeel_get_values packs them: query order, DESCENDING keys within a query, bytes as stored;
+ *            the .index offsets start at 0 in out->data, key_size = 8 + klen, out->items_written = the total.  Row q's
+ *            entries are entry numbers [first, first + count).  A caller asks for the previous page with end = the last
+ *            (smallest) key returned: end is exclusive, so no key suffix is needed.
+ *   Stops.   As dbeel_reader_get_ranges: a failed bound search or a table with no index record gives DBEEL_RANGE_STOPPED
+ *            with that stop, and nothing is read for the query's records.
+ *   Damage.  Only a suffix of every span is read.  Let A'_q be the merge, under G_q's rule, of every table's span records
+ *            for q, each cut just above the first record met walking down from seek_t(end) - 1 that fails dbeel_scan's
+ *            decode (ERR / PANIC as the scan classifies it) or whose key is not strictly below the key of the record
+ *            after it.  The row is then either the last min(limit, |A'_q|) entries of A'_q in descending order (MORE iff
+ *            |A'_q| > limit), or DBEEL_RANGE_STOPPED with stop = (table, ERR / PANIC, record) of a record that fails the
+ *            decode, or DBEEL_RANGE_UNSORTED with stop = (table, DBEEL_SCAN_STOP_NONE, r) of a record r whose key is not
+ *            below record r + 1's.  The last record of every non-empty span is always read.  One query's damage never
+ *            changes another query's row.
+ *   Reads.   The bound searches of dbeel_reader_get_ranges; per query and table, index records from seek_t(end) - 1
+ *            downward, never below seek_t(start), in chunks that end at seek_t(end) and double for the tables that hold
+ *            back the merge; the .data windows of exactly the records staged, each never wider than its records.  Leaf
+ *            slices, staged index slices and windows go through an attached page cache.  Nothing else is read.
+ *   Memory, Errors and dbeel_last_stats as dbeel_reader_get_ranges (DBEEL_RANGE_UNSORTED's stop.record here is the
+ *            record not below its successor).  A flag other than DBEEL_RANGE_KEEP_TOMBSTONES is DBEEL_ERR_INVALID_ARG. */
+int dbeel_reader_get_ranges_reverse(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, const uint32_t *limits,
+                                    uint32_t flags, dbeel_out *out, dbeel_range_row *rows);
 void dbeel_reader_close(dbeel_reader *r);
 
 /* Page cache for readers: the reference reads every .data / .index byte of a lookup or seek through a per-shard cache of

@@ -11,7 +11,15 @@ callback reads (a separate untimed pass through a logging callback); parity on e
 get_ranges equal the first entries of get_range's answer (all of it when that answer is shorter than the limit and its
 range reached the end of the key space).  Prints the GPU name and power limit of the run.  Results: DESIGN.md section 7,
 "Limited range reads".
-Usage: tools/reader_ranges_bench.py [keys_per_run (default 1000000)] [--rounds R] [--out result.json]"""
+With --reverse, range reads from the end (dbeel_reader_get_ranges_reverse) on the same tree: per batch, limit and end
+key distribution (uniform or Zipf(1.1), as the starts above), the last `limit` entries below each end key against the
+forward mirror -- get_ranges of the same number of entries from the other side of the same key -- and against get_range
+in non-overlapping calls reversed and cut on the host, its ranges starting 2 * limit keys below the end; and the last 10
+entries of the whole key space against its first 10 and against get_range of the whole key space plus a host tail cut.
+Parity on every round: every reverse query's entries equal the last entries of get_range's answer, reversed (all of it
+when that answer is shorter than the limit and its range started at the bottom of the key space).  Results: DESIGN.md
+section 7, "Range reads from the end".
+Usage: tools/reader_ranges_bench.py [keys_per_run (default 1000000)] [--rounds R] [--reverse] [--out result.json]"""
 import json
 import os
 import shutil
@@ -45,9 +53,20 @@ def entries(data, index, first, count):
     return bytes(data[a:b])
 
 
-def truncated_get_range(reader, ranges, limit):
-    """get_range in calls of up to 256 ranges that do not overlap (calls_of), every answer cut to its first `limit` entries on the host:
-    [(entry bytes, entries in the whole answer)], and the calls' dbeel_last_stats summed."""
+def last_entries(data, index, n, limit):
+    """The last `limit` of the n entries of one get_range answer, in descending key order, as one byte string."""
+    ix = np.asarray(index, np.uint8).reshape(-1, 16)
+    out = []
+    for k in range(n - 1, max(0, n - limit) - 1, -1):
+        off, fs = int(ix[k, :8].view("<u8")[0]), int(ix[k, 12:16].view("<u4")[0])
+        out.append(bytes(data[off:off + fs]))
+    return b"".join(out)
+
+
+def truncated_get_range(reader, ranges, limit, reverse=False):
+    """get_range in calls of up to 256 ranges that do not overlap (calls_of), every answer cut to its first `limit` entries
+    on the host (reverse: its last, in descending order): [(entry bytes, entries in the whole answer)], and the calls'
+    dbeel_last_stats summed."""
     uniq = sorted(set(ranges))  # a caller asks a repeated range once
     out, tot = {}, {"input_bytes": 0, "entries_out": 0, "partitions": 0, "reads": 0}  # reads: the counting reader's
     for call in calls_of(uniq):
@@ -57,7 +76,7 @@ def truncated_get_range(reader, ranges, limit):
             tot[k] += int(st[k])
         for q, (d, i) in zip(call, got):
             n = i.size // 16
-            out[uniq[q]] = (entries(d, i, 0, min(n, limit)), n)
+            out[uniq[q]] = (last_entries(d, i, n, limit) if reverse else entries(d, i, 0, min(n, limit)), n)
     return [out[x] for x in ranges], tot
 
 
@@ -83,6 +102,7 @@ def main():
     argv = sys.argv[1:]
     opt = lambda k, d: argv[argv.index(k) + 1] if k in argv else d
     out_path, rounds = opt("--out", None), int(opt("--rounds", "3"))
+    reverse = "--reverse" in argv
     pos = [a for a in argv if not a.startswith("--") and a not in (out_path, str(rounds))]
     kpr = int(pos[0]) if pos else 1_000_000
     cfg = W.CFG2 if kpr == 1_000_000 else W.scaled(W.CFG2, kpr)
@@ -94,7 +114,7 @@ def main():
     del runs
     base = "/dev/shm" if os.path.isdir("/dev/shm") else None
     d = tempfile.mkdtemp(prefix="reader_ranges_bench_", dir=base)
-    result = {"gpu": gpu, "power_limit": power, "rows": []}
+    result = {"gpu": gpu, "power_limit": power, "reverse": reverse, "rows": []}
     try:
         for k, (td, ti, tb) in enumerate(tables):
             sstable.write_run_files(d, 2 * k, (td, ti), tb)
@@ -156,16 +176,74 @@ def main():
             result["rows"].append(row)
             print(json.dumps(row), flush=True)
 
+        def run_row_reverse(name, make, limit, r_count):
+            arms = ("get_ranges_reverse", "get_ranges_forward_mirror", "get_range_reversed")
+            t = {a: [] for a in arms}
+            st, parity = {}, True
+            for r in range(r_count + 1):  # round 0 warms up
+                rq, fq, gr = make()
+                t0 = time.perf_counter()
+                rows, data, index = reader.get_ranges(rq, limit, reverse=True)
+                t1 = time.perf_counter()
+                st[arms[0]] = eng.stats()
+                reader.get_ranges(fq, limit)
+                t2 = time.perf_counter()
+                st[arms[1]] = eng.stats()
+                want, st[arms[2]] = truncated_get_range(reader, gr, limit, reverse=True)
+                t3 = time.perf_counter()
+                for q, (w, n_all) in enumerate(want):
+                    got = entries(data, index, int(rows[q]["first"]), int(rows[q]["count"]))
+                    more = bool(rows[q]["flags"] & capi.RANGE_MORE)
+                    if gr[q][0] == b"":  # both asked the rest of the key space below the end
+                        parity = parity and got == w and more == (n_all > limit)
+                    elif n_all >= limit:
+                        parity = parity and got == w and (more or n_all == limit)
+                    else:  # the guessed start cut get_range's answer short
+                        parity = parity and got[:len(w)] == w
+                if r:
+                    t[arms[0]].append(t1 - t0)
+                    t[arms[1]].append(t2 - t1)
+                    t[arms[2]].append(t3 - t2)
+            counting.get_ranges(rq, limit, reverse=True)
+            n_reads = {arms[0]: len(counting.last_stream_reads)}
+            rounds_c = {arms[0]: int(eng.stats()["partitions"])}
+            counting.get_ranges(fq, limit)
+            n_reads[arms[1]] = len(counting.last_stream_reads)
+            rounds_c[arms[1]] = int(eng.stats()["partitions"])
+            n_reads[arms[2]] = truncated_get_range(counting, gr, limit, reverse=True)[1]["reads"]
+            row = {"row": name, "parity": bool(parity), "arms": {}}
+            for arm in arms:
+                row["arms"][arm] = {"wall_ms": float(np.median(t[arm])) * 1e3, "bytes_read": int(st[arm]["input_bytes"]),
+                                    "reads": n_reads[arm], "rounds": int(st[arm]["partitions"]) if arm in rounds_c else None,
+                                    "entries": int(st[arm]["entries_out"])}
+                if arm in rounds_c:
+                    row["arms"][arm]["rounds_counting_reader"] = rounds_c[arm]
+            result["rows"].append(row)
+            print(json.dumps(row), flush=True)
+
         for batch in BATCHES:
             for limit in LIMITS:
                 for dist in ("uniform", "zipf"):
+                    if reverse:  # the last `limit` entries below keys[j]; the mirror: the first `limit` from keys[j] on
+                        def make(batch=batch, limit=limit, dist=dist):
+                            js = starts(batch, dist)
+                            rq = [(b"", keys[j].tobytes()) for j in js]
+                            fq = [(keys[j].tobytes(), TOP) for j in js]
+                            gr = [(keys[j - 2 * limit].tobytes() if j >= 2 * limit else b"", keys[j].tobytes()) for j in js]
+                            return rq, fq, gr
+                        run_row_reverse(f"batch {batch}, limit {limit}, {dist} ends", make, limit, rounds)
+                        continue
+
                     def make(batch=batch, limit=limit, dist=dist):
                         js = starts(batch, dist)
                         qs = [(keys[j].tobytes(), TOP) for j in js]
                         gr = [(keys[j].tobytes(), keys[j + 2 * limit].tobytes() if j + 2 * limit < nk else TOP) for j in js]
                         return qs, gr
                     run_row(f"batch {batch}, limit {limit}, {dist}", make, limit, rounds)
-        run_row("whole key space, limit 10", lambda: ([(b"", TOP)], [(b"", TOP)]), 10, min(rounds, 2))
+        if reverse:
+            run_row_reverse("whole key space, last 10", lambda: ([(b"", TOP)], [(b"", TOP)], [(b"", TOP)]), 10, min(rounds, 2))
+        else:
+            run_row("whole key space, limit 10", lambda: ([(b"", TOP)], [(b"", TOP)]), 10, min(rounds, 2))
         counting.close()
         reader.close()
         tree.close()
