@@ -49,6 +49,7 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_gpu_numa_node", "dbeel_bind_to_gpu", "dbeel_memtable_cuts_device", "dbeel_engine_stream",
            "dbeel_scan_bound", "dbeel_scan", "dbeel_scan_device", "dbeel_scan_stream", "dbeel_get_values",
            "dbeel_get_values_device", "dbeel_get_values_stream", "dbeel_reader_open", "dbeel_reader_get_values",
+           "dbeel_readers_get_values",
            "dbeel_reader_scan", "dbeel_reader_get_range", "dbeel_reader_get_ranges",
            "dbeel_reader_get_ranges_reverse", "dbeel_reader_close", "dbeel_page_cache_create", "dbeel_page_cache_destroy",
            "dbeel_reader_attach_page_cache", "dbeel_page_cache_stats"]
@@ -132,6 +133,12 @@ class LookupResult(C.Structure):
 
 
 LOOKUP_DTYPE = np.dtype([("table", "<i4"), ("bloom_rejects", "<u4"), ("record", "<u8")])
+MAX_READER_BATCHES = 1024  # DBEEL_MAX_READER_BATCHES
+
+
+class ReaderBatch(C.Structure):
+    _fields_ = [("reader", C.c_void_p), ("keys", C.c_void_p), ("key_offsets", C.c_void_p), ("n_keys", C.c_uint64),
+                ("mode", C.c_uint32), ("reserved", C.c_uint32)]
 
 
 def pack_keys(keys: Sequence[bytes]) -> Tuple[np.ndarray, np.ndarray]:
@@ -233,6 +240,8 @@ def lib():
         L.dbeel_reader_get_values.restype = C.c_int
         L.dbeel_reader_get_values.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.POINTER(Out),
                                               C.c_void_p]
+        L.dbeel_readers_get_values.restype = C.c_int
+        L.dbeel_readers_get_values.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(Out), C.c_void_p]
         L.dbeel_reader_scan.restype = C.c_int
         L.dbeel_reader_scan.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, SCAN_WRITE_FN, C.c_void_p,
                                         C.POINTER(JobResult), C.POINTER(ScanStop)]
@@ -1008,6 +1017,72 @@ class Engine:
         self._check(lib().dbeel_reader_open(self._h, st.arr, len(st.keep), C.byref(st.io), fence_bytes, C.byref(h)),
                     "dbeel_reader_open")
         return Reader(h, self, st)
+
+    def readers_get_values(self, batches, caps: Optional[Tuple[int, int]] = None, fail_read_at=None):
+        """dbeel_readers_get_values: the batches [(reader, keys, mode), ...] of many readers in one call.  Returns
+        [(rows, data, index)] per batch, each what reader.get_values(keys, mode) returns alone (index offsets into its own
+        data).  caps = (data_cap, index_cap) for the whole call, by default retried once with the sizes needed as
+        Reader.get_values does.  Each reader's last_stream_reads = its reads in this call; fail_read_at = {reader: n} makes
+        the n-th read of that reader's callback in the call return 4242."""
+        fail_read_at = fail_read_at or {}
+        arr = (ReaderBatch * max(1, len(batches)))()
+        keep, counts, readers = [], [], []
+        for j, (r, keys, mode) in enumerate(batches):
+            if not r._h:
+                raise ValueError("reader is closed")
+            blob, off = pack_keys(list(keys))
+            keep.append((blob, off))
+            counts.append(len(keys))
+            arr[j] = ReaderBatch(r._h, blob.ctypes.data if blob.size else None, off.ctypes.data, len(keys), mode, 0)
+            if all(r is not x for x in readers):
+                readers.append(r)
+        sts = [r._st for r in readers if r._st is not None]
+        for r in readers:
+            if r._st is not None:
+                r._st.fail_read_at = fail_read_at.get(r, -1)
+        n = sum(counts)
+        rows = np.zeros(max(1, n), dtype=LOOKUP_DTYPE)
+        dc0 = sum(sum(d for d, _ in r._st.sizes) if r._st is not None else r._data_cap for r in readers)
+        dc, ic = caps if caps is not None else (min(dc0, 64 << 20), 16 * n)
+        try:
+            for attempt in range(2):
+                od, oi = np.empty(max(1, dc), np.uint8), np.empty(max(1, ic), np.uint8)
+                out = Out(od.ctypes.data, dc, 0, oi.ctypes.data, ic, 0, None, 0, 0, 0)
+                for st in sts:
+                    st.log.clear()
+                rc = lib().dbeel_readers_get_values(self._h, arr, len(batches), C.byref(out), rows.ctypes.data)
+                for st in sts:
+                    st.last_reads = list(st.log)
+                if rc == 0:
+                    break
+                err = DbeelError(rc, f"dbeel_readers_get_values: {lib().dbeel_last_error(self._h).decode()}")
+                if rc == ERR_CAPACITY:
+                    err.needed = (int(out.data_len), int(out.index_len))
+                    err.rows = rows[:n].copy()
+                if caps is not None or attempt or rc != ERR_CAPACITY:
+                    raise err
+                dc, ic = err.needed
+        finally:
+            for r in readers:
+                if r._st is not None:
+                    r._st.fail_read_at = -1
+                    r.last_stream_reads = r._st.last_reads
+        # split the packed output: batch b's answered rows are its entries, in row order
+        data, index = od[:out.data_len], oi[:out.index_len]
+        rows = rows[:n]
+        answered = (rows["table"] >= 0) & ((rows["bloom_rejects"] & LOOKUP_BAD_ENTRY) == 0)
+        res, q0, item0 = [], 0, 0
+        for c in counts:
+            items = int(answered[q0:q0 + c].sum())
+            ix = index[16 * item0:16 * (item0 + items)].copy()
+            offs = ix.view("<u8")[0::2] if items else np.zeros(0, np.uint64)
+            d0 = int(offs[0]) if items else 0
+            d1 = int(offs[-1] + ix.view("<u4")[-1]) if items else 0
+            if items:
+                offs -= np.uint64(d0)
+            res.append((rows[q0:q0 + c].copy(), data[d0:d1].copy(), ix))
+            q0, item0 = q0 + c, item0 + items
+        return res
 
     def open_page_cache(self, nbytes: int) -> PageCache:
         """dbeel_page_cache_create: a PageCache of nbytes // 4096 page slots in one device allocation made now."""

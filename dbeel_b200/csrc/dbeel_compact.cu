@@ -2417,74 +2417,130 @@ int reader_load_fences(dbeel_engine *e, const dbeel_scan_io *io, uint32_t ti, db
 // their slots and the image from them; host_too brings the image back to host (the .index slices, whose records the host
 // reads).  The pages become resident only once their reads have succeeded.  The caller has synchronised the stream since
 // its last use of stage_out and of the cache's staging.  The callback's code comes back unchanged, with `what`.
-struct GvsPart { uint32_t t; const GvsStaged *s; };
+struct GvsPart {
+    uint32_t t; // the table's position in its reader's (or the call's) tables: the callback's table argument
+    const GvsStaged *s;
+    const dbeel_reader *r = nullptr;
+    const dbeel_scan_io *io = nullptr;
+};
 
-int gvs_load(dbeel_engine *e, const dbeel_scan_io *io, const dbeel_reader *r, uint32_t kind, const std::vector<GvsPart> &parts,
-             uint8_t *host, uint8_t *dev, uint64_t from, uint64_t to, bool host_too, const char *what) {
-    dbeel_page_cache *c = r ? r->cache : nullptr;
+int gvs_load(dbeel_engine *e, uint32_t kind, const std::vector<GvsPart> &parts, uint8_t *host, uint8_t *dev, uint64_t from,
+             uint64_t to, bool host_too, const char *what) {
     cudaStream_t s = e->stream;
     int rc;
-    PagePlan p;
-    if (c) {
+    // the parts of each page cache, in order of first appearance, as one request each
+    std::vector<dbeel_page_cache *> cs;
+    std::vector<std::vector<size_t>> of;
+    std::vector<PagePlan> plans;
+    for (size_t k = 0; k < parts.size(); k++) {
+        dbeel_page_cache *c = parts[k].r ? parts[k].r->cache : nullptr;
+        if (!c) continue;
+        const size_t ci = std::find(cs.begin(), cs.end(), c) - cs.begin();
+        if (ci == cs.size()) { cs.push_back(c); of.emplace_back(); }
+        of[ci].push_back(k);
+    }
+    std::vector<uint8_t> direct(parts.size(), 1);
+    uint64_t stage_bytes = 0;
+    for (size_t ci = 0; ci < cs.size(); ci++) {
         std::vector<PagePart> pp;
-        for (const GvsPart &g : parts) {
-            const TableDesc &d = r->tables[g.t]->desc;
-            pp.push_back(PagePart{r->tables[g.t]->id, kind, kind == DBEEL_STREAM_DATA ? d.data_len : 16 * d.n, {}});
-            for (size_t k = 0; k < g.s->runs.size(); k++) pp.back().ranges.push_back(PageRange{g.s->runs[k].lo, g.s->runs[k].hi, g.s->pos[k]});
+        for (size_t k : of[ci]) {
+            const GvsPart &g = parts[k];
+            const TableDesc &d = g.r->tables[g.t]->desc;
+            pp.push_back(PagePart{g.r->tables[g.t]->id, kind, kind == DBEEL_STREAM_DATA ? d.data_len : 16 * d.n, {}});
+            for (size_t j = 0; j < g.s->runs.size(); j++) pp.back().ranges.push_back(PageRange{g.s->runs[j].lo, g.s->runs[j].hi, g.s->pos[j]});
         }
-        p = c->pc.plan(pp, StreamPump::kPiece);
+        plans.push_back(cs[ci]->pc.plan(pp, StreamPump::kPiece));
+        const PagePlan &p = plans.back();
+        if (p.bypass) continue;
+        for (size_t k : of[ci]) direct[k] = 0;
+        stage_bytes = std::max(stage_bytes, align_up(p.img_bytes, kAlign) + sizeof(PageCopy) * p.moves.size());
     }
-    if (!c || p.bypass) {
-        for (const GvsPart &g : parts)
-            if ((rc = gvs_read(e, io, g.t, kind, *g.s, host))) return fail(e, rc, what);
-        if (to > from) CU(cudaMemcpyAsync(dev + from, host + from, to - from, cudaMemcpyHostToDevice, s));
-        return DBEEL_OK;
+    auto drop = [&](size_t from_ci) { // plans not carried out leave their caches as they were
+        for (size_t ci = from_ci; ci < cs.size(); ci++)
+            if (!plans[ci].bypass) cs[ci]->pc.commit(plans[ci], false);
+    };
+    rc = stage_bytes ? ensure_device(e, &e->stage_out, &e->stage_out_cap, std::max<uint64_t>(stage_bytes, 256)) : DBEEL_OK;
+    if (rc) { drop(0); return rc; }
+    // uncached parts (no cache, or a request larger than its cache): read into host, the whole image down in one copy,
+    // before any page copy writes its own parts over it
+    bool any_direct = false, any_paged = false;
+    for (size_t k = 0; k < parts.size(); k++) {
+        if (!direct[k]) { any_paged = true; continue; }
+        any_direct = true;
+        if ((rc = gvs_read(e, parts[k].io, parts[k].t, kind, *parts[k].s, host))) { drop(0); return fail(e, rc, what); }
     }
-    const uint64_t o_copy = align_up(p.img_bytes, kAlign), bytes = o_copy + sizeof(PageCopy) * p.moves.size();
-    rc = ensure_host(e, &c->host, &c->host_cap, std::max<uint64_t>(bytes, 256));
-    if (!rc) rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, std::max<uint64_t>(bytes, 256));
-    if (rc) { c->pc.commit(p, false); return rc; }
-    for (const PageRead &x : p.reads) e->stats.input_bytes += x.len;
-    rc = parallel_pieces(p.reads.size(), [&](size_t k) {
-        const PageRead &x = p.reads[k];
-        return io->read(io->ctx, parts[x.part].t, kind, x.off, x.len, c->host + x.img);
-    });
-    if (rc) { c->pc.commit(p, false); return fail(e, rc, what); }
-    const uint64_t src[3] = {(uint64_t)e->stage_out, (uint64_t)e->stage_out, (uint64_t)c->pool}; // by PageMove::how
-    const uint64_t dst[3] = {(uint64_t)c->pool, (uint64_t)dev, (uint64_t)dev};
-    PageCopy *pc = reinterpret_cast<PageCopy *>(c->host + o_copy);
-    for (size_t k = 0; k < p.moves.size(); k++) {
-        const PageMove &m = p.moves[k];
-        pc[k] = PageCopy{src[m.how] + m.src, dst[m.how] + m.dst, m.len, 0};
+    if (any_direct && to > from) {
+        const cudaError_t ce = cudaMemcpyAsync(dev + from, host + from, to - from, cudaMemcpyHostToDevice, s);
+        if (ce != cudaSuccess) { drop(0); return fail(e, DBEEL_ERR_CUDA, "cudaMemcpyAsync", ce); }
     }
-    cudaError_t ce = cudaSuccess;
-    if (!p.moves.empty()) {
-        ce = cudaMemcpyAsync(e->stage_out, c->host, bytes, cudaMemcpyHostToDevice, s);
-        if (ce == cudaSuccess) {
-            launch_k(e, k_page_copy, (uint32_t)((32 * p.moves.size() + 255) / 256), 256, 0, s, reinterpret_cast<const PageCopy *>(e->stage_out + o_copy),
-                     (uint64_t)p.moves.size());
-            ce = cudaGetLastError();
+    for (size_t ci = 0; ci < cs.size(); ci++) {
+        dbeel_page_cache *c = cs[ci];
+        PagePlan &p = plans[ci];
+        if (p.bypass) continue;
+        const uint64_t o_copy = align_up(p.img_bytes, kAlign), bytes = o_copy + sizeof(PageCopy) * p.moves.size();
+        rc = ensure_host(e, &c->host, &c->host_cap, std::max<uint64_t>(bytes, 256));
+        if (rc) { drop(ci); return rc; }
+        for (const PageRead &x : p.reads) e->stats.input_bytes += x.len;
+        rc = parallel_pieces(p.reads.size(), [&](size_t k) {
+            const PageRead &x = p.reads[k];
+            const GvsPart &g = parts[of[ci][x.part]];
+            return g.io->read(g.io->ctx, g.t, kind, x.off, x.len, c->host + x.img);
+        });
+        if (rc) { drop(ci); return fail(e, rc, what); }
+        const uint64_t src[3] = {(uint64_t)e->stage_out, (uint64_t)e->stage_out, (uint64_t)c->pool}; // by PageMove::how
+        const uint64_t dst[3] = {(uint64_t)c->pool, (uint64_t)dev, (uint64_t)dev};
+        PageCopy *pc = reinterpret_cast<PageCopy *>(c->host + o_copy);
+        for (size_t k = 0; k < p.moves.size(); k++) {
+            const PageMove &m = p.moves[k];
+            pc[k] = PageCopy{src[m.how] + m.src, dst[m.how] + m.dst, m.len, 0};
         }
+        cudaError_t ce = cudaSuccess;
+        if (!p.moves.empty()) {
+            ce = cudaMemcpyAsync(e->stage_out, c->host, bytes, cudaMemcpyHostToDevice, s);
+            if (ce == cudaSuccess) {
+                launch_k(e, k_page_copy, (uint32_t)((32 * p.moves.size() + 255) / 256), 256, 0, s, reinterpret_cast<const PageCopy *>(e->stage_out + o_copy),
+                         (uint64_t)p.moves.size());
+                ce = cudaGetLastError();
+            }
+        }
+        c->pc.commit(p, ce == cudaSuccess); // the copies that read a slot are enqueued before any later fill of it
+        if (ce != cudaSuccess) { drop(ci + 1); return fail(e, DBEEL_ERR_CUDA, "k_page_copy", ce); }
     }
-    c->pc.commit(p, ce == cudaSuccess); // the copies that read a slot are enqueued before any later fill of it
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "k_page_copy", ce);
-    if (host_too && to > from) {
+    if (any_paged && host_too && to > from) {
         CU(cudaMemcpyAsync(host + from, dev + from, to - from, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
     }
     return DBEEL_OK;
 }
 
-// One group of touched leaves (group_leaves), ascending (table, leaf), on the device for k_lookup_leaf / k_seek_leaf: per
-// table its index slices into stage_in behind the header (through ring_in, and back to it), then the .data windows of
+// Every part through `io` and reader r's page cache (r may be null: no cache).
+int gvs_load(dbeel_engine *e, const dbeel_scan_io *io, const dbeel_reader *r, uint32_t kind, std::vector<GvsPart> parts,
+             uint8_t *host, uint8_t *dev, uint64_t from, uint64_t to, bool host_too, const char *what) {
+    for (GvsPart &g : parts) {
+        g.r = r;
+        g.io = io;
+    }
+    return gvs_load(e, kind, parts, host, dev, from, to, host_too, what);
+}
+
+// Where the touched leaves of part t of a group come from: the reader (null: none) and io its reads go through, the table's
+// position there, its .data length and the longest key of the batch that searches it.
+struct LeafSrc {
+    const dbeel_reader *r;
+    const dbeel_scan_io *io;
+    uint32_t table;
+    uint64_t data_len, max_klen;
+};
+
+// One group of touched leaves (group_leaves), ascending (part, leaf), on the device for k_lookup_leaf / k_seek_leaf: per
+// part its index slices into stage_in behind the header (through ring_in, and back to it), then the .data windows of
 // those slices (leaf_window) into stage_in2 (through ring_out).  The header at stage_in is GvsLeaf[nl] | first[nt + 1]
-// (nt = data_len.size()): table t's leaves are [first[t], first[t + 1]), each biased so that record r of the table lies
+// (nt = src.size()): part t's leaves are [first[t], first[t + 1]), each biased so that record r of the table lies
 // at index + r and file offset o at data + o (a leaf whose records all point past the file never dereferences data:
 // probe() reports them corrupt first).  Through gvs_load, so with a page cache this writes stage_out: reader_scan_key's
 // per-call fences live there, and its k_seek_fence has completed (a synchronise) before the first group is loaded.
-int gvs_load_leaves(dbeel_engine *e, const dbeel_scan_io *io, const dbeel_reader *r, const TouchedLeaf *lv, uint32_t nl,
-                    const std::vector<uint64_t> &data_len, uint64_t max_klen) {
-    const uint32_t nt = (uint32_t)data_len.size();
+int gvs_load_leaves(dbeel_engine *e, const std::vector<LeafSrc> &src, const TouchedLeaf *lv, uint32_t nl) {
+    const uint32_t nt = (uint32_t)src.size();
     std::vector<uint32_t> first(nt + 1, 0);
     for (uint32_t k = 0; k < nl; k++) first[lv[k].t + 1]++;
     for (uint32_t t = 0; t < nt; t++) first[t + 1] += first[t];
@@ -2498,12 +2554,12 @@ int gvs_load_leaves(dbeel_engine *e, const dbeel_scan_io *io, const dbeel_reader
         for (uint32_t k = first[t]; k < first[t + 1]; k++) x.push_back({16 * lv[k].a, 16 * lv[k].b});
         ss[t] = gvs_stage(std::move(x), kLookupMergeGap, end);
         end = ss[t].end;
-        parts.push_back(GvsPart{t, &ss[t]});
+        parts.push_back(GvsPart{src[t].table, &ss[t], src[t].r, src[t].io});
     }
     int rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, end);
     if (!rc) rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, end);
     if (rc) return rc;
-    if ((rc = gvs_load(e, io, r, DBEEL_STREAM_INDEX, parts, e->ring_in, e->stage_in, hdr, end, true, "stream read callback failed (.index, leaves)")))
+    if ((rc = gvs_load(e, DBEEL_STREAM_INDEX, parts, e->ring_in, e->stage_in, hdr, end, true, "stream read callback failed (.index, leaves)")))
         return rc;
     std::vector<ByteRange> win(nl);
     std::vector<uint8_t> has(nl, 0);
@@ -2513,18 +2569,18 @@ int gvs_load_leaves(dbeel_engine *e, const dbeel_scan_io *io, const dbeel_reader
         if (first[t] == first[t + 1]) continue;
         std::vector<ByteRange> wr;
         for (uint32_t k = first[t]; k < first[t + 1]; k++)
-            if (leaf_window(e->ring_in + ss[t].at(16 * lv[k].a), lv[k].b - lv[k].a, data_len[t], max_klen, &win[k])) {
+            if (leaf_window(e->ring_in + ss[t].at(16 * lv[k].a), lv[k].b - lv[k].a, src[t].data_len, src[t].max_klen, &win[k])) {
                 has[k] = 1;
                 wr.push_back(win[k]);
             }
         sw[t] = gvs_stage(std::move(wr), 0, wend);
         wend = sw[t].end;
-        if (!sw[t].runs.empty()) parts.push_back(GvsPart{t, &sw[t]});
+        if (!sw[t].runs.empty()) parts.push_back(GvsPart{src[t].table, &sw[t], src[t].r, src[t].io});
     }
     rc = ensure_host(e, &e->ring_out, &e->ring_out_cap, std::max<uint64_t>(wend, 256));
     if (!rc) rc = ensure_device(e, &e->stage_in2, &e->stage_in2_cap, std::max<uint64_t>(wend, 256));
     if (rc) return rc;
-    if ((rc = gvs_load(e, io, r, DBEEL_STREAM_DATA, parts, e->ring_out, e->stage_in2, 0, wend, false, "stream read callback failed (.data, leaves)")))
+    if ((rc = gvs_load(e, DBEEL_STREAM_DATA, parts, e->ring_out, e->stage_in2, 0, wend, false, "stream read callback failed (.data, leaves)")))
         return rc;
     GvsLeaf *hl = reinterpret_cast<GvsLeaf *>(e->ring_in);
     for (uint32_t k = 0; k < nl; k++) {
@@ -2540,14 +2596,371 @@ int gvs_load_leaves(dbeel_engine *e, const dbeel_scan_io *io, const dbeel_reader
     return DBEEL_OK;
 }
 
-// Per table, newest first: k_gvs_filter -> fences read, k_lookup_fence -> touched leaves read in groups under the partition
-// budget, k_lookup_leaf per group and k_gvs_copy for the group's hits (their entries leave the window for the hit heap).
-// Then the entries of hits at fences are read into the heap, k_gvs_hit decodes every hit and split_emit writes `out` in
-// query order, as dbeel_get_values does.  Every phase ends in a stream synchronise before its pinned
-// buffers are refilled.
-// With a reader, the filters are already on the device and a table whose cached fences serve the batch
+// One batch of a batched read from files: dbeel_get_values_stream's (r null: its tables' filters staged here, reads
+// through io) or a reader's (its resident filters and cached fences, reads through its io and page cache).
+struct GvsBatch {
+    dbeel_reader *r = nullptr;
+    const dbeel_scan_io *io = nullptr;
+    std::vector<TableDesc> td; // oldest first
+    const uint8_t *keys = nullptr;
+    const uint64_t *key_off = nullptr;
+    uint64_t n_keys = 0, max_klen = 0;
+    uint32_t mode = 0;
+};
+
+// The batches' searches, one level at a time: level j pairs every batch b with its table T_b - 1 - j (newest first).  Per
+// level, for all pairs together: one k_gvs_filter; one read-back of the pairs' open-query counts when some pair's fence
+// decision needs it; the per-call fences of the pairs that need them in one image, and one k_lookup_fence; one read-back of
+// the touched leaves; then the leaves in groups (group_leaves over pairs), k_lookup_leaf per group and k_gvs_copy for the
+// group's hits (their entries leave the window for the hit heap).  Then the entries of hits at fences are read into the
+// heap, k_gvs_hit decodes every hit and split_emit writes `out` in query order, as dbeel_get_values does.  Every phase ends
+// in a stream synchronise before its pinned buffers are refilled.
+// Each pair's decisions are its batch's solo call's: a reader table whose cached fences serve the batch
 // (reader_uses_cache) descends them instead of reading its fences; when the depth the batch wants cannot exceed the cached
-// one for any number of open queries, k_gvs_filter and k_lookup_fence go back to back with no read-back between them.
+// one for any number of open queries, the decision is made before the filter and needs no count.
+// The caller has checked the arguments, taken the engine and cleared stats and out; results has Σ n_keys rows.
+int gvs_walk(dbeel_engine *e, const std::vector<GvsBatch> &bs, dbeel_out *out, dbeel_lookup_result *results) {
+    const uint32_t nb = (uint32_t)bs.size();
+    uint64_t n_keys = 0;
+    std::vector<uint64_t> row0(nb + 1, 0);
+    uint32_t levels = 0;
+    for (uint32_t b = 0; b < nb; b++) {
+        row0[b + 1] = row0[b] + bs[b].n_keys;
+        if (bs[b].n_keys) levels = std::max(levels, (uint32_t)bs[b].td.size());
+    }
+    n_keys = row0[nb];
+    if (n_keys == 0) return DBEEL_OK;
+    cudaError_t ce = cudaSetDevice(e->device);
+    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    cudaStream_t s = e->stream;
+    const uint32_t n = (uint32_t)n_keys;
+    const uint64_t budget = e->partition_bytes;
+    // the keys of every batch back to back (one batch: as given), and each query's batch
+    std::vector<uint8_t> kcat;
+    std::vector<uint64_t> ocat;
+    std::vector<uint32_t> qb;
+    const uint8_t *keys = bs[0].keys;
+    const uint64_t *key_off = bs[0].key_off;
+    if (nb > 1) {
+        ocat.resize(n_keys + 1);
+        qb.resize(n_keys);
+        for (uint32_t b = 0; b < nb; b++) {
+            const GvsBatch &B = bs[b];
+            if (!B.n_keys) continue;
+            const uint64_t k0 = B.key_off[0], base = kcat.size();
+            for (uint64_t i = 0; i < B.n_keys; i++) {
+                ocat[row0[b] + i] = base + (B.key_off[i] - k0);
+                qb[row0[b] + i] = b;
+            }
+            kcat.insert(kcat.end(), B.keys + k0, B.keys + B.key_off[B.n_keys]);
+        }
+        ocat[n_keys] = kcat.size();
+        keys = kcat.data();
+        key_off = ocat.data();
+    }
+    const uint64_t key_bytes = key_off[n_keys];
+    // the touched flags of a level: at most 2^max(lookup_depth(n_keys), cached depth) per pair
+    uint64_t touched_max = 1;
+    for (uint32_t j = 0; j < levels; j++) {
+        uint64_t t = 0;
+        for (const GvsBatch &B : bs) {
+            if (!B.n_keys || j >= B.td.size()) continue;
+            const uint32_t ti = (uint32_t)B.td.size() - 1 - j;
+            const TableDesc &d = B.td[ti];
+            uint32_t dmax = lookup_depth(B.n_keys, d.n, d.data_len, 8 + B.max_klen, budget);
+            if (B.r) dmax = std::max(dmax, (uint32_t)B.r->tables[ti]->depth);
+            t += 1ull << dmax;
+        }
+        touched_max = std::max(touched_max, t);
+    }
+
+    // ---- per-query state and the split's workspace
+    uint64_t off = 0;
+    const uint64_t o_keys = carve_ws(&off, key_bytes + 16), o_off = carve_ws(&off, 8ull * (n + 1)), o_batch = carve_ws(&off, 4ull * n);
+    const uint64_t o_rows = carve_ws(&off, 16ull * n), o_hix = carve_ws(&off, 16ull * n), o_state = carve_ws(&off, sizeof(SearchState) * n);
+    const uint64_t o_node = carve_ws(&off, 4ull * n), o_src = carve_ws(&off, 8ull * n), o_hoff = carve_ws(&off, 8ull * n);
+    const uint64_t o_touched = carve_ws(&off, touched_max), o_cnt = carve_ws(&off, 8ull * nb), o_need = carve_ws(&off, 8);
+    const uint64_t o_cursor = carve_ws(&off, 8), o_pairs = carve_ws(&off, sizeof(GvsPair) * nb);
+    const SplitLayout w = carve_split(&off, n, 1);
+    int rc = ensure_device(e, &e->ws, &e->ws_cap, off);
+    const uint64_t pin_tot = align_up(w.header2_bytes, 64);
+    // the pinned block during the levels: touched flags | open counts | the pairs as the filter reads them | as the rest do
+    const uint64_t p_cnt = align_up(touched_max, 64), p_fpairs = align_up(p_cnt + 8ull * nb, 64);
+    const uint64_t p_pairs = align_up(p_fpairs + sizeof(GvsPair) * nb, 64), p_end = p_pairs + sizeof(GvsPair) * nb;
+    if (!rc) rc = ensure_pinned(e, std::max<uint64_t>(pin_tot + 8ull * 4, p_end));
+    if (rc) return rc;
+    uint8_t *ws = e->ws;
+    CU(cudaEventRecord(e->ev[EV_START], s));
+    for (uint64_t q = 0; q < n_keys; q++) results[q] = dbeel_lookup_result{-1, 0, 0};
+    static_assert(sizeof(dbeel_lookup_result) == 16, "result rows are written as uint4");
+    if (key_bytes) CU(cudaMemcpyAsync(ws + o_keys, keys, key_bytes, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_off, key_off, 8ull * (n + 1), cudaMemcpyHostToDevice, s));
+    if (nb > 1) CU(cudaMemcpyAsync(ws + o_batch, qb.data(), 4ull * n, cudaMemcpyHostToDevice, s));
+    else CU(cudaMemsetAsync(ws + o_batch, 0, 4ull * n, s));
+    CU(cudaMemcpyAsync(ws + o_rows, results, 16ull * n, cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(ws + o_src, 0, 8ull * n, s));
+    CU(cudaMemsetAsync(ws + o_hoff, 0xFF, 8ull * n, s)); // kGvsNoEntry
+    CU(cudaMemsetAsync(ws + o_cursor, 0, 8, s));
+    GvsQueries gq{ws + o_keys, reinterpret_cast<const uint64_t *>(ws + o_off), reinterpret_cast<const uint32_t *>(ws + o_batch), n_keys,
+                  reinterpret_cast<uint4 *>(ws + o_rows), reinterpret_cast<uint4 *>(ws + o_hix), reinterpret_cast<SearchState *>(ws + o_state),
+                  reinterpret_cast<uint32_t *>(ws + o_node), reinterpret_cast<unsigned long long *>(ws + o_src),
+                  reinterpret_cast<unsigned long long *>(ws + o_hoff)};
+    unsigned long long *d_need = reinterpret_cast<unsigned long long *>(ws + o_need), *d_cursor = reinterpret_cast<unsigned long long *>(ws + o_cursor);
+    // The hit heap (stage_out2) holds every answered entry until split_emit gathers them; it grows keeping what it holds.
+    uint64_t heap_bound = 0;
+    auto heap_reserve = [&](uint64_t need) -> int {
+        if (need <= e->stage_out2_cap) return DBEEL_OK;
+        uint8_t *old = e->stage_out2;
+        const uint64_t old_cap = e->stage_out2_cap;
+        e->stage_out2 = nullptr;
+        e->stage_out2_cap = 0;
+        int rc2 = ensure_device(e, &e->stage_out2, &e->stage_out2_cap, need);
+        if (!rc2 && old && heap_bound) CU(cudaMemcpyAsync(e->stage_out2, old, std::min(old_cap, heap_bound), cudaMemcpyDeviceToDevice, s));
+        CU(cudaStreamSynchronize(s));
+        if (old) cudaFree(old);
+        return rc2;
+    };
+    unsigned long long *d_cnt = reinterpret_cast<unsigned long long *>(ws + o_cnt);
+    uint8_t *d_touched = ws + o_touched;
+    GvsPair *d_pairs = reinterpret_cast<GvsPair *>(ws + o_pairs);
+    const uint32_t grid = (n + 255) / 256;
+    uint32_t launches = 0, groups = 0;
+    // the page caches of the batches' readers (group_leaves over pairs keeps each one's leaves within its capacity)
+    std::vector<dbeel_page_cache *> caches;
+    std::vector<uint64_t> cache_bytes;
+    std::vector<int32_t> cache_of(nb, -1);
+    for (uint32_t b = 0; b < nb; b++) {
+        dbeel_page_cache *c = bs[b].r ? bs[b].r->cache : nullptr;
+        if (!c) continue;
+        const size_t ci = std::find(caches.begin(), caches.end(), c) - caches.begin();
+        if (ci == caches.size()) {
+            caches.push_back(c);
+            cache_bytes.push_back(kPageBytes * c->pc.capacity());
+        }
+        cache_of[b] = (int32_t)ci;
+    }
+
+    std::vector<GvsPair> pairs(nb);
+    std::vector<ProbeTree> pt_call(nb);
+    std::vector<const ProbeTree *> pts(nb);
+    std::vector<uint64_t> touched_at(nb);
+    for (uint32_t j = 0; j < levels; j++) {
+        // ---- the filter, with the decisions that need no count of open queries: the depth the batch wants grows with
+        // that count, which is at most its n_keys
+        std::vector<uint8_t> decided(nb, 0);
+        bool need_count = false;
+        for (uint32_t b = 0; b < nb; b++) {
+            const GvsBatch &B = bs[b];
+            GvsPair &P = pairs[b];
+            P = GvsPair{};
+            P.mode = B.mode;
+            if (!B.n_keys || j >= B.td.size()) continue;
+            const uint32_t ti = (uint32_t)B.td.size() - 1 - j;
+            P.t = B.td[ti];
+            P.table = ti;
+            P.live = 1;
+            dbeel_reader_table *rt = B.r ? B.r->tables[ti].get() : nullptr;
+            dbeel_reader_table::Fences *cache = rt ? &rt->fences[B.mode] : nullptr;
+            const uint32_t cd = rt ? (uint32_t)rt->depth : 0;
+            if (cache && cache->loaded && cd > 0 &&
+                reader_uses_cache(B.max_klen, lookup_depth(B.n_keys, P.t.n, P.t.data_len, 8 + B.max_klen, budget), cd)) {
+                decided[b] = 1;
+                P.depth = cd;
+                pts[b] = &cache->pt;
+                P.fix = reinterpret_cast<const uint4 *>(cache->dev);
+                P.ffr = reinterpret_cast<const unsigned long long *>(cache->dev + (16ull << cd));
+            } else {
+                need_count = true;
+            }
+        }
+        memcpy(e->pin + p_fpairs, pairs.data(), sizeof(GvsPair) * nb);
+        CU(cudaMemcpyAsync(d_pairs, e->pin + p_fpairs, sizeof(GvsPair) * nb, cudaMemcpyHostToDevice, s));
+        CU(cudaMemsetAsync(d_cnt, 0, 8ull * nb, s));
+        launch_k(e, k_gvs_filter, grid, 256, 0, s, gq, static_cast<const GvsPair *>(d_pairs), d_cnt);
+        launches++;
+        if (need_count) {
+            CU(cudaMemcpyAsync(e->pin + p_cnt, d_cnt, 8ull * nb, cudaMemcpyDeviceToHost, s));
+            CU(cudaStreamSynchronize(s));
+        }
+
+        // ---- the other decisions; fences: the index records of the open internal nodes, then their key frames (or the
+        // reader's copies)
+        std::vector<GvsFenceReads> frs(nb);
+        std::vector<uint64_t> img_at(nb, ~0ull);
+        uint64_t img_bytes = 0, tbytes = 0;
+        bool any = false, any_fence = false;
+        for (uint32_t b = 0; b < nb; b++) {
+            const GvsBatch &B = bs[b];
+            GvsPair &P = pairs[b];
+            if (!P.live) continue;
+            if (!decided[b]) {
+                const uint64_t m = rd64(e->pin + p_cnt + 8ull * b);
+                if (m == 0) { // no query reaches the table: nothing of it is read
+                    P.live = 0;
+                    continue;
+                }
+                const uint32_t ti = P.table;
+                dbeel_reader_table *rt = B.r ? B.r->tables[ti].get() : nullptr;
+                dbeel_reader_table::Fences *cache = rt ? &rt->fences[B.mode] : nullptr;
+                const uint32_t cd = rt ? (uint32_t)rt->depth : 0;
+                uint32_t depth = lookup_depth(m, P.t.n, P.t.data_len, 8 + B.max_klen, budget);
+                if (cache && reader_uses_cache(B.max_klen, depth, cd)) {
+                    depth = cd;
+                    if (!cache->loaded) {
+                        if ((rc = reader_load_fences(e, B.io, ti, rt, B.mode))) return rc;
+                        CU(cudaStreamSynchronize(s)); // its image goes down from ring_out, which the next pair refills
+                    }
+                    pts[b] = &cache->pt;
+                    P.fix = reinterpret_cast<const uint4 *>(cache->dev);
+                    P.ffr = reinterpret_cast<const unsigned long long *>(cache->dev + (16ull << cd));
+                } else {
+                    plan_probe_tree(B.mode, P.t.n, depth, &pt_call[b]);
+                    pts[b] = &pt_call[b];
+                    if (depth > 0) {
+                        if ((rc = gvs_read_fences(e, B.io, ti, pt_call[b], P.t.data_len, B.max_klen, &frs[b]))) return rc;
+                        img_at[b] = align_up(img_bytes, kAlign);
+                        img_bytes = img_at[b] + frs[b].image_bytes();
+                    }
+                }
+                P.depth = depth;
+            }
+            touched_at[b] = tbytes;
+            P.touched = d_touched + tbytes;
+            tbytes += 1ull << P.depth;
+            any = true;
+            any_fence = any_fence || P.depth > 0;
+        }
+        if (!any) continue;
+        if (img_bytes) {
+            if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, img_bytes))) return rc;
+            if ((rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, img_bytes))) return rc;
+            for (uint32_t b = 0; b < nb; b++) {
+                if (img_at[b] == ~0ull) continue;
+                gvs_fence_image(frs[b], pairs[b].t.data_len, e->ring_in + img_at[b], e->stage_in + img_at[b]);
+                pairs[b].fix = reinterpret_cast<const uint4 *>(e->stage_in + img_at[b]);
+                pairs[b].ffr = reinterpret_cast<const unsigned long long *>(e->stage_in + img_at[b] + (16ull << pairs[b].depth));
+            }
+            CU(cudaMemcpyAsync(e->stage_in, e->ring_in, img_bytes, cudaMemcpyHostToDevice, s));
+        }
+        CU(cudaMemsetAsync(d_touched, 0, tbytes, s));
+        for (uint32_t b = 0; b < nb; b++)
+            if (pairs[b].live && pairs[b].depth == 0) CU(cudaMemsetAsync(d_touched + touched_at[b], 1, 1, s));
+        memcpy(e->pin + p_pairs, pairs.data(), sizeof(GvsPair) * nb);
+        CU(cudaMemcpyAsync(d_pairs, e->pin + p_pairs, sizeof(GvsPair) * nb, cudaMemcpyHostToDevice, s));
+        if (any_fence) {
+            launch_k(e, k_lookup_fence, grid, 256, 0, s, gq, static_cast<const GvsPair *>(d_pairs));
+            launches++;
+        }
+        CU(cudaMemcpyAsync(e->pin, d_touched, tbytes, cudaMemcpyDeviceToHost, s));
+        CU(cudaGetLastError());
+        CU(cudaStreamSynchronize(s));
+
+        // ---- leaves, in groups of about `budget` bytes (with page caches, each cache's leaves at most its capacity)
+        std::vector<TouchedLeaf> lv;
+        std::vector<LeafPair> lp(nb);
+        std::vector<LeafSrc> src(nb);
+        for (uint32_t b = 0; b < nb; b++) {
+            const GvsPair &P = pairs[b];
+            lp[b] = LeafPair{P.t.n, P.t.data_len, bs[b].max_klen, cache_of[b]};
+            src[b] = LeafSrc{bs[b].r, bs[b].io, P.table, P.t.data_len, bs[b].max_klen};
+            if (P.live) touched_leaves(*pts[b], b, e->pin + touched_at[b], &lv);
+        }
+        const std::vector<size_t> cut = group_leaves(lv, lp, budget, cache_bytes);
+        for (size_t gi = 0; gi + 1 < cut.size(); gi++) {
+            const uint32_t nl = (uint32_t)(cut[gi + 1] - cut[gi]);
+            if ((rc = gvs_load_leaves(e, src, lv.data() + cut[gi], nl))) return rc;
+            CU(cudaMemsetAsync(d_need, 0, 8, s));
+            launch_k(e, k_lookup_leaf, grid, 256, 0, s, gq, static_cast<const GvsPair *>(d_pairs), reinterpret_cast<const GvsLeaf *>(e->stage_in),
+                     reinterpret_cast<const uint32_t *>(e->stage_in + sizeof(GvsLeaf) * nl), d_need);
+            CU(cudaMemcpyAsync(e->pin, d_need, 8, cudaMemcpyDeviceToHost, s));
+            CU(cudaGetLastError());
+            CU(cudaStreamSynchronize(s));
+            launches++;
+            if (const uint64_t need = rd64(e->pin)) { // the group's hits leave the window for the heap before it is reused
+                if ((rc = heap_reserve(heap_bound + need))) return rc;
+                heap_bound += need;
+                launch_k(e, k_gvs_copy, (uint32_t)((32 * n_keys + 255) / 256), 256, 0, s, gq, e->stage_out2, d_cursor);
+                CU(cudaGetLastError());
+                CU(cudaStreamSynchronize(s));
+                launches++;
+            }
+            groups++;
+        }
+    }
+
+    // ---- hits at fences: their entries, one record each (runs that touch as one read), per pair into the heap behind
+    // the copies
+    std::vector<uint4> hix(n);
+    std::vector<unsigned long long> hoff(n);
+    CU(cudaMemcpyAsync(results, ws + o_rows, 16ull * n, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(hix.data(), ws + o_hix, 16ull * n, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(hoff.data(), ws + o_hoff, 8ull * n, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    std::vector<uint32_t> pair0(nb + 1, 0); // batch b's tables are pairs [pair0[b], pair0[b + 1]) of the entry reads
+    for (uint32_t b = 0; b < nb; b++) pair0[b + 1] = pair0[b] + (uint32_t)bs[b].td.size();
+    std::vector<std::vector<ByteRange>> er(pair0[nb]);
+    auto fence_entry = [&](uint32_t b, uint64_t q, ByteRange *r) { // a fence hit whose entry k_gvs_hit can decode
+        if (hoff[q] != kGvsFenceHit) return false;
+        const uint4 ix = hix[q];
+        const uint64_t o = (uint64_t)ix.x | ((uint64_t)ix.y << 32), dl = bs[b].td[results[q].table].data_len;
+        if (!gvs_entry_fits(o, ix.z, ix.w, key_off[q + 1] - key_off[q], dl)) return false;
+        *r = ByteRange{o, o + ix.w};
+        return true;
+    };
+    bool any_fence_hit = false;
+    for (uint32_t b = 0; b < nb; b++)
+        for (uint64_t q = row0[b]; q < row0[b + 1]; q++) {
+            ByteRange r;
+            if (fence_entry(b, q, &r)) er[pair0[b] + results[q].table].push_back(r);
+            any_fence_hit = any_fence_hit || hoff[q] == kGvsFenceHit;
+        }
+    if (any_fence_hit) {
+        const uint64_t base = align_up(heap_bound, kAlign);
+        std::vector<GvsStaged> sh(pair0[nb]);
+        std::vector<GvsPart> parts;
+        uint64_t staged = 0;
+        for (uint32_t b = 0; b < nb; b++)
+            for (uint32_t i = 0; i < bs[b].td.size(); i++) {
+                GvsStaged &x = sh[pair0[b] + i];
+                x = gvs_stage(std::move(er[pair0[b] + i]), 0, staged);
+                staged = x.end;
+                if (!x.runs.empty()) parts.push_back(GvsPart{i, &x, bs[b].r, bs[b].io});
+            }
+        if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, std::max<uint64_t>(staged, 256)))) return rc;
+        if ((rc = heap_reserve(base + staged + 256))) return rc;
+        if ((rc = gvs_load(e, DBEEL_STREAM_DATA, parts, e->ring_in, e->stage_out2 + base, 0, staged, false, "stream read callback failed (.data, entries)")))
+            return rc;
+        for (uint32_t b = 0; b < nb; b++)
+            for (uint64_t q = row0[b]; q < row0[b + 1]; q++) {
+                ByteRange r;
+                if (hoff[q] != kGvsFenceHit) continue;
+                hoff[q] = fence_entry(b, q, &r) ? base + sh[pair0[b] + results[q].table].at(r.lo) : kGvsNoEntry;
+            }
+        CU(cudaMemcpyAsync(ws + o_hoff, hoff.data(), 8ull * n, cudaMemcpyHostToDevice, s));
+        CU(cudaStreamSynchronize(s));
+    }
+    ScanParams sp = {};
+    RouteParams rp;
+    Params p;
+    split_bind(w, ws, &sp, &rp, &p);
+    CU(cudaMemsetAsync(ws + w.o_tot, 0, 8ull * 3, s));
+    CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
+    launch_k(e, k_gvs_hit, grid, 256, 0, s, gq, static_cast<const uint8_t *>(e->stage_out2), LookupEmit{sp.dest, sp.flat});
+    launches++;
+    CU(cudaMemcpyAsync(results, ws + o_rows, 16ull * n, cudaMemcpyDeviceToHost, s)); // back with the sizes: filled on ERR_CAPACITY too
+    e->stats.entries_in = n_keys;
+    e->stats.partitions = groups;
+    uint64_t items = 0, bytes = 0;
+    rc = split_emit(e, w, sp, rp, p, pin_tot, false, out, &launches, &items, &bytes, [](const unsigned long long *) {});
+    if (rc == DBEEL_ERR_CAPACITY) {
+        out->data_len = bytes;
+        out->index_len = 16 * items;
+        return fail(e, DBEEL_ERR_CAPACITY, "the entries found are larger than the output buffers (data_len / index_len: the sizes needed)");
+    }
+    return rc;
+}
+
+// dbeel_get_values_stream and dbeel_reader_get_values: one batch.
 int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys, const uint64_t *key_off,
                             uint64_t n_keys, uint32_t mode, const dbeel_scan_io *io, dbeel_out *out, dbeel_lookup_result *results,
                             dbeel_reader *reader = nullptr) {
@@ -2572,222 +2985,33 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
     if (!keys && key_bytes) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     cudaError_t ce = cudaSetDevice(e->device);
     if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
-    cudaStream_t s = e->stream;
-    const uint32_t n = (uint32_t)n_keys;
-    uint64_t max_klen = 0;
-    for (uint64_t q = 0; q < n_keys; q++) max_klen = std::max(max_klen, key_off[q + 1] - key_off[q]);
-
-    // ---- per-query state and the split's workspace
-    uint64_t off = 0;
-    const uint64_t o_keys = carve_ws(&off, key_bytes + 16), o_off = carve_ws(&off, 8ull * (n + 1));
-    const uint64_t o_rows = carve_ws(&off, 16ull * n), o_hix = carve_ws(&off, 16ull * n), o_state = carve_ws(&off, sizeof(SearchState) * n);
-    const uint64_t o_node = carve_ws(&off, 4ull * n), o_src = carve_ws(&off, 8ull * n), o_hoff = carve_ws(&off, 8ull * n);
-    const uint64_t o_touched = carve_ws(&off, 1ull << kLookupMaxDepth), o_cnt = carve_ws(&off, 8), o_need = carve_ws(&off, 8);
-    const uint64_t o_cursor = carve_ws(&off, 8);
-    const SplitLayout w = carve_split(&off, n, 1);
-    int rc = ensure_device(e, &e->ws, &e->ws_cap, off);
-    const uint64_t pin_tot = align_up(w.header2_bytes, 64);
-    if (!rc) rc = ensure_pinned(e, std::max<uint64_t>(pin_tot + 8ull * 4, (1ull << kLookupMaxDepth) + 64));
-    if (rc) return rc;
+    int rc;
     uint64_t bloom_bytes = 0;
     for (uint32_t i = 0; i < n_tables; i++) bloom_bytes += align_up(tables[i].bloom_len + 16, kAlign);
     if ((rc = ensure_device(e, &e->bloom_dev, &e->bloom_dev_cap, std::max<uint64_t>(bloom_bytes, 256)))) return rc;
-    uint8_t *ws = e->ws;
-    std::vector<TableDesc> td(n_tables);
-    std::vector<uint64_t> nrecs(n_tables), data_lens(n_tables);
+    std::vector<GvsBatch> bs(1);
+    GvsBatch &B = bs[0];
+    B.r = reader;
+    B.io = io;
+    B.keys = static_cast<const uint8_t *>(keys);
+    B.key_off = key_off;
+    B.n_keys = n_keys;
+    B.mode = mode;
+    for (uint64_t q = 0; q < n_keys; q++) B.max_klen = std::max(B.max_klen, key_off[q + 1] - key_off[q]);
+    B.td.resize(n_tables);
     uint64_t bpos = 0;
     for (uint32_t i = 0; i < n_tables; i++) {
         const dbeel_table &t = tables[i];
-        td[i] = TableDesc{nullptr, t.data_len, nullptr, t.index_len / DBEEL_INDEX_ENTRY_SIZE, nullptr, 0, 0, 0, 0, {0, 0, 0, 0}};
-        if (reader) td[i] = reader->tables[i]->desc; // tables[] carries no filter: it is resident
-        nrecs[i] = td[i].n;
-        data_lens[i] = td[i].data_len;
+        B.td[i] = TableDesc{nullptr, t.data_len, nullptr, t.index_len / DBEEL_INDEX_ENTRY_SIZE, nullptr, 0, 0, 0, 0, {0, 0, 0, 0}};
+        if (reader) B.td[i] = reader->tables[i]->desc; // tables[] carries no filter: it is resident
         if (!t.bloom_len) continue;
         const uint8_t *b = static_cast<const uint8_t *>(t.bloom);
-        if ((rc = parse_bloom(e, b, b + t.bloom_len - kBloomTrailer, t.bloom_len, &td[i]))) return rc;
-        CU(cudaMemcpyAsync(e->bloom_dev + bpos, b, t.bloom_len, cudaMemcpyHostToDevice, s));
-        td[i].words = reinterpret_cast<const uint32_t *>(e->bloom_dev + bpos + 8);
+        if ((rc = parse_bloom(e, b, b + t.bloom_len - kBloomTrailer, t.bloom_len, &B.td[i]))) return rc;
+        CU(cudaMemcpyAsync(e->bloom_dev + bpos, b, t.bloom_len, cudaMemcpyHostToDevice, e->stream));
+        B.td[i].words = reinterpret_cast<const uint32_t *>(e->bloom_dev + bpos + 8);
         bpos += align_up(t.bloom_len + 16, kAlign);
     }
-    CU(cudaEventRecord(e->ev[EV_START], s));
-    for (uint64_t q = 0; q < n_keys; q++) results[q] = dbeel_lookup_result{-1, 0, 0};
-    static_assert(sizeof(dbeel_lookup_result) == 16, "result rows are written as uint4");
-    if (key_bytes) CU(cudaMemcpyAsync(ws + o_keys, keys, key_bytes, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ws + o_off, key_off, 8ull * (n + 1), cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ws + o_rows, results, 16ull * n, cudaMemcpyHostToDevice, s));
-    CU(cudaMemsetAsync(ws + o_src, 0, 8ull * n, s));
-    CU(cudaMemsetAsync(ws + o_hoff, 0xFF, 8ull * n, s)); // kGvsNoEntry
-    CU(cudaMemsetAsync(ws + o_cursor, 0, 8, s));
-    GvsQueries gq{ws + o_keys, reinterpret_cast<const uint64_t *>(ws + o_off), n_keys, reinterpret_cast<uint4 *>(ws + o_rows),
-                  reinterpret_cast<uint4 *>(ws + o_hix), reinterpret_cast<SearchState *>(ws + o_state), reinterpret_cast<uint32_t *>(ws + o_node),
-                  reinterpret_cast<unsigned long long *>(ws + o_src), reinterpret_cast<unsigned long long *>(ws + o_hoff), mode};
-    unsigned long long *d_need = reinterpret_cast<unsigned long long *>(ws + o_need), *d_cursor = reinterpret_cast<unsigned long long *>(ws + o_cursor);
-    // The hit heap (stage_out2) holds every answered entry until split_emit gathers them; it grows keeping what it holds.
-    uint64_t heap_bound = 0;
-    auto heap_reserve = [&](uint64_t need) -> int {
-        if (need <= e->stage_out2_cap) return DBEEL_OK;
-        uint8_t *old = e->stage_out2;
-        const uint64_t old_cap = e->stage_out2_cap;
-        e->stage_out2 = nullptr;
-        e->stage_out2_cap = 0;
-        int rc2 = ensure_device(e, &e->stage_out2, &e->stage_out2_cap, need);
-        if (!rc2 && old && heap_bound) CU(cudaMemcpyAsync(e->stage_out2, old, std::min(old_cap, heap_bound), cudaMemcpyDeviceToDevice, s));
-        CU(cudaStreamSynchronize(s));
-        if (old) cudaFree(old);
-        return rc2;
-    };
-    unsigned long long *d_cnt = reinterpret_cast<unsigned long long *>(ws + o_cnt);
-    uint8_t *d_touched = ws + o_touched;
-    const uint32_t grid = (n + 255) / 256;
-    uint32_t launches = 0, groups = 0;
-    const uint64_t budget = e->partition_bytes;
-    const bool paged = reader && reader->cache;
-    const uint64_t group_bytes = paged ? std::min(budget, kPageBytes * reader->cache->pc.capacity()) : budget;
-
-    for (uint32_t ti = n_tables; ti-- > 0;) { // sstables.iter().rev(): newest first
-        const TableDesc &t = td[ti];
-        const uint64_t data_len = t.data_len, nrec = t.n;
-        dbeel_reader_table *rt = reader ? reader->tables[ti].get() : nullptr;
-        dbeel_reader_table::Fences *cache = rt ? &rt->fences[mode] : nullptr;
-        const uint32_t cached_depth = rt ? (uint32_t)rt->depth : 0;
-        // whether the cached fences serve the batch, decided before the filter runs when no count of open queries can
-        // change it: the depth the batch wants grows with that count, which is at most n_keys
-        bool use_cache = cache && cache->loaded && cached_depth > 0 &&
-                         reader_uses_cache(max_klen, lookup_depth(n_keys, nrec, data_len, 8 + max_klen, budget), cached_depth);
-        CU(cudaMemsetAsync(d_cnt, 0, 8, s));
-        launch_k(e, k_gvs_filter, grid, 256, 0, s, gq, t, d_cnt);
-        launches++;
-        uint32_t depth = cached_depth;
-        if (!use_cache) {
-            CU(cudaMemcpyAsync(e->pin, d_cnt, 8, cudaMemcpyDeviceToHost, s));
-            CU(cudaStreamSynchronize(s));
-            const uint64_t m = rd64(e->pin);
-            if (m == 0) continue; // no query reaches the table: nothing of it is read
-            depth = lookup_depth(m, nrec, data_len, 8 + max_klen, budget);
-            use_cache = cache && reader_uses_cache(max_klen, depth, cached_depth);
-            if (use_cache) {
-                depth = cached_depth;
-                if (!cache->loaded && (rc = reader_load_fences(e, io, ti, rt, mode))) return rc;
-            }
-        }
-        ProbeTree pt_call;
-        if (!use_cache) plan_probe_tree(mode, nrec, depth, &pt_call);
-        const ProbeTree &pt = use_cache ? cache->pt : pt_call;
-        const uint64_t leaf0 = 1ull << depth;
-        CU(cudaMemsetAsync(d_touched, 0, leaf0, s));
-
-        // ---- fences: the index records of the open internal nodes, then their key frames (or the reader's copies)
-        if (depth > 0) {
-            if (!use_cache) {
-                GvsFenceReads fr;
-                if ((rc = gvs_read_fences(e, io, ti, pt, data_len, max_klen, &fr))) return rc;
-                const uint64_t bytes = fr.image_bytes();
-                if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, bytes))) return rc;
-                if ((rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, bytes))) return rc;
-                gvs_fence_image(fr, data_len, e->ring_in, e->stage_in);
-                CU(cudaMemcpyAsync(e->stage_in, e->ring_in, bytes, cudaMemcpyHostToDevice, s));
-            }
-            const uint8_t *f = use_cache ? cache->dev : e->stage_in; // fix[leaf0] | ffr[leaf0] | ...
-            GvsFences gf{reinterpret_cast<const uint4 *>(f), reinterpret_cast<const unsigned long long *>(f + 16 * leaf0), depth, ti, nrec, d_touched};
-            launch_k(e, k_lookup_fence, grid, 256, 0, s, gq, gf);
-            launches++;
-        } else {
-            CU(cudaMemsetAsync(d_touched, 1, 1, s));
-        }
-        CU(cudaMemcpyAsync(e->pin, d_touched, leaf0, cudaMemcpyDeviceToHost, s));
-        CU(cudaGetLastError());
-        CU(cudaStreamSynchronize(s));
-
-        // ---- leaves, in groups of about `budget` bytes (with a page cache, at most its capacity)
-        std::vector<TouchedLeaf> lv;
-        touched_leaves(pt, ti, e->pin, &lv);
-        const std::vector<size_t> cut = group_leaves(lv, nrecs, data_lens, max_klen, group_bytes, paged);
-        for (size_t gi = 0; gi + 1 < cut.size(); gi++) {
-            const uint32_t nl = (uint32_t)(cut[gi + 1] - cut[gi]);
-            if ((rc = gvs_load_leaves(e, io, reader, lv.data() + cut[gi], nl, data_lens, max_klen))) return rc;
-            CU(cudaMemsetAsync(d_need, 0, 8, s));
-            launch_k(e, k_lookup_leaf, grid, 256, 0, s, gq, t, reinterpret_cast<const GvsLeaf *>(e->stage_in), nl, depth, ti, d_need);
-            CU(cudaMemcpyAsync(e->pin, d_need, 8, cudaMemcpyDeviceToHost, s));
-            CU(cudaGetLastError());
-            CU(cudaStreamSynchronize(s));
-            launches++;
-            if (const uint64_t need = rd64(e->pin)) { // the group's hits leave the window for the heap before it is reused
-                if ((rc = heap_reserve(heap_bound + need))) return rc;
-                heap_bound += need;
-                launch_k(e, k_gvs_copy, (uint32_t)((32 * n_keys + 255) / 256), 256, 0, s, gq, e->stage_out2, d_cursor);
-                CU(cudaGetLastError());
-                CU(cudaStreamSynchronize(s));
-                launches++;
-            }
-            groups++;
-        }
-    }
-
-    // ---- hits at fences: their entries, one record each (runs that touch as one read), into the heap behind the copies
-    std::vector<uint4> hix(n);
-    std::vector<unsigned long long> hoff(n);
-    CU(cudaMemcpyAsync(results, ws + o_rows, 16ull * n, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(hix.data(), ws + o_hix, 16ull * n, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(hoff.data(), ws + o_hoff, 8ull * n, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    std::vector<std::vector<ByteRange>> er(n_tables);
-    auto fence_entry = [&](uint64_t q, ByteRange *r) { // a fence hit whose entry k_gvs_hit can decode
-        if (hoff[q] != kGvsFenceHit) return false;
-        const uint4 ix = hix[q];
-        const uint64_t o = (uint64_t)ix.x | ((uint64_t)ix.y << 32), dl = tables[results[q].table].data_len;
-        if (!gvs_entry_fits(o, ix.z, ix.w, key_off[q + 1] - key_off[q], dl)) return false;
-        *r = ByteRange{o, o + ix.w};
-        return true;
-    };
-    bool any_fence_hit = false;
-    for (uint64_t q = 0; q < n_keys; q++) {
-        ByteRange r;
-        if (fence_entry(q, &r)) er[results[q].table].push_back(r);
-        any_fence_hit = any_fence_hit || hoff[q] == kGvsFenceHit;
-    }
-    if (any_fence_hit) {
-        const uint64_t base = align_up(heap_bound, kAlign);
-        std::vector<GvsStaged> sh(n_tables);
-        uint64_t staged = 0;
-        for (uint32_t i = 0; i < n_tables; i++) {
-            sh[i] = gvs_stage(std::move(er[i]), 0, staged);
-            staged = sh[i].end;
-        }
-        if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, std::max<uint64_t>(staged, 256)))) return rc;
-        if ((rc = heap_reserve(base + staged + 256))) return rc;
-        std::vector<GvsPart> parts;
-        for (uint32_t i = 0; i < n_tables; i++)
-            if (!sh[i].runs.empty()) parts.push_back(GvsPart{i, &sh[i]});
-        if ((rc = gvs_load(e, io, reader, DBEEL_STREAM_DATA, parts, e->ring_in, e->stage_out2 + base, 0, staged, false,
-                           "stream read callback failed (.data, entries)")))
-            return rc;
-        for (uint64_t q = 0; q < n_keys; q++) {
-            ByteRange r;
-            if (hoff[q] != kGvsFenceHit) continue;
-            hoff[q] = fence_entry(q, &r) ? base + sh[results[q].table].at(r.lo) : kGvsNoEntry;
-        }
-        CU(cudaMemcpyAsync(ws + o_hoff, hoff.data(), 8ull * n, cudaMemcpyHostToDevice, s));
-        CU(cudaStreamSynchronize(s));
-    }
-    ScanParams sp = {};
-    RouteParams rp;
-    Params p;
-    split_bind(w, ws, &sp, &rp, &p);
-    CU(cudaMemsetAsync(ws + w.o_tot, 0, 8ull * 3, s));
-    CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
-    launch_k(e, k_gvs_hit, grid, 256, 0, s, gq, static_cast<const uint8_t *>(e->stage_out2), LookupEmit{sp.dest, sp.flat});
-    launches++;
-    CU(cudaMemcpyAsync(results, ws + o_rows, 16ull * n, cudaMemcpyDeviceToHost, s)); // back with the sizes: filled on ERR_CAPACITY too
-    e->stats.entries_in = n_keys;
-    e->stats.partitions = groups;
-    uint64_t items = 0, bytes = 0;
-    rc = split_emit(e, w, sp, rp, p, pin_tot, false, out, &launches, &items, &bytes, [](const unsigned long long *) {});
-    if (rc == DBEEL_ERR_CAPACITY) {
-        out->data_len = bytes;
-        out->index_len = 16 * items;
-        return fail(e, DBEEL_ERR_CAPACITY, "the entries found are larger than the output buffers (data_len / index_len: the sizes needed)");
-    }
-    return rc;
+    return gvs_walk(e, bs, out, results);
 }
 
 
@@ -3293,9 +3517,11 @@ int reader_seek(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, uint3
     std::vector<TouchedLeaf> lv;
     for (uint32_t t = 0; t < nseek; t++) touched_leaves(*pts[t], t, touched.data() + touched_at[t], &lv);
     const std::vector<size_t> cut = group_leaves(lv, nrecs, data_lens, max_klen, group_bytes, paged);
+    std::vector<LeafSrc> src(nseek);
+    for (uint32_t t = 0; t < nseek; t++) src[t] = LeafSrc{r, io, t, data_lens[t], max_klen};
     for (size_t g = 0; g + 1 < cut.size(); g++) {
         const uint32_t nl = (uint32_t)(cut[g + 1] - cut[g]);
-        if ((rc = gvs_load_leaves(e, io, r, lv.data() + cut[g], nl, data_lens, max_klen))) return rc;
+        if ((rc = gvs_load_leaves(e, src, lv.data() + cut[g], nl))) return rc;
         launch_k(e, k_seek_leaf, grid, 256, 0, s, sq, reinterpret_cast<const TableDesc *>(ws + o_td),
                  reinterpret_cast<const uint32_t *>(ws + o_depth), reinterpret_cast<const GvsLeaf *>(e->stage_in),
                  reinterpret_cast<const uint32_t *>(e->stage_in + sizeof(GvsLeaf) * nl));
@@ -4313,6 +4539,45 @@ int dbeel_reader_get_values(dbeel_reader *r, const void *keys, const uint64_t *k
     REFUSE_WHILE_ASYNC(r->e);
     const std::vector<dbeel_table> tables = reader_tables(r);
     return get_values_stream_entry(r->e, tables.data(), (uint32_t)tables.size(), keys, key_offsets, n_keys, mode, &r->io, out, results, r);
+}
+
+int dbeel_readers_get_values(dbeel_engine *e, const dbeel_reader_batch *batches, uint32_t n_batches, dbeel_out *out,
+                             dbeel_lookup_result *results) {
+    REFUSE_WHILE_ASYNC(e);
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (!batches || !out || !results) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    if (n_batches == 0 || n_batches > DBEEL_MAX_READER_BATCHES) return fail(e, DBEEL_ERR_INVALID_ARG, "n_batches is 0 or above DBEEL_MAX_READER_BATCHES");
+    uint64_t n_keys = 0;
+    for (uint32_t b = 0; b < n_batches; b++) {
+        const dbeel_reader_batch &x = batches[b];
+        if (!x.reader) return fail(e, DBEEL_ERR_INVALID_ARG, "null reader");
+        if (x.reader->e != e) return fail(e, DBEEL_ERR_INVALID_ARG, "a reader of another engine");
+        if (x.mode > DBEEL_LOOKUP_EXACT) return fail(e, DBEEL_ERR_INVALID_ARG, "unknown lookup mode");
+        if (x.reserved) return fail(e, DBEEL_ERR_INVALID_ARG, "reserved is not 0");
+        if (!x.key_offsets) return fail(e, DBEEL_ERR_INVALID_ARG, "null key_offsets");
+        if (x.n_keys >= 0xFFFFFFF0ull - n_keys) return fail(e, DBEEL_ERR_INVALID_ARG, "2^32 - 16 keys or more");
+        if (!x.keys && x.key_offsets[x.n_keys] > x.key_offsets[0]) return fail(e, DBEEL_ERR_INVALID_ARG, "null keys with key bytes");
+        n_keys += x.n_keys;
+    }
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    e->stats = dbeel_stats{};
+    out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
+    std::vector<GvsBatch> bs(n_batches);
+    for (uint32_t b = 0; b < n_batches; b++) {
+        const dbeel_reader_batch &x = batches[b];
+        GvsBatch &B = bs[b];
+        B.r = x.reader;
+        B.io = &x.reader->io;
+        B.keys = static_cast<const uint8_t *>(x.keys);
+        B.key_off = x.key_offsets;
+        B.n_keys = x.n_keys;
+        B.mode = x.mode;
+        for (uint64_t q = 0; q < x.n_keys; q++) B.max_klen = std::max(B.max_klen, x.key_offsets[q + 1] - x.key_offsets[q]);
+        for (const ReaderTableRef &t : x.reader->tables) B.td.push_back(t->desc);
+    }
+    return gvs_walk(e, bs, out, results);
 }
 
 int dbeel_reader_scan(dbeel_reader *r, uint32_t kind, const void *ranges, uint32_t n_ranges,

@@ -195,19 +195,70 @@ inline void touched_leaves(const ProbeTree &pt, uint32_t t, const uint8_t *touch
 // index bytes plus table t's mean entry (ceil(data_len[t] / n[t]), 0 for an empty table), and 8 + max_klen for a probe
 // frame; with a page cache (paged), two more pages, as its slice and window each end in pages of their own.  A group
 // holds at least one leaf.  Group g is leaves [cut[g], cut[g + 1]) of the returned cut.
+inline uint64_t leaf_bytes(const TouchedLeaf &l, uint64_t n, uint64_t data_len, uint64_t max_klen, bool paged) {
+    return (l.b - l.a) * (16 + (n ? (data_len + n - 1) / n : 0)) + 8 + max_klen + (paged ? 2 * kPageBytes : 0);
+}
+
 inline std::vector<size_t> group_leaves(const std::vector<TouchedLeaf> &leaves, const std::vector<uint64_t> &n,
                                         const std::vector<uint64_t> &data_len, uint64_t max_klen, uint64_t group_bytes, bool paged) {
     std::vector<size_t> cut = {0};
     uint64_t est = 0;
     for (size_t k = 0; k < leaves.size(); k++) {
         const TouchedLeaf &l = leaves[k];
-        const uint64_t per_rec = 16 + (n[l.t] ? (data_len[l.t] + n[l.t] - 1) / n[l.t] : 0);
-        const uint64_t bytes = (l.b - l.a) * per_rec + 8 + max_klen + (paged ? 2 * kPageBytes : 0);
+        const uint64_t bytes = leaf_bytes(l, n[l.t], data_len[l.t], max_klen, paged);
         if (k > cut.back() && est + bytes > group_bytes) {
             cut.push_back(k);
             est = 0;
         }
         est += bytes;
+    }
+    if (!leaves.empty()) cut.push_back(leaves.size());
+    return cut;
+}
+
+// ---- batched reads across readers (dbeel_readers_get_values): one level of many (batch, table) pairs
+//
+// Pair p of a level: its table's n and data_len, its batch's longest key, and the page cache its leaves go through
+// (cache_bytes index, or -1 for none).  TouchedLeaf.t is the pair.
+struct LeafPair {
+    uint64_t n, data_len, max_klen;
+    int32_t cache;
+};
+
+// Cuts the touched leaves of a level, ascending pair, into groups.  Pair p's leaves are first cut exactly as its solo call
+// cuts them (group_leaves with the partition budget, or with min(budget, its cache's bytes) when paged): those units keep
+// every read of the pair inside the reads of its solo call, as the .index slices of a unit merge across the same gaps.
+// Whole units then fill groups in order while the group's estimate stays within `budget` and the leaves of each cache c
+// within cache_bytes[c]; a group holds at least one unit.
+inline std::vector<size_t> group_leaves(const std::vector<TouchedLeaf> &leaves, const std::vector<LeafPair> &pairs, uint64_t budget,
+                                        const std::vector<uint64_t> &cache_bytes) {
+    std::vector<size_t> cut = {0};
+    uint64_t est = 0;
+    std::vector<uint64_t> est_c(cache_bytes.size(), 0);
+    for (size_t k0 = 0; k0 < leaves.size();) {
+        const uint32_t p = leaves[k0].t;
+        const LeafPair &lp = pairs[p];
+        size_t k1 = k0;
+        while (k1 < leaves.size() && leaves[k1].t == p) k1++;
+        const bool paged = lp.cache >= 0;
+        const std::vector<uint64_t> n1 = {lp.n}, dl1 = {lp.data_len};
+        std::vector<TouchedLeaf> local(leaves.begin() + k0, leaves.begin() + k1);
+        for (TouchedLeaf &l : local) l.t = 0;
+        const std::vector<size_t> unit = group_leaves(local, n1, dl1, lp.max_klen,
+                                                      paged ? std::min(budget, cache_bytes[lp.cache]) : budget, paged);
+        for (size_t u = 0; u + 1 < unit.size(); u++) {
+            uint64_t bytes = 0;
+            for (size_t k = unit[u]; k < unit[u + 1]; k++) bytes += leaf_bytes(local[k], lp.n, lp.data_len, lp.max_klen, paged);
+            const size_t at = k0 + unit[u];
+            if (at > cut.back() && (est + bytes > budget || (paged && est_c[lp.cache] + bytes > cache_bytes[lp.cache]))) {
+                cut.push_back(at);
+                est = 0;
+                std::fill(est_c.begin(), est_c.end(), 0);
+            }
+            est += bytes;
+            if (paged) est_c[lp.cache] += bytes;
+        }
+        k0 = k1;
     }
     if (!leaves.empty()) cut.push_back(leaves.size());
     return cut;

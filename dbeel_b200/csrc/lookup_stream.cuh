@@ -1,10 +1,13 @@
-// lookup_stream.cuh -- dbeel_get_values_stream: the search of lookup.cuh on tables that are not on the device, only the parts
-// of them the batch's searches reach (host/lookup_plan.h).  Per table, newest first, for the queries still open:
+// lookup_stream.cuh -- dbeel_get_values_stream, dbeel_reader_get_values and dbeel_readers_get_values: the search of lookup.cuh
+// on tables that are not on the device, only the parts of them the batches' searches reach (host/lookup_plan.h).  The
+// queries of every batch run together, one level at a time: level j pairs each batch b with its own table T_b - 1 - j
+// (newest first), described by the level's GvsPair[b], and a query finds its pair through its batch id.  Per level, for the
+// queries still open:
 //
-//   k_gvs_filter   the table's bloom filter; an open query that passes starts its search at the root (node 1)
-//   k_lookup_fence the top D probes on the staged fences (index record + key frame per probe-tree node); ends in a hit, a
-//                  corrupt record, "not in this table", or a leaf (node 2^D + leaf) whose records are staged next
-//   k_lookup_leaf  resumes the search inside a staged leaf: the table's TableDesc with .index / .data biased to the slice and
+//   k_gvs_filter   the pair's bloom filter; an open query that passes starts its search at the root (node 1)
+//   k_lookup_fence the top D probes on the pair's staged fences (index record + key frame per probe-tree node); ends in a
+//                  hit, a corrupt record, "not in this table", or a leaf (node 2^D + leaf) whose records are staged next
+//   k_lookup_leaf  resumes the search inside a staged leaf: the pair's TableDesc with .index / .data biased to the slice and
 //                  the window, so probe() checks the same bounds against the file's data_len as k_lookup does
 //   k_gvs_copy     copies the entries of the group's hits out of the window into the hit heap before the window is reused
 //   k_page_copy    with a page cache attached to a reader: assembles the staged slices, windows and entries from its pages
@@ -22,6 +25,7 @@ namespace dbeel {
 struct GvsQueries {
     const uint8_t *keys;
     const uint64_t *key_off;
+    const uint32_t *batch; // the query's batch: its pair is the level's pairs[batch]
     uint64_t n_keys;
     uint4 *rows;          // {table, rejects | flags, record lo, record hi}; table = ~0 while not found
     uint4 *hit_ix;        // the hit's index record
@@ -29,7 +33,18 @@ struct GvsQueries {
     uint32_t *node;       // 0 = nothing to do in the current table, else its probe-tree node
     unsigned long long *hit_src; // a leaf hit's entry inside the staged window, until k_gvs_copy has copied it (else 0)
     unsigned long long *hit_off; // the entry's offset in the hit heap, kGvsNoEntry or kGvsFenceHit
-    uint32_t mode;
+};
+
+// One (batch, table) pair of a level.  t: the table (its filter in words; data / index unset); fences: per node
+// k < 2^depth the index record fix[k] and the device address of its key frame ffr[k] (0 = the probe reports the record
+// corrupt); touched[leaf] is set for every leaf a search ends in.  table: the table's position in its batch's tables.
+// live = 0: the batch has no table at this level.
+struct GvsPair {
+    TableDesc t;
+    const uint4 *fix;
+    const unsigned long long *ffr;
+    uint8_t *touched;
+    uint32_t depth, table, mode, live;
 };
 
 constexpr unsigned long long kGvsNoEntry = ~0ull;      // no hit, or a hit whose entry cannot decode
@@ -43,14 +58,18 @@ __host__ __device__ __forceinline__ bool gvs_entry_fits(uint64_t off, uint64_t k
 
 __device__ __forceinline__ bool gvs_closed(const uint4 &r) { return r.x != 0xFFFFFFFFu || (r.y & kLookupCorrupt); }
 
-__global__ void __launch_bounds__(256) k_gvs_filter(GvsQueries g, TableDesc t, unsigned long long *n_open) {
+// n_open[b]: the open queries of batch b that reach its table
+__global__ void __launch_bounds__(256) k_gvs_filter(GvsQueries g, const GvsPair *pairs, unsigned long long *n_open) {
     pdl_trigger();
     pdl_wait();
     const uint64_t q = (uint64_t)blockIdx.x * 256u + threadIdx.x;
     if (q >= g.n_keys) return;
     g.node[q] = 0;
+    const uint32_t b = g.batch[q];
+    if (!pairs[b].live) return;
     uint4 r = g.rows[q];
     if (gvs_closed(r)) return;
+    const TableDesc &t = pairs[b].t;
     const uint64_t k0 = g.key_off[q];
     const uint8_t *key = g.keys + k0;
     const uint64_t klen = g.key_off[q + 1] - k0;
@@ -71,13 +90,12 @@ __global__ void __launch_bounds__(256) k_gvs_filter(GvsQueries g, TableDesc t, u
         }
     }
     if (t.n == 0) return;
-    g.state[q] = search_init(g.mode, t.n);
+    g.state[q] = search_init(pairs[b].mode, t.n);
     g.node[q] = 1;
-    atomicAdd(n_open, 1ull);
+    atomicAdd(&n_open[b], 1ull);
 }
 
-// fences: per node k < 2^depth the index record fix[k] and the device address of its key frame ffr[k] (0 = the probe
-// reports the record corrupt); touched[leaf] is set for every leaf a search ends in.
+// One table's fences as GvsPair holds them, for k_seek_fence (scan_seek.cuh).
 struct GvsFences {
     const uint4 *fix;
     const unsigned long long *ffr;
@@ -87,13 +105,16 @@ struct GvsFences {
     uint8_t *touched;
 };
 
-__global__ void __launch_bounds__(256) k_lookup_fence(GvsQueries g, GvsFences f) {
+__global__ void __launch_bounds__(256) k_lookup_fence(GvsQueries g, const GvsPair *pairs) {
     pdl_trigger();
     pdl_wait();
     const uint64_t q = (uint64_t)blockIdx.x * 256u + threadIdx.x;
     if (q >= g.n_keys) return;
     uint32_t node = g.node[q];
     if (node == 0) return;
+    const GvsPair &f = pairs[g.batch[q]];
+    const uint32_t mode = f.mode;
+    const uint64_t n = f.t.n;
     const uint64_t k0 = g.key_off[q];
     const uint8_t *key = g.keys + k0;
     const uint64_t klen = g.key_off[q + 1] - k0;
@@ -101,7 +122,7 @@ __global__ void __launch_bounds__(256) k_lookup_fence(GvsQueries g, GvsFences f)
     const uint32_t leaf0 = 1u << f.depth;
     while (node < leaf0) {
         const unsigned long long fr = f.ffr[node];
-        const uint64_t pos = search_pos(g.mode, s);
+        const uint64_t pos = search_pos(mode, s);
         if (fr == 0) { // as probe(): offset or length prefix past the end of .data
             g.rows[q].y |= kLookupCorrupt;
             node = 0;
@@ -117,7 +138,7 @@ __global__ void __launch_bounds__(256) k_lookup_fence(GvsQueries g, GvsFences f)
             node = 0;
             break;
         }
-        search_step(g.mode, f.n, &s, c);
+        search_step(mode, n, &s, c);
         if (s.done) { node = 0; break; }
         node = 2 * node + (c < 0 ? 1u : 0u);
     }
@@ -128,8 +149,8 @@ __global__ void __launch_bounds__(256) k_lookup_fence(GvsQueries g, GvsFences f)
     }
 }
 
-// The staged leaves of one group, ascending leaf ids; data / index are biased so that file offset o / record r of the table
-// are at data + o / index + r.
+// The staged leaves of one group, ascending (pair, leaf); data / index are biased so that file offset o / record r of the
+// pair's table are at data + o / index + r.
 struct GvsLeaf {
     const uint8_t *data;
     const uint4 *index;
@@ -139,21 +160,27 @@ struct GvsLeaf {
 
 // A hit whose entry fits (gvs_entry_fits) leaves its window address in hit_src and adds the heap bytes k_gvs_copy will
 // take for it to *heap_need.
-__global__ void __launch_bounds__(256) k_lookup_leaf(GvsQueries g, TableDesc t, const GvsLeaf *leaves, uint32_t n_leaves,
-                                                     uint32_t depth, uint32_t table, unsigned long long *heap_need) {
+// Pair b's leaves are leaves[first[b] .. first[b + 1]).
+__global__ void __launch_bounds__(256) k_lookup_leaf(GvsQueries g, const GvsPair *pairs, const GvsLeaf *leaves, const uint32_t *first,
+                                                     unsigned long long *heap_need) {
     pdl_trigger();
     pdl_wait();
     const uint64_t q = (uint64_t)blockIdx.x * 256u + threadIdx.x;
     if (q >= g.n_keys) return;
-    const uint32_t node = g.node[q], leaf0 = 1u << depth;
+    const uint32_t node = g.node[q];
+    if (node == 0) return;
+    const uint32_t b = g.batch[q];
+    const GvsPair &p = pairs[b];
+    const uint32_t leaf0 = 1u << p.depth, mode = p.mode;
     if (node < leaf0) return;
     const uint32_t leaf = node - leaf0;
-    uint32_t lo = 0, hi = n_leaves; // the group's leaf, if it holds it
+    uint32_t lo = first[b], hi = first[b + 1]; // the group's leaf, if it holds it
     while (lo < hi) {
         const uint32_t mid = (lo + hi) / 2;
         if (leaves[mid].leaf < leaf) lo = mid + 1; else hi = mid;
     }
-    if (lo == n_leaves || leaves[lo].leaf != leaf) return;
+    if (lo == first[b + 1] || leaves[lo].leaf != leaf) return;
+    TableDesc t = p.t;
     t.data = leaves[lo].data;
     t.index = leaves[lo].index;
     const uint64_t k0 = g.key_off[q];
@@ -163,7 +190,7 @@ __global__ void __launch_bounds__(256) k_lookup_leaf(GvsQueries g, TableDesc t, 
     bool bad = false;
     while (!s.done) {
         uint4 ix;
-        const uint64_t pos = search_pos(g.mode, s);
+        const uint64_t pos = search_pos(mode, s);
         const int c = probe(t, pos, key, klen, &bad, &ix);
         if (bad) {
             g.rows[q].y |= kLookupCorrupt;
@@ -171,7 +198,7 @@ __global__ void __launch_bounds__(256) k_lookup_leaf(GvsQueries g, TableDesc t, 
         }
         if (c == 0) {
             const uint4 r = g.rows[q];
-            g.rows[q] = make_uint4(table, r.y, (uint32_t)pos, (uint32_t)(pos >> 32));
+            g.rows[q] = make_uint4(p.table, r.y, (uint32_t)pos, (uint32_t)(pos >> 32));
             g.hit_ix[q] = ix;
             const uint64_t off = (uint64_t)ix.x | ((uint64_t)ix.y << 32), fs = ix.w;
             if (gvs_entry_fits(off, ix.z, fs, klen, t.data_len)) { // the window covers [off, off + fs) (lookup_plan.h)
@@ -180,7 +207,7 @@ __global__ void __launch_bounds__(256) k_lookup_leaf(GvsQueries g, TableDesc t, 
             }
             break;
         }
-        search_step(g.mode, t.n, &s, c);
+        search_step(mode, t.n, &s, c);
     }
     g.node[q] = 0;
 }

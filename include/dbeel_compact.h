@@ -483,6 +483,42 @@ int dbeel_reader_open(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tab
 int dbeel_reader_get_values(dbeel_reader *r, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
                             dbeel_out *out, dbeel_lookup_result *results);
 
+/* Batched reads across readers: the point-read batches of many readers (a node's shards and collections, each a tree) in
+ * one call.  Batch b asks batches[b].reader for n_keys keys (keys / key_offsets as for dbeel_reader_get_values) in its own
+ * mode (DBEEL_LOOKUP_REFERENCE or DBEEL_LOOKUP_EXACT); reserved must be 0.  A reader may appear in several batches, and a
+ * batch may have no keys.
+ * Result: exactly dbeel_reader_get_values(batches[b].reader, ...) for b = 0, 1, ... in order, concatenated.  results has
+ * sum(n_keys) rows in batch order; a row's table is a position in its own reader's tables; the flags and bloom_rejects are
+ * the solo call's, on damaged tables too, and one batch's damage or misses never change another batch's rows.  out packs
+ * the answered entries in row order as dbeel_get_values packs them: batch b's .data / .index are its solo call's output,
+ * appended, its .index offsets shifted by the .data bytes before it; items_written is the total.
+ * Reads: the batches run together one table level at a time (level j: every batch's table T_b - 1 - j, newest first), so a
+ * level costs one filter, fence and touched-leaf pass for all batches, not one per batch.  Each (batch, table) pair makes
+ * its solo call's decisions: cached or per-call fences and their depth, from that batch's longest key and open queries.
+ * Every read goes through the pair's own reader's io->read and page cache, and lies inside what the solo calls, made in
+ * batch order on readers in the same state, read for that table and file kind: a pair's leaves are loaded in the groups
+ * its solo call cuts, and groups of different pairs share a load while they fit the partition budget and each page
+ * cache's capacity.  With no page cache, input_bytes is at most the sum of the solo calls'.  A cache whose leaves of one
+ * group do not fit it reads them uncached, as a solo call does.
+ * Errors leave every reader, the engine and every page cache usable: DBEEL_ERR_INVALID_ARG for null batches / out /
+ * results or a null reader, a reader of another engine, n_batches of 0 or above DBEEL_MAX_READER_BATCHES, an unknown mode
+ * or nonzero reserved, a null key_offsets, null keys with key bytes, or sum(n_keys) >= 2^32 - 16; DBEEL_ERR_CAPACITY as
+ * dbeel_get_values (every row filled, out->data_len / index_len = the sizes needed for the whole call, nothing written);
+ * a callback's nonzero return unchanged; DBEEL_ERR_BUSY while another call runs on the engine.
+ * dbeel_last_stats: input_bytes = every byte read through every reader's callback, entries_in = sum(n_keys),
+ * entries_out / output_bytes = what was returned, partitions = leaf groups run, kernel_launches summed over the call. */
+#define DBEEL_MAX_READER_BATCHES 1024u
+typedef struct dbeel_reader_batch {
+    dbeel_reader *reader;
+    const void *keys;            /* as dbeel_reader_get_values */
+    const uint64_t *key_offsets; /* n_keys + 1 byte offsets */
+    uint64_t n_keys;
+    uint32_t mode;               /* DBEEL_LOOKUP_REFERENCE or DBEEL_LOOKUP_EXACT, per batch */
+    uint32_t reserved;           /* 0 */
+} dbeel_reader_batch;
+int dbeel_readers_get_values(dbeel_engine *e, const dbeel_reader_batch *batches, uint32_t n_batches, dbeel_out *out,
+                             dbeel_lookup_result *results);
+
 /* Range scans on a reader: dbeel_scan_stream's call on the reader's tables (a snapshot: a tree reader keeps its tables'
  * files open while the tree flushes and compacts).  kind / ranges / n_ranges / results / stop mean what they mean for
  * dbeel_scan_stream, with its argument checks and limits (kind, 1 <= n_ranges <= DBEEL_MAX_SCAN_RANGES, a non-null write,
