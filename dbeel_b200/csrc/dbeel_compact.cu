@@ -29,7 +29,6 @@
 #include "lookup_stream.cuh"
 #include "route.cuh"
 #include "scan.cuh"
-#include "scan_seek.cuh"
 #include "wal.cuh"
 #include "host/page_cache.h"
 #include "host/reader_tables.h"
@@ -2532,13 +2531,12 @@ struct LeafSrc {
     uint64_t data_len, max_klen;
 };
 
-// One group of touched leaves (group_leaves), ascending (part, leaf), on the device for k_lookup_leaf / k_seek_leaf: per
+// One group of touched leaves (group_leaves), ascending (part, leaf), on the device for k_lookup_leaf: per
 // part its index slices into stage_in behind the header (through ring_in, and back to it), then the .data windows of
 // those slices (leaf_window) into stage_in2 (through ring_out).  The header at stage_in is GvsLeaf[nl] | first[nt + 1]
 // (nt = src.size()): part t's leaves are [first[t], first[t + 1]), each biased so that record r of the table lies
 // at index + r and file offset o at data + o (a leaf whose records all point past the file never dereferences data:
-// probe() reports them corrupt first).  Through gvs_load, so with a page cache this writes stage_out: reader_scan_key's
-// per-call fences live there, and its k_seek_fence has completed (a synchronise) before the first group is loaded.
+// probe() reports them corrupt first).  Through gvs_load, so with a page cache this also writes stage_out.
 int gvs_load_leaves(dbeel_engine *e, const std::vector<LeafSrc> &src, const TouchedLeaf *lv, uint32_t nl) {
     const uint32_t nt = (uint32_t)src.size();
     std::vector<uint32_t> first(nt + 1, 0);
@@ -2608,13 +2606,168 @@ struct GvsBatch {
     uint32_t mode = 0;
 };
 
+// The hit heap (stage_out2) holds every answered entry of a walk until split_emit gathers them; it grows to `need` bytes
+// keeping the `keep` it holds.
+int gvs_heap_reserve(dbeel_engine *e, uint64_t need, uint64_t keep) {
+    if (need <= e->stage_out2_cap) return DBEEL_OK;
+    uint8_t *old = e->stage_out2;
+    const uint64_t old_cap = e->stage_out2_cap;
+    e->stage_out2 = nullptr;
+    e->stage_out2_cap = 0;
+    int rc = ensure_device(e, &e->stage_out2, &e->stage_out2_cap, need);
+    if (!rc && old && keep) CU(cudaMemcpyAsync(e->stage_out2, old, std::min(old_cap, keep), cudaMemcpyDeviceToDevice, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    if (old) cudaFree(old);
+    return rc;
+}
+
+// What the levels of a walk share: its queries on the device, where a level's pairs and touched flags go (the pairs go
+// down from e->pin + p_pairs, the touched flags come back to e->pin), the leaf kernel's heap counter and the hit heap.
+struct GvsLevel {
+    GvsQueries gq;
+    uint32_t grid;
+    GvsPair *d_pairs;
+    uint8_t *d_touched;
+    uint64_t p_pairs;
+    unsigned long long *d_need, *d_cursor;
+    uint64_t heap_bound = 0; // the heap bytes the copies so far may have used
+    uint32_t launches = 0, groups = 0;
+};
+
+// One level of a walk, from its pairs with their open-query counts known to its last leaf group.  A live pair whose pts[p]
+// the caller has set has its fences (depth, fix, ffr) chosen; the others choose here from count[p] open queries (0: the
+// pair is dropped): the reader table's cached fences when they serve the queries (reader_uses_cache), else fences read
+// for this call into one image in stage_in.  Then one k_lookup_fence, one read-back of the touched leaves, and the leaves
+// in groups (group_leaves over pairs, each reader's page cache a cache of its own), each with one k_lookup_leaf and, when
+// the group's hits need heap bytes, one k_gvs_copy that moves their entries out of the window before it is reused.
+// src[p]: where pair p's leaves come from.  Every phase ends in a stream synchronise before its pinned buffers are refilled.
+template <bool kSeek>
+int gvs_level(dbeel_engine *e, GvsLevel &L, std::vector<GvsPair> &pairs, const std::vector<LeafSrc> &src, const std::vector<uint64_t> &count,
+              std::vector<const ProbeTree *> &pts) {
+    cudaStream_t s = e->stream;
+    const uint64_t budget = e->partition_bytes;
+    const uint32_t np = (uint32_t)pairs.size();
+    int rc;
+    // ---- fences: the index records of the open internal nodes, then their key frames (or the reader's copies)
+    std::vector<ProbeTree> pt_call(np);
+    std::vector<GvsFenceReads> frs(np);
+    std::vector<uint64_t> img_at(np, ~0ull), touched_at(np);
+    uint64_t img_bytes = 0, tbytes = 0;
+    bool any = false, any_fence = false;
+    for (uint32_t b = 0; b < np; b++) {
+        const LeafSrc &S = src[b];
+        GvsPair &P = pairs[b];
+        if (!P.live) continue;
+        if (!pts[b]) {
+            const uint64_t m = count[b];
+            if (m == 0) { // no query reaches the table: nothing of it is read
+                P.live = 0;
+                continue;
+            }
+            const uint32_t ti = P.table;
+            dbeel_reader_table *rt = S.r ? S.r->tables[ti].get() : nullptr;
+            dbeel_reader_table::Fences *cache = rt ? &rt->fences[P.mode] : nullptr;
+            const uint32_t cd = rt ? (uint32_t)rt->depth : 0;
+            uint32_t depth = lookup_depth(m, P.t.n, P.t.data_len, 8 + S.max_klen, budget);
+            if (cache && reader_uses_cache(S.max_klen, depth, cd)) {
+                depth = cd;
+                if (!cache->loaded) {
+                    if ((rc = reader_load_fences(e, S.io, ti, rt, P.mode))) return rc;
+                    CU(cudaStreamSynchronize(s)); // its image goes down from ring_out, which the next pair refills
+                }
+                pts[b] = &cache->pt;
+                P.fix = reinterpret_cast<const uint4 *>(cache->dev);
+                P.ffr = reinterpret_cast<const unsigned long long *>(cache->dev + (16ull << cd));
+            } else {
+                plan_probe_tree(P.mode, P.t.n, depth, &pt_call[b]);
+                pts[b] = &pt_call[b];
+                if (depth > 0) {
+                    if ((rc = gvs_read_fences(e, S.io, ti, pt_call[b], P.t.data_len, S.max_klen, &frs[b]))) return rc;
+                    img_at[b] = align_up(img_bytes, kAlign);
+                    img_bytes = img_at[b] + frs[b].image_bytes();
+                }
+            }
+            P.depth = depth;
+        }
+        touched_at[b] = tbytes;
+        P.touched = L.d_touched + tbytes;
+        tbytes += 1ull << P.depth;
+        any = true;
+        any_fence = any_fence || P.depth > 0;
+    }
+    if (!any) return DBEEL_OK;
+    if (img_bytes) {
+        if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, img_bytes))) return rc;
+        if ((rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, img_bytes))) return rc;
+        for (uint32_t b = 0; b < np; b++) {
+            if (img_at[b] == ~0ull) continue;
+            gvs_fence_image(frs[b], pairs[b].t.data_len, e->ring_in + img_at[b], e->stage_in + img_at[b]);
+            pairs[b].fix = reinterpret_cast<const uint4 *>(e->stage_in + img_at[b]);
+            pairs[b].ffr = reinterpret_cast<const unsigned long long *>(e->stage_in + img_at[b] + (16ull << pairs[b].depth));
+        }
+        CU(cudaMemcpyAsync(e->stage_in, e->ring_in, img_bytes, cudaMemcpyHostToDevice, s));
+    }
+    CU(cudaMemsetAsync(L.d_touched, 0, tbytes, s));
+    for (uint32_t b = 0; b < np; b++)
+        if (pairs[b].live && pairs[b].depth == 0) CU(cudaMemsetAsync(L.d_touched + touched_at[b], 1, 1, s));
+    memcpy(e->pin + L.p_pairs, pairs.data(), sizeof(GvsPair) * np);
+    CU(cudaMemcpyAsync(L.d_pairs, e->pin + L.p_pairs, sizeof(GvsPair) * np, cudaMemcpyHostToDevice, s));
+    if (any_fence) {
+        launch_k(e, k_lookup_fence<kSeek>, L.grid, 256, 0, s, L.gq, static_cast<const GvsPair *>(L.d_pairs));
+        L.launches++;
+    }
+    CU(cudaMemcpyAsync(e->pin, L.d_touched, tbytes, cudaMemcpyDeviceToHost, s));
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(s));
+
+    // ---- leaves, in groups of about `budget` bytes (with page caches, each cache's leaves at most its capacity)
+    std::vector<uint64_t> cache_bytes;
+    std::vector<dbeel_page_cache *> caches;
+    std::vector<TouchedLeaf> lv;
+    std::vector<LeafPair> lp(np);
+    for (uint32_t b = 0; b < np; b++) {
+        const GvsPair &P = pairs[b];
+        dbeel_page_cache *c = src[b].r ? src[b].r->cache : nullptr;
+        int32_t ci = -1;
+        if (c) {
+            ci = (int32_t)(std::find(caches.begin(), caches.end(), c) - caches.begin());
+            if (ci == (int32_t)caches.size()) {
+                caches.push_back(c);
+                cache_bytes.push_back(kPageBytes * c->pc.capacity());
+            }
+        }
+        lp[b] = LeafPair{P.t.n, P.t.data_len, src[b].max_klen, ci};
+        if (P.live) touched_leaves(*pts[b], b, e->pin + touched_at[b], &lv);
+    }
+    const std::vector<size_t> cut = group_leaves(lv, lp, budget, cache_bytes);
+    for (size_t gi = 0; gi + 1 < cut.size(); gi++) {
+        const uint32_t nl = (uint32_t)(cut[gi + 1] - cut[gi]);
+        if ((rc = gvs_load_leaves(e, src, lv.data() + cut[gi], nl))) return rc;
+        CU(cudaMemsetAsync(L.d_need, 0, 8, s));
+        launch_k(e, k_lookup_leaf<kSeek>, L.grid, 256, 0, s, L.gq, static_cast<const GvsPair *>(L.d_pairs),
+                 reinterpret_cast<const GvsLeaf *>(e->stage_in), reinterpret_cast<const uint32_t *>(e->stage_in + sizeof(GvsLeaf) * nl), L.d_need);
+        CU(cudaMemcpyAsync(e->pin, L.d_need, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaGetLastError());
+        CU(cudaStreamSynchronize(s));
+        L.launches++;
+        if (const uint64_t need = rd64(e->pin)) { // the group's hits leave the window for the heap before it is reused
+            if ((rc = gvs_heap_reserve(e, L.heap_bound + need, L.heap_bound))) return rc;
+            L.heap_bound += need;
+            launch_k(e, k_gvs_copy, (uint32_t)((32 * L.gq.n_keys + 255) / 256), 256, 0, s, L.gq, e->stage_out2, L.d_cursor);
+            CU(cudaGetLastError());
+            CU(cudaStreamSynchronize(s));
+            L.launches++;
+        }
+        L.groups++;
+    }
+    return DBEEL_OK;
+}
+
 // The batches' searches, one level at a time: level j pairs every batch b with its table T_b - 1 - j (newest first).  Per
 // level, for all pairs together: one k_gvs_filter; one read-back of the pairs' open-query counts when some pair's fence
-// decision needs it; the per-call fences of the pairs that need them in one image, and one k_lookup_fence; one read-back of
-// the touched leaves; then the leaves in groups (group_leaves over pairs), k_lookup_leaf per group and k_gvs_copy for the
-// group's hits (their entries leave the window for the hit heap).  Then the entries of hits at fences are read into the
-// heap, k_gvs_hit decodes every hit and split_emit writes `out` in query order, as dbeel_get_values does.  Every phase ends
-// in a stream synchronise before its pinned buffers are refilled.
+// decision needs it; then gvs_level.  Then the entries of hits at fences are read into the heap, k_gvs_hit decodes every
+// hit and split_emit writes `out` in query order, as dbeel_get_values does.  Every phase ends in a stream synchronise
+// before its pinned buffers are refilled.
 // Each pair's decisions are its batch's solo call's: a reader table whose cached fences serve the batch
 // (reader_uses_cache) descends them instead of reading its fences; when the depth the batch wants cannot exceed the cached
 // one for any number of open queries, the decision is made before the filter and needs no count.
@@ -2705,66 +2858,36 @@ int gvs_walk(dbeel_engine *e, const std::vector<GvsBatch> &bs, dbeel_out *out, d
                   reinterpret_cast<uint4 *>(ws + o_rows), reinterpret_cast<uint4 *>(ws + o_hix), reinterpret_cast<SearchState *>(ws + o_state),
                   reinterpret_cast<uint32_t *>(ws + o_node), reinterpret_cast<unsigned long long *>(ws + o_src),
                   reinterpret_cast<unsigned long long *>(ws + o_hoff)};
-    unsigned long long *d_need = reinterpret_cast<unsigned long long *>(ws + o_need), *d_cursor = reinterpret_cast<unsigned long long *>(ws + o_cursor);
-    // The hit heap (stage_out2) holds every answered entry until split_emit gathers them; it grows keeping what it holds.
-    uint64_t heap_bound = 0;
-    auto heap_reserve = [&](uint64_t need) -> int {
-        if (need <= e->stage_out2_cap) return DBEEL_OK;
-        uint8_t *old = e->stage_out2;
-        const uint64_t old_cap = e->stage_out2_cap;
-        e->stage_out2 = nullptr;
-        e->stage_out2_cap = 0;
-        int rc2 = ensure_device(e, &e->stage_out2, &e->stage_out2_cap, need);
-        if (!rc2 && old && heap_bound) CU(cudaMemcpyAsync(e->stage_out2, old, std::min(old_cap, heap_bound), cudaMemcpyDeviceToDevice, s));
-        CU(cudaStreamSynchronize(s));
-        if (old) cudaFree(old);
-        return rc2;
-    };
+    GvsLevel L{gq, (n + 255) / 256, reinterpret_cast<GvsPair *>(ws + o_pairs), ws + o_touched, p_pairs,
+               reinterpret_cast<unsigned long long *>(ws + o_need), reinterpret_cast<unsigned long long *>(ws + o_cursor)};
     unsigned long long *d_cnt = reinterpret_cast<unsigned long long *>(ws + o_cnt);
-    uint8_t *d_touched = ws + o_touched;
-    GvsPair *d_pairs = reinterpret_cast<GvsPair *>(ws + o_pairs);
-    const uint32_t grid = (n + 255) / 256;
-    uint32_t launches = 0, groups = 0;
-    // the page caches of the batches' readers (group_leaves over pairs keeps each one's leaves within its capacity)
-    std::vector<dbeel_page_cache *> caches;
-    std::vector<uint64_t> cache_bytes;
-    std::vector<int32_t> cache_of(nb, -1);
-    for (uint32_t b = 0; b < nb; b++) {
-        dbeel_page_cache *c = bs[b].r ? bs[b].r->cache : nullptr;
-        if (!c) continue;
-        const size_t ci = std::find(caches.begin(), caches.end(), c) - caches.begin();
-        if (ci == caches.size()) {
-            caches.push_back(c);
-            cache_bytes.push_back(kPageBytes * c->pc.capacity());
-        }
-        cache_of[b] = (int32_t)ci;
-    }
 
     std::vector<GvsPair> pairs(nb);
-    std::vector<ProbeTree> pt_call(nb);
-    std::vector<const ProbeTree *> pts(nb);
-    std::vector<uint64_t> touched_at(nb);
+    std::vector<LeafSrc> src(nb);
+    std::vector<uint64_t> count(nb);
     for (uint32_t j = 0; j < levels; j++) {
         // ---- the filter, with the decisions that need no count of open queries: the depth the batch wants grows with
         // that count, which is at most its n_keys
-        std::vector<uint8_t> decided(nb, 0);
+        std::vector<const ProbeTree *> pts(nb, nullptr);
         bool need_count = false;
         for (uint32_t b = 0; b < nb; b++) {
             const GvsBatch &B = bs[b];
             GvsPair &P = pairs[b];
             P = GvsPair{};
             P.mode = B.mode;
+            src[b] = LeafSrc{B.r, B.io, 0, 0, B.max_klen};
             if (!B.n_keys || j >= B.td.size()) continue;
             const uint32_t ti = (uint32_t)B.td.size() - 1 - j;
             P.t = B.td[ti];
             P.table = ti;
             P.live = 1;
+            src[b].table = ti;
+            src[b].data_len = P.t.data_len;
             dbeel_reader_table *rt = B.r ? B.r->tables[ti].get() : nullptr;
             dbeel_reader_table::Fences *cache = rt ? &rt->fences[B.mode] : nullptr;
             const uint32_t cd = rt ? (uint32_t)rt->depth : 0;
             if (cache && cache->loaded && cd > 0 &&
                 reader_uses_cache(B.max_klen, lookup_depth(B.n_keys, P.t.n, P.t.data_len, 8 + B.max_klen, budget), cd)) {
-                decided[b] = 1;
                 P.depth = cd;
                 pts[b] = &cache->pt;
                 P.fix = reinterpret_cast<const uint4 *>(cache->dev);
@@ -2774,118 +2897,16 @@ int gvs_walk(dbeel_engine *e, const std::vector<GvsBatch> &bs, dbeel_out *out, d
             }
         }
         memcpy(e->pin + p_fpairs, pairs.data(), sizeof(GvsPair) * nb);
-        CU(cudaMemcpyAsync(d_pairs, e->pin + p_fpairs, sizeof(GvsPair) * nb, cudaMemcpyHostToDevice, s));
+        CU(cudaMemcpyAsync(L.d_pairs, e->pin + p_fpairs, sizeof(GvsPair) * nb, cudaMemcpyHostToDevice, s));
         CU(cudaMemsetAsync(d_cnt, 0, 8ull * nb, s));
-        launch_k(e, k_gvs_filter, grid, 256, 0, s, gq, static_cast<const GvsPair *>(d_pairs), d_cnt);
-        launches++;
+        launch_k(e, k_gvs_filter, L.grid, 256, 0, s, gq, static_cast<const GvsPair *>(L.d_pairs), d_cnt);
+        L.launches++;
         if (need_count) {
             CU(cudaMemcpyAsync(e->pin + p_cnt, d_cnt, 8ull * nb, cudaMemcpyDeviceToHost, s));
             CU(cudaStreamSynchronize(s));
+            memcpy(count.data(), e->pin + p_cnt, 8ull * nb);
         }
-
-        // ---- the other decisions; fences: the index records of the open internal nodes, then their key frames (or the
-        // reader's copies)
-        std::vector<GvsFenceReads> frs(nb);
-        std::vector<uint64_t> img_at(nb, ~0ull);
-        uint64_t img_bytes = 0, tbytes = 0;
-        bool any = false, any_fence = false;
-        for (uint32_t b = 0; b < nb; b++) {
-            const GvsBatch &B = bs[b];
-            GvsPair &P = pairs[b];
-            if (!P.live) continue;
-            if (!decided[b]) {
-                const uint64_t m = rd64(e->pin + p_cnt + 8ull * b);
-                if (m == 0) { // no query reaches the table: nothing of it is read
-                    P.live = 0;
-                    continue;
-                }
-                const uint32_t ti = P.table;
-                dbeel_reader_table *rt = B.r ? B.r->tables[ti].get() : nullptr;
-                dbeel_reader_table::Fences *cache = rt ? &rt->fences[B.mode] : nullptr;
-                const uint32_t cd = rt ? (uint32_t)rt->depth : 0;
-                uint32_t depth = lookup_depth(m, P.t.n, P.t.data_len, 8 + B.max_klen, budget);
-                if (cache && reader_uses_cache(B.max_klen, depth, cd)) {
-                    depth = cd;
-                    if (!cache->loaded) {
-                        if ((rc = reader_load_fences(e, B.io, ti, rt, B.mode))) return rc;
-                        CU(cudaStreamSynchronize(s)); // its image goes down from ring_out, which the next pair refills
-                    }
-                    pts[b] = &cache->pt;
-                    P.fix = reinterpret_cast<const uint4 *>(cache->dev);
-                    P.ffr = reinterpret_cast<const unsigned long long *>(cache->dev + (16ull << cd));
-                } else {
-                    plan_probe_tree(B.mode, P.t.n, depth, &pt_call[b]);
-                    pts[b] = &pt_call[b];
-                    if (depth > 0) {
-                        if ((rc = gvs_read_fences(e, B.io, ti, pt_call[b], P.t.data_len, B.max_klen, &frs[b]))) return rc;
-                        img_at[b] = align_up(img_bytes, kAlign);
-                        img_bytes = img_at[b] + frs[b].image_bytes();
-                    }
-                }
-                P.depth = depth;
-            }
-            touched_at[b] = tbytes;
-            P.touched = d_touched + tbytes;
-            tbytes += 1ull << P.depth;
-            any = true;
-            any_fence = any_fence || P.depth > 0;
-        }
-        if (!any) continue;
-        if (img_bytes) {
-            if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, img_bytes))) return rc;
-            if ((rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, img_bytes))) return rc;
-            for (uint32_t b = 0; b < nb; b++) {
-                if (img_at[b] == ~0ull) continue;
-                gvs_fence_image(frs[b], pairs[b].t.data_len, e->ring_in + img_at[b], e->stage_in + img_at[b]);
-                pairs[b].fix = reinterpret_cast<const uint4 *>(e->stage_in + img_at[b]);
-                pairs[b].ffr = reinterpret_cast<const unsigned long long *>(e->stage_in + img_at[b] + (16ull << pairs[b].depth));
-            }
-            CU(cudaMemcpyAsync(e->stage_in, e->ring_in, img_bytes, cudaMemcpyHostToDevice, s));
-        }
-        CU(cudaMemsetAsync(d_touched, 0, tbytes, s));
-        for (uint32_t b = 0; b < nb; b++)
-            if (pairs[b].live && pairs[b].depth == 0) CU(cudaMemsetAsync(d_touched + touched_at[b], 1, 1, s));
-        memcpy(e->pin + p_pairs, pairs.data(), sizeof(GvsPair) * nb);
-        CU(cudaMemcpyAsync(d_pairs, e->pin + p_pairs, sizeof(GvsPair) * nb, cudaMemcpyHostToDevice, s));
-        if (any_fence) {
-            launch_k(e, k_lookup_fence, grid, 256, 0, s, gq, static_cast<const GvsPair *>(d_pairs));
-            launches++;
-        }
-        CU(cudaMemcpyAsync(e->pin, d_touched, tbytes, cudaMemcpyDeviceToHost, s));
-        CU(cudaGetLastError());
-        CU(cudaStreamSynchronize(s));
-
-        // ---- leaves, in groups of about `budget` bytes (with page caches, each cache's leaves at most its capacity)
-        std::vector<TouchedLeaf> lv;
-        std::vector<LeafPair> lp(nb);
-        std::vector<LeafSrc> src(nb);
-        for (uint32_t b = 0; b < nb; b++) {
-            const GvsPair &P = pairs[b];
-            lp[b] = LeafPair{P.t.n, P.t.data_len, bs[b].max_klen, cache_of[b]};
-            src[b] = LeafSrc{bs[b].r, bs[b].io, P.table, P.t.data_len, bs[b].max_klen};
-            if (P.live) touched_leaves(*pts[b], b, e->pin + touched_at[b], &lv);
-        }
-        const std::vector<size_t> cut = group_leaves(lv, lp, budget, cache_bytes);
-        for (size_t gi = 0; gi + 1 < cut.size(); gi++) {
-            const uint32_t nl = (uint32_t)(cut[gi + 1] - cut[gi]);
-            if ((rc = gvs_load_leaves(e, src, lv.data() + cut[gi], nl))) return rc;
-            CU(cudaMemsetAsync(d_need, 0, 8, s));
-            launch_k(e, k_lookup_leaf, grid, 256, 0, s, gq, static_cast<const GvsPair *>(d_pairs), reinterpret_cast<const GvsLeaf *>(e->stage_in),
-                     reinterpret_cast<const uint32_t *>(e->stage_in + sizeof(GvsLeaf) * nl), d_need);
-            CU(cudaMemcpyAsync(e->pin, d_need, 8, cudaMemcpyDeviceToHost, s));
-            CU(cudaGetLastError());
-            CU(cudaStreamSynchronize(s));
-            launches++;
-            if (const uint64_t need = rd64(e->pin)) { // the group's hits leave the window for the heap before it is reused
-                if ((rc = heap_reserve(heap_bound + need))) return rc;
-                heap_bound += need;
-                launch_k(e, k_gvs_copy, (uint32_t)((32 * n_keys + 255) / 256), 256, 0, s, gq, e->stage_out2, d_cursor);
-                CU(cudaGetLastError());
-                CU(cudaStreamSynchronize(s));
-                launches++;
-            }
-            groups++;
-        }
+        if ((rc = gvs_level<false>(e, L, pairs, src, count, pts))) return rc;
     }
 
     // ---- hits at fences: their entries, one record each (runs that touch as one read), per pair into the heap behind
@@ -2915,7 +2936,7 @@ int gvs_walk(dbeel_engine *e, const std::vector<GvsBatch> &bs, dbeel_out *out, d
             any_fence_hit = any_fence_hit || hoff[q] == kGvsFenceHit;
         }
     if (any_fence_hit) {
-        const uint64_t base = align_up(heap_bound, kAlign);
+        const uint64_t base = align_up(L.heap_bound, kAlign);
         std::vector<GvsStaged> sh(pair0[nb]);
         std::vector<GvsPart> parts;
         uint64_t staged = 0;
@@ -2927,7 +2948,7 @@ int gvs_walk(dbeel_engine *e, const std::vector<GvsBatch> &bs, dbeel_out *out, d
                 if (!x.runs.empty()) parts.push_back(GvsPart{i, &x, bs[b].r, bs[b].io});
             }
         if ((rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, std::max<uint64_t>(staged, 256)))) return rc;
-        if ((rc = heap_reserve(base + staged + 256))) return rc;
+        if ((rc = gvs_heap_reserve(e, base + staged + 256, L.heap_bound))) return rc;
         if ((rc = gvs_load(e, DBEEL_STREAM_DATA, parts, e->ring_in, e->stage_out2 + base, 0, staged, false, "stream read callback failed (.data, entries)")))
             return rc;
         for (uint32_t b = 0; b < nb; b++)
@@ -2945,13 +2966,13 @@ int gvs_walk(dbeel_engine *e, const std::vector<GvsBatch> &bs, dbeel_out *out, d
     split_bind(w, ws, &sp, &rp, &p);
     CU(cudaMemsetAsync(ws + w.o_tot, 0, 8ull * 3, s));
     CU(cudaMemsetAsync(sp.stop, 0xFF, 8, s));
-    launch_k(e, k_gvs_hit, grid, 256, 0, s, gq, static_cast<const uint8_t *>(e->stage_out2), LookupEmit{sp.dest, sp.flat});
-    launches++;
+    launch_k(e, k_gvs_hit, L.grid, 256, 0, s, gq, static_cast<const uint8_t *>(e->stage_out2), LookupEmit{sp.dest, sp.flat});
+    L.launches++;
     CU(cudaMemcpyAsync(results, ws + o_rows, 16ull * n, cudaMemcpyDeviceToHost, s)); // back with the sizes: filled on ERR_CAPACITY too
     e->stats.entries_in = n_keys;
-    e->stats.partitions = groups;
+    e->stats.partitions = L.groups;
     uint64_t items = 0, bytes = 0;
-    rc = split_emit(e, w, sp, rp, p, pin_tot, false, out, &launches, &items, &bytes, [](const unsigned long long *) {});
+    rc = split_emit(e, w, sp, rp, p, pin_tot, false, out, &L.launches, &items, &bytes, [](const unsigned long long *) {});
     if (rc == DBEEL_ERR_CAPACITY) {
         out->data_len = bytes;
         out->index_len = 16 * items;
@@ -3404,13 +3425,14 @@ inline bool key_less(const uint8_t *a, uint64_t al, const uint8_t *b, uint64_t b
 }
 
 // seek_t(bound) of dbeel_reader_scan (dbeel_compact.h) for every table t < nseek and every bound b of kb[boff[b] ..
-// + blen[b]): res / bad / bix[t * nb + b] = k_seek_leaf's result, its smallest corrupt probe (~0: none) and that probe's
-// index record.  Fences (cached or read for this call) on the device in one pass (k_seek_fence), then the touched leaves in
-// groups of about the partition budget (k_seek_leaf).  depth_queries sizes per-call fences (lookup_depth).
-int reader_seek(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, uint32_t nseek, const uint8_t *kb, uint64_t key_bytes,
+// + blen[b]): res / bad / bix[t * nb + b] = the search's result (~0: it failed), its corrupt probe (~0: none) and that
+// probe's index record.  One level of gvs_level<true>: query q = t * nb + b searches pair t, reader table t in
+// DBEEL_LOOKUP_EXACT (its exact-mode fence cache), with no filter; every pair counts depth_queries open queries, which size
+// the fences (lookup_depth).
+int reader_seek(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, uint32_t nseek, const uint8_t *kb,
                 const std::vector<uint64_t> &boff, const std::vector<uint64_t> &blen, uint64_t depth_queries,
                 std::vector<unsigned long long> *res_out, std::vector<unsigned long long> *bad_out, std::vector<uint4> *bix_out) {
-    const uint64_t nb = boff.size(), Q = nb * nseek; // pair q: table q / nb, bound q % nb
+    const uint64_t nb = boff.size(), Q = nb * nseek;
     uint64_t max_klen = 0;
     for (uint64_t b = 0; b < nb; b++) max_klen = std::max(max_klen, blen[b]);
     if (!Q) return DBEEL_OK;
@@ -3418,126 +3440,110 @@ int reader_seek(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, uint3
     if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     cudaStream_t s = e->stream;
     const uint64_t budget = e->partition_bytes;
-    int rc;
-    // ---- fences per table: the reader's (loaded now if this is the first exact-mode call that reaches the table)
-    // or read for this call into one host image, staged to stage_out
-    std::vector<uint32_t> depth(nseek);
-    std::vector<ProbeTree> pt_call(nseek);
-    std::vector<const ProbeTree *> pts(nseek);
-    std::vector<GvsFences> gf(nseek);
-    std::vector<GvsFenceReads> frs(nseek);
-    std::vector<uint64_t> img_at(nseek, ~0ull), touched_at(nseek + 1, 0), nrecs(nseek), data_lens(nseek);
-    uint64_t img_bytes = 0;
-    for (uint32_t t = 0; t < nseek; t++) {
-        dbeel_reader_table *rt = r->tables[t].get();
-        dbeel_reader_table::Fences &cache = rt->fences[DBEEL_LOOKUP_EXACT];
-        const uint64_t n = rt->desc.n, dl = rt->desc.data_len;
-        nrecs[t] = n;
-        data_lens[t] = dl;
-        const uint32_t want = lookup_depth(depth_queries, n, dl, 8 + max_klen, budget);
-        const bool use_cache = reader_uses_cache(max_klen, want, (uint32_t)rt->depth);
-        depth[t] = use_cache ? (uint32_t)rt->depth : want;
-        const uint64_t leaf0 = 1ull << depth[t];
-        touched_at[t + 1] = touched_at[t] + leaf0;
-        gf[t] = GvsFences{nullptr, nullptr, depth[t], t, n, nullptr};
-        if (use_cache) {
-            if (!cache.loaded) {
-                if ((rc = reader_load_fences(e, io, t, rt, DBEEL_LOOKUP_EXACT))) return rc;
-                CU(cudaStreamSynchronize(s)); // its image goes down from ring_out, which the next table refills
-            }
-            pts[t] = &cache.pt;
-            if (depth[t]) {
-                gf[t].fix = reinterpret_cast<const uint4 *>(cache.dev);
-                gf[t].ffr = reinterpret_cast<const unsigned long long *>(cache.dev + 16 * leaf0);
-            }
-            continue;
-        }
-        plan_probe_tree(DBEEL_LOOKUP_EXACT, n, depth[t], &pt_call[t]);
-        pts[t] = &pt_call[t];
-        if (!depth[t]) continue;
-        if ((rc = gvs_read_fences(e, io, t, pt_call[t], dl, max_klen, &frs[t]))) return rc;
-        img_at[t] = align_up(img_bytes, kAlign);
-        img_bytes = img_at[t] + frs[t].image_bytes();
-    }
-    std::vector<uint8_t> img(img_bytes);
-    if (img_bytes) {
-        if ((rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, img_bytes))) return rc;
-        for (uint32_t t = 0; t < nseek; t++) {
-            if (img_at[t] == ~0ull) continue;
-            gvs_fence_image(frs[t], data_lens[t], img.data() + img_at[t], e->stage_out + img_at[t]);
-            gf[t].fix = reinterpret_cast<const uint4 *>(e->stage_out + img_at[t]);
-            gf[t].ffr = reinterpret_cast<const unsigned long long *>(e->stage_out + img_at[t] + 16 * (1ull << depth[t]));
-        }
-    }
-
-    // ---- per-pair state in the workspace
-    uint64_t off = 0;
-    const uint64_t o_keys = carve_ws(&off, key_bytes + 16), o_koff = carve_ws(&off, 8 * Q), o_klen = carve_ws(&off, 8 * Q);
-    const uint64_t o_tab = carve_ws(&off, 4 * Q), o_state = carve_ws(&off, sizeof(SearchState) * Q), o_node = carve_ws(&off, 4 * Q);
-    const uint64_t o_res = carve_ws(&off, 8 * Q), o_bad = carve_ws(&off, 8 * Q), o_bix = carve_ws(&off, 16 * Q);
-    const uint64_t o_gf = carve_ws(&off, sizeof(GvsFences) * nseek), o_td = carve_ws(&off, sizeof(TableDesc) * nseek);
-    const uint64_t o_depth = carve_ws(&off, 4ull * nseek), o_touched = carve_ws(&off, touched_at[nseek]);
-    if ((rc = ensure_device(e, &e->ws, &e->ws_cap, off))) return rc;
-    uint8_t *ws = e->ws;
-    std::vector<uint64_t> qoff(Q), qlen(Q);
-    std::vector<uint32_t> qtab(Q);
-    std::vector<TableDesc> td(nseek);
+    // the bounds once per table, so that query q's key is keys[ko[q] .. ko[q + 1])
+    std::vector<uint8_t> keys;
+    std::vector<uint64_t> ko(Q + 1);
+    std::vector<uint32_t> qt(Q);
     for (uint64_t q = 0; q < Q; q++) {
-        qoff[q] = boff[q % nb];
-        qlen[q] = blen[q % nb];
-        qtab[q] = (uint32_t)(q / nb);
+        ko[q] = keys.size();
+        qt[q] = (uint32_t)(q / nb);
+        keys.insert(keys.end(), kb + boff[q % nb], kb + boff[q % nb] + blen[q % nb]);
     }
-    for (uint32_t t = 0; t < nseek; t++) {
-        gf[t].touched = ws + o_touched + touched_at[t];
-        td[t] = r->tables[t]->desc;
-    }
-    if (key_bytes) CU(cudaMemcpyAsync(ws + o_keys, kb, key_bytes, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ws + o_koff, qoff.data(), 8 * Q, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ws + o_klen, qlen.data(), 8 * Q, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ws + o_tab, qtab.data(), 4 * Q, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ws + o_gf, gf.data(), sizeof(GvsFences) * nseek, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ws + o_td, td.data(), sizeof(TableDesc) * nseek, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(ws + o_depth, depth.data(), 4ull * nseek, cudaMemcpyHostToDevice, s));
-    if (!img.empty()) CU(cudaMemcpyAsync(e->stage_out, img.data(), img.size(), cudaMemcpyHostToDevice, s));
-    CU(cudaMemsetAsync(ws + o_touched, 0, touched_at[nseek], s));
-    SeekQueries sq{ws + o_keys, reinterpret_cast<const uint64_t *>(ws + o_koff), reinterpret_cast<const uint64_t *>(ws + o_klen),
-                   reinterpret_cast<const uint32_t *>(ws + o_tab), Q, reinterpret_cast<SearchState *>(ws + o_state),
-                   reinterpret_cast<uint32_t *>(ws + o_node), reinterpret_cast<unsigned long long *>(ws + o_res),
-                   reinterpret_cast<unsigned long long *>(ws + o_bad), reinterpret_cast<uint4 *>(ws + o_bix)};
-    const uint32_t grid = (uint32_t)((Q + 255) / 256);
-    launch_k(e, k_seek_fence, grid, 256, 0, s, sq, reinterpret_cast<const GvsFences *>(ws + o_gf));
-    std::vector<uint8_t> touched(touched_at[nseek]);
-    CU(cudaMemcpyAsync(touched.data(), ws + o_touched, touched.size(), cudaMemcpyDeviceToHost, s));
-    CU(cudaGetLastError());
-    CU(cudaStreamSynchronize(s));
-
-    // ---- touched leaves, in groups of about `budget` bytes (with a page cache, at most its capacity)
-    const bool paged = r->cache != nullptr;
-    const uint64_t group_bytes = paged ? std::min(budget, kPageBytes * r->cache->pc.capacity()) : budget;
-    std::vector<TouchedLeaf> lv;
-    for (uint32_t t = 0; t < nseek; t++) touched_leaves(*pts[t], t, touched.data() + touched_at[t], &lv);
-    const std::vector<size_t> cut = group_leaves(lv, nrecs, data_lens, max_klen, group_bytes, paged);
+    ko[Q] = keys.size();
+    std::vector<GvsPair> pairs(nseek);
     std::vector<LeafSrc> src(nseek);
-    for (uint32_t t = 0; t < nseek; t++) src[t] = LeafSrc{r, io, t, data_lens[t], max_klen};
-    for (size_t g = 0; g + 1 < cut.size(); g++) {
-        const uint32_t nl = (uint32_t)(cut[g + 1] - cut[g]);
-        if ((rc = gvs_load_leaves(e, src, lv.data() + cut[g], nl))) return rc;
-        launch_k(e, k_seek_leaf, grid, 256, 0, s, sq, reinterpret_cast<const TableDesc *>(ws + o_td),
-                 reinterpret_cast<const uint32_t *>(ws + o_depth), reinterpret_cast<const GvsLeaf *>(e->stage_in),
-                 reinterpret_cast<const uint32_t *>(e->stage_in + sizeof(GvsLeaf) * nl));
-        CU(cudaGetLastError());
-        CU(cudaStreamSynchronize(s));
+    uint64_t touched_max = 0; // at most 2^max(lookup_depth, cached depth) per pair
+    for (uint32_t t = 0; t < nseek; t++) {
+        const TableDesc &d = r->tables[t]->desc;
+        pairs[t] = GvsPair{d, nullptr, nullptr, nullptr, 0, t, DBEEL_LOOKUP_EXACT, 1};
+        pairs[t].t.words = nullptr;
+        src[t] = LeafSrc{r, io, t, d.data_len, max_klen};
+        touched_max += 1ull << std::max(lookup_depth(depth_queries, d.n, d.data_len, 8 + max_klen, budget), (uint32_t)r->tables[t]->depth);
     }
+
+    // ---- per-query state; the pinned block: touched flags | the pairs as the filter reads them | as the rest do
+    uint64_t off = 0;
+    const uint64_t o_keys = carve_ws(&off, keys.size() + 16), o_off = carve_ws(&off, 8 * (Q + 1)), o_batch = carve_ws(&off, 4 * Q);
+    const uint64_t o_rows = carve_ws(&off, 16 * Q), o_hix = carve_ws(&off, 16 * Q), o_state = carve_ws(&off, sizeof(SearchState) * Q);
+    const uint64_t o_node = carve_ws(&off, 4 * Q), o_touched = carve_ws(&off, touched_max), o_cnt = carve_ws(&off, 8ull * nseek);
+    const uint64_t o_need = carve_ws(&off, 8), o_pairs = carve_ws(&off, sizeof(GvsPair) * nseek);
+    const uint64_t p_fpairs = align_up(touched_max, 64), p_pairs = align_up(p_fpairs + sizeof(GvsPair) * nseek, 64);
+    int rc = ensure_device(e, &e->ws, &e->ws_cap, off);
+    if (!rc) rc = ensure_pinned(e, p_pairs + sizeof(GvsPair) * nseek);
+    if (rc) return rc;
+    uint8_t *ws = e->ws;
+    std::vector<uint4> rows(Q, make_uint4(0xFFFFFFFFu, 0, 0, 0)), hix(Q);
+    if (!keys.empty()) CU(cudaMemcpyAsync(ws + o_keys, keys.data(), keys.size(), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_off, ko.data(), 8 * (Q + 1), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_batch, qt.data(), 4 * Q, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(ws + o_rows, rows.data(), 16 * Q, cudaMemcpyHostToDevice, s));
+    GvsQueries gq{ws + o_keys, reinterpret_cast<const uint64_t *>(ws + o_off), reinterpret_cast<const uint32_t *>(ws + o_batch), Q,
+                  reinterpret_cast<uint4 *>(ws + o_rows), reinterpret_cast<uint4 *>(ws + o_hix), reinterpret_cast<SearchState *>(ws + o_state),
+                  reinterpret_cast<uint32_t *>(ws + o_node), nullptr, nullptr};
+    GvsLevel L{gq, (uint32_t)((Q + 255) / 256), reinterpret_cast<GvsPair *>(ws + o_pairs), ws + o_touched, p_pairs,
+               reinterpret_cast<unsigned long long *>(ws + o_need), nullptr};
+    unsigned long long *d_cnt = reinterpret_cast<unsigned long long *>(ws + o_cnt);
+    memcpy(e->pin + p_fpairs, pairs.data(), sizeof(GvsPair) * nseek);
+    CU(cudaMemcpyAsync(L.d_pairs, e->pin + p_fpairs, sizeof(GvsPair) * nseek, cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(d_cnt, 0, 8ull * nseek, s));
+    launch_k(e, k_gvs_filter, L.grid, 256, 0, s, gq, static_cast<const GvsPair *>(L.d_pairs), d_cnt);
+    std::vector<const ProbeTree *> pts(nseek, nullptr);
+    if ((rc = gvs_level<true>(e, L, pairs, src, std::vector<uint64_t>(nseek, depth_queries), pts))) return rc;
 
     // ---- the bounds and the failed searches
-    res_out->assign(Q, 0);
-    bad_out->assign(Q, 0);
-    bix_out->assign(Q, make_uint4(0, 0, 0, 0));
-    CU(cudaMemcpyAsync(res_out->data(), ws + o_res, 8 * Q, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(bad_out->data(), ws + o_bad, 8 * Q, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(bix_out->data(), ws + o_bix, 16 * Q, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(rows.data(), ws + o_rows, 16 * Q, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(hix.data(), ws + o_hix, 16 * Q, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
+    res_out->assign(Q, ~0ull);
+    bad_out->assign(Q, ~0ull);
+    bix_out->assign(Q, make_uint4(0, 0, 0, 0));
+    for (uint64_t q = 0; q < Q; q++) {
+        const uint64_t rec = (uint64_t)rows[q].z | ((uint64_t)rows[q].w << 32);
+        if (rows[q].y & kLookupCorrupt) {
+            (*bad_out)[q] = rec;
+            (*bix_out)[q] = hix[q];
+        } else if (rows[q].x != 0xFFFFFFFFu) {
+            (*res_out)[q] = rec;
+        }
+    }
     return DBEEL_OK;
+}
+
+// The bounds of the key ranges d < n that can hold a record (start < end; range d is kb[ko[2d] .. ko[2d + 1]) ..
+// kb[ko[2d + 1] .. ko[2d + 2])) as offsets into kb and lengths: start, end, start, end, ...  Returns those ranges.
+std::vector<uint32_t> range_bounds(const uint8_t *kb, const std::vector<uint64_t> &ko, uint32_t n, std::vector<uint64_t> *boff,
+                                   std::vector<uint64_t> *blen) {
+    std::vector<uint32_t> live;
+    for (uint32_t d = 0; d < n; d++) {
+        if (!key_less(kb + ko[2 * d], ko[2 * d + 1] - ko[2 * d], kb + ko[2 * d + 1], ko[2 * d + 2] - ko[2 * d + 1])) continue;
+        live.push_back(d);
+        for (uint32_t k = 2 * d; k < 2 * d + 2; k++) {
+            boff->push_back(ko[k]);
+            blen->push_back(ko[k + 1] - ko[k]);
+        }
+    }
+    return live;
+}
+
+// The tables before the first one with no index record: a key-range read stops there with PANIC at its record 0.
+uint32_t seek_tables(const dbeel_reader *r) {
+    for (uint32_t t = 0; t < r->tables.size(); t++)
+        if (r->tables[t]->desc.n == 0) return t;
+    return (uint32_t)r->tables.size();
+}
+
+// The stop of table t's bound searches [q0, q1) of reader_seek's bad / bix: the smallest corrupt probe, PANIC when its index
+// record alone shows it, as dbeel_scan on reaching the record; table -1 when none failed.
+dbeel_scan_stop seek_stop(const dbeel_reader *r, uint32_t t, const std::vector<unsigned long long> &bad, const std::vector<uint4> &bix,
+                          uint64_t q0, uint64_t q1) {
+    uint64_t worst = q1;
+    for (uint64_t q = q0; q < q1; q++)
+        if (bad[q] != ~0ull && (worst == q1 || bad[q] < bad[worst])) worst = q;
+    if (worst == q1) return dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
+    const uint4 ix = bix[worst];
+    const uint64_t o = (uint64_t)ix.x | ((uint64_t)ix.y << 32), dl = r->tables[t]->desc.data_len;
+    const bool panic = ix.w == 0 || o > dl || ix.w > dl - o;
+    return dbeel_scan_stop{(int32_t)t, panic ? DBEEL_SCAN_STOP_PANIC : DBEEL_SCAN_STOP_ERR, bad[worst]};
 }
 
 // Steps 1-2 of a key-range read on a reader (dbeel_reader_scan, dbeel_reader_get_range): the bound searches of every table
@@ -3550,18 +3556,9 @@ int reader_spans(dbeel_engine *e, dbeel_reader *r, const void *ranges, uint32_t 
     const uint8_t *kb = key_bytes ? static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0] : nullptr;
     std::vector<uint64_t> ko(2 * nd + 1);
     for (uint32_t k = 0; k <= 2 * nd; k++) ko[k] = kr->key_offsets[k] - kr->key_offsets[0];
-    std::vector<uint64_t> boff, blen; // the bounds of the ranges that can take a record: start, end, start, end, ...
-    for (uint32_t d = 0; d < nd; d++) {
-        if (!key_less(kb + ko[2 * d], ko[2 * d + 1] - ko[2 * d], kb + ko[2 * d + 1], ko[2 * d + 2] - ko[2 * d + 1])) continue;
-        for (uint32_t k = 2 * d; k < 2 * d + 2; k++) {
-            boff.push_back(ko[k]);
-            blen.push_back(ko[k + 1] - ko[k]);
-        }
-    }
-    const uint32_t nt = (uint32_t)r->tables.size();
-    uint32_t nseek = nt; // the tables before the first one with no index record (a PANIC at its record 0)
-    for (uint32_t t = 0; t < nt; t++)
-        if (r->tables[t]->desc.n == 0) { nseek = t; break; }
+    std::vector<uint64_t> boff, blen;
+    range_bounds(kb, ko, nd, &boff, &blen);
+    const uint32_t nt = (uint32_t)r->tables.size(), nseek = seek_tables(r);
     *host_stop = nseek < nt ? dbeel_scan_stop{(int32_t)nseek, DBEEL_SCAN_STOP_PANIC, 0} : dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
     const uint64_t nb = boff.size();
     uint32_t cutoff = nseek;
@@ -3569,23 +3566,17 @@ int reader_spans(dbeel_engine *e, dbeel_reader *r, const void *ranges, uint32_t 
     if (nb && nseek) {
         std::vector<unsigned long long> res, bad;
         std::vector<uint4> bix;
-        if (const int rc = reader_seek(e, r, io, nseek, kb, key_bytes, boff, blen, 2ull * nd, &res, &bad, &bix)) return rc;
-        for (uint32_t t = 0; t < nseek && cutoff == nseek; t++) {
-            uint64_t worst = ~0ull;
-            uint4 ix = make_uint4(0, 0, 0, 0);
-            std::vector<ScanSpan> sp;
-            for (uint64_t q = nb * t; q < nb * (t + 1); q += 2) {
-                for (uint64_t j = q; j < q + 2; j++)
-                    if (bad[j] < worst) { worst = bad[j]; ix = bix[j]; }
-                if (res[q] < res[q + 1] && res[q + 1] != ~0ull) sp.push_back(ScanSpan{res[q], res[q + 1]});
-            }
-            if (worst != ~0ull) { // as dbeel_scan on reaching the record: PANIC when its index record alone shows it
-                const uint64_t o = (uint64_t)ix.x | ((uint64_t)ix.y << 32), dl = r->tables[t]->desc.data_len;
-                const bool panic = ix.w == 0 || o > dl || ix.w > dl - o;
-                *host_stop = dbeel_scan_stop{(int32_t)t, panic ? DBEEL_SCAN_STOP_PANIC : DBEEL_SCAN_STOP_ERR, worst};
+        if (const int rc = reader_seek(e, r, io, nseek, kb, boff, blen, 2ull * nd, &res, &bad, &bix)) return rc;
+        for (uint32_t t = 0; t < nseek; t++) {
+            const dbeel_scan_stop st = seek_stop(r, t, bad, bix, nb * t, nb * (t + 1));
+            if (st.table >= 0) {
+                *host_stop = st;
                 cutoff = t;
                 break;
             }
+            std::vector<ScanSpan> sp;
+            for (uint64_t q = nb * t; q < nb * (t + 1); q += 2)
+                if (res[q] < res[q + 1] && res[q + 1] != ~0ull) sp.push_back(ScanSpan{res[q], res[q + 1]});
             std::sort(sp.begin(), sp.end(), [](const ScanSpan &a, const ScanSpan &b) { return a.lo < b.lo; });
             for (const ScanSpan &x : sp) {
                 if (!(*spans)[t].empty() && x.lo <= (*spans)[t].back().hi) (*spans)[t].back().hi = std::max((*spans)[t].back().hi, x.hi);
@@ -3634,7 +3625,7 @@ int reader_seek_batched(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *i
         }
         std::vector<unsigned long long> rs, bd;
         std::vector<uint4> bx;
-        if (const int rc = reader_seek(e, r, io, nt, blob.data(), blob.size(), bo, bl, j1 - j0, &rs, &bd, &bx)) return rc;
+        if (const int rc = reader_seek(e, r, io, nt, blob.data(), bo, bl, j1 - j0, &rs, &bd, &bx)) return rc;
         const uint64_t m = j1 - j0;
         for (uint64_t q = 0; q < rs.size(); q++) {
             const uint64_t at = (q / m) * nb + j0 + q % m;
@@ -3974,20 +3965,9 @@ int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const
 int reader_get_ranges(dbeel_engine *e, dbeel_reader *r, const uint8_t *kb, const std::vector<uint64_t> &ko, uint32_t nq,
                       const uint32_t *limits, bool keep_tombstones, bool desc, const dbeel_scan_io *io, dbeel_out *out,
                       dbeel_range_row *rows) {
-    const uint32_t nt = (uint32_t)r->tables.size();
-    uint32_t nseek = nt; // the tables before the first one with no index record
-    for (uint32_t t = 0; t < nt; t++)
-        if (r->tables[t]->desc.n == 0) { nseek = t; break; }
-    std::vector<uint32_t> vq; // the queries with start < end
+    const uint32_t nt = (uint32_t)r->tables.size(), nseek = seek_tables(r);
     std::vector<uint64_t> boff, blen;
-    for (uint32_t q = 0; q < nq; q++) {
-        if (!key_less(kb + ko[2 * q], ko[2 * q + 1] - ko[2 * q], kb + ko[2 * q + 1], ko[2 * q + 2] - ko[2 * q + 1])) continue;
-        vq.push_back(q);
-        for (uint32_t k = 2 * q; k < 2 * q + 2; k++) {
-            boff.push_back(ko[k]);
-            blen.push_back(ko[k + 1] - ko[k]);
-        }
-    }
+    const std::vector<uint32_t> vq = range_bounds(kb, ko, nq, &boff, &blen); // the queries with start < end
     const dbeel_scan_stop empty_stop{(int32_t)nseek, DBEEL_SCAN_STOP_PANIC, 0};
     if (nseek < nt)
         for (uint32_t q = 0; q < nq; q++) { rows[q].flags = DBEEL_RANGE_STOPPED; rows[q].stop = empty_stop; }
@@ -4011,13 +3991,10 @@ int reader_get_ranges(dbeel_engine *e, dbeel_reader *r, const uint8_t *kb, const
         bool any = false;
         for (uint32_t t = 0; t < nseek; t++) {
             const uint64_t a = t * nb + 2 * j, b = a + 1;
-            if (bad[a] != ~0ull || bad[b] != ~0ull) { // as reader_spans: the smallest corrupt probe, PANIC when its index record shows it
-                const uint64_t c = bad[a] <= bad[b] ? a : b;
-                const uint4 ix = bix[c];
-                const uint64_t o = (uint64_t)ix.x | ((uint64_t)ix.y << 32), dl = r->tables[t]->desc.data_len;
-                const bool panic = ix.w == 0 || o > dl || ix.w > dl - o;
+            const dbeel_scan_stop stop = seek_stop(r, t, bad, bix, a, b + 1);
+            if (stop.table >= 0) {
                 rows[q].flags = DBEEL_RANGE_STOPPED;
-                rows[q].stop = dbeel_scan_stop{(int32_t)t, panic ? DBEEL_SCAN_STOP_PANIC : DBEEL_SCAN_STOP_ERR, bad[c]};
+                rows[q].stop = stop;
                 any = false;
                 break;
             }

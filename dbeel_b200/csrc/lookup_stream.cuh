@@ -15,6 +15,10 @@
 // Hits at fences have no window: their entries are read one record each after the last table.  Then k_gvs_hit decodes
 // every hit's entry from the heap the way k_lookup_emit decodes it.
 // Per query: its row (dbeel_lookup_result), the hit's index record, its search state and node, and where its entry is.
+//
+// The key-range reads' bound searches (dbeel_reader_scan and the range reads: for every table and bound, the first record
+// whose key is not less than the bound) are one level of this with a pair per reader table, no filter, and the fence and
+// leaf kernels' kSeek form.
 #pragma once
 
 #include "lookup.cuh"
@@ -95,16 +99,17 @@ __global__ void __launch_bounds__(256) k_gvs_filter(GvsQueries g, const GvsPair 
     atomicAdd(&n_open[b], 1ull);
 }
 
-// One table's fences as GvsPair holds them, for k_seek_fence (scan_seek.cuh).
-struct GvsFences {
-    const uint4 *fix;
-    const unsigned long long *ffr;
-    uint32_t depth;
-    uint32_t table;
-    uint64_t n;
-    uint8_t *touched;
-};
+// kSeek: the row of a bound search (dbeel_reader_scan's seek_t: lookup.cuh's exact-mode search with no exit on equality)
+// becomes {table, flags | `flags`, record lo, record hi}.
+__device__ __forceinline__ void gvs_seek_row(const GvsQueries &g, uint64_t q, uint32_t table, uint32_t flags, uint64_t rec) {
+    const uint4 r = g.rows[q];
+    g.rows[q] = make_uint4(table, r.y | flags, (uint32_t)rec, (uint32_t)(rec >> 32));
+}
 
+// kSeek: a comparison c == 0 goes on to child 2k, as a lower-bound search does (so a reader's DBEEL_LOOKUP_EXACT fences
+// serve it as they are); a finished search leaves s.a in the row's record; a corrupt probe leaves kLookupCorrupt, the
+// probed record in the row and its index record in hit_ix.  hit_off, hit_src and heap_need are not touched.
+template <bool kSeek>
 __global__ void __launch_bounds__(256) k_lookup_fence(GvsQueries g, const GvsPair *pairs) {
     pdl_trigger();
     pdl_wait();
@@ -124,22 +129,33 @@ __global__ void __launch_bounds__(256) k_lookup_fence(GvsQueries g, const GvsPai
         const unsigned long long fr = f.ffr[node];
         const uint64_t pos = search_pos(mode, s);
         if (fr == 0) { // as probe(): offset or length prefix past the end of .data
-            g.rows[q].y |= kLookupCorrupt;
+            if constexpr (kSeek) {
+                gvs_seek_row(g, q, 0xFFFFFFFFu, kLookupCorrupt, pos);
+                g.hit_ix[q] = f.fix[node];
+            } else {
+                g.rows[q].y |= kLookupCorrupt;
+            }
             node = 0;
             break;
         }
         const uint8_t *frame = reinterpret_cast<const uint8_t *>(fr);
         const int c = cmp_key_bytes(frame + 8, ld_bytes_le<true>(frame, 8), key, klen);
-        if (c == 0) {
-            const uint4 r = g.rows[q];
-            g.rows[q] = make_uint4(f.table, r.y, (uint32_t)pos, (uint32_t)(pos >> 32));
-            g.hit_ix[q] = f.fix[node];
-            g.hit_off[q] = kGvsFenceHit;
+        if constexpr (!kSeek) {
+            if (c == 0) {
+                const uint4 r = g.rows[q];
+                g.rows[q] = make_uint4(f.table, r.y, (uint32_t)pos, (uint32_t)(pos >> 32));
+                g.hit_ix[q] = f.fix[node];
+                g.hit_off[q] = kGvsFenceHit;
+                node = 0;
+                break;
+            }
+        }
+        search_step(mode, n, &s, c);
+        if (s.done) {
+            if constexpr (kSeek) gvs_seek_row(g, q, f.table, 0, s.a);
             node = 0;
             break;
         }
-        search_step(mode, n, &s, c);
-        if (s.done) { node = 0; break; }
         node = 2 * node + (c < 0 ? 1u : 0u);
     }
     g.node[q] = node;
@@ -159,8 +175,9 @@ struct GvsLeaf {
 };
 
 // A hit whose entry fits (gvs_entry_fits) leaves its window address in hit_src and adds the heap bytes k_gvs_copy will
-// take for it to *heap_need.
+// take for it to *heap_need.  kSeek: as k_lookup_fence<true>.
 // Pair b's leaves are leaves[first[b] .. first[b + 1]).
+template <bool kSeek>
 __global__ void __launch_bounds__(256) k_lookup_leaf(GvsQueries g, const GvsPair *pairs, const GvsLeaf *leaves, const uint32_t *first,
                                                      unsigned long long *heap_need) {
     pdl_trigger();
@@ -193,22 +210,31 @@ __global__ void __launch_bounds__(256) k_lookup_leaf(GvsQueries g, const GvsPair
         const uint64_t pos = search_pos(mode, s);
         const int c = probe(t, pos, key, klen, &bad, &ix);
         if (bad) {
-            g.rows[q].y |= kLookupCorrupt;
-            break;
-        }
-        if (c == 0) {
-            const uint4 r = g.rows[q];
-            g.rows[q] = make_uint4(p.table, r.y, (uint32_t)pos, (uint32_t)(pos >> 32));
-            g.hit_ix[q] = ix;
-            const uint64_t off = (uint64_t)ix.x | ((uint64_t)ix.y << 32), fs = ix.w;
-            if (gvs_entry_fits(off, ix.z, fs, klen, t.data_len)) { // the window covers [off, off + fs) (lookup_plan.h)
-                g.hit_src[q] = reinterpret_cast<unsigned long long>(t.data + off);
-                atomicAdd(heap_need, (unsigned long long)((fs + 15) / 16 * 16 + 16));
+            if constexpr (kSeek) {
+                gvs_seek_row(g, q, 0xFFFFFFFFu, kLookupCorrupt, pos);
+                g.hit_ix[q] = ix;
+            } else {
+                g.rows[q].y |= kLookupCorrupt;
             }
             break;
         }
+        if constexpr (!kSeek) {
+            if (c == 0) {
+                const uint4 r = g.rows[q];
+                g.rows[q] = make_uint4(p.table, r.y, (uint32_t)pos, (uint32_t)(pos >> 32));
+                g.hit_ix[q] = ix;
+                const uint64_t off = (uint64_t)ix.x | ((uint64_t)ix.y << 32), fs = ix.w;
+                if (gvs_entry_fits(off, ix.z, fs, klen, t.data_len)) { // the window covers [off, off + fs) (lookup_plan.h)
+                    g.hit_src[q] = reinterpret_cast<unsigned long long>(t.data + off);
+                    atomicAdd(heap_need, (unsigned long long)((fs + 15) / 16 * 16 + 16));
+                }
+                break;
+            }
+        }
         search_step(mode, t.n, &s, c);
     }
+    if constexpr (kSeek)
+        if (s.done) gvs_seek_row(g, q, p.table, 0, s.a);
     g.node[q] = 0;
 }
 
