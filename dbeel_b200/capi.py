@@ -51,7 +51,7 @@ EXPORTS = ["dbeel_abi_version", "dbeel_engine_create", "dbeel_engine_destroy", "
            "dbeel_get_values_device", "dbeel_get_values_stream", "dbeel_reader_open", "dbeel_reader_get_values",
            "dbeel_readers_get_values",
            "dbeel_reader_scan", "dbeel_reader_get_range", "dbeel_reader_get_ranges",
-           "dbeel_reader_get_ranges_reverse", "dbeel_reader_close", "dbeel_page_cache_create", "dbeel_page_cache_destroy",
+           "dbeel_reader_get_ranges_reverse", "dbeel_readers_get_ranges", "dbeel_reader_close", "dbeel_page_cache_create", "dbeel_page_cache_destroy",
            "dbeel_reader_attach_page_cache", "dbeel_page_cache_stats"]
 
 
@@ -139,6 +139,15 @@ MAX_READER_BATCHES = 1024  # DBEEL_MAX_READER_BATCHES
 class ReaderBatch(C.Structure):
     _fields_ = [("reader", C.c_void_p), ("keys", C.c_void_p), ("key_offsets", C.c_void_p), ("n_keys", C.c_uint64),
                 ("mode", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class RangeBatch(C.Structure):
+    """dbeel_range_batch: one reader's limited range reads in dbeel_readers_get_ranges."""
+    _fields_ = [("reader", C.c_void_p), ("ranges", KeyRanges), ("limits", C.c_void_p), ("n_ranges", C.c_uint32),
+                ("flags", C.c_uint32), ("reverse", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+DbeelRangeBatch = RangeBatch
 
 
 def pack_keys(keys: Sequence[bytes]) -> Tuple[np.ndarray, np.ndarray]:
@@ -254,6 +263,8 @@ def lib():
         L.dbeel_reader_get_ranges_reverse.restype = C.c_int
         L.dbeel_reader_get_ranges_reverse.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32,
                                                       C.POINTER(Out), C.c_void_p]
+        L.dbeel_readers_get_ranges.restype = C.c_int
+        L.dbeel_readers_get_ranges.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(Out), C.c_void_p]
         L.dbeel_reader_close.restype = None
         L.dbeel_reader_close.argtypes = [C.c_void_p]
         L.dbeel_page_cache_create.restype = C.c_int
@@ -1081,6 +1092,82 @@ class Engine:
             if items:
                 offs -= np.uint64(d0)
             res.append((rows[q0:q0 + c].copy(), data[d0:d1].copy(), ix))
+            q0, item0 = q0 + c, item0 + items
+        return res
+
+    def readers_get_ranges(self, batches, caps: Optional[Tuple[int, int]] = None, fail_read_at=None):
+        """dbeel_readers_get_ranges: the limited range reads [(reader, ranges, limits, reverse, keep_tombstones), ...] of
+        many readers in one call; limits is an int (every range) or one per range.  Returns [(rows, data, index)] per batch,
+        each what reader.get_ranges(ranges, limits, keep_tombstones, reverse=reverse) returns alone (first and the index
+        offsets rebased to the batch's own output).  caps = (data_cap, index_cap) for the whole call, by default retried
+        once with the sizes needed.  Each reader's last_stream_reads = its reads in this call; fail_read_at = {reader: n}
+        makes the n-th read of that reader's callback in the call return 4242."""
+        fail_read_at = fail_read_at or {}
+        arr = (RangeBatch * max(1, len(batches)))()
+        keep, counts, readers, total = [], [], [], 0
+        for j, (r, ranges, limits, reverse, keep_tombstones) in enumerate(batches):
+            if not r._h:
+                raise ValueError("reader is closed")
+            n = len(ranges)
+            lim = np.ascontiguousarray(np.full(n, limits, np.uint32) if isinstance(limits, (int, np.integer))
+                                       else np.array([int(x) for x in limits], np.uint32))
+            if lim.size != n:
+                raise ValueError("one limit per range")
+            blob, off = pack_keys([bytes(k) for pair in ranges for k in pair])
+            keep.append((blob, off, lim))
+            counts.append(n)
+            total += int(lim.sum())
+            arr[j] = RangeBatch(r._h, KeyRanges(blob.ctypes.data if blob.size else None, off.ctypes.data),
+                                lim.ctypes.data if n else None, n, RANGE_KEEP_TOMBSTONES if keep_tombstones else 0,
+                                1 if reverse else 0, 0)
+            if all(r is not x for x in readers):
+                readers.append(r)
+        sts = [r._st for r in readers if r._st is not None]
+        for r in readers:
+            if r._st is not None:
+                r._st.fail_read_at = fail_read_at.get(r, -1)
+        n = sum(counts)
+        rows = np.zeros(max(1, n), RANGE_ROW_DTYPE)
+        dc0 = sum(sum(d for d, _ in r._st.sizes) if r._st is not None else r._data_cap for r in readers)
+        dc, ic = caps if caps is not None else (min(dc0, 64 << 20), min(16 * total, 16 << 20))
+        try:
+            for attempt in range(2):
+                od, oi = np.empty(max(1, dc), np.uint8), np.empty(max(1, ic), np.uint8)
+                out = Out(od.ctypes.data, dc, 0, oi.ctypes.data, ic, 0, None, 0, 0, 0)
+                for st in sts:
+                    st.log.clear()
+                rc = lib().dbeel_readers_get_ranges(self._h, arr, len(batches), C.byref(out), rows.ctypes.data)
+                for st in sts:
+                    st.last_reads = list(st.log)
+                if rc == 0:
+                    break
+                err = DbeelError(rc, f"dbeel_readers_get_ranges: {lib().dbeel_last_error(self._h).decode()}")
+                if rc == ERR_CAPACITY:
+                    err.needed = (int(out.data_len), int(out.index_len))
+                    err.rows = rows[:n].copy()
+                if caps is not None or attempt or rc != ERR_CAPACITY:
+                    raise err
+                dc, ic = err.needed
+        finally:
+            for r in readers:
+                if r._st is not None:
+                    r._st.fail_read_at = -1
+                    r.last_stream_reads = r._st.last_reads
+        # split the packed output: batch b's rows hold its entries [first, first + count), in row order
+        data, index = od[:out.data_len], oi[:out.index_len]
+        rows = rows[:n]
+        res, q0, item0 = [], 0, 0
+        for c in counts:
+            rb = rows[q0:q0 + c].copy()
+            items = int(rb["count"].sum())
+            rb["first"] -= np.uint64(item0)
+            ix = index[16 * item0:16 * (item0 + items)].copy()
+            offs = ix.view("<u8")[0::2] if items else np.zeros(0, np.uint64)
+            d0 = int(offs[0]) if items else 0
+            d1 = int(offs[-1] + ix.view("<u4")[-1]) if items else 0
+            if items:
+                offs -= np.uint64(d0)
+            res.append((rb, data[d0:d1].copy(), ix))
             q0, item0 = q0 + c, item0 + items
         return res
 

@@ -2512,16 +2512,6 @@ int gvs_load(dbeel_engine *e, uint32_t kind, const std::vector<GvsPart> &parts, 
     return DBEEL_OK;
 }
 
-// Every part through `io` and reader r's page cache (r may be null: no cache).
-int gvs_load(dbeel_engine *e, const dbeel_scan_io *io, const dbeel_reader *r, uint32_t kind, std::vector<GvsPart> parts,
-             uint8_t *host, uint8_t *dev, uint64_t from, uint64_t to, bool host_too, const char *what) {
-    for (GvsPart &g : parts) {
-        g.r = r;
-        g.io = io;
-    }
-    return gvs_load(e, kind, parts, host, dev, from, to, host_too, what);
-}
-
 // Where the touched leaves of part t of a group come from: the reader (null: none) and io its reads go through, the table's
 // position there, its .data length and the longest key of the batch that searches it.
 struct LeafSrc {
@@ -3424,17 +3414,30 @@ inline bool key_less(const uint8_t *a, uint64_t al, const uint8_t *b, uint64_t b
     return c < 0 || (c == 0 && al < bl);
 }
 
-// seek_t(bound) of dbeel_reader_scan (dbeel_compact.h) for every table t < nseek and every bound b of kb[boff[b] ..
-// + blen[b]): res / bad / bix[t * nb + b] = the search's result (~0: it failed), its corrupt probe (~0: none) and that
-// probe's index record.  One level of gvs_level<true>: query q = t * nb + b searches pair t, reader table t in
-// DBEEL_LOOKUP_EXACT (its exact-mode fence cache), with no filter; every pair counts depth_queries open queries, which size
-// the fences (lookup_depth).
-int reader_seek(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, uint32_t nseek, const uint8_t *kb,
-                const std::vector<uint64_t> &boff, const std::vector<uint64_t> &blen, uint64_t depth_queries,
-                std::vector<unsigned long long> *res_out, std::vector<unsigned long long> *bad_out, std::vector<uint4> *bix_out) {
-    const uint64_t nb = boff.size(), Q = nb * nseek;
-    uint64_t max_klen = 0;
-    for (uint64_t b = 0; b < nb; b++) max_klen = std::max(max_klen, blen[b]);
+// One reader's part of a seek: seek_t(bound) of dbeel_reader_scan (dbeel_compact.h) for every table t < nseek of r and every
+// bound b of kb[boff[b] .. + blen[b]), through io; res / bad / bix[t * nb + b] = the search's result (~0: it failed), its
+// corrupt probe (~0: none) and that probe's index record.
+struct SeekPart {
+    dbeel_reader *r;
+    const dbeel_scan_io *io;
+    uint32_t nseek;
+    const uint8_t *kb;
+    std::vector<uint64_t> boff, blen;
+    uint64_t depth_queries; // the open queries every pair counts, which size its fences (lookup_depth)
+    std::vector<unsigned long long> res, bad;
+    std::vector<uint4> bix;
+};
+
+// The parts' bound searches as one level of gvs_level<true>: part i's table t is a pair, reader table t in
+// DBEEL_LOOKUP_EXACT (its exact-mode fence cache) with no filter, with the part's depth_queries and longest bound, so that
+// the depth and cache decisions are each part's own; query t * nb + b of a part searches its pair t.
+int reader_seek(dbeel_engine *e, std::vector<SeekPart> &sp) {
+    uint64_t Q = 0;
+    uint32_t np = 0;
+    for (const SeekPart &x : sp) {
+        Q += x.boff.size() * x.nseek;
+        np += x.nseek;
+    }
     if (!Q) return DBEEL_OK;
     cudaError_t ce = cudaSetDevice(e->device);
     if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
@@ -3442,34 +3445,41 @@ int reader_seek(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, uint3
     const uint64_t budget = e->partition_bytes;
     // the bounds once per table, so that query q's key is keys[ko[q] .. ko[q + 1])
     std::vector<uint8_t> keys;
-    std::vector<uint64_t> ko(Q + 1);
+    std::vector<uint64_t> ko(Q + 1), count;
     std::vector<uint32_t> qt(Q);
-    for (uint64_t q = 0; q < Q; q++) {
-        ko[q] = keys.size();
-        qt[q] = (uint32_t)(q / nb);
-        keys.insert(keys.end(), kb + boff[q % nb], kb + boff[q % nb] + blen[q % nb]);
+    std::vector<GvsPair> pairs;
+    std::vector<LeafSrc> src;
+    uint64_t touched_max = 0; // at most 2^max(lookup_depth, cached depth) per pair
+    for (uint64_t i = 0, q = 0; i < sp.size(); i++) {
+        const SeekPart &x = sp[i];
+        const uint64_t nb = x.boff.size();
+        uint64_t max_klen = 0;
+        for (uint64_t b = 0; b < nb; b++) max_klen = std::max(max_klen, x.blen[b]);
+        for (uint32_t t = 0; t < x.nseek; t++) {
+            for (uint64_t b = 0; b < nb; b++, q++) {
+                ko[q] = keys.size();
+                qt[q] = (uint32_t)pairs.size();
+                keys.insert(keys.end(), x.kb + x.boff[b], x.kb + x.boff[b] + x.blen[b]);
+            }
+            const TableDesc &d = x.r->tables[t]->desc;
+            pairs.push_back(GvsPair{d, nullptr, nullptr, nullptr, 0, t, DBEEL_LOOKUP_EXACT, 1});
+            pairs.back().t.words = nullptr;
+            src.push_back(LeafSrc{x.r, x.io, t, d.data_len, max_klen});
+            count.push_back(x.depth_queries);
+            touched_max += 1ull << std::max(lookup_depth(x.depth_queries, d.n, d.data_len, 8 + max_klen, budget), (uint32_t)x.r->tables[t]->depth);
+        }
     }
     ko[Q] = keys.size();
-    std::vector<GvsPair> pairs(nseek);
-    std::vector<LeafSrc> src(nseek);
-    uint64_t touched_max = 0; // at most 2^max(lookup_depth, cached depth) per pair
-    for (uint32_t t = 0; t < nseek; t++) {
-        const TableDesc &d = r->tables[t]->desc;
-        pairs[t] = GvsPair{d, nullptr, nullptr, nullptr, 0, t, DBEEL_LOOKUP_EXACT, 1};
-        pairs[t].t.words = nullptr;
-        src[t] = LeafSrc{r, io, t, d.data_len, max_klen};
-        touched_max += 1ull << std::max(lookup_depth(depth_queries, d.n, d.data_len, 8 + max_klen, budget), (uint32_t)r->tables[t]->depth);
-    }
 
     // ---- per-query state; the pinned block: touched flags | the pairs as the filter reads them | as the rest do
     uint64_t off = 0;
     const uint64_t o_keys = carve_ws(&off, keys.size() + 16), o_off = carve_ws(&off, 8 * (Q + 1)), o_batch = carve_ws(&off, 4 * Q);
     const uint64_t o_rows = carve_ws(&off, 16 * Q), o_hix = carve_ws(&off, 16 * Q), o_state = carve_ws(&off, sizeof(SearchState) * Q);
-    const uint64_t o_node = carve_ws(&off, 4 * Q), o_touched = carve_ws(&off, touched_max), o_cnt = carve_ws(&off, 8ull * nseek);
-    const uint64_t o_need = carve_ws(&off, 8), o_pairs = carve_ws(&off, sizeof(GvsPair) * nseek);
-    const uint64_t p_fpairs = align_up(touched_max, 64), p_pairs = align_up(p_fpairs + sizeof(GvsPair) * nseek, 64);
+    const uint64_t o_node = carve_ws(&off, 4 * Q), o_touched = carve_ws(&off, touched_max), o_cnt = carve_ws(&off, 8ull * np);
+    const uint64_t o_need = carve_ws(&off, 8), o_pairs = carve_ws(&off, sizeof(GvsPair) * np);
+    const uint64_t p_fpairs = align_up(touched_max, 64), p_pairs = align_up(p_fpairs + sizeof(GvsPair) * np, 64);
     int rc = ensure_device(e, &e->ws, &e->ws_cap, off);
-    if (!rc) rc = ensure_pinned(e, p_pairs + sizeof(GvsPair) * nseek);
+    if (!rc) rc = ensure_pinned(e, p_pairs + sizeof(GvsPair) * np);
     if (rc) return rc;
     uint8_t *ws = e->ws;
     std::vector<uint4> rows(Q, make_uint4(0xFFFFFFFFu, 0, 0, 0)), hix(Q);
@@ -3483,28 +3493,33 @@ int reader_seek(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, uint3
     GvsLevel L{gq, (uint32_t)((Q + 255) / 256), reinterpret_cast<GvsPair *>(ws + o_pairs), ws + o_touched, p_pairs,
                reinterpret_cast<unsigned long long *>(ws + o_need), nullptr};
     unsigned long long *d_cnt = reinterpret_cast<unsigned long long *>(ws + o_cnt);
-    memcpy(e->pin + p_fpairs, pairs.data(), sizeof(GvsPair) * nseek);
-    CU(cudaMemcpyAsync(L.d_pairs, e->pin + p_fpairs, sizeof(GvsPair) * nseek, cudaMemcpyHostToDevice, s));
-    CU(cudaMemsetAsync(d_cnt, 0, 8ull * nseek, s));
+    memcpy(e->pin + p_fpairs, pairs.data(), sizeof(GvsPair) * np);
+    CU(cudaMemcpyAsync(L.d_pairs, e->pin + p_fpairs, sizeof(GvsPair) * np, cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(d_cnt, 0, 8ull * np, s));
     launch_k(e, k_gvs_filter, L.grid, 256, 0, s, gq, static_cast<const GvsPair *>(L.d_pairs), d_cnt);
-    std::vector<const ProbeTree *> pts(nseek, nullptr);
-    if ((rc = gvs_level<true>(e, L, pairs, src, std::vector<uint64_t>(nseek, depth_queries), pts))) return rc;
+    std::vector<const ProbeTree *> pts(np, nullptr);
+    if ((rc = gvs_level<true>(e, L, pairs, src, count, pts))) return rc;
 
     // ---- the bounds and the failed searches
     CU(cudaMemcpyAsync(rows.data(), ws + o_rows, 16 * Q, cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(hix.data(), ws + o_hix, 16 * Q, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
-    res_out->assign(Q, ~0ull);
-    bad_out->assign(Q, ~0ull);
-    bix_out->assign(Q, make_uint4(0, 0, 0, 0));
-    for (uint64_t q = 0; q < Q; q++) {
-        const uint64_t rec = (uint64_t)rows[q].z | ((uint64_t)rows[q].w << 32);
-        if (rows[q].y & kLookupCorrupt) {
-            (*bad_out)[q] = rec;
-            (*bix_out)[q] = hix[q];
-        } else if (rows[q].x != 0xFFFFFFFFu) {
-            (*res_out)[q] = rec;
+    for (uint64_t i = 0, q0 = 0; i < sp.size(); i++) {
+        SeekPart &x = sp[i];
+        const uint64_t m = x.boff.size() * x.nseek;
+        x.res.assign(m, ~0ull);
+        x.bad.assign(m, ~0ull);
+        x.bix.assign(m, make_uint4(0, 0, 0, 0));
+        for (uint64_t k = 0; k < m; k++) {
+            const uint64_t q = q0 + k, rec = (uint64_t)rows[q].z | ((uint64_t)rows[q].w << 32);
+            if (rows[q].y & kLookupCorrupt) {
+                x.bad[k] = rec;
+                x.bix[k] = hix[q];
+            } else if (rows[q].x != 0xFFFFFFFFu) {
+                x.res[k] = rec;
+            }
         }
+        q0 += m;
     }
     return DBEEL_OK;
 }
@@ -3564,9 +3579,10 @@ int reader_spans(dbeel_engine *e, dbeel_reader *r, const void *ranges, uint32_t 
     uint32_t cutoff = nseek;
     spans->assign(nseek, {});
     if (nb && nseek) {
-        std::vector<unsigned long long> res, bad;
-        std::vector<uint4> bix;
-        if (const int rc = reader_seek(e, r, io, nseek, kb, boff, blen, 2ull * nd, &res, &bad, &bix)) return rc;
+        std::vector<SeekPart> sp{SeekPart{r, io, nseek, kb, boff, blen, 2ull * nd, {}, {}, {}}};
+        if (const int rc = reader_seek(e, sp)) return rc;
+        const std::vector<unsigned long long> &res = sp[0].res, &bad = sp[0].bad;
+        const std::vector<uint4> &bix = sp[0].bix;
         for (uint32_t t = 0; t < nseek; t++) {
             const dbeel_scan_stop st = seek_stop(r, t, bad, bix, nb * t, nb * (t + 1));
             if (st.table >= 0) {
@@ -3602,38 +3618,42 @@ int reader_scan_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *tables,
     return rc;
 }
 
-// reader_seek for many bounds (kb[boff[b] .. + blen[b])) in batches whose search state (kSeekPairBytes per table and
-// bound, plus the bound's bytes) fits the partition budget: res / bad / bix[t * nb + b] as one reader_seek would give them.
-int reader_seek_batched(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, uint32_t nt, const uint8_t *kb,
-                        const std::vector<uint64_t> &boff, const std::vector<uint64_t> &blen, std::vector<unsigned long long> *res,
-                        std::vector<unsigned long long> *bad, std::vector<uint4> *bix) {
+// reader_seek for many bounds, of one or many readers: each part's res / bad / bix as one reader_seek would give them.  The
+// bounds are cut into seek batches whose search state (kSeekPairBytes per table and bound, plus the bound's bytes) fits
+// the partition budget, each part's as its solo call cuts them, and seek batches of consecutive parts share one
+// reader_seek while they fit it together (pack_batches).
+int reader_seek_batched(dbeel_engine *e, std::vector<SeekPart> &parts) {
     constexpr uint64_t kSeekPairBytes = 128;
-    const uint64_t nb = boff.size();
-    res->assign(nt * nb, ~0ull);
-    bad->assign(nt * nb, ~0ull);
-    bix->assign(nt * nb, make_uint4(0, 0, 0, 0));
-    for (uint64_t j0 = 0; j0 < nb;) {
-        std::vector<uint8_t> blob;
-        std::vector<uint64_t> bo, bl;
-        uint64_t j1 = j0, bytes = 0;
-        while (j1 < nb && (j1 == j0 || bytes + blen[j1] + kSeekPairBytes * nt <= e->partition_bytes)) {
-            bytes += blen[j1] + kSeekPairBytes * nt;
-            bo.push_back(blob.size());
-            bl.push_back(blen[j1]);
-            blob.insert(blob.end(), kb + boff[j1], kb + boff[j1] + blen[j1]);
-            j1++;
+    std::vector<std::vector<uint64_t>> cost(parts.size());
+    for (size_t i = 0; i < parts.size(); i++) {
+        SeekPart &x = parts[i];
+        const uint64_t nb = x.boff.size();
+        x.res.assign(x.nseek * nb, ~0ull);
+        x.bad.assign(x.nseek * nb, ~0ull);
+        x.bix.assign(x.nseek * nb, make_uint4(0, 0, 0, 0));
+        if (x.nseek)
+            for (uint64_t j = 0; j < nb; j++) cost[i].push_back(x.blen[j] + kSeekPairBytes * x.nseek);
+    }
+    for (const std::vector<BatchSpan> &group : pack_batches(cost, std::vector<int32_t>(parts.size(), -1), e->partition_bytes, {})) {
+        std::vector<SeekPart> sp;
+        for (const BatchSpan &u : group) {
+            const SeekPart &x = parts[u.batch];
+            sp.push_back(SeekPart{x.r, x.io, x.nseek, x.kb, {}, {}, u.k1 - u.k0, {}, {}, {}});
+            sp.back().boff.assign(x.boff.begin() + u.k0, x.boff.begin() + u.k1);
+            sp.back().blen.assign(x.blen.begin() + u.k0, x.blen.begin() + u.k1);
         }
-        std::vector<unsigned long long> rs, bd;
-        std::vector<uint4> bx;
-        if (const int rc = reader_seek(e, r, io, nt, blob.data(), bo, bl, j1 - j0, &rs, &bd, &bx)) return rc;
-        const uint64_t m = j1 - j0;
-        for (uint64_t q = 0; q < rs.size(); q++) {
-            const uint64_t at = (q / m) * nb + j0 + q % m;
-            (*res)[at] = rs[q];
-            (*bad)[at] = bd[q];
-            (*bix)[at] = bx[q];
+        if (const int rc = reader_seek(e, sp)) return rc;
+        for (size_t i = 0; i < group.size(); i++) {
+            const BatchSpan &u = group[i];
+            SeekPart &x = parts[u.batch];
+            const uint64_t nb = x.boff.size(), m = u.k1 - u.k0;
+            for (uint64_t q = 0; q < sp[i].res.size(); q++) {
+                const uint64_t at = (q / m) * nb + u.k0 + q % m;
+                x.res[at] = sp[i].res[q];
+                x.bad[at] = sp[i].bad[q];
+                x.bix[at] = sp[i].bix[q];
+            }
         }
-        j0 = j1;
     }
     return DBEEL_OK;
 }
@@ -3691,9 +3711,9 @@ int reader_get_range_key(dbeel_engine *e, dbeel_reader *r, const dbeel_table *ta
             blen.push_back(k.size());
             blob.insert(blob.end(), k.begin(), k.end());
         }
-        std::vector<unsigned long long> res, bad;
-        std::vector<uint4> bix;
-        if (const int src = reader_seek_batched(e, r, io, nt, blob.data(), boff, blen, &res, &bad, &bix)) return src;
+        std::vector<SeekPart> sp{SeekPart{r, io, nt, blob.data(), boff, blen, 0, {}, {}, {}}};
+        if (const int src = reader_seek_batched(e, sp)) return src;
+        const std::vector<unsigned long long> &res = sp[0].res, &bad = sp[0].bad;
         pos->assign(res.size(), ~0ull);
         for (uint64_t q = 0; q < res.size(); q++) (*pos)[q] = bad[q] != ~0ull ? ~0ull : res[q];
         return 0;
@@ -3749,42 +3769,62 @@ int reader_range_entry(dbeel_reader *r, bool get_range, uint32_t kind, const voi
     return rc;
 }
 
-// ---- dbeel_reader_get_ranges
-// One query of a call: its span [lo, hi) per searched table, the chunk width per table, and where its entries went.
+// ---- dbeel_reader_get_ranges / _reverse, dbeel_readers_get_ranges
+// One batch of a range-read walk: its reader, the io its reads go through, its ranges (kb and ko as range_bounds takes
+// them), limits, tombstone rule and direction.
+struct RangeBatch {
+    dbeel_reader *r;
+    const dbeel_scan_io *io;
+    const uint8_t *kb;
+    std::vector<uint64_t> ko;
+    uint32_t nq;
+    const uint32_t *limits;
+    bool keep_tombstones, desc;
+};
+
+// One query of a call: its batch and limit, its span [lo, hi) per searched table of its reader, the chunk width per table,
+// and where its entries went.
 struct LimitState {
+    uint32_t batch = 0, limit = 0;
     std::vector<uint64_t> lo, hi, w;
     int32_t em = -1; // emission that holds its entries
     uint32_t at = 0; // its first entry there
 };
 
-// One merge round of a group of live queries (range_limit.cuh): per (query, table) pair the records [lo, lo + w) cut at hi
-// -- desc: [hi - w, hi) cut at lo -- their .index slices, then the .data windows of the records whose index record stays
-// inside .data, both through gvs_load -- decoded, merged and ranked on the device.  A query is finished when it is damaged,
-// when it has limit + 1 survivors on the complete side of its frontier, or when every pair reached its span's far end; the
-// entries of the finished ones go through the split and phase 2 into emission `em` (host memory).  The pairs that set an
-// unfinished query's frontier double their width; that query goes to *next.
-int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const uint32_t *qs, uint32_t gq, const uint32_t *limits,
-                bool keep_tombstones, bool desc, std::vector<LimitState> &st, dbeel_range_row *rows,
-                std::vector<std::vector<uint8_t>> *em, std::vector<uint32_t> *next, uint32_t *launches, uint64_t *gather_bytes) {
-    const uint32_t nseek = (uint32_t)st[qs[0]].lo.size();
+// One merge round of a group of live queries, of any batches (range_limit.cuh): per (query, table) pair the records
+// [lo, lo + w) cut at hi -- reverse: [hi - w, hi) cut at lo -- their .index slices, then the .data windows of the records
+// whose index record stays inside .data, both through gvs_load with each part on its own batch's reader and io, decoded,
+// merged and ranked on the device.  A (batch, table) slot is tbase[batch] + table.  A query is finished when it is
+// damaged, when it has limit + 1 survivors on the complete side of its frontier, or when every pair reached its span's far
+// end; the entries of the finished ones go through the split and phase 2 into emission `em` (host memory).  The pairs that
+// set an unfinished query's frontier double their width; that query goes to *next.  Everything a query's row depends on is
+// its own state, so its row is the same in any group.
+int limit_round(dbeel_engine *e, const std::vector<RangeBatch> &bs, const std::vector<uint32_t> &tbase, const uint32_t *qs, uint32_t gq,
+                std::vector<LimitState> &st, dbeel_range_row *rows, std::vector<std::vector<uint8_t>> *em, std::vector<uint32_t> *next,
+                uint32_t *launches, uint64_t *gather_bytes) {
+    const uint32_t nslot = tbase.back();
     cudaStream_t s = e->stream;
     int rc;
     std::vector<LimitPair> pairs;
-    std::vector<uint32_t> ptab;
+    std::vector<uint32_t> ptab, slot_b(nslot);
     std::vector<uint64_t> pbase; // the table's record number of the pair's first staged record
     std::vector<LimitQuery> lq(gq);
-    std::vector<std::vector<ByteRange>> ir(nseek);
+    std::vector<std::vector<ByteRange>> ir(nslot);
+    for (uint32_t b = 0; b + 1 < tbase.size(); b++)
+        for (uint32_t k = tbase[b]; k < tbase[b + 1]; k++) slot_b[k] = b;
     uint32_t n = 0;
     for (uint32_t g = 0; g < gq; g++) {
         const LimitState &q = st[qs[g]];
-        lq[g] = LimitQuery{(uint32_t)pairs.size(), 0, n, 0, limits[qs[g]], 0};
-        for (uint32_t t = 0; t < nseek; t++) {
+        const RangeBatch &B = bs[q.batch];
+        const bool desc = B.desc;
+        lq[g] = LimitQuery{(uint32_t)pairs.size(), 0, n, 0, q.limit, (uint16_t)desc, (uint16_t)B.keep_tombstones};
+        for (uint32_t t = 0; t < q.lo.size(); t++) {
             if (q.hi[t] <= q.lo[t]) continue;
             const uint64_t c = std::min(q.w[t], q.hi[t] - q.lo[t]), b = desc ? q.hi[t] - c : q.lo[t];
             pairs.push_back(LimitPair{n, (uint32_t)c, g, (desc ? b > q.lo[t] : b + c < q.hi[t]) ? 1u : 0u});
             ptab.push_back(t);
             pbase.push_back(b);
-            ir[t].push_back({16 * b, 16 * (b + c)});
+            ir[tbase[q.batch] + t].push_back({16 * b, 16 * (b + c)});
             n += (uint32_t)c;
         }
         lq[g].pair1 = (uint32_t)pairs.size();
@@ -3793,58 +3833,61 @@ int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const
     const uint32_t np = (uint32_t)pairs.size();
     e->stats.entries_in += n;
     // ---- the .index slices (back to host too), then the windows of the records
-    std::vector<GvsStaged> ss(nseek), sw(nseek);
+    std::vector<GvsStaged> ss(nslot), sw(nslot);
     std::vector<GvsPart> parts;
+    auto part = [&](uint32_t k, const GvsStaged *x) {
+        const RangeBatch &B = bs[slot_b[k]];
+        return GvsPart{k - tbase[slot_b[k]], x, B.r, B.io};
+    };
     uint64_t end = 0;
-    for (uint32_t t = 0; t < nseek; t++) {
-        if (ir[t].empty()) continue;
-        ss[t] = gvs_stage(std::move(ir[t]), 0, end);
-        end = ss[t].end;
-        parts.push_back(GvsPart{t, &ss[t]});
+    for (uint32_t k = 0; k < nslot; k++) {
+        if (ir[k].empty()) continue;
+        ss[k] = gvs_stage(std::move(ir[k]), 0, end);
+        end = ss[k].end;
+        parts.push_back(part(k, &ss[k]));
     }
     rc = ensure_host(e, &e->ring_in, &e->ring_in_cap, end);
     if (!rc) rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, end);
     if (rc) return rc;
-    if ((rc = gvs_load(e, io, r, DBEEL_STREAM_INDEX, parts, e->ring_in, e->stage_in, 0, end, true, "stream read callback failed (.index, ranges)")))
+    if ((rc = gvs_load(e, DBEEL_STREAM_INDEX, parts, e->ring_in, e->stage_in, 0, end, true, "stream read callback failed (.index, ranges)")))
         return rc;
     std::vector<uint4> rec(n);
-    std::vector<uint32_t> rpair(n);
-    std::vector<std::vector<ByteRange>> wr(nseek);
+    std::vector<uint32_t> rpair(n), pslot(np);
+    std::vector<std::vector<ByteRange>> wr(nslot);
     for (uint32_t k = 0; k < np; k++) {
-        const uint32_t t = ptab[k];
-        const uint64_t dl = r->tables[t]->desc.data_len;
+        const uint32_t b = st[qs[pairs[k].query]].batch, t = ptab[k], sl = pslot[k] = tbase[b] + t;
+        const uint64_t dl = bs[b].r->tables[t]->desc.data_len;
         for (uint32_t j = 0; j < pairs[k].count; j++) {
-            const uint8_t *ix = e->ring_in + ss[t].at(16 * (pbase[k] + j));
+            const uint8_t *ix = e->ring_in + ss[sl].at(16 * (pbase[k] + j));
             const uint64_t off = rd_le(ix, 8), fs = rd_le(ix + 12, 4);
             const bool panic = fs == 0 || off > dl || fs > dl - off; // as k_scan_classify: the index record alone shows it
             rec[pairs[k].first + j] = make_uint4(0, 0, panic ? kScanStopPanic : 0u, (uint32_t)fs);
             rpair[pairs[k].first + j] = k;
-            if (!panic) wr[t].push_back({off, off + fs});
+            if (!panic) wr[sl].push_back({off, off + fs});
         }
     }
     uint64_t wend = 0;
     parts.clear();
-    for (uint32_t t = 0; t < nseek; t++) {
-        sw[t] = gvs_stage(std::move(wr[t]), 0, wend);
-        wend = sw[t].end;
-        if (!sw[t].runs.empty()) parts.push_back(GvsPart{t, &sw[t]});
+    for (uint32_t k = 0; k < nslot; k++) {
+        sw[k] = gvs_stage(std::move(wr[k]), 0, wend);
+        wend = sw[k].end;
+        if (!sw[k].runs.empty()) parts.push_back(part(k, &sw[k]));
     }
     rc = ensure_host(e, &e->ring_out, &e->ring_out_cap, std::max<uint64_t>(wend, 256));
     if (!rc) rc = ensure_device(e, &e->stage_in2, &e->stage_in2_cap, std::max<uint64_t>(wend, 256));
     if (rc) return rc;
-    if ((rc = gvs_load(e, io, r, DBEEL_STREAM_DATA, parts, e->ring_out, e->stage_in2, 0, wend, false, "stream read callback failed (.data, ranges)")))
+    if ((rc = gvs_load(e, DBEEL_STREAM_DATA, parts, e->ring_out, e->stage_in2, 0, wend, false, "stream read callback failed (.data, ranges)")))
         return rc;
     for (uint32_t k = 0; k < np; k++) {
-        const uint32_t t = ptab[k];
+        const uint32_t sl = pslot[k];
         for (uint32_t j = 0; j < pairs[k].count; j++) {
             uint4 &x = rec[pairs[k].first + j];
             if (x.z) continue;
-            const uint64_t a = reinterpret_cast<uint64_t>(e->stage_in2 + sw[t].at(rd_le(e->ring_in + ss[t].at(16 * (pbase[k] + j)), 8)));
+            const uint64_t a = reinterpret_cast<uint64_t>(e->stage_in2 + sw[sl].at(rd_le(e->ring_in + ss[sl].at(16 * (pbase[k] + j)), 8)));
             x.x = (uint32_t)a;
             x.y = (uint32_t)(a >> 32);
         }
     }
-
     // ---- workspace: the round's arrays, then the split of the selected records
     const uint32_t tiles = (n + kRangeTile - 1) / kRangeTile;
     uint64_t off = 0;
@@ -3872,7 +3915,7 @@ int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const
     split_bind(w, ws, &sp, &rp, &p);
     LimitParams lp{reinterpret_cast<const LimitPair *>(ws + o_pairs), reinterpret_cast<const LimitQuery *>(ws + o_q),
                    reinterpret_cast<const uint4 *>(ws + o_rec), reinterpret_cast<const uint32_t *>(ws + o_rpair), n, gq,
-                   keep_tombstones ? 1u : 0u, desc ? 1u : 0u, reinterpret_cast<uint4 *>(ws + o_flat), reinterpret_cast<unsigned long long *>(ws + o_pfx),
+                   reinterpret_cast<uint4 *>(ws + o_flat), reinterpret_cast<unsigned long long *>(ws + o_pfx),
                    reinterpret_cast<uint32_t *>(ws + o_code), reinterpret_cast<uint32_t *>(ws + o_pbad), reinterpret_cast<uint32_t *>(ws + o_setter),
                    reinterpret_cast<uint32_t *>(ws + o_front), reinterpret_cast<uint4 *>(ws + o_qout), reinterpret_cast<const uint32_t *>(ws + o_pre),
                    reinterpret_cast<uint32_t *>(ws + o_pre), reinterpret_cast<uint32_t *>(ws + o_rank), reinterpret_cast<const uint32_t *>(ws + o_qsel),
@@ -3903,13 +3946,14 @@ int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const
     std::vector<uint32_t> qsel(gq, ~0u), done;
     uint32_t n_sel = 0;
     for (uint32_t g = 0; g < gq; g++) {
-        const uint32_t qi = qs[g], lim = limits[qi];
+        const uint32_t qi = qs[g];
         dbeel_range_row &row = rows[qi];
         LimitState &q = st[qi];
+        const uint32_t lim = q.limit;
         const uint4 o = qout[g];
         if (o.z != ~0u) {
             const uint32_t t = ptab[o.z];
-            const uint64_t rec_no = pbase[o.z] + (desc ? pairs[o.z].count - 1 - o.w : o.w); // o.w: from the chunk's fixed end
+            const uint64_t rec_no = pbase[o.z] + (lq[g].desc ? pairs[o.z].count - 1 - o.w : o.w); // o.w: from the chunk's fixed end
             row.flags = o.y == kLimitUnsorted ? DBEEL_RANGE_UNSORTED : DBEEL_RANGE_STOPPED;
             row.stop = dbeel_scan_stop{(int32_t)t, o.y == kLimitUnsorted ? DBEEL_SCAN_STOP_NONE : o.y, rec_no};
             continue;
@@ -3959,86 +4003,116 @@ int limit_round(dbeel_engine *e, dbeel_reader *r, const dbeel_scan_io *io, const
     return DBEEL_OK;
 }
 
-// dbeel_reader_get_ranges, or dbeel_reader_get_ranges_reverse when `desc` (dbeel_compact.h): the bound searches
-// (reader_seek_batched), the spans and seek stops per query, then merge rounds over groups of the live queries of about the
-// partition budget (limit_round) until every query is finished, then the rows and `out` from the emissions, in query order.
-int reader_get_ranges(dbeel_engine *e, dbeel_reader *r, const uint8_t *kb, const std::vector<uint64_t> &ko, uint32_t nq,
-                      const uint32_t *limits, bool keep_tombstones, bool desc, const dbeel_scan_io *io, dbeel_out *out,
-                      dbeel_range_row *rows) {
-    const uint32_t nt = (uint32_t)r->tables.size(), nseek = seek_tables(r);
-    std::vector<uint64_t> boff, blen;
-    const std::vector<uint32_t> vq = range_bounds(kb, ko, nq, &boff, &blen); // the queries with start < end
-    const dbeel_scan_stop empty_stop{(int32_t)nseek, DBEEL_SCAN_STOP_PANIC, 0};
-    if (nseek < nt)
-        for (uint32_t q = 0; q < nq; q++) { rows[q].flags = DBEEL_RANGE_STOPPED; rows[q].stop = empty_stop; }
-    std::vector<unsigned long long> res, bad;
-    std::vector<uint4> bix;
+// The range-read walk of dbeel_reader_get_ranges / _reverse (one batch) and dbeel_readers_get_ranges (dbeel_compact.h): the
+// bound searches of every batch (reader_seek_batched over one part per batch), the spans and seek stops per query, then
+// merge rounds over groups of the live queries of all batches (pack_batches: each batch's groups of about the partition
+// budget as its solo call cuts them, packed whole) until every query is finished, then the rows and `out` from the
+// emissions, in global query order (batch order, then query order), `first` and the .index offsets running across batches.
+// Query q of batch b is row row0[b] + q.  The caller has checked the arguments, taken the engine and cleared stats, out and
+// rows.
+int reader_get_ranges(dbeel_engine *e, const std::vector<RangeBatch> &bs, dbeel_out *out, dbeel_range_row *rows) {
+    const uint32_t nbat = (uint32_t)bs.size();
+    std::vector<uint32_t> row0(nbat + 1, 0), tbase(nbat + 1, 0), nseek(nbat);
+    std::vector<std::vector<uint32_t>> vq(nbat); // the queries with start < end
+    std::vector<SeekPart> sp(nbat);
+    for (uint32_t b = 0; b < nbat; b++) {
+        const RangeBatch &B = bs[b];
+        const uint32_t nt = (uint32_t)B.r->tables.size();
+        nseek[b] = seek_tables(B.r);
+        row0[b + 1] = row0[b] + B.nq;
+        tbase[b + 1] = tbase[b] + nseek[b];
+        sp[b] = SeekPart{B.r, B.io, nseek[b], B.kb, {}, {}, 0, {}, {}, {}};
+        vq[b] = range_bounds(B.kb, B.ko, B.nq, &sp[b].boff, &sp[b].blen);
+        const dbeel_scan_stop empty_stop{(int32_t)nseek[b], DBEEL_SCAN_STOP_PANIC, 0};
+        if (nseek[b] < nt)
+            for (uint32_t q = row0[b]; q < row0[b + 1]; q++) { rows[q].flags = DBEEL_RANGE_STOPPED; rows[q].stop = empty_stop; }
+    }
     int rc;
-    if (!vq.empty() && nseek)
-        if ((rc = reader_seek_batched(e, r, io, nseek, kb, boff, blen, &res, &bad, &bix))) return rc;
+    if ((rc = reader_seek_batched(e, sp))) return rc;
     cudaError_t ce = cudaSetDevice(e->device);
     if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     CU(cudaEventRecord(e->ev[EV_START], e->stream));
-    const uint64_t nb = boff.size();
-    std::vector<LimitState> st(nq);
+    std::vector<LimitState> st(row0[nbat]);
     std::vector<uint32_t> live;
-    for (uint64_t j = 0; j < vq.size(); j++) {
-        const uint32_t q = vq[j];
-        LimitState &x = st[q];
-        x.lo.assign(nseek, 0);
-        x.hi.assign(nseek, 0);
-        x.w.assign(nseek, (uint64_t)limits[q] + 1);
-        bool any = false;
-        for (uint32_t t = 0; t < nseek; t++) {
-            const uint64_t a = t * nb + 2 * j, b = a + 1;
-            const dbeel_scan_stop stop = seek_stop(r, t, bad, bix, a, b + 1);
-            if (stop.table >= 0) {
-                rows[q].flags = DBEEL_RANGE_STOPPED;
-                rows[q].stop = stop;
-                any = false;
-                break;
-            }
-            if (res[a] < res[b] && res[b] != ~0ull) {
-                x.lo[t] = res[a];
-                x.hi[t] = res[b];
-                any = true;
-            }
+    for (uint32_t b = 0; b < nbat; b++) {
+        const RangeBatch &B = bs[b];
+        const uint64_t nb = sp[b].boff.size();
+        for (uint32_t q = row0[b]; q < row0[b + 1]; q++) {
+            st[q].batch = b;
+            st[q].limit = B.limits[q - row0[b]];
         }
-        if (any && !rows[q].flags) live.push_back(q);
+        if (!sp[b].nseek) continue;
+        for (uint64_t j = 0; j < vq[b].size(); j++) {
+            const uint32_t q = row0[b] + vq[b][j];
+            LimitState &x = st[q];
+            x.lo.assign(nseek[b], 0);
+            x.hi.assign(nseek[b], 0);
+            x.w.assign(nseek[b], (uint64_t)x.limit + 1);
+            bool any = false;
+            for (uint32_t t = 0; t < nseek[b]; t++) {
+                const uint64_t a = t * nb + 2 * j, c = a + 1;
+                const dbeel_scan_stop stop = seek_stop(B.r, t, sp[b].bad, sp[b].bix, a, c + 1);
+                if (stop.table >= 0) {
+                    rows[q].flags = DBEEL_RANGE_STOPPED;
+                    rows[q].stop = stop;
+                    any = false;
+                    break;
+                }
+                if (sp[b].res[a] < sp[b].res[c] && sp[b].res[c] != ~0ull) {
+                    x.lo[t] = sp[b].res[a];
+                    x.hi[t] = sp[b].res[c];
+                    any = true;
+                }
+            }
+            if (any && !rows[q].flags) live.push_back(q);
+        }
     }
 
     // ---- rounds: the live queries in groups of about the budget (their chunks' index records and mean entries)
-    std::vector<uint64_t> mean(nseek);
-    for (uint32_t t = 0; t < nseek; t++) mean[t] = (r->tables[t]->desc.data_len + r->tables[t]->desc.n - 1) / r->tables[t]->desc.n;
+    std::vector<std::vector<uint64_t>> mean(nbat);
+    std::vector<int32_t> cache(nbat, -1);
+    std::vector<dbeel_page_cache *> caches;
+    std::vector<uint64_t> cache_bytes;
+    for (uint32_t b = 0; b < nbat; b++) {
+        const dbeel_reader *r = bs[b].r;
+        for (uint32_t t = 0; t < nseek[b]; t++) mean[b].push_back((r->tables[t]->desc.data_len + r->tables[t]->desc.n - 1) / r->tables[t]->desc.n);
+        if (!r->cache) continue;
+        cache[b] = (int32_t)(std::find(caches.begin(), caches.end(), r->cache) - caches.begin());
+        if (cache[b] == (int32_t)caches.size()) {
+            caches.push_back(r->cache);
+            cache_bytes.push_back(kPageBytes * r->cache->pc.capacity());
+        }
+    }
     // per staged record: its .index record, its mean entry and the round's workspace (LimitParams' arrays, the split)
     constexpr uint64_t kLimitRecordBytes = 16 + 128;
-    const uint64_t page_bytes = r->cache ? 2 * kPageBytes : 0;
     std::vector<std::vector<uint8_t>> em; // emission k: data at 2k, index at 2k + 1
     uint32_t launches = 0;
     uint64_t gather_bytes = 0;
     while (!live.empty()) {
         std::vector<uint32_t> next;
-        for (size_t g0 = 0; g0 < live.size();) {
-            size_t g1 = g0;
-            uint64_t bytes = 0;
-            while (g1 < live.size()) {
-                const LimitState &x = st[live[g1]];
-                uint64_t cost = 0;
-                for (uint32_t t = 0; t < nseek; t++)
-                    if (x.hi[t] > x.lo[t]) cost += std::min(x.w[t], x.hi[t] - x.lo[t]) * (kLimitRecordBytes + mean[t]) + page_bytes;
-                if (g1 > g0 && bytes + cost > e->partition_bytes) break;
-                bytes += cost;
-                g1++;
-            }
-            if ((rc = limit_round(e, r, io, live.data() + g0, (uint32_t)(g1 - g0), limits, keep_tombstones, desc, st, rows, &em,
-                                  &next, &launches, &gather_bytes)))
-                return rc;
-            g0 = g1;
+        std::vector<std::vector<uint64_t>> cost(nbat);
+        std::vector<uint32_t> live0(nbat + 1, 0); // batch b's live queries are live[live0[b] ..]
+        for (const uint32_t q : live) {
+            const LimitState &x = st[q];
+            const uint64_t page_bytes = bs[x.batch].r->cache ? 2 * kPageBytes : 0;
+            uint64_t c = 0;
+            for (uint32_t t = 0; t < x.lo.size(); t++)
+                if (x.hi[t] > x.lo[t]) c += std::min(x.w[t], x.hi[t] - x.lo[t]) * (kLimitRecordBytes + mean[x.batch][t]) + page_bytes;
+            cost[x.batch].push_back(c);
+            live0[x.batch + 1]++;
+        }
+        for (uint32_t b = 0; b < nbat; b++) live0[b + 1] += live0[b];
+        for (const std::vector<BatchSpan> &group : pack_batches(cost, cache, e->partition_bytes, cache_bytes)) {
+            std::vector<uint32_t> qs;
+            for (const BatchSpan &u : group)
+                qs.insert(qs.end(), live.begin() + live0[u.batch] + u.k0, live.begin() + live0[u.batch] + u.k1);
+            if ((rc = limit_round(e, bs, tbase, qs.data(), (uint32_t)qs.size(), st, rows, &em, &next, &launches, &gather_bytes))) return rc;
         }
         live.swap(next);
     }
 
     // ---- out: every query's entries, in query order, offsets rebased
+    const uint32_t nq = row0[nbat];
     uint64_t items = 0, bytes = 0;
     for (uint32_t q = 0; q < nq; q++) {
         rows[q].first = items;
@@ -4080,42 +4154,66 @@ int reader_get_ranges(dbeel_engine *e, dbeel_reader *r, const uint8_t *kb, const
     return DBEEL_OK;
 }
 
+// The checks of one batch of key ranges with limits (dbeel_reader_get_ranges): its key offsets (ko, from 0), limits and
+// flags; *total grows by its limits.
+int range_batch_args(dbeel_engine *e, const dbeel_key_ranges *kr, uint32_t nq, const uint32_t *limits, uint32_t flags,
+                     std::vector<uint64_t> *ko, uint64_t *total) {
+    if (flags & ~DBEEL_RANGE_KEEP_TOMBSTONES) return fail(e, DBEEL_ERR_INVALID_ARG, "unknown flag");
+    if (!nq) return DBEEL_OK;
+    if (!kr->key_offsets || !limits) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    for (uint32_t q = 0; q < nq; q++) {
+        if (limits[q] == 0 || limits[q] > DBEEL_RANGE_LIMIT_MAX) return fail(e, DBEEL_ERR_INVALID_ARG, "a limit must be 1 .. DBEEL_RANGE_LIMIT_MAX");
+        *total += limits[q];
+    }
+    if (*total >= 0xFFFFFFF0ull) return fail(e, DBEEL_ERR_INVALID_ARG, "the limits sum to 2^32 - 16 or more");
+    ko->resize(2ull * nq + 1);
+    for (uint64_t k = 0; k <= 2ull * nq; k++) {
+        if (k && kr->key_offsets[k] < kr->key_offsets[k - 1]) return fail(e, DBEEL_ERR_INVALID_ARG, "key_offsets must not decrease");
+        (*ko)[k] = kr->key_offsets[k] - kr->key_offsets[0];
+    }
+    if ((*ko)[2ull * nq] && !kr->keys) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    return DBEEL_OK;
+}
+
+// Takes the engine, runs the walk over the checked batches (one ReaderScanIo each, so input_bytes counts every byte read
+// through every reader's callback) and leaves rows cleared after any error other than capacity.
+int ranges_entry(dbeel_engine *e, std::vector<RangeBatch> &bs, dbeel_out *out, dbeel_range_row *rows) {
+    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    BusyGuard g(e);
+    e->err.clear();
+    e->stats = dbeel_stats{};
+    out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
+    uint64_t nq = 0;
+    for (const RangeBatch &B : bs) nq += B.nq;
+    for (uint64_t q = 0; q < nq; q++) rows[q] = dbeel_range_row{0, 0, 0, dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0}};
+    std::vector<ReaderScanIo> x(bs.size());
+    std::vector<dbeel_scan_io> io(bs.size());
+    for (size_t b = 0; b < bs.size(); b++) {
+        x[b].rio = &bs[b].r->io;
+        io[b] = dbeel_scan_io{reader_scan_read, nullptr, &x[b]};
+        bs[b].io = &io[b];
+    }
+    const int rc = reader_get_ranges(e, bs, out, rows);
+    if (rc && rc != DBEEL_ERR_CAPACITY) {
+        cudaStreamSynchronize(e->stream); // nothing of this call may touch the engine's buffers after it returns
+        for (uint64_t q = 0; q < nq; q++) rows[q] = dbeel_range_row{0, 0, 0, dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0}};
+    }
+    e->stats.input_bytes = 0;
+    for (const ReaderScanIo &y : x) e->stats.input_bytes += y.bytes;
+    return rc;
+}
+
 int reader_get_ranges_entry(dbeel_reader *r, const dbeel_key_ranges *kr, uint32_t nq, const uint32_t *limits, uint32_t flags,
                             bool desc, dbeel_out *out, dbeel_range_row *rows) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
     dbeel_engine *e = r->e;
     if (!kr || !kr->key_offsets || !limits || !out || !rows) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     if (nq == 0) return fail(e, DBEEL_ERR_INVALID_ARG, "n_ranges must be at least 1");
-    if (flags & ~DBEEL_RANGE_KEEP_TOMBSTONES) return fail(e, DBEEL_ERR_INVALID_ARG, "unknown flag");
+    std::vector<RangeBatch> bs{RangeBatch{r, nullptr, nullptr, {}, nq, limits, (flags & DBEEL_RANGE_KEEP_TOMBSTONES) != 0, desc}};
     uint64_t total = 0;
-    for (uint32_t q = 0; q < nq; q++) {
-        if (limits[q] == 0 || limits[q] > DBEEL_RANGE_LIMIT_MAX) return fail(e, DBEEL_ERR_INVALID_ARG, "a limit must be 1 .. DBEEL_RANGE_LIMIT_MAX");
-        total += limits[q];
-    }
-    if (total >= 0xFFFFFFF0ull) return fail(e, DBEEL_ERR_INVALID_ARG, "the limits sum to 2^32 - 16 or more");
-    std::vector<uint64_t> ko(2ull * nq + 1);
-    for (uint64_t k = 0; k <= 2ull * nq; k++) {
-        if (k && kr->key_offsets[k] < kr->key_offsets[k - 1]) return fail(e, DBEEL_ERR_INVALID_ARG, "key_offsets must not decrease");
-        ko[k] = kr->key_offsets[k] - kr->key_offsets[0];
-    }
-    if (ko[2ull * nq] && !kr->keys) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
-    out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
-    for (uint32_t q = 0; q < nq; q++) rows[q] = dbeel_range_row{0, 0, 0, dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0}};
-    ReaderScanIo x;
-    x.rio = &r->io;
-    const dbeel_scan_io io{reader_scan_read, nullptr, &x};
-    const uint8_t *kb = ko[2ull * nq] ? static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0] : nullptr;
-    const int rc = reader_get_ranges(e, r, kb, ko, nq, limits, (flags & DBEEL_RANGE_KEEP_TOMBSTONES) != 0, desc, &io, out, rows);
-    if (rc && rc != DBEEL_ERR_CAPACITY) {
-        cudaStreamSynchronize(e->stream); // nothing of this call may touch the engine's buffers after it returns
-        for (uint32_t q = 0; q < nq; q++) rows[q] = dbeel_range_row{0, 0, 0, dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0}};
-    }
-    e->stats.input_bytes = x.bytes;
-    return rc;
+    if (const int rc = range_batch_args(e, kr, nq, limits, flags, &bs[0].ko, &total)) return rc;
+    if (bs[0].ko[2ull * nq]) bs[0].kb = static_cast<const uint8_t *>(kr->keys) + kr->key_offsets[0];
+    return ranges_entry(e, bs, out, rows);
 }
 
 } // namespace
@@ -4593,6 +4691,27 @@ int dbeel_reader_get_ranges_reverse(dbeel_reader *r, const dbeel_key_ranges *ran
     if (!r) return DBEEL_ERR_INVALID_ARG;
     REFUSE_WHILE_ASYNC(r->e);
     return reader_get_ranges_entry(r, ranges, n_ranges, limits, flags, true, out, rows);
+}
+
+int dbeel_readers_get_ranges(dbeel_engine *e, const dbeel_range_batch *batches, uint32_t n_batches, dbeel_out *out,
+                             dbeel_range_row *rows) {
+    REFUSE_WHILE_ASYNC(e);
+    if (!e) return DBEEL_ERR_INVALID_ARG;
+    if (!batches || !out || !rows) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
+    if (n_batches == 0 || n_batches > DBEEL_MAX_READER_BATCHES) return fail(e, DBEEL_ERR_INVALID_ARG, "n_batches is 0 or above DBEEL_MAX_READER_BATCHES");
+    std::vector<RangeBatch> bs(n_batches);
+    uint64_t total = 0;
+    for (uint32_t b = 0; b < n_batches; b++) {
+        const dbeel_range_batch &x = batches[b];
+        if (!x.reader) return fail(e, DBEEL_ERR_INVALID_ARG, "null reader");
+        if (x.reader->e != e) return fail(e, DBEEL_ERR_INVALID_ARG, "a reader of another engine");
+        if (x.reverse > 1) return fail(e, DBEEL_ERR_INVALID_ARG, "reverse is not 0 or 1");
+        if (x.reserved) return fail(e, DBEEL_ERR_INVALID_ARG, "reserved is not 0");
+        bs[b] = RangeBatch{x.reader, nullptr, nullptr, {}, x.n_ranges, x.limits, (x.flags & DBEEL_RANGE_KEEP_TOMBSTONES) != 0, x.reverse != 0};
+        if (const int rc = range_batch_args(e, &x.ranges, x.n_ranges, x.limits, x.flags, &bs[b].ko, &total)) return rc;
+        if (x.n_ranges && bs[b].ko[2ull * x.n_ranges]) bs[b].kb = static_cast<const uint8_t *>(x.ranges.keys) + x.ranges.key_offsets[0];
+    }
+    return ranges_entry(e, bs, out, rows);
 }
 
 int dbeel_page_cache_create(dbeel_engine *e, uint64_t bytes, dbeel_page_cache **out) {

@@ -264,6 +264,61 @@ inline std::vector<size_t> group_leaves(const std::vector<TouchedLeaf> &leaves, 
     return cut;
 }
 
+// ---- range reads across readers (dbeel_readers_get_ranges): seek batches and query groups of many batches
+//
+// Units of bytes[k], in order, cut into groups: a group takes the next unit while its bytes stay within `budget` and, for a
+// unit that goes through page cache cache[k] >= 0, the bytes of that cache's units within cache_bytes[cache[k]] (an empty
+// `cache`: none does); a group holds at least one unit.  Group g is units [cut[g], cut[g + 1]).
+inline std::vector<size_t> pack_in_order(const std::vector<uint64_t> &bytes, uint64_t budget, const std::vector<int32_t> &cache = {},
+                                         const std::vector<uint64_t> &cache_bytes = {}) {
+    std::vector<size_t> cut = {0};
+    uint64_t est = 0;
+    std::vector<uint64_t> est_c(cache_bytes.size(), 0);
+    for (size_t k = 0; k < bytes.size(); k++) {
+        const int32_t c = cache.empty() ? -1 : cache[k];
+        if (k > cut.back() && (est + bytes[k] > budget || (c >= 0 && est_c[c] + bytes[k] > cache_bytes[c]))) {
+            cut.push_back(k);
+            est = 0;
+            std::fill(est_c.begin(), est_c.end(), 0);
+        }
+        est += bytes[k];
+        if (c >= 0) est_c[c] += bytes[k];
+    }
+    if (!bytes.empty()) cut.push_back(bytes.size());
+    return cut;
+}
+
+// Units [k0, k1) of batch `batch`.
+struct BatchSpan {
+    uint32_t batch;
+    size_t k0, k1;
+};
+
+// The units of many batches in groups: batch b's units (cost[b], in order) are first cut as its solo call cuts them
+// (pack_in_order with the budget alone); those solo groups then fill groups whole, in batch order, while the budget and
+// each page cache's capacity hold (batch b goes through cache[b], -1 = none).  So every group of one batch is one of its
+// solo groups, and one batch is grouped exactly as its solo call groups it.
+inline std::vector<std::vector<BatchSpan>> pack_batches(const std::vector<std::vector<uint64_t>> &cost, const std::vector<int32_t> &cache,
+                                                        uint64_t budget, const std::vector<uint64_t> &cache_bytes) {
+    std::vector<BatchSpan> solo;
+    std::vector<uint64_t> bytes;
+    std::vector<int32_t> uc;
+    for (uint32_t b = 0; b < cost.size(); b++) {
+        const std::vector<size_t> cut = pack_in_order(cost[b], budget);
+        for (size_t g = 0; g + 1 < cut.size(); g++) {
+            solo.push_back(BatchSpan{b, cut[g], cut[g + 1]});
+            uint64_t x = 0;
+            for (size_t k = cut[g]; k < cut[g + 1]; k++) x += cost[b][k];
+            bytes.push_back(x);
+            uc.push_back(cache[b]);
+        }
+    }
+    const std::vector<size_t> cut = pack_in_order(bytes, budget, uc, cache_bytes);
+    std::vector<std::vector<BatchSpan>> out;
+    for (size_t g = 0; g + 1 < cut.size(); g++) out.emplace_back(solo.begin() + cut[g], solo.begin() + cut[g + 1]);
+    return out;
+}
+
 // ---- readers (dbeel_reader_*): fences kept on the device across batches
 //
 // A reader keeps, per table and mode, the fences of the top D_t levels of the probe tree: for every node k < 2^D_t its

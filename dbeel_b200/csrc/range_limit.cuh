@@ -1,7 +1,8 @@
-// range_limit.cuh -- one merge round of dbeel_reader_get_ranges / _reverse: per query, a prefix (forward) or a suffix
-// (reverse, LimitParams.desc) of every table's span records (a "pair" = one query and one table, its chunk staged as
+// range_limit.cuh -- one merge round of dbeel_reader_get_ranges / _reverse / dbeel_readers_get_ranges: per query, a
+// prefix (forward) or a suffix (reverse, LimitQuery.desc) of every table's span records (a "pair" = one query and one table, its chunk staged as
 // {entry address, index status, full_size} records), merged into the query's first (forward) or last (reverse) entries
 // under dbeel_reader_get_range's rule -- the newest table's version of a key wins, tombstones dropped unless asked for.
+// Direction and the tombstone rule are the query's own, so one round serves forward and reverse queries of many readers.
 // Pairs of a query lie together, tables ascending; a pair's records lie in record order in both directions.
 //
 //   k_limit_decode  per record: the scan's decode (PANIC / ERR), the flat split record {address, 8 + klen, full_size},
@@ -39,7 +40,9 @@ struct LimitPair {
 struct LimitQuery {
     uint32_t pair0, pair1; // its pairs
     uint32_t first, last;  // its records
-    uint32_t limit, pad;
+    uint32_t limit;
+    uint16_t desc;            // 1: reverse -- chunks end at the span's end, the last entries in descending key order
+    uint16_t keep_tombstones; // 1: tombstones are entries
 };
 
 struct LimitParams {
@@ -47,8 +50,7 @@ struct LimitParams {
     const LimitQuery *queries;
     const uint4 *rec;              // [n] {entry address (x, y), kScanStopPanic when the index record alone shows it, full_size}
     const uint32_t *rpair;         // [n] pair of every record
-    uint32_t n, n_queries, keep_tombstones;
-    uint32_t desc;                 // 1: reverse -- chunks end at the span's end, the last entries in descending key order
+    uint32_t n, n_queries;
     uint4 *flat;                   // [n] {entry address, 8 + klen, full_size}
     unsigned long long *pfx;       // [n]
     uint32_t *code;                // [n] 0 or the record's damage (kScanStopErr, kScanStopPanic, kLimitUnsorted)
@@ -114,14 +116,15 @@ __global__ void __launch_bounds__(256) k_limit_decode(LimitParams p) {
     p.pfx[i] = ok ? range_prefix(key, (uint32_t)kl) : 0ull;
     const uint32_t pr = p.rpair[i];
     const LimitPair pp = p.pairs[pr];
-    const uint32_t j = p.desc ? i + 1 : i - 1; // the neighbour: previous record (forward), next record (reverse)
+    const bool desc = p.queries[pp.query].desc;
+    const uint32_t j = desc ? i + 1 : i - 1; // the neighbour: previous record (forward), next record (reverse)
     uint64_t nkl = 0;
-    if (ok && (p.desc ? j < pp.first + pp.count : i > pp.first) && limit_decode(p.rec[j], &nkl)) {
+    if (ok && (desc ? j < pp.first + pp.count : i > pp.first) && limit_decode(p.rec[j], &nkl)) {
         const int c = scan_key_cmp(range_entry(p.rec[j]) + 8, nkl, key, kl);
-        if (p.desc ? c <= 0 : c >= 0) code = kLimitUnsorted;
+        if (desc ? c <= 0 : c >= 0) code = kLimitUnsorted;
     }
     p.code[i] = code;
-    if (code) atomicMin(&p.pair_bad[pr], p.desc ? pp.first + pp.count - 1 - i : i - pp.first);
+    if (code) atomicMin(&p.pair_bad[pr], desc ? pp.first + pp.count - 1 - i : i - pp.first);
 }
 
 __global__ void __launch_bounds__(256) k_limit_query(LimitParams p) {
@@ -130,11 +133,12 @@ __global__ void __launch_bounds__(256) k_limit_query(LimitParams p) {
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= p.n_queries) return;
     const LimitQuery Q = p.queries[q];
+    const bool desc = Q.desc;
     for (uint32_t k = Q.pair0; k < Q.pair1; k++) {
         const uint32_t b = p.pair_bad[k];
         if (b != ~0u) {
             const LimitPair pp = p.pairs[k];
-            p.qout[q] = make_uint4(0, p.code[p.desc ? pp.first + pp.count - 1 - b : pp.first + b], k, b);
+            p.qout[q] = make_uint4(0, p.code[desc ? pp.first + pp.count - 1 - b : pp.first + b], k, b);
             p.front[q] = ~0u;
             return;
         }
@@ -143,18 +147,18 @@ __global__ void __launch_bounds__(256) k_limit_query(LimitParams p) {
     for (uint32_t k = Q.pair0; k < Q.pair1; k++) {
         const LimitPair pp = p.pairs[k];
         if (!pp.truncated || !pp.count) continue;
-        const uint32_t j = p.desc ? pp.first : pp.first + pp.count - 1; // the staged record nearest the span's far end
+        const uint32_t j = desc ? pp.first : pp.first + pp.count - 1; // the staged record nearest the span's far end
         const uint4 r = p.flat[j];
         if (best == ~0u) { best = j; continue; }
         const int c = limit_cmp(p, j, p.pfx[j], range_entry(r) + 8, r.z - 8, best);
-        if (p.desc ? c > 0 : c < 0) best = j;
+        if (desc ? c > 0 : c < 0) best = j;
     }
     for (uint32_t k = Q.pair0; k < Q.pair1; k++) {
         const LimitPair pp = p.pairs[k];
         bool set = false;
         if (best != ~0u && pp.truncated && pp.count) {
             const uint4 r = p.flat[best];
-            set = limit_cmp(p, best, p.pfx[best], range_entry(r) + 8, r.z - 8, p.desc ? pp.first : pp.first + pp.count - 1) == 0;
+            set = limit_cmp(p, best, p.pfx[best], range_entry(r) + 8, r.z - 8, desc ? pp.first : pp.first + pp.count - 1) == 0;
         }
         p.setter[k] = set ? 1u : 0u;
     }
@@ -169,6 +173,7 @@ __global__ void __launch_bounds__(256) k_limit_flag(LimitParams p) {
     if (i >= p.n) return;
     const uint32_t pr = p.rpair[i];
     const uint32_t q = p.pairs[pr].query;
+    const LimitQuery Q = p.queries[q];
     bool keep = p.qout[q].y == 0;
     const uint4 r = p.flat[i];
     const uint8_t *k = range_entry(r) + 8;
@@ -177,11 +182,10 @@ __global__ void __launch_bounds__(256) k_limit_flag(LimitParams p) {
     const uint32_t f = p.front[q];
     if (keep && f != ~0u) {
         const int c = limit_cmp(p, i, pk, k, kl, f);
-        keep = p.desc ? c >= 0 : c <= 0;
+        keep = Q.desc ? c >= 0 : c <= 0;
     }
-    if (keep) keep = p.keep_tombstones || ld_u64_unaligned_narrow(k + kl) != 0;
-    const uint32_t pair1 = p.queries[q].pair1;
-    for (uint32_t x = pr + 1; keep && x < pair1; x++) { // a newer table staged the key
+    if (keep) keep = Q.keep_tombstones || ld_u64_unaligned_narrow(k + kl) != 0;
+    for (uint32_t x = pr + 1; keep && x < Q.pair1; x++) { // a newer table staged the key
         const LimitPair pp = p.pairs[x];
         const uint32_t at = limit_lower_bound(p, pp, pk, k, kl);
         if (at < pp.first + pp.count && limit_cmp(p, i, pk, k, kl, at) == 0) keep = false;
@@ -206,12 +210,12 @@ __global__ void __launch_bounds__(256) k_limit_rank(LimitParams p) {
     const uint32_t kl = r.z - 8;
     const unsigned long long pk = p.pfx[i];
     // reverse: survivors after it in its pair, and every other pair's at or above its key (none there equals it)
-    uint32_t rank = p.desc ? p.pre[mine.first + mine.count] - p.pre[i + 1] : p.pre[i] - p.pre[mine.first];
+    uint32_t rank = Q.desc ? p.pre[mine.first + mine.count] - p.pre[i + 1] : p.pre[i] - p.pre[mine.first];
     for (uint32_t x = Q.pair0; x < Q.pair1; x++) {
         if (x == pr) continue;
         const LimitPair pp = p.pairs[x];
         const uint32_t at = limit_lower_bound(p, pp, pk, k, kl);
-        rank += p.desc ? p.pre[pp.first + pp.count] - p.pre[at] : p.pre[at] - p.pre[pp.first];
+        rank += Q.desc ? p.pre[pp.first + pp.count] - p.pre[at] : p.pre[at] - p.pre[pp.first];
     }
     p.rank[i] = rank;
 }

@@ -680,6 +680,46 @@ int dbeel_reader_get_ranges(dbeel_reader *r, const dbeel_key_ranges *ranges, uin
  *            record not below its successor).  A flag other than DBEEL_RANGE_KEEP_TOMBSTONES is DBEEL_ERR_INVALID_ARG. */
 int dbeel_reader_get_ranges_reverse(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, const uint32_t *limits,
                                     uint32_t flags, dbeel_out *out, dbeel_range_row *rows);
+
+/* Range reads across readers: the limited range-read batches of many readers of one engine in one call (a node whose
+ * shards each have a page of a listing waiting, next pages and previous pages mixed), so that they share the bound
+ * searches and the merge rounds instead of paying them once per reader.  Batch b asks
+ * dbeel_reader_get_ranges(reader, &ranges, n_ranges, limits, flags, ...) when reverse is 0 and
+ * dbeel_reader_get_ranges_reverse(...) when it is 1; a batch of n_ranges 0 asks nothing.
+ * Result: exactly those solo calls for b = 0, 1, ... in order, concatenated.  rows has sum(n_ranges) rows in batch order;
+ * each row's count, flags and stop are its solo row's (stop.table is a position in that batch's own reader's tables), and
+ * its first is the solo row's first plus the entries of the batches before it.  out is the solo outputs appended: batch
+ * b's .index offsets are shifted by the .data bytes before it; items_written is the total.  One batch's damage, stops,
+ * empty tables or tombstone runs never change another batch's rows, also for two batches on the same reader, in the same
+ * or opposite directions.
+ * Reads: the bound searches of all batches run together: each batch's bounds are cut into its solo call's seek batches
+ * (the same depth and cache decisions per table), and seek batches of consecutive batches share one search while they fit
+ * the partition budget.  The merge rounds run the live queries of all batches together: each batch's groups are its solo
+ * call's, packed whole in batch order while they fit the budget and each page cache's capacity.  A query's chunks,
+ * doubling and finish test depend on its own state only, so its row is its solo row in any group.  Every read goes through
+ * the pair's own reader's io->read and page cache, and lies inside what the solo calls, made in batch order on readers in
+ * the same state, read for that table and file kind.  With no page cache, input_bytes is at most the sum of the solo
+ * calls'.
+ * Errors leave every reader, the engine and every page cache usable: DBEEL_ERR_INVALID_ARG for null batches / out / rows,
+ * n_batches of 0 or above DBEEL_MAX_READER_BATCHES, a null reader or a reader of another engine, a null key_offsets or
+ * limits in a batch with ranges, key_offsets that decrease, null keys with key bytes, a limit of 0 or above
+ * DBEEL_RANGE_LIMIT_MAX, a flag other than DBEEL_RANGE_KEEP_TOMBSTONES, reverse above 1 or nonzero reserved, or a sum of
+ * all limits >= 2^32 - 16; DBEEL_ERR_CAPACITY as dbeel_reader_get_ranges (every row filled, out->data_len / index_len =
+ * the sizes the whole call needs, nothing written); a callback's nonzero return unchanged; DBEEL_ERR_BUSY while another
+ * call runs on the engine.
+ * dbeel_last_stats: input_bytes = every byte read through every reader's callback, entries_in = index records staged,
+ * partitions = merge rounds run, kernel_launches and gather_bytes summed, entries_out / output_bytes = what was returned. */
+typedef struct dbeel_range_batch {
+    dbeel_reader *reader;
+    dbeel_key_ranges ranges; /* 2 * n_ranges + 1 key offsets, as dbeel_reader_get_ranges */
+    const uint32_t *limits;  /* n_ranges limits */
+    uint32_t n_ranges;       /* 0 allowed: the batch asks nothing */
+    uint32_t flags;          /* DBEEL_RANGE_KEEP_TOMBSTONES only */
+    uint32_t reverse;        /* 0: dbeel_reader_get_ranges, 1: dbeel_reader_get_ranges_reverse */
+    uint32_t reserved;       /* 0 */
+} dbeel_range_batch;
+int dbeel_readers_get_ranges(dbeel_engine *e, const dbeel_range_batch *batches, uint32_t n_batches, dbeel_out *out,
+                             dbeel_range_row *rows);
 void dbeel_reader_close(dbeel_reader *r);
 
 /* Page cache for readers: the reference reads every .data / .index byte of a lookup or seek through a per-shard cache of
