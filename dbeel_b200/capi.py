@@ -33,6 +33,7 @@ ERR_UNSORTED_RUN = 8
 ERR_CAPACITY = 2
 ERR_INVALID_ARG = 1
 ERR_NO_DEVICE = 9
+ERR_BUSY = 10
 FLAG_VERIFY_SORTED = 0x1
 FLAG_REFERENCE_READER = 0x2  # decode runs like read_next_entry (lsm_tree.rs:1158-1170): offset / key_size ignored, timestamps range-checked
 DEFAULT_BLOOM_MIN_SIZE = 1_048_576

@@ -42,6 +42,13 @@ namespace {
 constexpr uint64_t kAlign = 256;
 inline uint64_t align_up(uint64_t v, uint64_t a) { return (v + a - 1) / a * a; }
 
+// the offset of the next b bytes of a workspace being laid out at *off, each piece 256-byte aligned
+uint64_t carve_ws(uint64_t *off, uint64_t b) {
+    const uint64_t o = *off;
+    *off = align_up(*off + b, kAlign);
+    return o;
+}
+
 enum { EV_START = 0, EV_EXTRACT, EV_MERGE, EV_RESOLVE, EV_GATHER, EV_H2D0, EV_H2D1, EV_D2H0, EV_D2H1, EV_COUNT };
 
 } // namespace
@@ -80,7 +87,7 @@ struct dbeel_engine {
     uint64_t pin_cap = 0;
     dbeel_stats stats = {};
     std::string err;
-    bool busy = false;
+    std::atomic<bool> busy{false}; // a call holds the engine (Claim)
     std::vector<dbeel_reader *> readers; // open readers (dbeel_reader_open, dbeel_tree_reader_open): closed with the engine
     std::vector<dbeel_page_cache *> page_caches; // open page caches (dbeel_page_cache_create): destroyed with the engine
     // asynchronous jobs (dbeel_compact_submit)
@@ -104,7 +111,15 @@ struct dbeel_engine {
 
 namespace {
 
+// the engine whose asynchronous job runs on this thread (dbeel_compact_submit's worker)
+thread_local const dbeel_engine *t_job_engine = nullptr;
+
+// From dbeel_compact_submit until dbeel_poll / dbeel_wait reaps the job, e->err and e->stats are the job's: every other call
+// is refused with DBEEL_ERR_BUSY and touches neither (BUSY is an expected answer for a reactor that polls).
+bool refused(const dbeel_engine *e) { return e->async_state.load(std::memory_order_acquire) != 0 && t_job_engine != e; }
+
 int fail(dbeel_engine *e, int code, const char *what, cudaError_t ce = cudaSuccess) {
+    if (e && refused(e)) return DBEEL_ERR_BUSY; // an argument check ahead of the Claim: the job's error text stays
     char buf[512];
     if (ce != cudaSuccess)
         snprintf(buf, sizeof buf, "%s: %s (%s)", what, cudaGetErrorName(ce), cudaGetErrorString(ce));
@@ -132,6 +147,77 @@ int ensure_device(dbeel_engine *e, uint8_t **buf, uint64_t *cap, uint64_t need) 
     }
     if (ce != cudaSuccess) { cudaGetLastError(); return fail(e, DBEEL_ERR_NOMEM, "cudaMalloc(workspace)", ce); }
     *cap = want;
+    return DBEEL_OK;
+}
+
+// Taking the engine.  Every call that uses it holds a Claim from where it takes the engine until it returns: refused (rc =
+// DBEEL_ERR_BUSY, nothing touched) while an asynchronous job is unreaped, "engine busy" while another call holds it.  A
+// taken engine starts with no error text and zeroed stats, on its device.
+class Claim {
+  public:
+    explicit Claim(dbeel_engine *e) {
+        if (refused(e)) { rc = DBEEL_ERR_BUSY; return; }
+        if (e->busy.exchange(true, std::memory_order_acquire)) { rc = fail(e, DBEEL_ERR_BUSY, "engine busy"); return; }
+        e_ = e;
+        e->err.clear();
+        e->stats = dbeel_stats{};
+        const cudaError_t ce = cudaSetDevice(e->device);
+        if (ce != cudaSuccess) rc = fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    }
+    ~Claim() { if (e_) e_->busy.store(false, std::memory_order_release); }
+    Claim(const Claim &) = delete;
+    Claim &operator=(const Claim &) = delete;
+    int rc = DBEEL_OK;
+
+  private:
+    dbeel_engine *e_ = nullptr;
+};
+
+// Host staging of the entry points that take whole host buffers.  Every piece starts 256-byte aligned and has kStageSlack
+// bytes behind it: the kernels load an entry's 16-byte head as two ld_u64_unaligned (aligned 8-byte words) without
+// checking where the buffer ends, so a head that starts in a piece's last 16 bytes reads up to 23 bytes past them.
+constexpr uint64_t kStageSlack = 32;
+
+struct HostPiece {
+    const void *src;
+    uint64_t len;
+    const uint8_t *dev; // set by stage_host
+};
+
+// Lays the pieces back to back into stage_in and enqueues their copies on the engine's stream.
+int stage_host(dbeel_engine *e, std::vector<HostPiece> &pieces) {
+    uint64_t need = 0;
+    for (const HostPiece &p : pieces) need += align_up(p.len + kStageSlack, kAlign);
+    if (const int rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, need)) return rc;
+    uint64_t pos = 0;
+    for (HostPiece &p : pieces) {
+        p.dev = e->stage_in + pos;
+        if (p.len) CU(cudaMemcpyAsync(e->stage_in + pos, p.src, p.len, cudaMemcpyHostToDevice, e->stream));
+        pos += align_up(p.len + kStageSlack, kAlign);
+    }
+    return DBEEL_OK;
+}
+
+// *dout = outputs of data / index / bloom bytes in stage_out (bloom 0: none), with those capacities, nothing written yet.
+int stage_outputs(dbeel_engine *e, uint64_t data, uint64_t index, uint64_t bloom, dbeel_out *dout) {
+    const uint64_t o_index = align_up(data + kStageSlack, kAlign), o_bloom = o_index + align_up(index + kStageSlack, kAlign);
+    if (const int rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, o_bloom + (bloom ? align_up(bloom + kStageSlack, kAlign) : 0)))
+        return rc;
+    *dout = dbeel_out{e->stage_out, data, 0, e->stage_out + o_index, index, 0, bloom ? e->stage_out + o_bloom : nullptr, bloom, 0, 0};
+    return DBEEL_OK;
+}
+
+// Enqueues the copies of what was written into outputs from stage_outputs (the filter: bloom_len bytes) back to `out` and
+// sets its lengths; the caller synchronizes.
+int copy_back(dbeel_engine *e, const dbeel_out &dout, uint64_t bloom_len, dbeel_out *out) {
+    cudaStream_t s = e->stream;
+    if (dout.data_len) CU(cudaMemcpyAsync(out->data, dout.data, dout.data_len, cudaMemcpyDeviceToHost, s));
+    if (dout.index_len) CU(cudaMemcpyAsync(out->index, dout.index, dout.index_len, cudaMemcpyDeviceToHost, s));
+    if (bloom_len) CU(cudaMemcpyAsync(out->bloom, dout.bloom, bloom_len, cudaMemcpyDeviceToHost, s));
+    out->data_len = dout.data_len;
+    out->index_len = dout.index_len;
+    out->bloom_len = bloom_len;
+    out->items_written = dout.items_written;
     return DBEEL_OK;
 }
 
@@ -271,7 +357,7 @@ struct JobExtra {
 
 // The whole device-resident job.  `runs` / `out` hold device pointers.
 int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, const dbeel_compact_opts *o,
-                   bool flush, dbeel_out *out, bool record_start, const JobExtra *extra = nullptr) {
+                   bool flush, dbeel_out *out, const JobExtra *extra = nullptr) {
     JobShape sh;
     shape_of(runs, n_runs, o, flush, &sh);
     if (extra && (extra->external_bloom || extra->n_jobs)) sh.bloom_file = 0; // compact-many: per-job filters, sized by the caller
@@ -295,9 +381,7 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
         return fail(e, DBEEL_ERR_INVALID_ARG, "null output buffer");
 
     dbeel_stats &st = e->stats;
-    float h2d = st.ms_h2d; // set by the host wrapper before we get here
     memset(&st, 0, sizeof st);
-    st.ms_h2d = h2d;
     st.input_bytes = sh.data_total + sh.index_total;
     st.entries_in = sh.n_total;
     out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
@@ -363,41 +447,40 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
 
     // ---- carve the workspace
     uint64_t off = 0;
-    auto carve = [&](uint64_t bytes) { uint64_t o2 = off; off = align_up(off + bytes, kAlign); return o2; };
     // header block (host-initialised, one H2D copy): ctl | runs | first_bad | first_mismatch
-    const uint64_t o_ctl = carve(sizeof(Ctl));
-    const uint64_t o_runs = carve(sizeof(RunDesc) * n_runs);
-    const uint64_t o_fbad = carve(4ull * n_runs);
-    const uint64_t o_fmis = carve(4ull * n_runs);
-    const uint64_t o_groups = carve(jobs ? sizeof(GroupDesc) * (uint64_t)extra->n_jobs : 0);
+    const uint64_t o_ctl = carve_ws(&off, sizeof(Ctl));
+    const uint64_t o_runs = carve_ws(&off, sizeof(RunDesc) * n_runs);
+    const uint64_t o_fbad = carve_ws(&off, 4ull * n_runs);
+    const uint64_t o_fmis = carve_ws(&off, 4ull * n_runs);
+    const uint64_t o_groups = carve_ws(&off, jobs ? sizeof(GroupDesc) * (uint64_t)extra->n_jobs : 0);
     const uint64_t header_bytes = off;
     uint64_t o_seg[kMaxLevels + 1], o_tb[kMaxLevels];
-    for (uint32_t l = 0; l <= levels; l++) o_seg[l] = carve(sizeof(Seg) * p.nseg[l]);
-    for (uint32_t l = 0; l < levels; l++) o_tb[l] = carve(4ull * (p.nseg[l + 1] + 1));
+    for (uint32_t l = 0; l <= levels; l++) o_seg[l] = carve_ws(&off, sizeof(Seg) * p.nseg[l]);
+    for (uint32_t l = 0; l < levels; l++) o_tb[l] = carve_ws(&off, 4ull * (p.nseg[l + 1] + 1));
     const uint64_t tiles_ub = (uint64_t)(N + kFinNominal - 1) / kFinNominal + (p.nseg[0] + 1) / 2; // kFinNominal < kMergeTile: covers both
     const uint64_t bounds_ub = tiles_ub + (p.nseg[0] + 1) / 2 + 1;
-    const uint64_t o_part = carve(4 * bounds_ub);
-    const uint64_t o_pext = carve(4 * bounds_ub);
-    const uint64_t o_bnd = carve(16 * (bounds_ub + 1));
-    const uint64_t o_tbnd = carve(4 * (tiles_ub + 1));
+    const uint64_t o_part = carve_ws(&off, 4 * bounds_ub);
+    const uint64_t o_pext = carve_ws(&off, 4 * bounds_ub);
+    const uint64_t o_bnd = carve_ws(&off, 16 * (bounds_ub + 1));
+    const uint64_t o_tbnd = carve_ws(&off, 4 * (tiles_ub + 1));
     const uint64_t res_tiles = (uint64_t)(N + kResolveThreads - 1) / kResolveThreads;
-    const uint64_t o_tbytes = carve(res_tiles * 8), o_tcount = carve(res_tiles * 4);
+    const uint64_t o_tbytes = carve_ws(&off, res_tiles * 8), o_tcount = carve_ws(&off, res_tiles * 4);
     const uint64_t res_chunks = (res_tiles + 1023) / 1024;
-    const uint64_t o_cbytes = carve(res_chunks * 8), o_ccount = carve(res_chunks * 4);
-    const uint64_t o_reca = carve(16ull * N), o_recb = carve(16ull * N);
-    const uint64_t o_src = carve(8ull * N);
+    const uint64_t o_cbytes = carve_ws(&off, res_chunks * 8), o_ccount = carve_ws(&off, res_chunks * 4);
+    const uint64_t o_reca = carve_ws(&off, 16ull * N), o_recb = carve_ws(&off, 16ull * N);
+    const uint64_t o_src = carve_ws(&off, 8ull * N);
     const uint64_t n_groups = p.n_groups;
-    const uint64_t o_memtab = carve(n_groups ? 16ull * (n_groups + 1) : 0);
+    const uint64_t o_memtab = carve_ws(&off, n_groups ? 16ull * (n_groups + 1) : 0);
     const uint64_t gather_tiles = (sh.data_total + kGatherTileBytes - 1) / kGatherTileBytes;
-    const uint64_t o_tfirst = carve(4ull * (gather_tiles + 2));
+    const uint64_t o_tfirst = carve_ws(&off, 4ull * (gather_tiles + 2));
     const bool ref_reader = !flush && !jobs && (o->flags & DBEEL_FLAG_REFERENCE_READER);
-    const uint64_t o_fix = carve(ref_reader ? 16ull * N : 0);
+    const uint64_t o_fix = carve_ws(&off, ref_reader ? 16ull * N : 0);
     // single compaction: the last merge level, resolve, the offsets scan and the .index writes in one persistent kernel
     const bool fused_final = e->fused_final && e->fin_ctas_per_sm > 0 && !flush && !jobs && !many && levels >= 1;
     const uint64_t fin_tiles_ub = (uint64_t)(N + kFinNominal - 1) / kFinNominal + 1;
     p.fin_tile = fused_final ? (uint32_t)kFinNominal : 0u;
     const uint64_t scan_bytes = fused_final ? 16ull * fin_tiles_ub + 64 : 0;
-    const uint64_t o_scan = carve(scan_bytes);
+    const uint64_t o_scan = carve_ws(&off, scan_bytes);
     int rc = ensure_device(e, &e->ws, &e->ws_cap, off);
     if (rc) return rc;
     rc = ensure_pinned(e, header_bytes + align_up(sizeof(Ctl), 64) + 64 + (n_groups ? 16ull * (n_groups + 1) : 0));
@@ -492,7 +575,7 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
     // through cudaMemcpyAsync: a small copy on this stream would queue on a copy engine behind whatever bulk transfer
     // of the pipelined host path is in flight there (measured: every partition's kernels waited for the previous
     // partition's 200 MB D2H).  The compute stream carries kernels and event records only.
-    if (record_start) CU(cudaEventRecord(e->ev[EV_START], s)); // ms_total covers the header upload and the filter's memset too
+    CU(cudaEventRecord(e->ev[EV_START], s)); // ms_total covers the header upload and the filter's memset too
     launch_k(e, k_copy_words, (uint32_t)((header_bytes / 4 + 255) / 256), 256, 0, s, reinterpret_cast<uint32_t *>(ws),
              reinterpret_cast<const uint32_t *>(e->pin_dev), (uint32_t)(header_bytes / 4));
     launches++;
@@ -622,9 +705,9 @@ int run_job_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, cons
     st.entries_valid = hc->total;
     st.runs_truncated = hc->runs_truncated;
     st.index_repaired = (hc->flags & kFlagRepaired) ? 1 : 0;
-    if (record_start) cudaEventElapsedTime(&st.ms_total, e->ev[EV_START], e->ev[EV_GATHER]);
+    cudaEventElapsedTime(&st.ms_total, e->ev[EV_START], e->ev[EV_GATHER]);
     if (stage_ev) {
-        if (record_start) cudaEventElapsedTime(&st.ms_extract, e->ev[EV_START], e->ev[EV_EXTRACT]);
+        cudaEventElapsedTime(&st.ms_extract, e->ev[EV_START], e->ev[EV_EXTRACT]);
         cudaEventElapsedTime(&st.ms_merge, e->ev[EV_EXTRACT], e->ev[EV_MERGE]);
         cudaEventElapsedTime(&st.ms_resolve, e->ev[EV_MERGE], e->ev[EV_RESOLVE]);
         cudaEventElapsedTime(&st.ms_gather, e->ev[EV_RESOLVE], e->ev[EV_GATHER]);
@@ -991,7 +1074,7 @@ int run_job_host_pipelined(dbeel_engine *e, const dbeel_run *runs, uint32_t n_ru
         CU(cudaStreamWaitEvent(e->stream, e->ev_h2d[c & 1], 0));
         if (c >= 2) CU(cudaStreamWaitEvent(e->stream, e->ev_d2h[c & 1], 0)); // output buffer c&1 drained
         if (trace) CU(cudaEventRecord(tev[6 * c + 2], e->stream));
-        rc = run_job_device(e, dr.data(), n_runs, o, false, &dout, /*record_start=*/true, &ex); // syncs e->stream
+        rc = run_job_device(e, dr.data(), n_runs, o, false, &dout, &ex); // syncs e->stream
         if (rc) break;
         if (io) pump->release_input(c); // the kernels have read device buffer c & 1, which the H2D out of ring slot c mod R filled
         const dbeel_stats &ps = e->stats;
@@ -1076,6 +1159,33 @@ int run_job_host_pipelined(dbeel_engine *e, const dbeel_run *runs, uint32_t n_ru
     return DBEEL_OK;
 }
 
+// The host form of a device-resident job (dbeel_compact below the pipeline, dbeel_flush_many, dbeel_compact_many): the runs
+// go down into stage_in, run_job_device writes into `dout` (from stage_outputs), and what it wrote comes back into `out`, the
+// filter as bloom_len bytes.  ms_h2d / ms_d2h time the two copies.
+int run_job_staged(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, const dbeel_compact_opts *o, bool flush, dbeel_out *dout,
+                   uint64_t bloom_len, dbeel_out *out, const JobExtra *ex = nullptr) {
+    cudaStream_t s = e->stream;
+    std::vector<HostPiece> pieces;
+    for (uint32_t r = 0; r < n_runs; r++) {
+        pieces.push_back(HostPiece{runs[r].data, runs[r].data_len, nullptr});
+        pieces.push_back(HostPiece{runs[r].index, runs[r].index_len, nullptr});
+    }
+    CU(cudaEventRecord(e->ev[EV_H2D0], s));
+    int rc = stage_host(e, pieces);
+    if (rc) return rc;
+    CU(cudaEventRecord(e->ev[EV_H2D1], s));
+    std::vector<dbeel_run> dr(n_runs);
+    for (uint32_t r = 0; r < n_runs; r++) dr[r] = dbeel_run{pieces[2 * r].dev, runs[r].data_len, pieces[2 * r + 1].dev, runs[r].index_len};
+    if ((rc = run_job_device(e, dr.data(), n_runs, o, flush, dout, ex))) return rc;
+    CU(cudaEventRecord(e->ev[EV_D2H0], s));
+    if ((rc = copy_back(e, *dout, bloom_len, out))) return rc;
+    CU(cudaEventRecord(e->ev[EV_D2H1], s));
+    CU(cudaStreamSynchronize(s));
+    cudaEventElapsedTime(&e->stats.ms_h2d, e->ev[EV_H2D0], e->ev[EV_H2D1]);
+    cudaEventElapsedTime(&e->stats.ms_d2h, e->ev[EV_D2H0], e->ev[EV_D2H1]);
+    return DBEEL_OK;
+}
+
 // host buffers in / out around run_job_device
 int run_job_host(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, const dbeel_compact_opts *o, bool flush,
                  dbeel_out *out) {
@@ -1094,70 +1204,10 @@ int run_job_host(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, const 
         out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
     }
 
-    // device staging: every buffer 256-aligned with 16 bytes of slack behind it
-    uint64_t in_need = 0;
-    for (uint32_t r = 0; r < n_runs; r++)
-        in_need += align_up(runs[r].data_len + 16, kAlign) + align_up(runs[r].index_len + 16, kAlign);
-    uint64_t out_need = align_up(sh.data_total + 16, kAlign) + align_up(sh.n_total * 16 + 16, kAlign) +
-                        align_up(sh.bloom_file + 16, kAlign);
-    int rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, in_need);
-    if (rc) return rc;
-    rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, out_need);
-    if (rc) return rc;
-
-    cudaStream_t s = e->stream;
-    std::vector<dbeel_run> dr(n_runs);
-    CU(cudaEventRecord(e->ev[EV_H2D0], s));
-    uint64_t off = 0;
-    for (uint32_t r = 0; r < n_runs; r++) {
-        dr[r].data = e->stage_in + off;
-        dr[r].data_len = runs[r].data_len;
-        if (runs[r].data_len)
-            CU(cudaMemcpyAsync(e->stage_in + off, runs[r].data, runs[r].data_len, cudaMemcpyHostToDevice, s));
-        off += align_up(runs[r].data_len + 16, kAlign);
-        dr[r].index = e->stage_in + off;
-        dr[r].index_len = runs[r].index_len;
-        if (runs[r].index_len)
-            CU(cudaMemcpyAsync(e->stage_in + off, runs[r].index, runs[r].index_len, cudaMemcpyHostToDevice, s));
-        off += align_up(runs[r].index_len + 16, kAlign);
-    }
-    CU(cudaEventRecord(e->ev[EV_H2D1], s));
-    CU(cudaEventRecord(e->ev[EV_START], s));
-
-    dbeel_out dout = *out;
-    dout.data = e->stage_out;
-    dout.index = e->stage_out + align_up(sh.data_total + 16, kAlign);
-    dout.bloom = sh.bloom_file ? static_cast<uint8_t *>(dout.index) + align_up(sh.n_total * 16 + 16, kAlign) : nullptr;
-    rc = run_job_device(e, dr.data(), n_runs, o, flush, &dout, /*record_start=*/false);
-    // run_job_device zeroes stats; its START event is ours
-    if (rc) return rc;
-    dbeel_stats &st = e->stats;
-    if (sh.n_total) {
-        cudaEventElapsedTime(&st.ms_h2d, e->ev[EV_H2D0], e->ev[EV_H2D1]);
-        cudaEventElapsedTime(&st.ms_total, e->ev[EV_START], e->ev[EV_GATHER]);
-        // EV_EXTRACT is recorded only with stage events: on an event that was never recorded the call fails, and the error
-        // it leaves behind fails the next job's cudaGetLastError check
-        if (e->stage_events) cudaEventElapsedTime(&st.ms_extract, e->ev[EV_START], e->ev[EV_EXTRACT]);
-    }
-    CU(cudaEventRecord(e->ev[EV_D2H0], s));
-    if (dout.data_len) CU(cudaMemcpyAsync(out->data, dout.data, dout.data_len, cudaMemcpyDeviceToHost, s));
-    if (dout.index_len) CU(cudaMemcpyAsync(out->index, dout.index, dout.index_len, cudaMemcpyDeviceToHost, s));
-    if (dout.bloom_len) CU(cudaMemcpyAsync(out->bloom, dout.bloom, dout.bloom_len, cudaMemcpyDeviceToHost, s));
-    CU(cudaEventRecord(e->ev[EV_D2H1], s));
-    CU(cudaStreamSynchronize(s));
-    cudaEventElapsedTime(&st.ms_d2h, e->ev[EV_D2H0], e->ev[EV_D2H1]);
-    out->data_len = dout.data_len;
-    out->index_len = dout.index_len;
-    out->bloom_len = dout.bloom_len;
-    out->items_written = dout.items_written;
-    return DBEEL_OK;
+    dbeel_out dout;
+    const int rc = stage_outputs(e, sh.data_total, sh.n_total * 16, sh.bloom_file, &dout);
+    return rc ? rc : run_job_staged(e, runs, n_runs, o, flush, &dout, sh.bloom_file, out);
 }
-
-struct BusyGuard {
-    dbeel_engine *e;
-    explicit BusyGuard(dbeel_engine *e_) : e(e_) { e->busy = true; }
-    ~BusyGuard() { e->busy = false; }
-};
 
 // ------------------------------------------------------------------------------------ N3: the storage edge
 // dbeel_compact_stream for a job the pipeline does not take (too small to partition, an index the planner does not trust,
@@ -1224,18 +1274,13 @@ int stream_entry(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, const 
                  dbeel_out *out) {
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!out || !io || !io->read || !io->write || (n_runs && !runs)) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
-    if (e->async_state.load(std::memory_order_acquire) != 0) return DBEEL_ERR_BUSY;
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
+    const Claim c(e);
+    if (c.rc) return c.rc;
     dbeel_compact_opts o;
     default_opts(&o);
     if (opts) o = *opts;
     if (!(o.bloom_fp > 0.0 && o.bloom_fp < 1.0)) return fail(e, DBEEL_ERR_INVALID_ARG, "bloom_fp must be in (0,1)");
     if (n_runs > DBEEL_MAX_RUNS) return fail(e, DBEEL_ERR_TOO_MANY_RUNS, "too many runs");
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
-    e->stats.ms_h2d = 0;
     out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
     JobShape sh;
     shape_of(runs, n_runs, &o, false, &sh);
@@ -1252,17 +1297,13 @@ int entry(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, const dbeel_c
           bool flush, bool device) {
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!out || (n_runs && !runs)) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
+    const Claim c(e);
+    if (c.rc) return c.rc;
     dbeel_compact_opts o;
     default_opts(&o);
     if (opts) o = *opts;
     if (!(o.bloom_fp > 0.0 && o.bloom_fp < 1.0)) return fail(e, DBEEL_ERR_INVALID_ARG, "bloom_fp must be in (0,1)");
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
-    e->stats.ms_h2d = 0;
-    return device ? run_job_device(e, runs, n_runs, &o, flush, out, true) : run_job_host(e, runs, n_runs, &o, flush, out);
+    return device ? run_job_device(e, runs, n_runs, &o, flush, out) : run_job_host(e, runs, n_runs, &o, flush, out);
 }
 
 
@@ -1337,31 +1378,22 @@ int stage_lookup(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, 
             }
     } else { // host buffers: the tables, the keys and the offsets go down
         if (!keys && key_off[n_keys]) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
-        const uint64_t key_bytes = key_off[n_keys];
-        uint64_t need = align_up(key_bytes + 16, kAlign) + align_up((n_keys + 1) * 8, kAlign);
-        for (uint32_t i = 0; i < n_tables; i++)
-            need += align_up(tables[i].data_len + 16, kAlign) + align_up(tables[i].index_len + 16, kAlign) + align_up(tables[i].bloom_len + 16, kAlign);
-        rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, need);
-        if (rc) return rc;
-        uint64_t pos = 0;
-        auto put = [&](const void *src, uint64_t len, uint64_t slack) -> const uint8_t * {
-            uint8_t *dst = e->stage_in + pos;
-            pos += align_up(len + slack, kAlign);
-            if (len && cudaMemcpyAsync(dst, src, len, cudaMemcpyHostToDevice, s) != cudaSuccess) return nullptr;
-            return dst;
-        };
-        *d_keys = put(keys, key_bytes, 16);
-        *d_off = reinterpret_cast<const uint64_t *>(put(key_off, (n_keys + 1) * 8, 0));
-        if (!*d_keys || !*d_off) return fail(e, DBEEL_ERR_CUDA, "cudaMemcpyAsync(keys)", cudaGetLastError());
+        std::vector<HostPiece> pieces{{keys, key_off[n_keys], nullptr}, {key_off, (n_keys + 1) * 8, nullptr}};
         for (uint32_t i = 0; i < n_tables; i++) {
             const dbeel_table &t = tables[i];
-            const uint8_t *dd = put(t.data, t.data_len, 16), *di = put(t.index, t.index_len, 16), *db = put(t.bloom, t.bloom_len, 16);
-            if (!dd || !di || !db) return fail(e, DBEEL_ERR_CUDA, "cudaMemcpyAsync(table)", cudaGetLastError());
-            td[i] = TableDesc{dd, t.data_len, reinterpret_cast<const uint4 *>(di), t.index_len / DBEEL_INDEX_ENTRY_SIZE, nullptr, 0, 0, 0, 0, {0, 0, 0, 0}};
+            pieces.insert(pieces.end(), {{t.data, t.data_len, nullptr}, {t.index, t.index_len, nullptr}, {t.bloom, t.bloom_len, nullptr}});
+        }
+        if ((rc = stage_host(e, pieces))) return rc;
+        *d_keys = pieces[0].dev;
+        *d_off = reinterpret_cast<const uint64_t *>(pieces[1].dev);
+        for (uint32_t i = 0; i < n_tables; i++) {
+            const dbeel_table &t = tables[i];
+            const HostPiece *tp = &pieces[2 + 3 * i];
+            td[i] = TableDesc{tp[0].dev, t.data_len, reinterpret_cast<const uint4 *>(tp[1].dev), t.index_len / DBEEL_INDEX_ENTRY_SIZE, nullptr, 0, 0, 0, 0, {0, 0, 0, 0}};
             if (!t.bloom_len) continue;
             const uint8_t *b = static_cast<const uint8_t *>(t.bloom);
             if ((rc = parse_bloom(e, b, b + t.bloom_len - kBloomTrailer, t.bloom_len, &td[i]))) return rc;
-            td[i].words = reinterpret_cast<const uint32_t *>(db + 8);
+            td[i].words = reinterpret_cast<const uint32_t *>(tp[2].dev + 8);
         }
     }
     if (n_tables) {
@@ -1376,22 +1408,19 @@ int lookup_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, 
     static_assert(sizeof(dbeel_lookup_result) == 16, "result rows are written as uint4");
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (const int arc = lookup_args(e, tables, n_tables, key_off, n_keys, mode, results)) return arc;
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
+    const Claim c(e);
+    if (c.rc) return c.rc;
     if (n_keys == 0) return DBEEL_OK;
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     cudaStream_t s = e->stream;
     int rc = ensure_device(e, &e->ws, &e->ws_cap, std::max<uint64_t>(4096, n_tables * sizeof(TableDesc)));
-    if (!rc && !device) rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, n_keys * 16);
+    dbeel_out rows; // host callers: the rows before their D2H
+    if (!rc && !device) rc = stage_outputs(e, n_keys * 16, 0, 0, &rows);
     if (rc) return rc;
     const uint8_t *d_keys;
     const uint64_t *d_off;
     if ((rc = stage_lookup(e, tables, n_tables, keys, key_off, n_keys, device, 0, reinterpret_cast<TableDesc *>(e->ws), &d_keys, &d_off)))
         return rc;
-    uint4 *d_res = device ? reinterpret_cast<uint4 *>(results) : reinterpret_cast<uint4 *>(e->stage_out);
+    uint4 *d_res = reinterpret_cast<uint4 *>(device ? results : rows.data);
     LookupParams lp{reinterpret_cast<const TableDesc *>(e->ws), n_tables, mode, d_keys, d_off, n_keys, d_res};
     CU(cudaEventRecord(e->ev[EV_START], s));
     k_lookup<<<(uint32_t)((n_keys + 255) / 256), 256, 0, s>>>(lp);
@@ -1416,17 +1445,14 @@ int route_entry(dbeel_engine *e, const dbeel_run *batch, const uint32_t *ring, u
     if (n_shards > kRouteMaxShards) return fail(e, DBEEL_ERR_INVALID_ARG, "more shards than DBEEL_MAX_SHARDS");
     for (uint32_t s = 1; s < n_shards; s++)
         if (ring[s - 1] >= ring[s]) return fail(e, DBEEL_ERR_INVALID_ARG, "ring hashes must be strictly ascending");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
+    const Claim c(e);
+    if (c.rc) return c.rc;
     const uint64_t n64 = batch->index_len / DBEEL_INDEX_ENTRY_SIZE;
     for (uint32_t s = 0; s < n_shards; s++) { counts[s] = 0; if (bytes) bytes[s] = 0; }
     if (n64 >= 0xFFFFFFF0ull) return fail(e, DBEEL_ERR_TOO_MANY_ENTRIES, "too many arrivals in one batch");
     if (n64 == 0) return DBEEL_OK;
     if (out_index_cap < n64 * 16 || !out_index) return fail(e, DBEEL_ERR_CAPACITY, "routed index buffer too small");
     if (((uintptr_t)batch->index | (uintptr_t)out_index) & 15) return fail(e, DBEEL_ERR_INVALID_ARG, "index buffers must be 16-byte aligned");
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     RouteParams p;
     p.data = static_cast<const uint8_t *>(batch->data);
     p.data_len = batch->data_len;
@@ -1435,10 +1461,9 @@ int route_entry(dbeel_engine *e, const dbeel_run *batch, const uint32_t *ring, u
     p.n_shards = n_shards;
     p.n_blocks = (p.n + kRouteThreads - 1) / kRouteThreads;
     uint64_t off = 0;
-    auto carve = [&](uint64_t b) { uint64_t o2 = off; off = align_up(off + b, kAlign); return o2; };
-    const uint64_t o_ring = carve(4ull * n_shards), o_tot = carve(8ull * (3 * n_shards + 1));
-    const uint64_t o_hist = carve(4ull * p.n_blocks * n_shards), o_owner = carve(shard_of ? 0 : 4ull * p.n);
-    const uint64_t o_h64 = carve(out_hash64 ? 8ull * p.n : 0);
+    const uint64_t o_ring = carve_ws(&off, 4ull * n_shards), o_tot = carve_ws(&off, 8ull * (3 * n_shards + 1));
+    const uint64_t o_hist = carve_ws(&off, 4ull * p.n_blocks * n_shards), o_owner = carve_ws(&off, shard_of ? 0 : 4ull * p.n);
+    const uint64_t o_h64 = carve_ws(&off, out_hash64 ? 8ull * p.n : 0);
     int rc = ensure_device(e, &e->route_ws, &e->route_ws_cap, off);
     if (!rc) rc = ensure_pinned(e, 4096 + 8ull * (3 * n_shards + 1));
     if (rc) return rc;
@@ -1465,7 +1490,6 @@ int route_entry(dbeel_engine *e, const dbeel_run *batch, const uint32_t *ring, u
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(s));
     dbeel_stats &st = e->stats;
-    memset(&st, 0, sizeof st);
     st.entries_in = n64;
     st.kernel_launches = 5;
     cudaEventElapsedTime(&st.ms_total, e->ev[EV_START], e->ev[EV_GATHER]);
@@ -1485,11 +1509,8 @@ int cuts_entry(dbeel_engine *e, const void *key_hash64, const uint64_t *stream_s
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!stream_starts || !cuts || !cut_starts || !n_streams) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     if (capacity < 1 || capacity > kCutMaxCapacity) return fail(e, DBEEL_ERR_INVALID_ARG, "capacity above what the device cut supports (use dbeel_memtable_cut)");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    const Claim c(e);
+    if (c.rc) return c.rc;
     // a stream of n arrivals has at most n / capacity full memtables
     std::vector<uint32_t> base(n_streams + 1, 0);
     for (uint32_t s = 0; s < n_streams; s++) {
@@ -1502,9 +1523,8 @@ int cuts_entry(dbeel_engine *e, const void *key_hash64, const uint64_t *stream_s
     if (stream_starts[n_streams] == stream_starts[0]) return DBEEL_OK;
     if (!key_hash64) return fail(e, DBEEL_ERR_INVALID_ARG, "null key identities");
     uint64_t off = 0;
-    auto carve = [&](uint64_t b) { uint64_t o2 = off; off = align_up(off + b, kAlign); return o2; };
-    const uint64_t o_starts = carve(8ull * (n_streams + 1)), o_base = carve(4ull * n_streams), o_n = carve(4ull * n_streams);
-    const uint64_t o_cuts = carve(4ull * (total_max + 1));
+    const uint64_t o_starts = carve_ws(&off, 8ull * (n_streams + 1)), o_base = carve_ws(&off, 4ull * n_streams), o_n = carve_ws(&off, 4ull * n_streams);
+    const uint64_t o_cuts = carve_ws(&off, 4ull * (total_max + 1));
     const uint64_t hdr = o_n; // starts | base go down, n_cuts | cuts come back
     int rc = ensure_device(e, &e->route_ws, &e->route_ws_cap, off);
     if (!rc) rc = ensure_pinned(e, off);
@@ -1512,11 +1532,6 @@ int cuts_entry(dbeel_engine *e, const void *key_hash64, const uint64_t *stream_s
     memcpy(e->pin + o_starts, stream_starts, 8ull * (n_streams + 1));
     memcpy(e->pin + o_base, base.data(), 4ull * n_streams);
     cudaStream_t s = e->stream;
-    static bool attr_set = false;
-    if (!attr_set) {
-        CU(cudaFuncSetAttribute(k_memtable_cuts, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(12ull * kCutSlots)));
-        attr_set = true;
-    }
     CU(cudaEventRecord(e->ev[EV_START], s));
     k_copy_words<<<(uint32_t)((hdr / 4 + 255) / 256), 256, 0, s>>>(reinterpret_cast<uint32_t *>(e->route_ws), reinterpret_cast<const uint32_t *>(e->pin_dev),
                                                                     (uint32_t)(hdr / 4));
@@ -1536,7 +1551,6 @@ int cuts_entry(dbeel_engine *e, const void *key_hash64, const uint64_t *stream_s
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(s));
     dbeel_stats &st = e->stats;
-    memset(&st, 0, sizeof st);
     st.kernel_launches = 3;
     st.entries_in = stream_starts[n_streams] - stream_starts[0];
     cudaEventElapsedTime(&st.ms_total, e->ev[EV_START], e->ev[EV_GATHER]);
@@ -1557,72 +1571,61 @@ int cuts_entry(dbeel_engine *e, const void *key_hash64, const uint64_t *stream_s
 int wal_flush_entry(dbeel_engine *e, const void *wal, uint64_t wal_len, uint32_t capacity, dbeel_out *out, bool device) {
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!out || (wal_len && !wal)) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    e->err.clear();
+    const Claim c(e);
+    if (c.rc) return c.rc;
     out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
     const uint64_t n_pages64 = (wal_len + kWalPage - 1) / kWalPage;
     if (n_pages64 >= 0xFFFFFFF0ull) return fail(e, DBEEL_ERR_TOO_MANY_ENTRIES, "write-ahead log too large");
-    if (wal_len == 0) { e->stats = dbeel_stats{}; return DBEEL_OK; }
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    if (wal_len == 0) return DBEEL_OK;
     cudaStream_t s = e->stream;
     const uint32_t n_pages = (uint32_t)n_pages64, nodes = n_pages + 1;
     uint32_t levels = 0;
     while ((1ull << levels) < nodes) levels++;
 
     const uint8_t *d_wal = static_cast<const uint8_t *>(wal);
-    uint64_t data_cap_user = out->data_cap, index_cap_user = out->index_cap;
-    void *user_data = out->data, *user_index = out->index;
     float ms_h2d = 0;
-    const uint4 *d_index = nullptr;
-    {
-        BusyGuard g(e);
-        if (!device) { // host log: stage it down (the flush below writes into staging too)
-            int rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, align_up(wal_len + 32, kAlign));
-            if (rc) return rc;
-            CU(cudaEventRecord(e->ev[EV_H2D0], s));
-            CU(cudaMemcpyAsync(e->stage_in, wal, wal_len, cudaMemcpyHostToDevice, s));
-            CU(cudaEventRecord(e->ev[EV_H2D1], s));
-            d_wal = e->stage_in;
-        } else if ((uintptr_t)wal & 15) {
-            return fail(e, DBEEL_ERR_INVALID_ARG, "device log buffer must be 16-byte aligned");
-        }
-        // scratch: jump / cnt tables, per-page sizes, the arrival index, 3 totals
-        uint64_t off = 0;
-        auto carve = [&](uint64_t bytes) { uint64_t o2 = off; off = align_up(off + bytes, kAlign); return o2; };
-        const uint64_t o_jump = carve(4ull * (levels + 1) * nodes), o_cnt = carve(4ull * (levels + 1) * nodes);
-        const uint64_t o_sizes = carve(8ull * n_pages), o_index = carve(16ull * n_pages), o_tot = carve(32);
-        int rc = ensure_device(e, &e->wal_ws, &e->wal_ws_cap, off);
-        if (!rc) rc = ensure_pinned(e, 4096);
-        if (rc) return rc;
-        WalParams w;
-        w.wal = d_wal;
-        w.len = wal_len;
-        w.n_pages = n_pages;
-        w.levels = levels;
-        w.jump = reinterpret_cast<uint32_t *>(e->wal_ws + o_jump);
-        w.cnt = reinterpret_cast<uint32_t *>(e->wal_ws + o_cnt);
-        w.sizes = reinterpret_cast<uint2 *>(e->wal_ws + o_sizes);
-        w.index = reinterpret_cast<uint4 *>(e->wal_ws + o_index);
-        d_index = w.index;
-        w.totals = reinterpret_cast<unsigned long long *>(e->wal_ws + o_tot);
-        CU(cudaMemsetAsync(w.totals, 0, 32, s));
-        const uint32_t grid = (nodes + 255) / 256;
-        k_wal_parse<<<grid, 256, 0, s>>>(w);
-        for (uint32_t k = 0; k < levels; k++) k_wal_double<<<grid, 256, 0, s>>>(w, k);
-        k_wal_select<<<(n_pages + 255) / 256, 256, 0, s>>>(w);
-        k_publish<<<1, 256, 0, s>>>(reinterpret_cast<uint32_t *>(e->pin_dev), reinterpret_cast<const uint32_t *>(w.totals), 6,
-                                    nullptr, nullptr, 0);
-        CU(cudaGetLastError());
-        CU(cudaStreamSynchronize(s));
-        if (!device) cudaEventElapsedTime(&ms_h2d, e->ev[EV_H2D0], e->ev[EV_H2D1]);
+    if (!device) { // host log: stage it down (the flush below writes into staging too)
+        std::vector<HostPiece> log{{wal, wal_len, nullptr}};
+        CU(cudaEventRecord(e->ev[EV_H2D0], s));
+        if (const int rc = stage_host(e, log)) return rc;
+        CU(cudaEventRecord(e->ev[EV_H2D1], s));
+        d_wal = log[0].dev;
+    } else if ((uintptr_t)wal & 15) {
+        return fail(e, DBEEL_ERR_INVALID_ARG, "device log buffer must be 16-byte aligned");
     }
+    // scratch: jump / cnt tables, per-page sizes, the arrival index, 3 totals
+    uint64_t off = 0;
+    const uint64_t o_jump = carve_ws(&off, 4ull * (levels + 1) * nodes), o_cnt = carve_ws(&off, 4ull * (levels + 1) * nodes);
+    const uint64_t o_sizes = carve_ws(&off, 8ull * n_pages), o_index = carve_ws(&off, 16ull * n_pages), o_tot = carve_ws(&off, 32);
+    int rc = ensure_device(e, &e->wal_ws, &e->wal_ws_cap, off);
+    if (!rc) rc = ensure_pinned(e, 4096);
+    if (rc) return rc;
+    WalParams w;
+    w.wal = d_wal;
+    w.len = wal_len;
+    w.n_pages = n_pages;
+    w.levels = levels;
+    w.jump = reinterpret_cast<uint32_t *>(e->wal_ws + o_jump);
+    w.cnt = reinterpret_cast<uint32_t *>(e->wal_ws + o_cnt);
+    w.sizes = reinterpret_cast<uint2 *>(e->wal_ws + o_sizes);
+    w.index = reinterpret_cast<uint4 *>(e->wal_ws + o_index);
+    w.totals = reinterpret_cast<unsigned long long *>(e->wal_ws + o_tot);
+    CU(cudaMemsetAsync(w.totals, 0, 32, s));
+    const uint32_t grid = (nodes + 255) / 256;
+    k_wal_parse<<<grid, 256, 0, s>>>(w);
+    for (uint32_t k = 0; k < levels; k++) k_wal_double<<<grid, 256, 0, s>>>(w, k);
+    k_wal_select<<<(n_pages + 255) / 256, 256, 0, s>>>(w);
+    k_publish<<<1, 256, 0, s>>>(reinterpret_cast<uint32_t *>(e->pin_dev), reinterpret_cast<const uint32_t *>(w.totals), 6,
+                                nullptr, nullptr, 0);
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(s));
+    if (!device) cudaEventElapsedTime(&ms_h2d, e->ev[EV_H2D0], e->ev[EV_H2D1]);
     unsigned long long totals[3];
     memcpy(totals, e->pin, sizeof totals);
     const uint64_t n_rec = totals[0], bytes = totals[1];
     const uint32_t wal_launches = levels + 3;
     if (totals[2] & kWalTooLarge) return fail(e, DBEEL_ERR_ITEM_TOO_LARGE, "a logged entry exceeds u32::MAX bytes");
-    if (n_rec == 0) { e->stats = dbeel_stats{}; e->stats.kernel_launches = wal_launches; return DBEEL_OK; }
+    if (n_rec == 0) { e->stats.kernel_launches = wal_launches; return DBEEL_OK; }
 
     // ---- the flush: the log is the batch's .data, the selected records its (sparse) .index
     dbeel_compact_opts o;
@@ -1630,32 +1633,22 @@ int wal_flush_entry(dbeel_engine *e, const void *wal, uint64_t wal_len, uint32_t
     JobExtra ex;
     ex.sparse_offsets = true;
     ex.data_bytes = bytes;
-    dbeel_run batch{d_wal, wal_len, d_index, n_rec * 16};
-    if (data_cap_user < bytes || index_cap_user < n_rec * 16) return fail(e, DBEEL_ERR_CAPACITY, "output buffer too small for the replayed entries");
-    int rc;
+    dbeel_run batch{d_wal, wal_len, w.index, n_rec * 16};
+    if (out->data_cap < bytes || out->index_cap < n_rec * 16) return fail(e, DBEEL_ERR_CAPACITY, "output buffer too small for the replayed entries");
     if (device) {
-        BusyGuard g(e);
-        e->stats.ms_h2d = 0;
-        rc = run_job_device(e, &batch, 1, &o, true, out, true, &ex);
+        rc = run_job_device(e, &batch, 1, &o, true, out, &ex);
     } else {
-        BusyGuard g(e);
-        rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, align_up(bytes + 16, kAlign) + align_up(n_rec * 16 + 16, kAlign));
-        if (rc) return rc;
         dbeel_out dout = {};
-        dout.data = e->stage_out;
-        dout.data_cap = bytes;
-        dout.index = e->stage_out + align_up(bytes + 16, kAlign);
-        dout.index_cap = n_rec * 16;
-        e->stats.ms_h2d = ms_h2d;
-        rc = run_job_device(e, &batch, 1, &o, true, &dout, true, &ex);
+        rc = stage_outputs(e, bytes, n_rec * 16, 0, &dout);
+        if (!rc) rc = run_job_device(e, &batch, 1, &o, true, &dout, &ex);
         if (!rc && dout.items_written <= capacity) {
-            if (dout.data_len) CU(cudaMemcpyAsync(user_data, dout.data, dout.data_len, cudaMemcpyDeviceToHost, s));
-            if (dout.index_len) CU(cudaMemcpyAsync(user_index, dout.index, dout.index_len, cudaMemcpyDeviceToHost, s));
+            rc = copy_back(e, dout, 0, out);
             CU(cudaStreamSynchronize(s));
         }
         out->data_len = dout.data_len;
         out->index_len = dout.index_len;
         out->items_written = dout.items_written;
+        e->stats.ms_h2d = ms_h2d;
     }
     if (rc) return rc;
     e->stats.kernel_launches += wal_launches;
@@ -1701,9 +1694,8 @@ int compact_many_entry(dbeel_engine *e, const dbeel_job *jobs, uint32_t n_jobs, 
                        dbeel_job_result *results, bool device) {
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!out || (n_jobs && (!jobs || !results))) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g0(e);
-    e->err.clear();
+    const Claim c(e);
+    if (c.rc) return c.rc;
     out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
     JobShapes js;
     int rc = job_shapes(e, jobs, n_jobs, bloom_min_size, fp, &js);
@@ -1713,9 +1705,7 @@ int compact_many_entry(dbeel_engine *e, const dbeel_job *jobs, uint32_t n_jobs, 
     if (js.entries >= 0xFFFFFFFEull) return fail(e, DBEEL_ERR_TOO_MANY_ENTRIES, "too many entries");
     if (out->data_cap < js.data || out->index_cap < js.index || out->bloom_cap < js.bloom)
         return fail(e, DBEEL_ERR_CAPACITY, "output buffer smaller than dbeel_compact_many_bound");
-    if (n_jobs == 0 || js.entries == 0) { e->stats = dbeel_stats{}; return DBEEL_OK; }
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
+    if (n_jobs == 0 || js.entries == 0) return DBEEL_OK;
     cudaStream_t s = e->stream;
 
     // all runs back to back; host buffers are staged down first
@@ -1730,28 +1720,9 @@ int compact_many_entry(dbeel_engine *e, const dbeel_job *jobs, uint32_t n_jobs, 
     first[n_jobs] = (uint32_t)flat.size();
     dbeel_out dout = *out;
     if (!device) {
-        uint64_t in_need = 0;
-        for (auto &r : flat) {
+        for (auto &r : flat)
             if ((r.data_len && !r.data) || (r.index_len && !r.index)) return fail(e, DBEEL_ERR_INVALID_ARG, "null run buffer");
-            in_need += align_up(r.data_len + 32, kAlign) + align_up(r.index_len + 16, kAlign);
-        }
-        rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, in_need);
-        if (!rc) rc = ensure_device(e, &e->stage_out, &e->stage_out_cap,
-                                    align_up(js.data + 16, kAlign) + align_up(js.index + 16, kAlign) + align_up(js.bloom + 16, kAlign));
-        if (rc) return rc;
-        uint64_t pos = 0;
-        for (auto &r : flat) {
-            const void *hd = r.data, *hi = r.index;
-            r.data = e->stage_in + pos;
-            if (r.data_len) CU(cudaMemcpyAsync(e->stage_in + pos, hd, r.data_len, cudaMemcpyHostToDevice, s));
-            pos += align_up(r.data_len + 32, kAlign);
-            r.index = e->stage_in + pos;
-            if (r.index_len) CU(cudaMemcpyAsync(e->stage_in + pos, hi, r.index_len, cudaMemcpyHostToDevice, s));
-            pos += align_up(r.index_len + 16, kAlign);
-        }
-        dout.data = e->stage_out;
-        dout.index = e->stage_out + align_up(js.data + 16, kAlign);
-        dout.bloom = e->stage_out + align_up(js.data + 16, kAlign) + align_up(js.index + 16, kAlign);
+        if ((rc = stage_outputs(e, js.data, js.index, js.bloom, &dout))) return rc;
     } else if ((uintptr_t)out->bloom & 15) {
         return fail(e, DBEEL_ERR_INVALID_ARG, "device output buffers must be 16-byte aligned");
     }
@@ -1789,18 +1760,12 @@ int compact_many_entry(dbeel_engine *e, const dbeel_job *jobs, uint32_t n_jobs, 
     ex.job_keep = keep.data();
     ex.job_bloom = bloom.data();
     ex.job_results = results;
-    e->stats.ms_h2d = 0;
-    rc = run_job_device(e, flat.data(), (uint32_t)flat.size(), &o, false, &dout, true, &ex);
+    rc = device ? run_job_device(e, flat.data(), (uint32_t)flat.size(), &o, false, &dout, &ex)
+                : run_job_staged(e, flat.data(), (uint32_t)flat.size(), &o, false, &dout, js.bloom, out, &ex);
     if (rc) return rc;
     for (uint32_t g = 0; g < n_jobs; g++) {
         results[g].bloom_off = js.bloom_off[g];
         results[g].bloom_len = js.shape[g].bloom_file;
-    }
-    if (!device) {
-        if (dout.data_len) CU(cudaMemcpyAsync(out->data, dout.data, dout.data_len, cudaMemcpyDeviceToHost, s));
-        if (dout.index_len) CU(cudaMemcpyAsync(out->index, dout.index, dout.index_len, cudaMemcpyDeviceToHost, s));
-        if (js.bloom) CU(cudaMemcpyAsync(out->bloom, dout.bloom, js.bloom, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
     }
     out->data_len = dout.data_len;
     out->index_len = dout.index_len;
@@ -1835,12 +1800,6 @@ int scan_args(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uin
 void clear_scan(dbeel_job_result *results, uint32_t nd, dbeel_scan_stop *stop) {
     for (uint32_t d = 0; d < nd; d++) results[d] = dbeel_job_result{0, 0, 0, 0, 0, 0, 0};
     *stop = dbeel_scan_stop{-1, DBEEL_SCAN_STOP_NONE, 0};
-}
-
-uint64_t carve_ws(uint64_t *off, uint64_t b) {
-    const uint64_t o = *off;
-    *off = align_up(*off + b, kAlign);
-    return o;
 }
 
 // ---- the ranges as the kernels read them (ScanParams.hash_ranges / key_off / keys), carved behind what the caller put
@@ -2048,10 +2007,8 @@ int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
     if (!out) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     uint64_t key_bytes = 0;
     if (const int arc = scan_args(e, tables, n_tables, kind, ranges, n_ranges, results, stop, &key_bytes)) return arc;
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
+    const Claim c(e);
+    if (c.rc) return c.rc;
     out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
     clear_scan(results, n_ranges, stop);
     uint64_t n64 = 0, data_total = 0, index_total = 0;
@@ -2079,28 +2036,17 @@ int scan_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, ui
         *stop = dbeel_scan_stop{(int32_t)t, (uint32_t)(key & 3), (key >> 12) - base[t]};
     };
     if (n == 0) { set_stop(stop0); return DBEEL_OK; }
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     cudaStream_t s = e->stream;
 
-    // host tables go down whole (16 bytes of slack behind every buffer: the 8-byte header loads may run past an entry)
+    // host tables go down whole
     std::vector<ScanTable> td(n_tables);
     if (!device) {
-        uint64_t need = 0;
-        for (uint32_t t = 0; t < n_tables; t++) need += align_up(tables[t].data_len + 32, kAlign) + align_up(tables[t].index_len + 16, kAlign);
-        int rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, need);
-        if (rc) return rc;
-        uint64_t pos = 0;
-        for (uint32_t t = 0; t < n_tables; t++) {
-            const dbeel_table &tb = tables[t];
-            uint8_t *dd = e->stage_in + pos;
-            pos += align_up(tb.data_len + 32, kAlign);
-            uint8_t *di = e->stage_in + pos;
-            pos += align_up(tb.index_len + 16, kAlign);
-            if (tb.data_len) CU(cudaMemcpyAsync(dd, tb.data, tb.data_len, cudaMemcpyHostToDevice, s));
-            if (tb.index_len) CU(cudaMemcpyAsync(di, tb.index, tb.index_len, cudaMemcpyHostToDevice, s));
-            td[t] = ScanTable{dd, tb.data_len, reinterpret_cast<const uint4 *>(di), base[t + 1] - base[t], base[t]};
-        }
+        std::vector<HostPiece> pieces;
+        for (uint32_t t = 0; t < n_tables; t++)
+            pieces.insert(pieces.end(), {{tables[t].data, tables[t].data_len, nullptr}, {tables[t].index, tables[t].index_len, nullptr}});
+        if (const int rc = stage_host(e, pieces)) return rc;
+        for (uint32_t t = 0; t < n_tables; t++)
+            td[t] = ScanTable{pieces[2 * t].dev, tables[t].data_len, reinterpret_cast<const uint4 *>(pieces[2 * t + 1].dev), base[t + 1] - base[t], base[t]};
     } else {
         for (uint32_t t = 0; t < n_tables; t++)
             td[t] = ScanTable{static_cast<const uint8_t *>(tables[t].data), tables[t].data_len, static_cast<const uint4 *>(tables[t].index),
@@ -2174,14 +2120,10 @@ int get_values_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tabl
     if (n_keys >= 0xFFFFFFF0ull) return fail(e, DBEEL_ERR_INVALID_ARG, "2^32 - 16 keys or more");
     if (device && (((uintptr_t)out->data | (uintptr_t)out->index) & 15))
         return fail(e, DBEEL_ERR_INVALID_ARG, "device output buffers must be 16-byte aligned");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
+    const Claim c(e);
+    if (c.rc) return c.rc;
     out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
     if (n_keys == 0) return DBEEL_OK;
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     cudaStream_t s = e->stream;
     const uint32_t n = (uint32_t)n_keys;
     uint64_t off = 0;
@@ -2773,8 +2715,6 @@ int gvs_walk(dbeel_engine *e, const std::vector<GvsBatch> &bs, dbeel_out *out, d
     }
     n_keys = row0[nb];
     if (n_keys == 0) return DBEEL_OK;
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     cudaStream_t s = e->stream;
     const uint32_t n = (uint32_t)n_keys;
     const uint64_t budget = e->partition_bytes;
@@ -2979,10 +2919,8 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
     if (!out || !io || !io->read) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     if (const int arc = lookup_args(e, tables, n_tables, key_off, n_keys, mode, results)) return arc;
     if (n_keys >= 0xFFFFFFF0ull) return fail(e, DBEEL_ERR_INVALID_ARG, "2^32 - 16 keys or more");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
+    const Claim c(e);
+    if (c.rc) return c.rc;
     out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
     if (n_keys == 0) return DBEEL_OK;
     for (uint32_t i = 0; i < n_tables; i++) { // as stage_lookup; .data and .index come through the callback
@@ -2994,8 +2932,6 @@ int get_values_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t
     }
     const uint64_t key_bytes = key_off[n_keys];
     if (!keys && key_bytes) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     int rc;
     uint64_t bloom_bytes = 0;
     for (uint32_t i = 0; i < n_tables; i++) bloom_bytes += align_up(tables[i].bloom_len + 16, kAlign);
@@ -3052,8 +2988,6 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
         if (plan.panic_table >= 0) *stop = dbeel_scan_stop{plan.panic_table, DBEEL_SCAN_STOP_PANIC, plan.panic_record};
     };
     if (np == 0) { host_stop(); return DBEEL_OK; }
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     cudaStream_t s = e->stream;
 
     // ---- 2. slot layouts: [ScanTable per slice | per slice: index slice (+16), .data window (+32)], 256-byte aligned pieces
@@ -3258,7 +3192,7 @@ int run_scan_plan(dbeel_engine *e, const dbeel_table *tables, const ScanPlan &pl
             rc = enqueue_kernels(c + 1);
             if (rc) break;
         }
-        ce = cudaEventSynchronize(e->ev_comp[c & 1]);
+        const cudaError_t ce = cudaEventSynchronize(e->ev_comp[c & 1]);
         if (ce != cudaSuccess) { rc = fail(e, DBEEL_ERR_CUDA, "scan kernels", ce); break; }
         pump.release_input(c); // H2D c (out of ring slot c mod R) has completed
         memcpy(hdr.data(), e->pin + pin_pub + (c & 1) * pub_stride, 8 * pub_words);
@@ -3370,10 +3304,8 @@ int scan_stream_entry(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tab
     if (!io || !io->read || !io->write) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     uint64_t key_bytes = 0;
     if (const int arc = scan_args(e, tables, n_tables, kind, ranges, n_ranges, results, stop, &key_bytes)) return arc;
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
+    const Claim c(e);
+    if (c.rc) return c.rc;
     clear_scan(results, n_ranges, stop);
     return plan_and_run_scan(e, tables, n_tables, kind, ranges, n_ranges, key_bytes, io, results, stop, nullptr);
 }
@@ -3439,8 +3371,6 @@ int reader_seek(dbeel_engine *e, std::vector<SeekPart> &sp) {
         np += x.nseek;
     }
     if (!Q) return DBEEL_OK;
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     cudaStream_t s = e->stream;
     const uint64_t budget = e->partition_bytes;
     // the bounds once per table, so that query q's key is keys[ko[q] .. ko[q + 1])
@@ -3747,10 +3677,8 @@ int reader_range_entry(dbeel_reader *r, bool get_range, uint32_t kind, const voi
     const uint32_t nt = (uint32_t)tables.size();
     uint64_t key_bytes = 0;
     if (const int arc = scan_args(e, tables.data(), nt, kind, ranges, n_ranges, results, stop, &key_bytes)) return arc;
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
+    const Claim c(e);
+    if (c.rc) return c.rc;
     clear_scan(results, n_ranges, stop);
     ReaderScanIo x;
     x.rio = &r->io;
@@ -4029,8 +3957,6 @@ int reader_get_ranges(dbeel_engine *e, const std::vector<RangeBatch> &bs, dbeel_
     }
     int rc;
     if ((rc = reader_seek_batched(e, sp))) return rc;
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     CU(cudaEventRecord(e->ev[EV_START], e->stream));
     std::vector<LimitState> st(row0[nbat]);
     std::vector<uint32_t> live;
@@ -4178,10 +4104,8 @@ int range_batch_args(dbeel_engine *e, const dbeel_key_ranges *kr, uint32_t nq, c
 // Takes the engine, runs the walk over the checked batches (one ReaderScanIo each, so input_bytes counts every byte read
 // through every reader's callback) and leaves rows cleared after any error other than capacity.
 int ranges_entry(dbeel_engine *e, std::vector<RangeBatch> &bs, dbeel_out *out, dbeel_range_row *rows) {
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
+    const Claim c(e);
+    if (c.rc) return c.rc;
     out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
     uint64_t nq = 0;
     for (const RangeBatch &B : bs) nq += B.nq;
@@ -4222,8 +4146,8 @@ namespace dbeel {
 
 int reader_table_create(dbeel_engine *e, const dbeel_table &t, ReaderTableRef *out) {
     if (!e) return DBEEL_ERR_INVALID_ARG;
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
+    const Claim c(e);
+    if (c.rc) return c.rc;
     // the table checks of dbeel_get_values_stream, and its filter parsed as there
     if (t.index_len % DBEEL_INDEX_ENTRY_SIZE) return fail(e, DBEEL_ERR_INVALID_ARG, "index length is not a multiple of 16");
     if (t.bloom_len && !t.bloom) return fail(e, DBEEL_ERR_INVALID_ARG, "null table buffer");
@@ -4235,7 +4159,6 @@ int reader_table_create(dbeel_engine *e, const dbeel_table &t, ReaderTableRef *o
     if (t.bloom_len) {
         const uint8_t *b = static_cast<const uint8_t *>(t.bloom);
         if (const int rc = parse_bloom(e, b, b + t.bloom_len - kBloomTrailer, t.bloom_len, &rt->desc)) return rc;
-        CU(cudaSetDevice(e->device));
         if (cudaMalloc(reinterpret_cast<void **>(&rt->bloom_dev), t.bloom_len) != cudaSuccess) {
             cudaGetLastError();
             rt->bloom_dev = nullptr;
@@ -4253,7 +4176,8 @@ int reader_open_tables(dbeel_engine *e, std::vector<ReaderTableRef> tables, cons
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!out || !io.read) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     if (tables.size() > 65536) return fail(e, DBEEL_ERR_TOO_MANY_RUNS, "more than 65536 tables");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    const Claim c(e);
+    if (c.rc) return c.rc;
     const size_t nt = tables.size();
     std::vector<uint64_t> n(nt), data_len(nt);
     std::vector<int32_t> fixed(nt);
@@ -4306,7 +4230,8 @@ int dbeel_engine_create(int device, dbeel_engine **out) {
     if (const char *v = getenv("DBEEL_PARTITION_TAPER")) e->partition_taper = atoi(v) != 0;
     if (const char *v = getenv("DBEEL_STREAM_RING")) e->stream_ring = std::max(2, atoi(v));
     if (const char *v = getenv("DBEEL_PARTITION_MB")) e->partition_bytes = (uint64_t)(atoi(v) > 0 ? atoi(v) : 128) << 20;
-    if (cudaFuncSetAttribute(k_merge_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * kMergeBufRecs * sizeof(Rec))) != cudaSuccess) {
+    if (cudaFuncSetAttribute(k_merge_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * kMergeBufRecs * sizeof(Rec))) != cudaSuccess ||
+        cudaFuncSetAttribute(k_memtable_cuts, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(12ull * kCutSlots)) != cudaSuccess) {
         dbeel_engine_destroy(e);
         return DBEEL_ERR_CUDA;
     }
@@ -4404,14 +4329,8 @@ int dbeel_compact_bound(const dbeel_run *runs, uint32_t n_runs, const dbeel_comp
     return DBEEL_OK;
 }
 
-// While an asynchronous job runs, the worker thread owns e->err and e->stats: a refused call returns the code without
-// touching either (BUSY is an expected answer for a reactor that polls).
-#define REFUSE_WHILE_ASYNC(e)                                                                  \
-    if ((e) && (e)->async_state.load(std::memory_order_acquire) != 0) return DBEEL_ERR_BUSY
-
 int dbeel_compact(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, const dbeel_compact_opts *opts,
                   dbeel_out *out) {
-    REFUSE_WHILE_ASYNC(e);
     return entry(e, runs, n_runs, opts, out, false, false);
 }
 
@@ -4422,7 +4341,6 @@ int dbeel_compact_stream(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs
 
 int dbeel_compact_device(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs, const dbeel_compact_opts *opts,
                          dbeel_out *out) {
-    REFUSE_WHILE_ASYNC(e);
     return entry(e, runs, n_runs, opts, out, false, true);
 }
 
@@ -4441,6 +4359,7 @@ int dbeel_compact_submit(dbeel_engine *e, const dbeel_run *runs, uint32_t n_runs
         e->async_opts.bloom_seed = e->async_seed;
     }
     e->worker = std::thread([e, out]() {
+        t_job_engine = e; // its Claim is not refused by its own job
         e->async_status = entry(e, e->async_runs.data(), (uint32_t)e->async_runs.size(), &e->async_opts, out, false, false);
         e->async_state.store(2, std::memory_order_release);
     });
@@ -4466,7 +4385,6 @@ int dbeel_wait(dbeel_engine *e) {
 }
 
 int dbeel_flush(dbeel_engine *e, const dbeel_run *batch, dbeel_out *out) {
-    REFUSE_WHILE_ASYNC(e);
     return entry(e, batch, batch ? 1 : 0, nullptr, out, true, false);
 }
 
@@ -4474,13 +4392,10 @@ static int flush_many_entry(dbeel_engine *e, const dbeel_run *batches, uint32_t 
                             bool device, bool sparse = false, uint64_t payload_bound = 0) {
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!out || !table || (n && !batches)) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
+    const Claim c(e);
+    if (c.rc) return c.rc;
     dbeel_compact_opts o;
     default_opts(&o);
-    cudaError_t ce = cudaSetDevice(e->device);
-    if (ce != cudaSuccess) return fail(e, DBEEL_ERR_CUDA, "cudaSetDevice", ce);
     for (uint32_t i = 0; i < n; i++) table[i] = dbeel_flush_table{0, 0, 0, 0, 0};
     JobExtra ex;
     ex.flush_table = table;
@@ -4488,120 +4403,81 @@ static int flush_many_entry(dbeel_engine *e, const dbeel_run *batches, uint32_t 
         ex.sparse_offsets = true;
         ex.data_bytes = payload_bound;
     }
-    if (device) return run_job_device(e, batches, n, &o, true, out, true, &ex);
+    if (device) return run_job_device(e, batches, n, &o, true, out, &ex);
     // host buffers: stage everything down, run, bring the concatenated SSTables back
-    uint64_t in_need = 0, dsum = 0, isum = 0;
+    uint64_t dsum = 0, isum = 0;
     for (uint32_t r = 0; r < n; r++) {
         if ((batches[r].data_len && !batches[r].data) || (batches[r].index_len && !batches[r].index))
             return fail(e, DBEEL_ERR_INVALID_ARG, "null batch buffer");
-        in_need += align_up(batches[r].data_len + 32, kAlign) + align_up(batches[r].index_len + 16, kAlign);
         dsum += batches[r].data_len;
         isum += batches[r].index_len / DBEEL_INDEX_ENTRY_SIZE * 16;
     }
     if (out->data_cap < dsum || out->index_cap < isum) return fail(e, DBEEL_ERR_CAPACITY, "output buffer too small");
-    int rc = ensure_device(e, &e->stage_in, &e->stage_in_cap, in_need);
-    if (!rc) rc = ensure_device(e, &e->stage_out, &e->stage_out_cap, align_up(dsum + 16, kAlign) + align_up(isum + 16, kAlign));
-    if (rc) return rc;
-    std::vector<dbeel_run> dr(n);
-    uint64_t pos = 0;
-    for (uint32_t r = 0; r < n; r++) {
-        dr[r] = dbeel_run{e->stage_in + pos, batches[r].data_len, nullptr, batches[r].index_len};
-        if (batches[r].data_len) CU(cudaMemcpyAsync(e->stage_in + pos, batches[r].data, batches[r].data_len, cudaMemcpyHostToDevice, e->stream));
-        pos += align_up(batches[r].data_len + 32, kAlign);
-        dr[r].index = e->stage_in + pos;
-        if (batches[r].index_len) CU(cudaMemcpyAsync(e->stage_in + pos, batches[r].index, batches[r].index_len, cudaMemcpyHostToDevice, e->stream));
-        pos += align_up(batches[r].index_len + 16, kAlign);
-    }
-    dbeel_out dout = *out;
-    dout.data = e->stage_out;
-    dout.index = e->stage_out + align_up(dsum + 16, kAlign);
-    dout.bloom = nullptr;
-    dout.bloom_cap = 0;
-    rc = run_job_device(e, dr.data(), n, &o, true, &dout, true, &ex);
-    if (rc) return rc;
-    if (dout.data_len) CU(cudaMemcpyAsync(out->data, dout.data, dout.data_len, cudaMemcpyDeviceToHost, e->stream));
-    if (dout.index_len) CU(cudaMemcpyAsync(out->index, dout.index, dout.index_len, cudaMemcpyDeviceToHost, e->stream));
-    CU(cudaStreamSynchronize(e->stream));
-    out->data_len = dout.data_len;
-    out->index_len = dout.index_len;
-    out->bloom_len = 0;
-    out->items_written = dout.items_written;
-    return DBEEL_OK;
+    dbeel_out dout;
+    const int rc = stage_outputs(e, dsum, isum, 0, &dout);
+    return rc ? rc : run_job_staged(e, batches, n, &o, true, &dout, 0, out, &ex);
 }
 
 int dbeel_flush_many(dbeel_engine *e, const dbeel_run *batches, uint32_t n_batches, dbeel_out *out, dbeel_flush_table *table) {
-    REFUSE_WHILE_ASYNC(e);
     return flush_many_entry(e, batches, n_batches, out, table, false);
 }
 
 int dbeel_flush_many_device(dbeel_engine *e, const dbeel_run *batches, uint32_t n_batches, dbeel_out *out,
                             dbeel_flush_table *table) {
-    REFUSE_WHILE_ASYNC(e);
     return flush_many_entry(e, batches, n_batches, out, table, true);
 }
 
 int dbeel_flush_many_sparse_device(dbeel_engine *e, const dbeel_run *batches, uint32_t n_batches, uint64_t payload_bound,
                                    dbeel_out *out, dbeel_flush_table *table) {
-    REFUSE_WHILE_ASYNC(e);
     return flush_many_entry(e, batches, n_batches, out, table, true, true, payload_bound);
 }
 
 int dbeel_route_device(dbeel_engine *e, const dbeel_run *batch, const uint32_t *ring_hashes, uint32_t n_shards, void *out_index,
                        uint64_t out_index_cap, uint32_t *shard_of, void *out_key_hash64, uint64_t *counts, uint64_t *payload_bytes) {
-    REFUSE_WHILE_ASYNC(e);
     return route_entry(e, batch, ring_hashes, n_shards, out_index, out_index_cap, shard_of, out_key_hash64, counts, payload_bytes);
 }
 
 int dbeel_memtable_cuts_device(dbeel_engine *e, const void *key_hash64, const uint64_t *stream_starts, uint32_t n_streams,
                                uint32_t capacity, uint32_t *cuts, uint32_t *cut_starts, uint32_t max_cuts_total) {
-    REFUSE_WHILE_ASYNC(e);
     return cuts_entry(e, key_hash64, stream_starts, n_streams, capacity, cuts, cut_starts, max_cuts_total);
 }
 
 int dbeel_flush_device(dbeel_engine *e, const dbeel_run *batch, dbeel_out *out) {
-    REFUSE_WHILE_ASYNC(e);
     return entry(e, batch, batch ? 1 : 0, nullptr, out, true, true);
 }
 
 int dbeel_get_many(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys, const uint64_t *key_offsets,
                    uint64_t n_keys, uint32_t mode, dbeel_lookup_result *results) {
-    REFUSE_WHILE_ASYNC(e);
     return lookup_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, results, false);
 }
 
 int dbeel_get_many_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys,
                           const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_lookup_result *results) {
-    REFUSE_WHILE_ASYNC(e);
     return lookup_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, results, true);
 }
 
 int dbeel_get_values(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys, const uint64_t *key_offsets,
                      uint64_t n_keys, uint32_t mode, dbeel_out *out, dbeel_lookup_result *results) {
-    REFUSE_WHILE_ASYNC(e);
     return get_values_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, out, results, false);
 }
 
 int dbeel_get_values_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys,
                             const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, dbeel_out *out, dbeel_lookup_result *results) {
-    REFUSE_WHILE_ASYNC(e);
     return get_values_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, out, results, true);
 }
 
 int dbeel_get_values_stream(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const void *keys,
                             const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode, const dbeel_scan_io *io,
                             dbeel_out *out, dbeel_lookup_result *results) {
-    REFUSE_WHILE_ASYNC(e);
     return get_values_stream_entry(e, tables, n_tables, keys, key_offsets, n_keys, mode, io, out, results);
 }
 
 int dbeel_reader_open(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, const dbeel_scan_io *io, uint64_t fence_bytes,
                       dbeel_reader **out) {
-    REFUSE_WHILE_ASYNC(e);
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!out || !io || !io->read) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     *out = nullptr;
     if (const int arc = lookup_args(e, tables, n_tables, nullptr, 0, DBEEL_LOOKUP_REFERENCE, nullptr)) return arc;
-    e->err.clear();
     std::vector<ReaderTableRef> rts(n_tables);
     for (uint32_t i = 0; i < n_tables; i++)
         if (const int rc = reader_table_create(e, tables[i], &rts[i])) return rc;
@@ -4611,14 +4487,12 @@ int dbeel_reader_open(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tab
 int dbeel_reader_get_values(dbeel_reader *r, const void *keys, const uint64_t *key_offsets, uint64_t n_keys, uint32_t mode,
                             dbeel_out *out, dbeel_lookup_result *results) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
-    REFUSE_WHILE_ASYNC(r->e);
     const std::vector<dbeel_table> tables = reader_tables(r);
     return get_values_stream_entry(r->e, tables.data(), (uint32_t)tables.size(), keys, key_offsets, n_keys, mode, &r->io, out, results, r);
 }
 
 int dbeel_readers_get_values(dbeel_engine *e, const dbeel_reader_batch *batches, uint32_t n_batches, dbeel_out *out,
                              dbeel_lookup_result *results) {
-    REFUSE_WHILE_ASYNC(e);
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!batches || !out || !results) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     if (n_batches == 0 || n_batches > DBEEL_MAX_READER_BATCHES) return fail(e, DBEEL_ERR_INVALID_ARG, "n_batches is 0 or above DBEEL_MAX_READER_BATCHES");
@@ -4634,10 +4508,8 @@ int dbeel_readers_get_values(dbeel_engine *e, const dbeel_reader_batch *batches,
         if (!x.keys && x.key_offsets[x.n_keys] > x.key_offsets[0]) return fail(e, DBEEL_ERR_INVALID_ARG, "null keys with key bytes");
         n_keys += x.n_keys;
     }
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    e->stats = dbeel_stats{};
+    const Claim c(e);
+    if (c.rc) return c.rc;
     out->data_len = out->index_len = out->bloom_len = out->items_written = 0;
     std::vector<GvsBatch> bs(n_batches);
     for (uint32_t b = 0; b < n_batches; b++) {
@@ -4659,7 +4531,6 @@ int dbeel_reader_scan(dbeel_reader *r, uint32_t kind, const void *ranges, uint32
                       int (*write)(void *ctx, uint32_t dest, uint32_t kind, uint64_t offset, const void *src, uint64_t len),
                       void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
-    REFUSE_WHILE_ASYNC(r->e);
     return reader_range_entry(r, false, kind, ranges, n_ranges, 0, write, ctx, results, stop);
 }
 
@@ -4675,27 +4546,23 @@ int dbeel_reader_get_range(dbeel_reader *r, const dbeel_key_ranges *ranges, uint
                            int (*write)(void *ctx, uint32_t dest, uint32_t kind, uint64_t offset, const void *src, uint64_t len),
                            void *ctx, dbeel_job_result *results, dbeel_scan_stop *stop) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
-    REFUSE_WHILE_ASYNC(r->e);
     return reader_range_entry(r, true, DBEEL_SCAN_KEY, ranges, n_ranges, flags, write, ctx, results, stop);
 }
 
 int dbeel_reader_get_ranges(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, const uint32_t *limits,
                             uint32_t flags, dbeel_out *out, dbeel_range_row *rows) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
-    REFUSE_WHILE_ASYNC(r->e);
     return reader_get_ranges_entry(r, ranges, n_ranges, limits, flags, false, out, rows);
 }
 
 int dbeel_reader_get_ranges_reverse(dbeel_reader *r, const dbeel_key_ranges *ranges, uint32_t n_ranges, const uint32_t *limits,
                                     uint32_t flags, dbeel_out *out, dbeel_range_row *rows) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
-    REFUSE_WHILE_ASYNC(r->e);
     return reader_get_ranges_entry(r, ranges, n_ranges, limits, flags, true, out, rows);
 }
 
 int dbeel_readers_get_ranges(dbeel_engine *e, const dbeel_range_batch *batches, uint32_t n_batches, dbeel_out *out,
                              dbeel_range_row *rows) {
-    REFUSE_WHILE_ASYNC(e);
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!batches || !out || !rows) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     if (n_batches == 0 || n_batches > DBEEL_MAX_READER_BATCHES) return fail(e, DBEEL_ERR_INVALID_ARG, "n_batches is 0 or above DBEEL_MAX_READER_BATCHES");
@@ -4715,17 +4582,14 @@ int dbeel_readers_get_ranges(dbeel_engine *e, const dbeel_range_batch *batches, 
 }
 
 int dbeel_page_cache_create(dbeel_engine *e, uint64_t bytes, dbeel_page_cache **out) {
-    REFUSE_WHILE_ASYNC(e);
     if (!e) return DBEEL_ERR_INVALID_ARG;
     if (!out) return fail(e, DBEEL_ERR_INVALID_ARG, "null argument");
     *out = nullptr;
     const uint64_t slots = bytes / kPageBytes;
     if (slots == 0) return fail(e, DBEEL_ERR_INVALID_ARG, "a page cache needs at least one 4096-byte page");
     if (slots > 0xFFFFFFFFull) return fail(e, DBEEL_ERR_INVALID_ARG, "a page cache holds at most 2^32 - 1 pages");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
-    BusyGuard g(e);
-    e->err.clear();
-    CU(cudaSetDevice(e->device));
+    const Claim claim(e);
+    if (claim.rc) return claim.rc;
     uint8_t *pool = nullptr;
     cudaError_t ce = cudaMalloc(reinterpret_cast<void **>(&pool), slots * kPageBytes);
     if (ce != cudaSuccess) { cudaGetLastError(); return fail(e, DBEEL_ERR_NOMEM, "cudaMalloc(page cache)", ce); }
@@ -4753,17 +4617,17 @@ void dbeel_page_cache_destroy(dbeel_page_cache *c) {
 int dbeel_reader_attach_page_cache(dbeel_reader *r, dbeel_page_cache *c) {
     if (!r) return DBEEL_ERR_INVALID_ARG;
     dbeel_engine *e = r->e;
-    REFUSE_WHILE_ASYNC(e);
     if (c && c->e != e) return fail(e, DBEEL_ERR_INVALID_ARG, "the page cache belongs to another engine");
-    if (e->busy) return fail(e, DBEEL_ERR_BUSY, "engine busy");
+    const Claim claim(e);
+    if (claim.rc) return claim.rc;
     r->cache = c;
     return DBEEL_OK;
 }
 
 int dbeel_page_cache_stats(const dbeel_page_cache *c, struct dbeel_page_cache_stats *out) {
     if (!c || !out) return DBEEL_ERR_INVALID_ARG;
-    REFUSE_WHILE_ASYNC(c->e);
-    if (c->e->busy) return DBEEL_ERR_BUSY;
+    const Claim claim(c->e);
+    if (claim.rc) return claim.rc;
     out->capacity_pages = c->pc.capacity();
     out->resident_pages = c->pc.resident();
     out->hits = c->pc.hits;
@@ -4783,13 +4647,11 @@ int dbeel_scan_bound(const dbeel_table *tables, uint32_t n_tables, uint64_t *dat
 
 int dbeel_scan(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges, uint32_t n_ranges,
                dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop) {
-    REFUSE_WHILE_ASYNC(e);
     return scan_entry(e, tables, n_tables, kind, ranges, n_ranges, out, results, stop, false);
 }
 
 int dbeel_scan_device(dbeel_engine *e, const dbeel_table *tables, uint32_t n_tables, uint32_t kind, const void *ranges,
                       uint32_t n_ranges, dbeel_out *out, dbeel_job_result *results, dbeel_scan_stop *stop) {
-    REFUSE_WHILE_ASYNC(e);
     return scan_entry(e, tables, n_tables, kind, ranges, n_ranges, out, results, stop, true);
 }
 
@@ -4812,23 +4674,19 @@ int dbeel_compact_many_bound(const dbeel_job *jobs, uint32_t n_jobs, uint64_t bl
 
 int dbeel_compact_many(dbeel_engine *e, const dbeel_job *jobs, uint32_t n_jobs, uint64_t bloom_min_size, double bloom_fp,
                        dbeel_out *out, dbeel_job_result *results) {
-    REFUSE_WHILE_ASYNC(e);
     return compact_many_entry(e, jobs, n_jobs, bloom_min_size, bloom_fp, out, results, false);
 }
 
 int dbeel_compact_many_device(dbeel_engine *e, const dbeel_job *jobs, uint32_t n_jobs, uint64_t bloom_min_size, double bloom_fp,
                               dbeel_out *out, dbeel_job_result *results) {
-    REFUSE_WHILE_ASYNC(e);
     return compact_many_entry(e, jobs, n_jobs, bloom_min_size, bloom_fp, out, results, true);
 }
 
 int dbeel_wal_flush(dbeel_engine *e, const void *wal, uint64_t wal_len, uint32_t capacity, dbeel_out *out) {
-    REFUSE_WHILE_ASYNC(e);
     return wal_flush_entry(e, wal, wal_len, capacity, out, false);
 }
 
 int dbeel_wal_flush_device(dbeel_engine *e, const void *wal, uint64_t wal_len, uint32_t capacity, dbeel_out *out) {
-    REFUSE_WHILE_ASYNC(e);
     return wal_flush_entry(e, wal, wal_len, capacity, out, true);
 }
 

@@ -63,7 +63,8 @@ enum {
     DBEEL_ERR_TOO_MANY_ENTRIES = 7,/* more than 2^32-2 input entries in one job             */
     DBEEL_ERR_UNSORTED_RUN = 8,    /* an input run violates "keys strictly ascending"       */
     DBEEL_ERR_NO_DEVICE = 9,       /* no CUDA device / not an sm_90 part                    */
-    DBEEL_ERR_BUSY = 10,           /* engine already has a job in flight                    */
+    DBEEL_ERR_BUSY = 10,           /* another call holds the engine, or a submitted job is  */
+                                   /* unreaped (then err / stats stay the job's)            */
     DBEEL_ERR_BAD_BLOOM = 11,      /* a .bloom file is not a bincode bloomfilter::Bloom      */
     DBEEL_ERR_TREE_FULL = 12       /* rbtree_arena ReachedCapacity (lib.rs:458-461)          */
 };
